@@ -1,5 +1,6 @@
-"""Builds libalazgpu.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libalazgpu.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU)."""
 import os
+import shutil
 import subprocess
 import sys
 
@@ -10,7 +11,7 @@ LIB = os.path.join(LIB_DIR, "libalazgpu.so")
 
 SOURCES = ["alz_api.cu", "alz_kernels.cu", "alz_ingest.cu", "alz_sort.cu", "alz_comm.cu", "alz_gnn.cu", "alz_sock.cu"]
 EXTRA = [os.path.join(HERE, "synth", "alz_synth_topo.c")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 
@@ -36,7 +37,8 @@ def build(force=False, verbose=False, prof=False):
     if not force and not prof and not needs_build():
         return LIB
     os.makedirs(LIB_DIR, exist_ok=True)
-    nvcc = os.environ.get("NVCC", "nvcc")
+    nvcc = os.environ.get("NVCC") or shutil.which("nvcc") or os.path.join(
+        os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
     srcs = [os.path.join(CSRC, s) for s in SOURCES] + EXTRA
     cmd = [nvcc] + NVCC_FLAGS + (["-DALZ_INGEST_PROF"] if prof else []) + (["-Xptxas", "-v"] if verbose else []) + \
         srcs + ["-o", out + ".tmp", "-ldl"]

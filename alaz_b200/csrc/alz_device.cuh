@@ -1,4 +1,4 @@
-// alz_device.cuh — device-side building blocks of libalazgpu (sm_100a).
+// alz_device.cuh — device-side building blocks of libalazgpu (sm_90a).
 //
 // Semantics restated from the reference (file:line = getanteon/alaz @ 828b997f):
 //   row-emit rule      aggregator/data.go:1364-1383 (processL7 switch), :1252-1255,
@@ -118,10 +118,8 @@ __device__ __forceinline__ uint32_t latency_bucket(uint64_t d) {
 // ---- open-addressed u64 dictionary -> dense accumulator rows ---------------------------
 // The dictionary only maps a key to a row number; rows are handed out densely
 // by an atomic counter, so the accumulators of the live keys stay contiguous
-// (190k live pairs x 280 B = 53 MB: L2-resident) however large the dictionary
-// was sized. v1 indexed the accumulators by dictionary slot and every
-// reduction missed L2 (profiles/r1_v2_ingest_ncu.txt: 11 GB DRAM reads for a
-// 3.2 GB stream).
+// however large the dictionary was sized. v1 indexed the accumulators by
+// dictionary slot and nearly every reduction missed L2.
 struct __align__(16) DictEnt {
   uint64_t key;   // kEmptyKey = free
   uint32_t row;   // kNoRow until the inserting thread has published it
@@ -163,7 +161,7 @@ struct AccTable {
   uint32_t* hist;     // [(max_rows + 3) * ALZ_NB] (edge table only)
   // Pair table rows are kept in 32-byte SECTORS, 16 per row (512 B): sector g = { cells 4g, 4g+1 | cells 4g+2, 4g+3 |
   // latency partial u64 | 5xx partial u64 }. A global reduction costs the SM one LSU pass per distinct sector an
-  // instruction touches, not per lane (scripts/micro/red_merge.cu on B200: a histogram increment and a latency add as
+  // instruction touches, not per lane (scripts/micro/red_merge.cu: a histogram increment and a latency add as
   // two instructions = 93 G events/s chip-wide whether or not they share a sector; as ONE red.u64 instruction with two
   // lanes on the same sector = 172 G/s, the price of a single reduction, 188 G/s). So an event's cell and latency live
   // in one sector and are added by a lane pair of one instruction; a row's latency / 5xx totals are the sums of its 16
@@ -224,8 +222,7 @@ __device__ __forceinline__ uint32_t ep_lookup(const EpEntry* __restrict__ tab, u
 // Pair-dictionary insert with the drop rule applied at admission: a NEW socket pair is only
 // inserted if its source address is a pod right now (setFromToV2's first test, data.go:829-832).
 // Unresolvable traffic is often high-cardinality (every event a new pair); letting it into the
-// dictionary cost a CAS, a row and two DRAM-missing reductions per event
-// (profiles/r1_v4_ingest_ncu.txt: 890k row allocations per 100M events, 190k of them real).
+// dictionary cost a CAS, a row and two DRAM-missing reductions per event.
 // Existing pairs are found without touching the endpoint table. Returns kDropRow for a rejected pair.
 constexpr uint32_t kDropRow = 0xFFFFFFFDu;
 __device__ __forceinline__ uint32_t find_or_insert_pair(const AccTable& t, uint64_t key, uint32_t kind,
@@ -293,14 +290,14 @@ __device__ __forceinline__ bool resolve_edge_hostkey(const EpEntry* __restrict__
   return true;
 }
 
-// 32-byte record, one 256-bit load (LDG.E.256 on sm_100a), streaming: bypass L1
+// 32-byte record, two 128-bit loads (the widest global load on sm_90a), streaming: bypass L1
 struct Rec { uint32_t w[8]; };
 __device__ __forceinline__ Rec load_rec(const alz_l7_rec* p) {
   Rec r;
-  asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]),
-                 "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7])
-               : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r.w[0]), "=r"(r.w[1]), "=r"(r.w[2]), "=r"(r.w[3]) : "l"(p));
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4+16];"
+               : "=r"(r.w[4]), "=r"(r.w[5]), "=r"(r.w[6]), "=r"(r.w[7]) : "l"(p));
   return r;
 }
 // field accessors of the packed words (layout of alz_l7_rec)

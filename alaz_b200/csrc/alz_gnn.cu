@@ -8,7 +8,7 @@
 //   CSR     : in-edges grouped by destination (stable sort by dst index, row
 //             offsets = exclusive scan of the in-degrees)
 //   layer   : mean of the in-neighbours' rows (coalesced 256-B row reads) ->
-//             [h_v || m_v] (128) x W (128 x 64) + b, ReLU; the GEMM runs on tcgen05
+//             [h_v || m_v] (128) x W (128 x 64) + b, ReLU; the GEMM runs on wgmma
 //             (sage_layer_tc_kernel, 3xTF32), an FP32 FFMA version is kept for comparison
 //   score   : sigma(a . [h2_u || h2_v || e_uv] + c), e_uv from the edge's
 //             integers and float64 histogram quantiles
@@ -198,20 +198,21 @@ __global__ void __launch_bounds__(256) sage_layer_kernel(const float* __restrict
 }
 
 // ---------------------------------------------------------------------------
-// The same layer on the 5th-gen tensor cores: the feature update
+// The same layer on the Hopper tensor cores: the feature update
 //   [h_v || mean_{u in N_in(v)} h_u]  (128 nodes x 128)  x  W (128 x 64)
 // is the path's one dense contraction. One persistent CTA per SM, tile = 128 nodes:
 //   gather   8 warps build the tile's 128 x 128 operand directly in shared memory in
-//            the UMMA K-major / no-swizzle layout (8 x 16-byte core matrices)
-//   MMA      one thread issues tcgen05.mma.cta_group::1.kind::tf32, M=128 N=64 K=8,
-//            accumulator in TMEM (64 columns)
-//   epilogue 4 warps tcgen05.ld their 32 lanes, add bias, ReLU, store rows
-// Precision: kind::tf32 keeps 10 mantissa bits, which would miss the 1e-5 bound, so
+//            the wgmma K-major / no-swizzle layout (8 x 16-byte core matrices)
+//   MMA      each of the two warpgroups issues wgmma.mma_async m64n64k8 .tf32 on its
+//            64 rows of the tile, accumulator in registers (32 fp32 per thread)
+//   epilogue every thread adds the bias to its accumulator fragment, ReLU, stores
+// Precision: tf32 keeps 10 mantissa bits, which would miss the 1e-5 bound, so
 // both operands are split x = hi + lo (hi = cvt.rna.tf32, lo = x - hi, exact) and
-// the product is accumulated as hi*hi + hi*lo + lo*hi (3xTF32): 48 MMAs per tile.
+// the product is accumulated as hi*hi + hi*lo + lo*hi (3xTF32): 48 wgmma per warpgroup per tile.
 // ---------------------------------------------------------------------------
 namespace tc {
 constexpr uint32_t TM = 128, TK = 128, TN = 64;
+constexpr uint32_t WG_M = 64;                             // rows of the tile per warpgroup
 constexpr uint32_t A_BYTES = TM * TK * 4, B_BYTES = TN * TK * 4;
 constexpr uint32_t A_LBO = (TM / 8) * 128, A_SBO = 128;   // K-adjacent cores TM/8 cores apart; row groups adjacent
 constexpr uint32_t B_LBO = (TN / 8) * 128, B_SBO = 128;
@@ -221,14 +222,11 @@ constexpr uint32_t B_LBO = (TN / 8) * 128, B_SBO = 128;
 __host__ __device__ inline uint32_t op_off(uint32_t r, uint32_t k, uint32_t rows) {
   return (k >> 2) * (rows / 8) * 128 + (r >> 3) * 128 + (r & 7) * 16 + (k & 3) * 4;
 }
-// UMMA shared-memory descriptor (sm_100): start >> 4, LBO >> 4 at bit 16, SBO >> 4 at bit 32,
-// version 1 at bit 46, layout type 0 (no swizzle) at bit 61
+// wgmma shared-memory descriptor (sm_90): start >> 4 at bit 0, LBO >> 4 at bit 16 (K-adjacent core matrices),
+// SBO >> 4 at bit 32 (adjacent 8-row groups), base offset 0, layout type 0 (no swizzle) at bit 62
 __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32) |
-         (1ull << 46);
+  return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
-// instruction descriptor: D = F32 (bit 4), A = B = TF32 (2 << 7, 2 << 10), both K-major, N >> 3 at bit 17, M >> 4 at bit 24
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((TN >> 3) << 17) | ((TM >> 4) << 24);
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t to_tf32(float x) {
@@ -236,17 +234,19 @@ __device__ __forceinline__ uint32_t to_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
   return u;
 }
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t accumulate) {
+// D (64 x 64 fp32, this warpgroup's fragment) += A (64 x 8) * B (8 x 64), both tf32 K-major in shared memory
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-      :: "r"(tmem_d), "l"(da), "l"(db), "r"(kIdesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db)
+      : "memory");
 }
 
 // ---- TMA-staged neighbour gather ---------------------------------------------------------
@@ -276,7 +276,7 @@ __device__ __forceinline__ void tma_row(uint32_t dst, const void* src, uint32_t 
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
-// operand row r, columns kbase + lane and kbase + 32 + lane <- (z0, z1), split hi/lo in the UMMA layout
+// operand row r, columns kbase + lane and kbase + 32 + lane <- (z0, z1), split hi/lo in the wgmma layout
 __device__ __forceinline__ void put_pair(uint8_t* sA_hi, uint8_t* sA_lo, uint32_t r, uint32_t kbase, uint32_t lane,
                                          float z0, float z1) {
   const float z[2] = {z0, z1};
@@ -304,30 +304,20 @@ __global__ void __launch_bounds__(256, 1) sage_layer_tc_kernel(const float* __re
   uint8_t* sA_lo = smem + A_BYTES;
   uint8_t* sB = smem + 2 * A_BYTES;                      // B_hi, then B_lo
   uint8_t* rings = smem + 2 * A_BYTES + 2 * B_BYTES;     // per warp: 2 slots of RING_ROWS rows
-  uint64_t* bars = reinterpret_cast<uint64_t*>(rings + 8 * 2 * RING_BYTES);   // [0] MMA done, [1 + 2w + slot] ring slots
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 1 + 16);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(rings + 8 * 2 * RING_BYTES);   // [2w + slot] ring slots
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
-  uint64_t* mbar = bars;
+  const uint32_t wg = warp >> 2;                         // warpgroup: rows 64 wg .. 64 wg + 63 of the tile
   const float* ring = reinterpret_cast<const float*>(rings + warp * 2 * RING_BYTES);
   const uint32_t ring_a = smem_u32(ring);
-  const uint32_t rbar = smem_u32(bars + 1 + 2 * warp);
+  const uint32_t rbar = smem_u32(bars + 2 * warp);
   uint32_t ring_uses[2] = {0u, 0u};
 
   for (uint32_t i = tid; i < 2 * B_BYTES / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(sB)[i] = reinterpret_cast<const uint4*>(Wcan)[i];
-  if (warp == 0) {   // TMEM: 64 columns for the 128 x 64 fp32 accumulator
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 64;" :: "r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  if (tid == 0) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(smem_u32(mbar)) : "memory");
   if (lane == 0) { mbar_init(rbar, 1u); mbar_init(rbar + 8u, 1u); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-  uint32_t parity = 0;
 
   for (uint32_t tile = blockIdx.x; tile * TM < n_v; tile += gridDim.x) {
     // ---- gather: warp w builds rows 16w .. 16w+15 of the operand (hi and lo parts)
@@ -399,59 +389,50 @@ __global__ void __launch_bounds__(256, 1) sage_layer_tc_kernel(const float* __re
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> tensor-core (async proxy) reads
     __syncthreads();
-    // ---- MMA: one thread, 3 passes x 16 K-steps of M128 N64 K8
-    if (tid == 0) {
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t a_hi = smem_u32(sA_hi), a_lo = smem_u32(sA_lo), b_hi = smem_u32(sB), b_lo = smem_u32(sB + B_BYTES);
+    // ---- MMA: each warpgroup, 3 passes x 16 K-steps of M64 N64 K8 over its 64 rows (8 row groups = 1 KB in)
+    float acc[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+    {
+      const uint32_t a_off = wg * (WG_M / 8) * 128;
+      const uint32_t a_hi = smem_u32(sA_hi) + a_off, a_lo = smem_u32(sA_lo) + a_off;
+      const uint32_t b_hi = smem_u32(sB), b_lo = smem_u32(sB + B_BYTES);
       const uint32_t pa[3] = {a_hi, a_hi, a_lo}, pb[3] = {b_hi, b_lo, b_hi};
-      uint32_t acc = 0;
+      asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
       for (int ps = 0; ps < 3; ++ps) {
+#pragma unroll
         for (uint32_t ks = 0; ks < TK / 8; ++ks) {
           const uint64_t da = smem_desc(pa[ps] + ks * 2 * A_LBO, A_LBO, A_SBO);
           const uint64_t db = smem_desc(pb[ps] + ks * 2 * B_LBO, B_LBO, B_SBO);
-          mma_tf32(tmem_base, da, db, acc);
-          acc = 1;
+          wgmma_tf32(acc, da, db);
         }
       }
-      asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-                   :: "r"(smem_u32(mbar)) : "memory");
+      asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+      asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
     }
-    // ---- epilogue: warps 0..3 own TMEM lanes 32w .. 32w+31
-    if (warp < 4) {
-      uint32_t done = 0;
-      while (!done) {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}\n"
-                     : "=r"(done) : "r"(smem_u32(mbar)), "r"(parity) : "memory");
-      }
-      __syncwarp();   // lane 0 of warp 0 comes from the MMA issue: .sync.aligned loads need the whole warp together
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t v = tile * TM + warp * 32 + lane;
-      float* orow = h_out + (size_t)v * D;
+    // ---- epilogue: accumulator fragment of warp w (of the warpgroup), lane l: rows 16w + l/4 (+8),
+    // columns 8j + 2 (l % 4) (+1) in acc[4j + {0,1}] (+ {2,3} for the row 8 further down)
+    {
+      const uint32_t r0 = tile * TM + wg * WG_M + (warp & 3u) * 16 + (lane >> 2);
 #pragma unroll
-      for (uint32_t c = 0; c < TN; c += 16) {
-        uint32_t acc[16];
-        tmem_ld16(tmem_base + ((warp * 32u) << 16) + c, acc);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      for (uint32_t half = 0; half < 2; ++half) {
+        const uint32_t v = r0 + half * 8;
         if (v < n_v) {
+          float* orow = h_out + (size_t)v * D;
 #pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            float4 o;
-            o.x = fmaxf(__uint_as_float(acc[j + 0]) + bias[c + j + 0], 0.f);
-            o.y = fmaxf(__uint_as_float(acc[j + 1]) + bias[c + j + 1], 0.f);
-            o.z = fmaxf(__uint_as_float(acc[j + 2]) + bias[c + j + 2], 0.f);
-            o.w = fmaxf(__uint_as_float(acc[j + 3]) + bias[c + j + 3], 0.f);
-            *reinterpret_cast<float4*>(orow + c + j) = o;
+          for (uint32_t j = 0; j < TN / 8; ++j) {
+            const uint32_t c = 8 * j + 2 * (lane & 3u);
+            float2 o;
+            o.x = fmaxf(acc[4 * j + 2 * half + 0] + bias[c + 0], 0.f);
+            o.y = fmaxf(acc[4 * j + 2 * half + 1] + bias[c + 1], 0.f);
+            *reinterpret_cast<float2*>(orow + c) = o;
           }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     }
-    parity ^= 1u;
-    __syncthreads();   // operand tile and accumulator are free again
+    __syncthreads();   // the operand tile is free again
   }
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 64;" :: "r"(tmem_base) : "memory");
 }
 }  // namespace tc
 
@@ -527,7 +508,7 @@ struct alz_gnn_state {
   unsigned long long* d_stats = nullptr;
   float *d_h[3] = {nullptr, nullptr, nullptr}, *d_W[2] = {nullptr, nullptr}, *d_b[2] = {nullptr, nullptr};
   float *d_a = nullptr, *d_scores = nullptr;
-  uint8_t* d_Wcan[2] = {nullptr, nullptr};   // per layer: W^T split hi/lo in the UMMA operand layout (64 KB)
+  uint8_t* d_Wcan[2] = {nullptr, nullptr};   // per layer: W^T split hi/lo in the wgmma operand layout (64 KB)
   bool use_tc = true;
   float c = 0.f;
   void* d_tmp = nullptr;
@@ -580,7 +561,7 @@ static int gnn_init_impl(alz_handle* h) {
     CK(cudaMemcpyAsync(g->d_b[l], w.b[l].data(), D * 4, cudaMemcpyHostToDevice, h->stream));
   }
   {
-    const char* simt = getenv("ALZ_GNN_SIMT");   // comparison knob: FP32 FFMA layer instead of tcgen05
+    const char* simt = getenv("ALZ_GNN_SIMT");   // comparison knob: FP32 FFMA layer instead of wgmma
     g->use_tc = !(simt && simt[0] == '1');
     std::vector<float> can(2 * tc::TN * tc::TK);
     for (int l = 0; l < 2; ++l) {

@@ -6,9 +6,8 @@
 // elected lane, L2 evict-first). Lanes copy their records from the ring into registers, the stage
 // goes back to the TMA as soon as those loads have returned, and the next two chunks are in flight
 // while the warp works: no per-lane address arithmetic, no scoreboard stall on the first use of a
-// streamed record (profiles/r2_ingest_phases.json: 3 % of a warp's time waits on the ring; with
-// plain loads, even prefetched into L2 by the TMA engine, it was 28 %), no cross-warp barrier
-// anywhere in the main loop.
+// streamed record (plain loads, even prefetched into L2 by the TMA engine, stall on it), no
+// cross-warp barrier anywhere in the main loop.
 //
 // Work per event, three tiers:
 //   hot   the event's socket pair is in the CTA's shared-memory table. A row holds a 16-bucket
@@ -67,7 +66,7 @@ constexpr uint32_t kBusy = kRowMask;       // entry whose row field is no row: c
 constexpr uint32_t kColdQ = 128;           // cold queue entries per warp (ring): up to 31 left over + 32 + 64 new ones
 constexpr uint32_t kSlowQ = 64;            // slow queue entries per warp (ring)
 constexpr uint32_t kQBytes = 16;           // queue entry {key u64, dur_lo u32, meta u32}
-constexpr uint32_t kSmemMax = 232448;      // 227 KB per CTA on sm_100
+constexpr uint32_t kSmemMax = 232448;      // 227 KB per CTA on sm_90
 constexpr int kU = 2;                      // events per lane per iteration
 constexpr uint32_t kChunk = 32u * kU;      // events per warp per iteration = one TMA copy
 
@@ -106,9 +105,8 @@ __device__ __forceinline__ void red_add_u64(uint64_t* p, uint64_t v) {
   asm volatile("red.relaxed.gpu.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 // the same with an L2 eviction-priority hint: the pair dictionary and the pair rows are the kernel's random-access
-// working set (~100 MB against 126 MB of L2, with 3.2 GB of records streaming through): marked evict-last they
-// stay resident (profiles/r2_ingest_v8_ncu.txt: 11 % of the dictionary probes went to DRAM without the hint,
-// enough for nearly every batch of 32 probes to wait for one)
+// working set (~100 MB at config 2, against 50 MB of L2 on an H100, with 3.2 GB of records streaming through): marked
+// evict-last, as much of it as fits stays resident instead of being pushed out by the stream
 __device__ __forceinline__ void red_add_u32_keep(uint32_t* p, uint32_t v, uint64_t pol) {
   asm volatile("red.relaxed.gpu.global.add.L2::cache_hint.u32 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
 }

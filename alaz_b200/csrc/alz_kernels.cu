@@ -1,4 +1,4 @@
-// alz_kernels.cu — sm_100a kernels of the aggregation hot path.
+// alz_kernels.cu — sm_90a kernels of the aggregation hot path.
 //
 // Plan (DESIGN.md §3): the reference resolves every event through the IP->UID
 // tables and then emits one row (aggregator/data.go:827-870, :1244). Grouping
@@ -12,8 +12,7 @@
 // lane walks the same statements under predicates and meets at __syncwarp()
 // between the divergent dictionary probes and the reductions. The first
 // version let lanes leave the probe loops on their own paths and the
-// reductions then issued with ~2 active lanes per instruction
-// (profiles/r1_v2_ingest_ncu.txt).
+// reductions then issued with ~2 active lanes per instruction.
 #include <algorithm>
 
 #include "alz_kernels.cuh"
@@ -184,7 +183,7 @@ __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const
 
 // pass 2, eight lanes per pair row (four rows per warp in flight): add the row into its edge row and
 // zero it. Each lane owns 8 histogram cells = two 16-byte loads; the one-warp-per-row version was bound
-// by its chain of dependent L2 round trips (profiles/r1_final_launches.csv: 0.15 ms per launch).
+// by its chain of dependent L2 round trips.
 __global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTable edges, Counters* ctr,
                                                          uint32_t* __restrict__ hot_bins) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;

@@ -10,6 +10,7 @@ stream), so the hot-pair list a fold leaves behind is a prediction for the next 
 not a replay of it; the very first window (no history) is timed separately.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5]
+                  [--dump-outputs DIR]
 
 Configs are BASELINE.json's (index into `configs`):
   2 (default, the one `metric` is quoted on at N=1): 10k services / 100M events per GPU per step
@@ -20,9 +21,8 @@ At N>1 every rank ingests its own shard of the global stream (events owned by
 alz_owner_rank(saddr)): weak scaling for config 2 (100M per rank), the named totals split
 over the ranks for 4 and 5.
 
-`--impl reference` times the CPU restatement of the reference aggregator (oracle/alz_oracle.c —
-the Go binary cannot be built here, SURVEY.md §8c) on the box's host cores, on a bounded
-sample of the same workload.
+`--impl reference` times the CPU restatement of the reference aggregator (oracle/alz_oracle.c;
+the reference is Go, SURVEY.md §8c) on the host's cores, on a bounded sample of the same workload.
 """
 import argparse
 import ctypes as C
@@ -77,6 +77,8 @@ def parse_args():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-gnn", action="store_true", help="skip the separate GNN-update timing (config 2)")
     ap.add_argument("--no-verify", action="store_true", help="skip the in-run parity check against the oracle")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed to DIR/<name>.npy (float64)")
     return ap.parse_args()
 
 
@@ -105,7 +107,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def measured_traffic(kernel, config):
@@ -121,7 +123,7 @@ def measured_traffic(kernel, config):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -293,6 +295,8 @@ def main():
     h = new_handle()
     if world > 1:
         comm_setup(h, dist, rank, world, torch)
+    if with_gnn:
+        gnn_score_device(h)   # allocates the GNN buffers (sized by max_edges) before the windows take what is left
 
     # ---- inputs resident in HBM before the timed region: R distinct windows, rotated
     free_b, _ = torch.cuda.mem_get_info()
@@ -348,18 +352,21 @@ def main():
     sampler.mark()
     ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(steps)]
     t_all0, t_all1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    p_edges, p_scores = None, None
     t_all0.record(stream)
     for k in range(steps):
         ev[k][0].record(stream)
         h.submit_device(d_win[(warmup + k) % R], N)
         ev[k][1].record(stream)
-        _, n_edges = h.flush_device()
+        p_edges, n_edges = h.flush_device()
         ev[k][2].record(stream)
         if with_gnn:
-            gnn_score_device(h)
+            p_scores, _ = gnn_score_device(h)
         ev[k][3].record(stream)
     t_all1.record(stream)
     barrier()
+    if args.dump_outputs and rank == 0 and p_edges is not None:   # every rank holds the same merged edges
+        dump_outputs(args.dump_outputs, h, abi, p_edges, n_edges, p_scores)
     total_ms = t_all0.elapsed_time(t_all1)
     ingest_ms = float(np.mean([e[0].elapsed_time(e[1]) for e in ev]))
     flush_ms = float(np.mean([e[1].elapsed_time(e[2]) for e in ev]))
@@ -473,6 +480,40 @@ def gnn_score_device(h):
     return p.value, n_out.value
 
 
+DUMP_MAX_EDGES = 1 << 16   # 72 float64 columns per edge: at most 38 MB of edge rows
+
+
+def dump_outputs(out_dir, h, abi, p_edges, n, p_scores):
+    """Writes the edge rows of the last timed step as float64 arrays, in canonical (from, to) order: all of them, or
+    a fixed seeded sample of DUMP_MAX_EDGES when there are more, and the GNN score of each written edge when the
+    step scores. totals.npy holds, over every edge, the edge count and the sums of count, of err5xx and of
+    lat_sum_ns >> 20 (whole 2^20-ns units, so that the sum stays exact in float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    e = h.d2h(p_edges, n, abi.EDGE_OUT)
+    scores = h.d2h(p_scores, n, np.float32) if p_scores is not None else None
+    order = np.lexsort((e["to"], e["to_type"], e["from"], e["from_type"]))
+    e = e[order]
+    pick = np.arange(n) if n <= DUMP_MAX_EDGES else \
+        np.sort(np.random.default_rng(SEED).choice(n, DUMP_MAX_EDGES, replace=False))
+    s = e[pick]
+    lat = s["lat_sum_ns"]
+    arrays = {
+        "edge_index": pick.astype(np.float64),
+        "edge_ends": np.stack([s["from_type"], s["from"], s["to_type"], s["to"]], axis=1).astype(np.float64),
+        "edge_count": s["count"].astype(np.float64),
+        "edge_err5xx": s["err5xx"].astype(np.float64),
+        # a u64 sum can exceed float64's 53-bit mantissa: stored exactly as its two 32-bit halves
+        "edge_lat_sum_ns_hi_lo": np.stack([lat >> np.uint64(32), lat & np.uint64(0xFFFFFFFF)], axis=1).astype(np.float64),
+        "edge_hist": s["hist"].astype(np.float64),
+        "totals": np.array([n, e["count"].sum(dtype=np.uint64), e["err5xx"].sum(dtype=np.uint64),
+                            (e["lat_sum_ns"] >> np.uint64(20)).sum(dtype=np.uint64)], dtype=np.float64),
+    }
+    if scores is not None:
+        arrays["edge_gnn_score"] = scores[order][pick].astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def verify_window(h, capi, abi, topo, d_ev, N, S, world, rank, dist, torch):
     """Re-run one window and check it: (a) every rank's merged edge array is byte-identical (64-bit sums over
     the device buffer, all-gathered); (b) on every rank, the edges whose source pod falls in a 1/64 sample are
@@ -562,7 +603,7 @@ def run_e2e(h, capi, abi, d_win, N, steps_dev, world, dist, torch):
         del r16
     out = capi.PinnedBuffer(h.max_edges, abi.EDGE_OUT, handle=h)
     n_out = C.c_size_t(0)
-    steps = max(3, min(steps_dev, 6))
+    steps = steps_dev
 
     def one(k):
         pin, pov, no = pins[k % W]

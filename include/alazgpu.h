@@ -1,5 +1,5 @@
 /*
- * alazgpu.h — C ABI of libalazgpu: the B200-native replacement for the
+ * alazgpu.h — C ABI of libalazgpu: the H100-native replacement for the
  * service-map aggregation hot path of getanteon/alaz (reference @ 828b997f).
  *
  * The reference has no FFI boundary for this path; the seam this library sits

@@ -1,6 +1,6 @@
 #!/bin/bash
 # Evidence for profiles/: launch list of the default bench command, one full capture of the ingest kernel
-# (warm caches), one of the GNN layer, SASS proof of the TMA / cp.async / tcgen05 instructions.
+# (warm caches), one of the GNN layer, SASS proof of the TMA / cp.async / wgmma instructions.
 set -u
 mkdir -p gpurun_out
 echo "== launch list"

@@ -5,7 +5,7 @@
 //   C  ONE red.u64 instruction, lane pairs: even lane the cell pair, odd lane the lat partial of the same sector
 //   D  one red.u32 only (lower bound)
 //   E  like C but four lanes per event all in one sector (cell, lat, err, count)
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o red_merge red_merge.cu
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o red_merge red_merge.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -49,7 +49,9 @@ template <int kMode>
 double run(uint32_t* hist, uint64_t* lat, uint64_t* sect, uint32_t ept, int lanes_per_event, const char* name) {
   cudaEvent_t a, b;
   cudaEventCreate(&a); cudaEventCreate(&b);
-  const int blocks = 148 * 4;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+  const int blocks = sms * 4;
   k<kMode><<<blocks, 512>>>(hist, lat, sect, ept);   // warm
   cudaEventRecord(a);
   for (int r = 0; r < 5; ++r) k<kMode><<<blocks, 512>>>(hist, lat, sect, ept);

@@ -1,7 +1,7 @@
-// Microbenchmark: what does a shared-memory atomic cost on sm_100a at full occupancy (32 warps / SM)?
+// Microbenchmark: what does a shared-memory atomic cost on sm_90a at full occupancy (32 warps / SM)?
 // Variants: no-return add, returning add, plain load+store RMW; address patterns: every lane its own word
 // (random rows), a hot word shared by a fraction of the lanes. Prints SM cycles per warp-instruction.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o smem_atomics smem_atomics.cu && ./smem_atomics
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o smem_atomics smem_atomics.cu && ./smem_atomics
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -41,14 +41,16 @@ __global__ void __launch_bounds__(1024, 1) k(uint32_t* out, long long* cycles, u
 template <int kMode>
 void run(const char* name, uint32_t hot) {
   uint32_t* out; long long* cyc;
-  cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 148 * 8);
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);   // one CTA per SM
+  cudaMalloc(&out, (size_t)sms * 1024 * 4); cudaMalloc(&cyc, (size_t)sms * 8);
   cudaFuncSetAttribute(k<kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWords * 4);
-  k<kMode><<<148, 1024, kWords * 4>>>(out, cyc, hot, 1);
-  k<kMode><<<148, 1024, kWords * 4>>>(out, cyc, hot, 2);
+  k<kMode><<<sms, 1024, kWords * 4>>>(out, cyc, hot, 1);
+  k<kMode><<<sms, 1024, kWords * 4>>>(out, cyc, hot, 2);
   cudaDeviceSynchronize();
-  long long h[148]; cudaMemcpy(h, cyc, sizeof h, cudaMemcpyDeviceToHost);
-  double s = 0; for (int i = 0; i < 148; ++i) s += (double)h[i];
-  s /= 148;
+  long long h[1024]; cudaMemcpy(h, cyc, (size_t)sms * 8, cudaMemcpyDeviceToHost);
+  double s = 0; for (int i = 0; i < sms; ++i) s += (double)h[i];
+  s /= sms;
   // 32 warps each issue kIters warp-instructions (mode 3: two atomics per iteration)
   printf("%-34s hot lanes/32 = %2u : %7.1f cycles per warp-iteration (all 32 warps), %6.2f per lane-op\n", name, hot,
          s / kIters / 32.0 * 32.0 / 32.0 * 32.0, s / kIters / 1024.0 / (kMode == 3 ? 2.0 : 1.0));
