@@ -171,18 +171,18 @@ __global__ void __launch_bounds__(256) sage_layer_kernel(const float* __restrict
   const uint32_t warps_per_grid = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; v < n_v; v += warps_per_grid) {
     const uint32_t beg = rowptr[v], end = rowptr[v + 1];
-    float m0 = 0.f, m1 = 0.f;
+    double m0 = 0.0, m1 = 0.0;                       // float64: a hub's many similar rows do not drift (SPEC §6)
     for (uint32_t p = beg; p < end; ++p) {          // CSR order: deterministic sum
       const float* hu = h_in + (size_t)col[p] * D;
-      m0 += hu[lane];
-      m1 += hu[32 + lane];
+      m0 += (double)hu[lane];
+      m1 += (double)hu[32 + lane];
     }
-    const float inv = end > beg ? 1.0f / (float)(end - beg) : 0.f;
+    const double inv = end > beg ? 1.0 / (double)(end - beg) : 0.0;
     const float* hv = h_in + (size_t)v * D;
     sz[warp][lane] = hv[lane];
     sz[warp][32 + lane] = hv[32 + lane];
-    sz[warp][64 + lane] = m0 * inv;
-    sz[warp][96 + lane] = m1 * inv;
+    sz[warp][64 + lane] = (float)(m0 * inv);
+    sz[warp][96 + lane] = (float)(m1 * inv);
     __syncwarp();
     float a0 = b[lane], a1 = b[32 + lane];
 #pragma unroll 8
@@ -356,12 +356,12 @@ __global__ void __launch_bounds__(256, 1) sage_layer_tc_kernel(const float* __re
     if (n_chunks > 1) issue(1, 0u);
     uint32_t r = 0;                                   // current row of the warp
     uint32_t row_end = n_rows ? rowptr[v0 + 1] : 0u, row_beg = e_beg;
-    float m0 = 0.f, m1 = 0.f;
+    double m0 = 0.0, m1 = 0.0;                        // float64 neighbour sums (SPEC §6), as in the SIMT layer
     auto close_rows_until = [&](uint32_t e) {         // rows that end at or before edge e are complete
       while (r < n_rows && row_end <= e) {
-        const float inv = row_end > row_beg ? 1.0f / (float)(row_end - row_beg) : 0.f;
-        put_pair(sA_hi, sA_lo, warp * 16 + r, 64u, lane, m0 * inv, m1 * inv);
-        m0 = m1 = 0.f;
+        const double inv = row_end > row_beg ? 1.0 / (double)(row_end - row_beg) : 0.0;
+        put_pair(sA_hi, sA_lo, warp * 16 + r, 64u, lane, (float)(m0 * inv), (float)(m1 * inv));
+        m0 = m1 = 0.0;
         ++r;
         row_beg = row_end;
         if (r < n_rows) row_end = rowptr[v0 + r + 1];
@@ -376,8 +376,8 @@ __global__ void __launch_bounds__(256, 1) sage_layer_tc_kernel(const float* __re
         close_rows_until(first + j);
         const float* row = ring + (slot * RING_ROWS + j) * D;
         last = row[lane];
-        m0 += last;
-        m1 += row[32 + lane];
+        m0 += (double)last;
+        m1 += (double)row[32 + lane];
       }
       __syncwarp();
       if (c + 2 < n_chunks) issue(c + 2, __float_as_uint(last) & zero_rt);   // the slot goes back to the TMA

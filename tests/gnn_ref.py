@@ -1,6 +1,7 @@
 """numpy float64 restatement of docs/SPEC.md §6 (GNN anomaly pass). TEST INFRASTRUCTURE ONLY:
 the oracle for alz_gnn_score. Shares no code with alaz_b200/csrc/alz_gnn.cu."""
 import numpy as np
+from scipy import sparse
 
 M64 = (1 << 64) - 1
 SEED = 0xA1A26E6E
@@ -89,23 +90,23 @@ def quantiles_vec(hist, q):
     return np.where(total > 0.0, val, 0.0)
 
 
-def run(edges):
-    """edges: alz_edge_out array (any order). Returns (node_keys, h2, scores) with scores in the input order."""
-    n_e = len(edges)
+def _graph(edges):
+    """Node keys, edge ends (u, v) and the float32-stored features h0 (SPEC §6). The per-node sums of count,
+    5xx and latency are u64 and wrap mod 2^64 like the edge accumulators (SPEC §3); they become float64 only
+    for the features."""
     fk = (edges["from_type"].astype(np.uint64) << np.uint64(32)) | edges["from"].astype(np.uint64)
     tk = (edges["to_type"].astype(np.uint64) << np.uint64(32)) | edges["to"].astype(np.uint64)
     nodes = np.unique(np.concatenate([fk, tk]))
     n_v = len(nodes)
     u = np.searchsorted(nodes, fk)
     v = np.searchsorted(nodes, tk)
-    st = np.zeros((n_v, 8), dtype=np.float64)
-    cnt = edges["count"].astype(np.float64)
-    err = edges["err5xx"].astype(np.float64)
-    lat = edges["lat_sum_ns"].astype(np.float64)
-    np.add.at(st[:, 0], u, cnt); np.add.at(st[:, 1], v, cnt)
-    np.add.at(st[:, 2], u, err); np.add.at(st[:, 3], v, err)
-    np.add.at(st[:, 4], u, lat); np.add.at(st[:, 5], v, lat)
-    np.add.at(st[:, 6], u, 1.0); np.add.at(st[:, 7], v, 1.0)
+    st = np.zeros((n_v, 8), dtype=np.uint64)
+    for k, f in enumerate(("count", "err5xx", "lat_sum_ns")):
+        x = edges[f].astype(np.uint64)
+        np.add.at(st[:, 2 * k], u, x)        # uint64 adds: mod 2^64
+        np.add.at(st[:, 2 * k + 1], v, x)
+    np.add.at(st[:, 6], u, np.uint64(1)); np.add.at(st[:, 7], v, np.uint64(1))
+    st = st.astype(np.float64)
 
     def ratio(a, b):
         return np.divide(a, b, out=np.zeros_like(a), where=b > 0)
@@ -117,18 +118,40 @@ def run(edges):
     h[:, 6] = np.log1p(st[:, 6]); h[:, 7] = np.log1p(st[:, 7])
     h[:, 8] = kind == 0; h[:, 9] = kind == 1; h[:, 10] = kind >= 2; h[:, 11] = 1.0   # outbound, by address or by Host header
     h = h.astype(np.float32).astype(np.float64)   # features are stored as float32
-    W, b, a, c = weights()
-    indeg = st[:, 7]
+    return nodes, u, v, st[:, 7], h
+
+
+def _layers(h, u, v, indeg, W, b):
+    """Two GraphSAGE-mean layers; the neighbour means are float64 sums (SPEC §6)."""
+    n_v = len(h)
+    # A[v, u] = 1 per edge u -> v: the neighbour sums as one sparse product, float64
+    A = sparse.csr_matrix((np.ones(len(u)), (v, u)), shape=(n_v, n_v))
     for l in range(2):
-        m = np.zeros((n_v, D), dtype=np.float64)
-        np.add.at(m, v, h[u])
+        m = np.asarray(A @ h)
         m = np.divide(m, indeg[:, None], out=np.zeros_like(m), where=indeg[:, None] > 0)
         z = np.concatenate([h, m], axis=1)
         h = np.maximum(z @ W[l] + b[l], 0.0)
+    return h
+
+
+def run(edges, with_scale=False):
+    """edges: alz_edge_out array (any order). Returns (node_keys, h2, scores) with scores in the input order.
+    with_scale: also the magnitude pass, the same two layers on |h0|, |W| and |b|: for every element of h2, the sum
+    of the absolute values of every term that went into it (the scale an elementwise error bound refers to)."""
+    n_e = len(edges)
+    nodes, u, v, indeg, h0 = _graph(edges)
+    W, b, a, c = weights()
+    h = _layers(h0, u, v, indeg, W, b)
+    cnt = edges["count"].astype(np.float64)
+    err = edges["err5xx"].astype(np.float64)
     e_feat = np.zeros((n_e, 4), dtype=np.float64)
     e_feat[:, 0] = np.log1p(cnt)
-    e_feat[:, 1] = ratio(err, cnt)
+    e_feat[:, 1] = np.divide(err, cnt, out=np.zeros_like(err), where=cnt > 0)
     e_feat[:, 2] = np.log1p(quantiles_vec(edges["hist"], 0.5))
     e_feat[:, 3] = np.log1p(quantiles_vec(edges["hist"], 0.99))
     zz = np.concatenate([h[u], h[v], e_feat], axis=1) @ a + c
-    return nodes, h, 1.0 / (1.0 + np.exp(-zz))
+    scores = 1.0 / (1.0 + np.exp(-zz))
+    if not with_scale:
+        return nodes, h, scores
+    scale = _layers(np.abs(h0), u, v, indeg, [np.abs(w) for w in W], [np.abs(x) for x in b])
+    return nodes, h, scores, scale
