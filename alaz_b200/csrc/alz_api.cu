@@ -100,11 +100,17 @@ static void free_table(AccTable* t) {
   cudaFree(t->err5xx); cudaFree(t->count); cudaFree(t->row_cnt); cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->hist); cudaFree(t->sect);
   memset(t, 0, sizeof(*t));
 }
-// all keys out of the dictionaries, row allocator back to zero (rows were zeroed by fold / gather)
-static int clear_dict(alz_handle* h, AccTable* t) {
+// all keys out of the dictionaries; the rows keep their indices until clear_dict resets the allocator
+static int clear_keys(alz_handle* h, AccTable* t) {
   CK(cudaMemsetAsync(t->dict, 0xFF, ((size_t)t->dict_mask + 1) * sizeof(DictEnt), h->stream));
   if (t->dict_rev) CK(cudaMemsetAsync(t->dict_rev, 0xFF, ((size_t)t->dict_rev_mask + 1) * sizeof(DictEnt), h->stream));
   if (t->dict_host) CK(cudaMemsetAsync(t->dict_host, 0xFF, ((size_t)t->dict_host_mask + 1) * sizeof(DictEnt), h->stream));
+  return ALZ_OK;
+}
+// all keys out of the dictionaries, row allocator back to zero (rows were zeroed by fold / emit)
+static int clear_dict(alz_handle* h, AccTable* t) {
+  int rc = clear_keys(h, t);
+  if (rc != ALZ_OK) return rc;
   CK(cudaMemsetAsync(t->n_rows, 0, 4, h->stream));
   return ALZ_OK;
 }
@@ -192,8 +198,19 @@ extern "C" int alz_create(const alz_config* cfg, alz_handle** out) {
     CKC(cudaMalloc(&h->d_keys[b], (size_t)h->cfg.max_edges * 8));
     CKC(cudaMalloc(&h->d_rows[b], (size_t)h->cfg.max_edges * 4));
   }
-  h->sort_tmp_bytes = sort_pairs_temp_bytes(h->cfg.max_edges);
+  // shared by the key sort and the scan of the bucket counts, which run one after the other in stream order
+  h->sort_tmp_bytes = std::max(sort_pairs_temp_bytes(h->cfg.max_edges), scan_temp_bytes(h->cfg.max_edges + 1));
   CKC(cudaMalloc(&h->d_sort_tmp, h->sort_tmp_bytes));
+  if (!(h->cfg.flags & ALZ_CFG_EAGER_JOIN)) {
+    const size_t n_cnt = (size_t)h->cfg.max_edges + 1;
+    h->bk.cap = h->cfg.max_pairs + kPairKinds;
+    CKC(cudaMalloc(&h->bk.cnt, n_cnt * 4));
+    CKC(cudaMemsetAsync(h->bk.cnt, 0, n_cnt * 4, h->stream));
+    CKC(cudaMalloc(&h->bk.off, n_cnt * 4));
+    CKC(cudaMalloc(&h->bk.rows, (size_t)h->bk.cap * 4));
+    CKC(cudaMalloc(&h->bk.n_stray, 4));
+    CKC(cudaMemsetAsync(h->bk.n_stray, 0, 4, h->stream));
+  }
   CKC(cudaMalloc(&h->d_out, (size_t)h->cfg.max_edges * sizeof(alz_edge_out)));
   CKC(cudaStreamSynchronize(h->stream));
 #undef CKC
@@ -231,6 +248,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   if (h->ev_patch) cudaEventDestroy(h->ev_patch);
   for (int i = 0; i < 3; ++i) if (h->ev_t[i]) cudaEventDestroy(h->ev_t[i]);
   cudaFree(h->d_sort_tmp); cudaFree(h->d_out);
+  cudaFree(h->bk.cnt); cudaFree(h->bk.off); cudaFree(h->bk.rows); cudaFree(h->bk.n_stray);
   if (h->own_stream) cudaStreamDestroy(h->own_stream);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   delete h;
@@ -485,6 +503,7 @@ static int fold_second_half(alz_handle* h) {
   CK(cudaGetLastError());
   int rc = clear_dict(h, &h->pairs);
   h->pending_since_fold = 0;
+  h->edges_dirty = true;
   return rc;
 }
 static int fold_locked(alz_handle* h) {
@@ -680,10 +699,13 @@ extern "C" int alz_submit_l7_raw(alz_handle* h, const void* raw, size_t n) {
 }
 
 // ---- window result ---------------------------------------------------------------------------
-// Fold + sort of the live edge keys (no reset). After it h->n_live edges sit in d_keys[1]/d_rows[1].
-// The edge count is final once the first half of the fold has run, so the counters are copied out right
-// there and the host waits on an event for THAT copy only: the second half of the fold is still
-// running on the GPU while the host sizes and enqueues the sort (r1 stalled the whole stream here).
+// Resolve + sort of the live edge keys (no reset). After it h->n_live edges sit in d_keys[1]/d_rows[1].
+// The edge count is final once fold_resolve_kernel has run, so the counters are copied out right there and
+// the host waits on an event for THAT copy only. What does not need the count is enqueued before the wait and
+// keeps the GPU busy while the host sizes and enqueues the sort:
+//  - one rank: the pair rows are bucketed by edge row and the pair dictionaries cleared (nothing probes them
+//    after the resolve); finish_flush sums each bucket straight into its output row;
+//  - several ranks: the rest of the fold into the edge table, which the merge reads (alz_comm.cu).
 // *overflow: the window lost rows (pair or edge table full); the flush still emits what it has.
 static int prepare_flush(alz_handle* h, bool* overflow) {
   *overflow = false;
@@ -692,7 +714,15 @@ static int prepare_flush(alz_handle* h, bool* overflow) {
   if (fold && (rc = fold_first_half(h)) != ALZ_OK) return rc;
   CK(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaEventRecord(h->ev_count, h->stream));
-  if (fold && (rc = fold_second_half(h)) != ALZ_OK) return rc;
+  if (fold && h->comm_nranks <= 1) {
+    launch_bucket_count(h->pairs, h->cfg.max_edges, h->bk, h->sms, h->stream);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    if ((rc = clear_keys(h, &h->pairs)) != ALZ_OK) return rc;
+    h->bucketed = true;
+  } else if (fold && (rc = fold_second_half(h)) != ALZ_OK) {
+    return rc;
+  }
   CK(cudaEventSynchronize(h->ev_count));
   h->n_live = h->h_ctr->edge_rows;
   if (h->n_live > h->cfg.max_edges) { h->n_live = h->cfg.max_edges; *overflow = true; }
@@ -708,12 +738,36 @@ static int prepare_flush(alz_handle* h, bool* overflow) {
   return ALZ_OK;
 }
 
+// Single rank: the output rows in key order, each the sum of its edge's pair rows (and of the edge accumulators
+// when a fold already ran in this window); the edge table and the pair rows are left zeroed for the next window.
 static int finish_flush(alz_handle* h) {
-  launch_gather_edges(h->edges, h->d_keys[1], h->d_rows[1], h->n_live, h->d_out, true, h->sms, h->stream);
-  h->launches += h->n_live ? 1 : 0;
+  const FlushBuckets* b = nullptr;
+  if (h->bucketed) {
+    // cnt[n_live] is zero (every edge row of a pair row is below n_live), so off[n_live] ends the last bucket
+    exclusive_scan_u32(h->d_sort_tmp, h->sort_tmp_bytes, h->bk.cnt, h->bk.off, h->n_live + 1, h->stream);
+    launch_bucket_fill(h->pairs, h->cfg.max_edges, h->bk, h->sms, h->stream);
+    h->launches += 1;
+    b = &h->bk;
+  }
+  const bool with_edges = h->edges_dirty || (h->cfg.flags & ALZ_CFG_EAGER_JOIN);
+  if (b || h->n_live) {
+    launch_emit_edges(h->pairs, h->edges, h->d_ctr, h->d_hot, h->d_keys[1], h->d_rows[1], h->n_live, b, with_edges,
+                      h->d_out, h->sms, h->stream);
+    h->launches += 1;
+  }
   CK(cudaGetLastError());
+  if (h->bucketed) {
+    CK(cudaMemsetAsync(h->bk.n_stray, 0, 4, h->stream));
+    launch_hot_select(h->pairs, h->d_hot, h->sms, h->stream);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    CK(cudaMemsetAsync(h->pairs.n_rows, 0, 4, h->stream));
+    h->bucketed = false;
+    h->pending_since_fold = 0;
+  }
   int rc = clear_dict(h, &h->edges);
   if (rc != ALZ_OK) return rc;
+  h->edges_dirty = false;
   h->last_n_edges = h->n_live;
   h->windows++;
   return ALZ_OK;
@@ -774,7 +828,16 @@ extern "C" int alz_window_flush(alz_handle* h, alz_edge_out* out, size_t cap, si
     int rc = prepare_flush(h, &overflow);
     *n_out = h->n_live;
     if (rc != ALZ_OK) return rc;
-    if (h->n_live > cap) { if (overflow) h->lost_reported = ~0ull; return ALZ_E_CAPACITY; }   // report the loss again next time
+    if (h->n_live > cap) {
+      if (overflow) h->lost_reported = ~0ull;   // report the loss again next time
+      if (h->bucketed) {                        // keep the window: the bucketed pair rows go into the edge table
+        CK(cudaMemsetAsync(h->bk.cnt, 0, ((size_t)h->cfg.max_edges + 1) * 4, h->stream));
+        CK(cudaMemsetAsync(h->bk.n_stray, 0, 4, h->stream));
+        h->bucketed = false;
+        if ((rc = fold_second_half(h)) != ALZ_OK) return rc;
+      }
+      return ALZ_E_CAPACITY;
+    }
     rc = finish_flush(h);
     if (rc != ALZ_OK) return rc;
     if (h->n_live) CK(cudaMemcpyAsync(out, h->d_out, (size_t)h->n_live * sizeof(alz_edge_out),

@@ -490,7 +490,7 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc) {
   }
   // local rows behind the header, in canonical order; the window is NOT reset yet
   if (n_local) {
-    launch_gather_edges(h->edges, h->d_keys[1], h->d_rows[1], n_local, c->d_send + 1, false, h->sms, s);
+    launch_gather_edges(h->edges, h->d_keys[1], h->d_rows[1], n_local, c->d_send + 1, h->sms, s);
     h->launches += 1;
   }
   for (int attempt = 0; attempt < 4; ++attempt) {

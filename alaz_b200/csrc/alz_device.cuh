@@ -165,7 +165,7 @@ struct AccTable {
   // two instructions = 93 G events/s chip-wide whether or not they share a sector; as ONE red.u64 instruction with two
   // lanes on the same sector = 172 G/s, the price of a single reduction, 188 G/s). So an event's cell and latency live
   // in one sector and are added by a lane pair of one instruction; a row's latency / 5xx totals are the sums of its 16
-  // partials (fold_pairs_kernel). A cell pair is added to as a u64: cells are u32 and a fold runs before any cell
+  // partials (take_pair_row, alz_kernels.cu). A cell pair is added to as a u64: cells are u32 and a fold runs before any cell
   // could reach 2^31 (alz_api.cu), so nothing carries from the low cell into the high one.
   uint64_t* sect;     // [(max_rows + 3) * kSectPerRow * 4] (pair table only; hist / lat_sum / err5xx are null there)
 };

@@ -80,6 +80,9 @@ struct alz_handle {
   size_t sort_tmp_bytes = 0;
   alz_edge_out* d_out = nullptr;
   uint32_t n_live = 0, last_n_edges = 0;
+  alz::FlushBuckets bk{};                 // single-rank flush: pair rows by edge row (not with ALZ_CFG_EAGER_JOIN)
+  bool bucketed = false;                  // prepare_flush bucketed the pair rows; finish_flush emits them
+  bool edges_dirty = false;               // a fold since the last flush left sums in the edge accumulators
   uint64_t lost_reported = 0;             // capacity_events already reported by an earlier flush
 
   // time-cut windows (alz_window_clock)

@@ -757,7 +757,7 @@ __global__ void win_advance_kernel(WinClock* win) {
 }
 
 // ---- hot-pair feedback: after a fold, pick the pairs that took the most events -----
-// fold_pairs_kernel left row_cnt[row], row_base[row] and a 128-bin (quarter-octave) histogram of the counts of
+// the fold (fold_pairs_kernel, or emit_edges_kernel at a single-rank flush) left row_cnt[row], row_base[row] and a 128-bin (quarter-octave) histogram of the counts of
 // the forward rows; thresholds = the lowest bins that keep tier A <= kHotA and A+B <= target. Every block derives
 // the same two thresholds from the bins itself (128 adds) instead of a separate launch.
 __global__ void __launch_bounds__(256) hot_emit_kernel(AccTable pairs, HotState* hot, uint32_t target_total) {
@@ -838,7 +838,7 @@ void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const AccT
 }
 void launch_window_advance(uint64_t* win, cudaStream_t s) { win_advance_kernel<<<1, 32, 0, s>>>((WinClock*)win); }
 
-// after fold_pairs_kernel(pairs, ..., hot->bins): choose next window's hot list
+// after fold_pairs_kernel / emit_edges_kernel filled hot->bins: choose next window's hot list
 void launch_hot_select(const AccTable& pairs, HotState* hot, int sms, cudaStream_t s) {
   hot_emit_kernel<<<(unsigned)sms * 2, 256, 0, s>>>(pairs, hot, Layout<kDefaultWarps, 8>::kPreload);
 }

@@ -5,7 +5,7 @@
 // commutes with that join, so the default plan here reduces the stream per
 // socket pair (saddr,daddr,direction) first — one dictionary probe and two
 // reductions per event — and joins only the DISTINCT pairs against the tables
-// (fold_pairs_kernel). ALZ_CFG_EAGER_JOIN keeps the textbook plan (join every
+// (fold_resolve_kernel). ALZ_CFG_EAGER_JOIN keeps the textbook plan (join every
 // event, then reduce) for comparison; both give bit-identical edges.
 //
 // Control flow in the per-event loops is kept warp-convergent on purpose: every
@@ -153,7 +153,7 @@ __global__ void __launch_bounds__(256) ingest_eager_kernel(const alz_l7_rec* __r
 // (the one-warp-per-row version spent its time in lane 0's probe chain).
 __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const EpEntry* __restrict__ ep,
                                                            uint32_t ep_mask, AccTable edges, HotState* hot) {
-  // the hot-list bookkeeping of this fold starts from zero (fold_pairs_kernel fills the bins, hot_emit
+  // the hot-list bookkeeping of this fold starts from zero (fold_pairs_kernel or emit_edges_kernel fills the bins, hot_emit
   // the list; both run after this kernel, the ingest launches that read the list ran before it)
   if (blockIdx.x == 0 && hot != nullptr) {
     if (threadIdx.x < 128) hot->bins[threadIdx.x] = 0u;
@@ -181,56 +181,86 @@ __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const
   }
 }
 
-// pass 2, eight lanes per pair row (four rows per warp in flight): add the row into its edge row and
-// zero it. Each lane owns 8 histogram cells = two 16-byte loads; the one-warp-per-row version was bound
-// by its chain of dependent L2 round trips.
+// One pair row taken by an 8-lane group (mask gmask): lane sl holds sectors 2sl and 2sl+1, that is 64 contiguous
+// bytes = cells 8sl..8sl+3 | lat, 5xx partials | cells 8sl+4..8sl+7 | partials. Leaves the next ingest its feedback
+// (row_base, row_cnt and the count bin of a forward row), zeroes what was not zero and returns the row's event count,
+// the same in all eight lanes. Every lane of the group calls it; `valid` is uniform over the group.
+struct PairSlice { uint4 a, pa, b, pb; };
+__device__ __forceinline__ uint64_t take_pair_row(const AccTable& pairs, uint32_t row, bool valid, uint32_t gmask,
+                                                  uint32_t* __restrict__ hot_bins, PairSlice& s) {
+  const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
+  uint4* cells = reinterpret_cast<uint4*>(pairs.sect + ((size_t)row * kSectPerRow + sl * 2u) * 4u);
+  s.a = make_uint4(0u, 0u, 0u, 0u); s.b = s.a; s.pa = s.a; s.pb = s.a;
+  if (valid) { s.a = cells[0]; s.pa = cells[1]; s.b = cells[2]; s.pb = cells[3]; }
+  const uint4 a = s.a, b = s.b;
+  uint64_t cnt = (uint64_t)a.x + a.y + a.z + a.w + b.x + b.y + b.z + b.w;
+  cnt += __shfl_xor_sync(gmask, cnt, 1);
+  cnt += __shfl_xor_sync(gmask, cnt, 2);
+  cnt += __shfl_xor_sync(gmask, cnt, 4);
+  if (pairs.row_base != nullptr) {   // every lane of the group takes part in the shuffles (uniform branch)
+    // the 16-bucket window (aligned to 4 buckets) that holds most of the row's events: group sums of 4 cells,
+    // two candidates per lane, arg-max over the row's eight lanes
+    const uint64_t g0 = (uint64_t)a.x + a.y + a.z + a.w, g1 = (uint64_t)b.x + b.y + b.z + b.w;   // groups 2sl, 2sl+1
+    const uint32_t seg = lane & ~7u;
+    const uint64_t n0 = __shfl_sync(gmask, g0, seg | ((sl + 1u) & 7u)), n1 = __shfl_sync(gmask, g1, seg | ((sl + 1u) & 7u));
+    const uint64_t m0 = __shfl_sync(gmask, g0, seg | ((sl + 2u) & 7u));
+    // candidate j covers groups j..j+3 (j <= 12); lanes past the end contribute nothing
+    uint64_t c0 = sl <= 6u ? g0 + g1 + n0 + n1 : 0ull;                    // j = 2 sl       (sl = 6 -> j = 12)
+    uint64_t c1 = sl <= 5u ? g1 + n0 + n1 + m0 : 0ull;                    // j = 2 sl + 1   (sl = 5 -> j = 11)
+    uint64_t best = c0 >= c1 ? (c0 << 4) | (2u * sl) : (c1 << 4) | (2u * sl + 1u);   // counts < 2^37: room for 4 index bits
+    for (int o = 1; o < 8; o <<= 1) { const uint64_t x = __shfl_xor_sync(gmask, best, o); best = x > best ? x : best; }
+    if (sl == 0 && valid && row < pairs.max_rows) pairs.row_base[row] = (uint8_t)(best & 15u);
+  }
+  if (!valid || cnt == 0) return cnt;  // unused sentinel row (allocated rows always hold >= 1 event)
+  if (sl == 0 && row < pairs.max_rows && pairs.row_cnt != nullptr) {    // feedback for the next ingest
+    const uint32_t c32 = cnt > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cnt;
+    pairs.row_cnt[row] = c32;
+    if (hot_bins != nullptr && pairs.row_kind[row] == kPairFwd) atomicAdd(&hot_bins[count_bin(c32)], 1u);
+  }
+  // zero what was not zero: a pair's latencies fall into a few of its 16 sectors, the rest was never written
+  const uint4 pa = s.pa, pb = s.pb;
+  if (a.x | a.y | a.z | a.w | pa.x | pa.y | pa.z | pa.w) { cells[0] = make_uint4(0u, 0u, 0u, 0u); cells[1] = make_uint4(0u, 0u, 0u, 0u); }
+  if (b.x | b.y | b.z | b.w | pb.x | pb.y | pb.z | pb.w) { cells[2] = make_uint4(0u, 0u, 0u, 0u); cells[3] = make_uint4(0u, 0u, 0u, 0u); }
+  return cnt;
+}
+__device__ __forceinline__ uint64_t lat_partial(const PairSlice& s) {
+  return (((uint64_t)s.pa.y << 32) | s.pa.x) + (((uint64_t)s.pb.y << 32) | s.pb.x);
+}
+__device__ __forceinline__ uint64_t err_partial(const PairSlice& s) {
+  return (((uint64_t)s.pa.w << 32) | s.pa.z) + (((uint64_t)s.pb.w << 32) | s.pb.z);
+}
+// events of a pair row that reaches no output row: its source is not a pod (kDropRow), or the edge table was full
+__device__ __forceinline__ void count_stray_events(Counters* ctr, uint32_t erow, uint64_t cnt) {
+  if (erow == kDropRow) atomicAdd(&ctr->src_unresolved, (unsigned long long)cnt);
+  else if (erow >= kLostRow) atomicAdd(&ctr->fold_lost_events, (unsigned long long)cnt);
+  // else: the edge row of the free-marker key, which no flush emits
+}
+
+// pass 2 of a fold in the middle of a window (a table commit, 2^31 pending events) or before a multi-rank merge,
+// eight lanes per pair row (four rows per warp in flight): add the row into its edge row and zero it. Each lane
+// owns 8 histogram cells = two 16-byte loads; the one-warp-per-row version was bound by its chain of dependent L2
+// round trips.
 __global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTable edges, Counters* ctr,
                                                          uint32_t* __restrict__ hot_bins) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
+  const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
-  const uint32_t n_iter = (n_rows + kPairKinds + groups_per_grid - 1u) / groups_per_grid;   // same trip count for every lane
   uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3;
   // rows [0, n_rows) plus the sentinel rows (index n_rows + kind stands for row max_rows + kind)
-  for (uint32_t it = 0; it < n_iter; ++it, i += groups_per_grid) {
-    const bool valid = i < n_rows + kPairKinds;
-    const uint32_t row = !valid ? 0u : (i >= n_rows) ? pairs.max_rows + (i - n_rows) : i;
-    // the lane's two sectors = 64 contiguous bytes: cells 8sl..8sl+3 | lat, 5xx partials | cells 8sl+4..8sl+7 | partials
-    uint4* cells = reinterpret_cast<uint4*>(pairs.sect + ((size_t)row * kSectPerRow + sl * 2u) * 4u);
-    uint4 a = make_uint4(0u, 0u, 0u, 0u), b = a, pa = a, pb = a;
-    if (valid) { a = cells[0]; pa = cells[1]; b = cells[2]; pb = cells[3]; }
-    uint64_t lat = ((((uint64_t)pa.y << 32) | pa.x) + (((uint64_t)pb.y << 32) | pb.x));
-    uint64_t e5 = ((((uint64_t)pa.w << 32) | pa.z) + (((uint64_t)pb.w << 32) | pb.z));
-    uint64_t cnt = (uint64_t)a.x + a.y + a.z + a.w + b.x + b.y + b.z + b.w;
+  for (; i < n_rows + kPairKinds; i += groups_per_grid) {
+    const uint32_t row = i >= n_rows ? pairs.max_rows + (i - n_rows) : i;
+    PairSlice s;
+    const uint64_t cnt = take_pair_row(pairs, row, true, gmask, hot_bins, s);
+    if (cnt == 0) continue;
+    uint64_t lat = lat_partial(s), e5 = err_partial(s);
     for (int o = 1; o < 8; o <<= 1) {
-      lat += __shfl_xor_sync(0xFFFFFFFFu, lat, o);
-      e5 += __shfl_xor_sync(0xFFFFFFFFu, e5, o);
-    }
-    cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, 1);
-    cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, 2);
-    cnt += __shfl_xor_sync(0xFFFFFFFFu, cnt, 4);
-    if (pairs.row_base != nullptr) {   // every lane of the warp takes part in the shuffles (uniform branch)
-      // the 16-bucket window (aligned to 4 buckets) that holds most of the row's events: group sums of 4 cells,
-      // two candidates per lane, arg-max over the row's eight lanes
-      const uint64_t g0 = (uint64_t)a.x + a.y + a.z + a.w, g1 = (uint64_t)b.x + b.y + b.z + b.w;   // groups 2sl, 2sl+1
-      const uint32_t seg = lane & ~7u;
-      const uint64_t n0 = __shfl_sync(0xFFFFFFFFu, g0, seg | ((sl + 1u) & 7u)), n1 = __shfl_sync(0xFFFFFFFFu, g1, seg | ((sl + 1u) & 7u));
-      const uint64_t m0 = __shfl_sync(0xFFFFFFFFu, g0, seg | ((sl + 2u) & 7u));
-      // candidate j covers groups j..j+3 (j <= 12); lanes past the end contribute nothing
-      uint64_t c0 = sl <= 6u ? g0 + g1 + n0 + n1 : 0ull;                    // j = 2 sl       (sl = 6 -> j = 12)
-      uint64_t c1 = sl <= 5u ? g1 + n0 + n1 + m0 : 0ull;                    // j = 2 sl + 1   (sl = 5 -> j = 11)
-      uint64_t best = c0 >= c1 ? (c0 << 4) | (2u * sl) : (c1 << 4) | (2u * sl + 1u);   // counts < 2^37: room for 4 index bits
-      for (int o = 1; o < 8; o <<= 1) { const uint64_t x = __shfl_xor_sync(0xFFFFFFFFu, best, o); best = x > best ? x : best; }
-      if (sl == 0 && valid && row < pairs.max_rows) pairs.row_base[row] = (uint8_t)(best & 15u);
-    }
-    if (!valid || cnt == 0) continue;  // unused sentinel row (allocated rows always hold >= 1 event)
-    if (sl == 0 && row < pairs.max_rows && pairs.row_cnt != nullptr) {    // feedback for the next ingest
-      const uint32_t c32 = cnt > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cnt;
-      pairs.row_cnt[row] = c32;
-      if (hot_bins != nullptr && pairs.row_kind[row] == kPairFwd) atomicAdd(&hot_bins[count_bin(c32)], 1u);
+      lat += __shfl_xor_sync(gmask, lat, o);
+      e5 += __shfl_xor_sync(gmask, e5, o);
     }
     const uint32_t erow = pairs.row_aux[row];
     if (erow < kDropRow) {
+      const uint4 a = s.a, b = s.b;
       uint32_t* dst = edges.hist + (size_t)erow * ALZ_NB + sl * 8u;
       if (a.x) atomicAdd(dst + 0, a.x);
       if (a.y) atomicAdd(dst + 1, a.y);
@@ -246,54 +276,144 @@ __global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTabl
         if (e5) atomicAdd((unsigned long long*)&edges.err5xx[erow], (unsigned long long)e5);
       }
     } else if (sl == 0) {
-      if (erow == kDropRow) atomicAdd(&ctr->src_unresolved, (unsigned long long)cnt);
-      else atomicAdd(&ctr->fold_lost_events, (unsigned long long)cnt);
+      count_stray_events(ctr, erow, cnt);
     }
-    // zero what was not zero: a pair's latencies fall into a few of its 16 sectors, the rest was never written
-    if (a.x | a.y | a.z | a.w | pa.x | pa.y | pa.z | pa.w) { cells[0] = make_uint4(0u, 0u, 0u, 0u); cells[1] = make_uint4(0u, 0u, 0u, 0u); }
-    if (b.x | b.y | b.z | b.w | pb.x | pb.y | pb.z | pb.w) { cells[2] = make_uint4(0u, 0u, 0u, 0u); cells[3] = make_uint4(0u, 0u, 0u, 0u); }
   }
 }
 
 // ---------------------------------------------------------------------------
 // flush: rows [0, n) of the edge table are the live edges. iota -> sort by key
-// (alz_sort.cu) -> gather into the caller-facing layout, zeroing the rows.
+// (alz_sort.cu) -> output rows in key order.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) iota_kernel(uint32_t* out, uint32_t n) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = i;
 }
 
+// the fixed part of an output row and the lane's 8 histogram cells (hist sits at byte 40 of a 296-byte row:
+// 8-byte aligned only)
+__device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uint64_t key, const uint32_t (&c)[8],
+                                               uint64_t count, uint64_t err5xx, uint64_t lat_sum) {
+  uint2* d2 = reinterpret_cast<uint2*>(&o->hist[sl * 8u]);
+  d2[0] = make_uint2(c[0], c[1]); d2[1] = make_uint2(c[2], c[3]);
+  d2[2] = make_uint2(c[4], c[5]); d2[3] = make_uint2(c[6], c[7]);
+  if (sl == 0) {
+    uint8_t ft, tt; uint32_t f, t;
+    unpack_edge_key(key, &ft, &f, &tt, &t);
+    o->from_type = ft; o->to_type = tt;
+    for (int k = 0; k < 6; ++k) o->_pad[k] = 0;
+    o->from = f; o->to = t;
+    o->count = count;
+    o->err5xx = err5xx;
+    o->lat_sum_ns = lat_sum;
+  }
+}
+
+// multi-rank flush: the live edge rows, as they are, into the send buffer (the window stays in the table until
+// every rank has taken part in the merge, alz_comm.cu)
 __global__ void __launch_bounds__(256) gather_edges_kernel(AccTable edges, const uint64_t* __restrict__ keys,
                                                            const uint32_t* __restrict__ rows, uint32_t n_live,
-                                                           alz_edge_out* __restrict__ out, bool reset) {
+                                                           alz_edge_out* __restrict__ out) {
   // eight lanes per edge, four edges per warp in flight; a lane moves 8 histogram cells (2 x 16 bytes)
   const uint32_t sl = threadIdx.x & 7u;
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_live; i += groups_per_grid) {
     const uint32_t row = rows[i];
-    alz_edge_out* o = &out[i];
-    uint4* cells = reinterpret_cast<uint4*>(edges.hist + (size_t)row * ALZ_NB + sl * 8u);
-    uint4* dst = reinterpret_cast<uint4*>(&o->hist[sl * 8u]);   // hist sits at byte 40 of a 296-byte row: 8-byte aligned only
+    const uint4* cells = reinterpret_cast<const uint4*>(edges.hist + (size_t)row * ALZ_NB + sl * 8u);
     const uint4 a = cells[0], b = cells[1];
-    uint2* d2 = reinterpret_cast<uint2*>(dst);
-    d2[0] = make_uint2(a.x, a.y); d2[1] = make_uint2(a.z, a.w);
-    d2[2] = make_uint2(b.x, b.y); d2[3] = make_uint2(b.z, b.w);
-    if (sl == 0) {
-      uint8_t ft, tt; uint32_t f, t;
-      unpack_edge_key(keys[i], &ft, &f, &tt, &t);
-      o->from_type = ft; o->to_type = tt;
-      for (int k = 0; k < 6; ++k) o->_pad[k] = 0;
-      o->from = f; o->to = t;
-      o->count = edges.count[row];
-      o->err5xx = edges.err5xx[row];
-      o->lat_sum_ns = edges.lat_sum[row];
+    const uint32_t c[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+    uint64_t count = 0, e5 = 0, lat = 0;
+    if (sl == 0) { count = edges.count[row]; e5 = edges.err5xx[row]; lat = edges.lat_sum[row]; }
+    store_edge_out(&out[i], sl, keys[i], c, count, e5, lat);
+  }
+}
+
+// ---------------------------------------------------------------------------
+// single-rank flush: the pair rows go straight into the output rows. fold_resolve_kernel gave every pair row its
+// edge row (row_aux); the rows are bucketed by edge row (count, exclusive scan, fill) and emit_edges_kernel sums
+// each bucket in registers into the output row of its edge. Every sum is an integer sum, so the order of the rows
+// in a bucket does not change the result.
+// ---------------------------------------------------------------------------
+// pair rows per edge row into cnt[]; a row that reaches no edge row (unresolved source, full edge table, the
+// free-marker edge key) goes to the back of row_list, *n_stray of them
+__global__ void __launch_bounds__(256) bucket_count_kernel(AccTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
+                                                           uint32_t* __restrict__ row_list, uint32_t list_cap,
+                                                           uint32_t* __restrict__ n_stray) {
+  const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_rows + kPairKinds; i += stride) {
+    const uint32_t row = i >= n_rows ? pairs.max_rows + (i - n_rows) : i;
+    const uint32_t erow = pairs.row_aux[row];
+    if (erow < max_edges) atomicAdd(&cnt[erow], 1u);
+    else row_list[list_cap - 1u - atomicAdd(n_stray, 1u)] = row;
+  }
+}
+// each row to its place in its edge's bucket; counts cnt[] back down to zero for the next flush
+__global__ void __launch_bounds__(256) bucket_fill_kernel(AccTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
+                                                          const uint32_t* __restrict__ off, uint32_t* __restrict__ row_list) {
+  const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_rows + kPairKinds; i += stride) {
+    const uint32_t row = i >= n_rows ? pairs.max_rows + (i - n_rows) : i;
+    const uint32_t erow = pairs.row_aux[row];
+    if (erow < max_edges) row_list[off[erow] + atomicSub(&cnt[erow], 1u) - 1u] = row;
+  }
+}
+
+// Output row i (edge row rows[i]) = the sum of the pair rows of its bucket, row_list[off[erow], off[erow + 1]),
+// plus, when a fold already ran in this window (with_edges), what the edge accumulators hold, which it zeroes.
+// Eight lanes per output row as in fold_pairs_kernel, plain stores only. The n_stray pair rows at the back of
+// row_list follow as groups n_live.. : they leave their feedback and their events in the counters. off == nullptr:
+// no pair rows to take (nothing was ingested since the last fold, or ALZ_CFG_EAGER_JOIN).
+__global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTable edges, Counters* ctr,
+                                                         uint32_t* __restrict__ hot_bins, const uint64_t* __restrict__ keys,
+                                                         const uint32_t* __restrict__ rows, uint32_t n_live,
+                                                         const uint32_t* __restrict__ off,
+                                                         const uint32_t* __restrict__ row_list, uint32_t list_cap,
+                                                         const uint32_t* __restrict__ n_stray, bool with_edges,
+                                                         alz_edge_out* __restrict__ out) {
+  const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
+  const uint32_t gmask = 0xFFu << (lane & ~7u);
+  const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
+  const uint32_t n_groups = n_live + (off != nullptr ? *n_stray : 0u);
+  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_groups; i += groups_per_grid) {
+    if (i >= n_live) {
+      const uint32_t row = row_list[list_cap - 1u - (i - n_live)];
+      PairSlice s;
+      const uint64_t cnt = take_pair_row(pairs, row, true, gmask, hot_bins, s);
+      if (sl == 0 && cnt != 0) count_stray_events(ctr, pairs.row_aux[row], cnt);
+      continue;
     }
-    if (reset) {
+    const uint32_t erow = rows[i];
+    uint32_t c[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+    uint64_t count = 0, lat = 0, e5 = 0;   // lane partials of the latency and 5xx sums; count in lane 0
+    if (with_edges) {
+      uint4* cells = reinterpret_cast<uint4*>(edges.hist + (size_t)erow * ALZ_NB + sl * 8u);
+      const uint4 a = cells[0], b = cells[1];
+      c[0] = a.x; c[1] = a.y; c[2] = a.z; c[3] = a.w; c[4] = b.x; c[5] = b.y; c[6] = b.z; c[7] = b.w;
       cells[0] = make_uint4(0u, 0u, 0u, 0u);
       cells[1] = make_uint4(0u, 0u, 0u, 0u);
-      if (sl == 0) { edges.count[row] = 0ull; edges.err5xx[row] = 0ull; edges.lat_sum[row] = 0ull; }
+      if (sl == 0) {
+        count = edges.count[erow]; lat = edges.lat_sum[erow]; e5 = edges.err5xx[erow];
+        edges.count[erow] = 0ull; edges.lat_sum[erow] = 0ull; edges.err5xx[erow] = 0ull;
+      }
     }
+    if (off != nullptr) {
+      const uint32_t end = off[erow + 1u];
+      for (uint32_t j = off[erow]; j < end; ++j) {
+        PairSlice s;
+        count += take_pair_row(pairs, row_list[j], true, gmask, hot_bins, s);
+        c[0] += s.a.x; c[1] += s.a.y; c[2] += s.a.z; c[3] += s.a.w;
+        c[4] += s.b.x; c[5] += s.b.y; c[6] += s.b.z; c[7] += s.b.w;
+        lat += lat_partial(s);
+        e5 += err_partial(s);
+      }
+    }
+    for (int o = 1; o < 8; o <<= 1) {
+      lat += __shfl_xor_sync(gmask, lat, o);
+      e5 += __shfl_xor_sync(gmask, e5, o);
+    }
+    store_edge_out(&out[i], sl, keys[i], c, count, e5, lat);
   }
 }
 
@@ -406,9 +526,22 @@ void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s) {
   iota_kernel<<<grid_for(sms, 4), 256, 0, s>>>(out, n);
 }
 void launch_gather_edges(const AccTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
-                         alz_edge_out* out, bool reset, int sms, cudaStream_t s) {
+                         alz_edge_out* out, int sms, cudaStream_t s) {
   if (n_live == 0) return;
-  gather_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(edges, keys, rows, n_live, out, reset);
+  gather_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(edges, keys, rows, n_live, out);
+}
+void launch_bucket_count(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
+  bucket_count_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, max_edges, b.cnt, b.rows, b.cap, b.n_stray);
+}
+void launch_bucket_fill(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
+  bucket_fill_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, max_edges, b.cnt, b.off, b.rows);
+}
+void launch_emit_edges(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
+                       const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
+                       int sms, cudaStream_t s) {
+  emit_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot ? hot->bins : nullptr, keys, rows, n_live,
+                                                     b ? b->off : nullptr, b ? b->rows : nullptr, b ? b->cap : 0u,
+                                                     b ? b->n_stray : nullptr, with_edges, out);
 }
 void launch_compact_raw(const uint8_t* raw, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s) {
   if (n == 0) return;

@@ -28,7 +28,21 @@ void launch_fold_add(const AccTable& pairs, const AccTable& edges, Counters* ctr
 void launch_ep_patch(EpEntry* tab, const void* patch, uint32_t n, int sms, cudaStream_t s);
 void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s);
 void launch_gather_edges(const AccTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
-                         alz_edge_out* out, bool reset, int sms, cudaStream_t s);
+                         alz_edge_out* out, int sms, cudaStream_t s);
+// single-rank flush scratch: pair rows bucketed by edge row (alz_kernels.cu, emit_edges_kernel)
+struct FlushBuckets {
+  uint32_t* cnt;       // [max_edges + 1] pair rows per edge row; all zero between flushes
+  uint32_t* off;       // [max_edges + 1] exclusive scan of cnt: bucket of edge row e = rows[off[e], off[e + 1])
+  uint32_t* rows;      // [cap] bucketed pair rows from the front, rows that reach no edge row from the back
+  uint32_t cap;        // max_pairs + kPairKinds
+  uint32_t* n_stray;   // rows at the back of `rows`
+};
+void launch_bucket_count(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
+void launch_bucket_fill(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
+// b == nullptr: no pair rows to take
+void launch_emit_edges(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
+                       const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
+                       int sms, cudaStream_t s);
 void launch_compact_raw(const uint8_t* raw, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s);
 void launch_synth(const alz_synth_view& v, uint64_t first, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s);
 void launch_synth_owned(const alz_synth_view& v, uint64_t first, uint64_t n, uint32_t nranks, uint32_t rank,
