@@ -218,6 +218,13 @@ class Handle:
         self._ck(self.L.alz_submit_l7_packed(self.h, C.c_void_p(host_ptr), n, C.c_void_p(ovf_ptr) if ovf_ptr else None,
                                              n_ovf), "alz_submit_l7_packed")
 
+    def submit_packed_device(self, dev_ptr, n, dev_ovf=None):
+        """alz_submit_l7_packed_device: n 16-B records already in device memory; dev_ovf the device array of overflow
+        durations their indices point into (None: no record has ALZ_REC16_DUR_OVERFLOW)."""
+        self._ck(self.L.alz_submit_l7_packed_device(self.h, C.c_void_p(dev_ptr), n,
+                                                    C.c_void_p(dev_ovf) if dev_ovf else None),
+                 "alz_submit_l7_packed_device")
+
     def submit_raw(self, raw):
         raw = np.ascontiguousarray(raw, dtype=np.uint8)
         n = raw.size // abi.BPF_L7_EVENT_SIZE

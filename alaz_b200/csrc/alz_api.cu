@@ -516,31 +516,49 @@ static int fold_locked(alz_handle* h) {
 int alz_internal_fold(alz_handle* h) { return fold_locked(h); }
 
 // ---- ingest ------------------------------------------------------------------------------
+// Pair-row cells are u32 and the ingest kernels add to them (a cell pair even as one u64) without looking at them:
+// a fold must run before any cell could reach 2^31. So the events between two folds never exceed kFoldEvery, and a
+// submit larger than what is left of that budget is launched in pieces with a fold between them.
+constexpr uint64_t kFoldEvery = 1ull << 31;
+
 // requires h->mu
 static int ingest_device(alz_handle* h, const void* d, uint64_t n, bool rec16, const uint64_t* d_ovf) {
   if (h->win_on && (rec16 || (h->cfg.flags & (ALZ_CFG_EAGER_JOIN | ALZ_CFG_NO_SMEM_CACHE)))) return ALZ_E_STATE;
-  if (rec16) {
-    if (h->cfg.flags & (ALZ_CFG_EAGER_JOIN | ALZ_CFG_NO_SMEM_CACHE)) return ALZ_E_UNSUPPORTED;
-    launch_ingest_pairs_rec16((const alz_l7_rec16*)d, n, d_ovf, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
-                              h->d_bloom, h->sms, h->stream);
-  } else if (h->cfg.flags & ALZ_CFG_EAGER_JOIN) {
-    launch_ingest_eager((const alz_l7_rec*)d, n, h->d_ep, h->ep_cap - 1, h->edges, h->d_ctr, h->sms, h->stream);
-  } else if (h->cfg.flags & ALZ_CFG_NO_SMEM_CACHE) {
-    launch_ingest_pairs_v1((const alz_l7_rec*)d, n, h->pairs, h->d_ctr, h->d_ep, h->ep_cap - 1, h->sms, h->stream);
-  } else if (h->win_on) {
-    launch_ingest_pairs_windowed((const alz_l7_rec*)d, n, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1, h->d_bloom,
-                                 h->d_win, h->win_off, h->d_defer[h->defer_cur], h->defer_cap, h->sms, h->stream);
-    h->launches += 1;
-  } else {
-    launch_ingest_pairs((const alz_l7_rec*)d, n, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1, h->d_bloom, h->sms,
-                        h->stream);
-  }
-  CK(cudaGetLastError());
-  h->launches += n ? 1 : 0;
-  h->events_in += n;
-  h->pending_since_fold += n;
-  // pair histograms are u32: fold before any bucket could wrap
-  if (h->pending_since_fold >= (1ull << 31)) return fold_locked(h);
+  if (rec16 && (h->cfg.flags & (ALZ_CFG_EAGER_JOIN | ALZ_CFG_NO_SMEM_CACHE))) return ALZ_E_UNSUPPORTED;
+  // the eager plan reduces into the edge table directly, whose cells wrap mod 2^32 as docs/SPEC.md §3 defines them
+  const bool eager = (h->cfg.flags & ALZ_CFG_EAGER_JOIN) != 0;
+  const size_t rec_bytes = rec16 ? sizeof(alz_l7_rec16) : sizeof(alz_l7_rec);
+  uint64_t done = 0;
+  do {
+    if (!eager && h->pending_since_fold >= kFoldEvery) {
+      const int rc = fold_locked(h);
+      if (rc != ALZ_OK) return rc;
+    }
+    const uint64_t m = eager ? n - done : std::min(n - done, kFoldEvery - h->pending_since_fold);
+    const void* p = (const char*)d + done * rec_bytes;
+    if (rec16) {   // overflow indices are absolute: every piece takes the same side array
+      launch_ingest_pairs_rec16((const alz_l7_rec16*)p, m, d_ovf, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
+                                h->d_bloom, h->sms, h->stream);
+    } else if (eager) {
+      launch_ingest_eager((const alz_l7_rec*)p, m, h->d_ep, h->ep_cap - 1, h->edges, h->d_ctr, h->sms, h->stream);
+    } else if (h->cfg.flags & ALZ_CFG_NO_SMEM_CACHE) {
+      launch_ingest_pairs_v1((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_ep, h->ep_cap - 1, h->sms, h->stream);
+    } else if (h->win_on) {
+      launch_ingest_pairs_windowed((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
+                                   h->d_bloom, h->d_win, h->win_off, h->d_defer[h->defer_cur], h->defer_cap, h->sms,
+                                   h->stream);
+      h->launches += 1;
+    } else {
+      launch_ingest_pairs((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1, h->d_bloom,
+                          h->sms, h->stream);
+    }
+    CK(cudaGetLastError());
+    h->launches += m ? 1 : 0;
+    h->events_in += m;
+    h->pending_since_fold += m;
+    done += m;
+  } while (done < n);
+  if (!eager && h->pending_since_fold >= kFoldEvery) return fold_locked(h);
   return ALZ_OK;
 }
 

@@ -304,7 +304,8 @@ __device__ __forceinline__ Rec load_rec(const alz_l7_rec* p) {
 __device__ __forceinline__ uint32_t rec_saddr(const Rec& r) { return r.w[0]; }
 __device__ __forceinline__ uint32_t rec_daddr(const Rec& r) { return r.w[1]; }
 __device__ __forceinline__ uint32_t rec_status(const Rec& r) { return r.w[3] & 0xFFFFu; }
-__device__ __forceinline__ uint32_t rec_protocol(const Rec& r) { return (r.w[3] >> 16) & 0x3Fu; }   // without the flag bits
+// without ALZ_PROTO_F_HOSTKEY; bit 7 is no flag of a 32-B record, so a byte with it set stays an undefined protocol
+__device__ __forceinline__ uint32_t rec_protocol(const Rec& r) { return (r.w[3] >> 16) & 0xBFu; }
 __device__ __forceinline__ bool rec_hostkey(const Rec& r) { return (r.w[3] & ((uint32_t)ALZ_PROTO_F_HOSTKEY << 16)) != 0u; }
 __device__ __forceinline__ uint32_t rec_mflags(const Rec& r) { return r.w[3] >> 24; }
 __device__ __forceinline__ uint64_t rec_duration(const Rec& r) { return ((uint64_t)r.w[5] << 32) | r.w[4]; }

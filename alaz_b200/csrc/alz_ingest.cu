@@ -636,7 +636,9 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
         if (p & ALZ_REC16_DUR_OVERFLOW) dur[u] = live[u] ? __ldg(&dur_ovf[w[u][3]]) : 0ull;
       }
       const bool hk = (p & ALZ_PROTO_F_HOSTKEY) != 0u;             // daddr is a Host-header id: own key space, cold tier
-      p &= 0x3Fu;
+      // bit 7 is ALZ_REC16_DUR_OVERFLOW on packed records; on 32-B records it is no flag, and a byte with it set is
+      // no protocol (class 0 below, as for any value > 8)
+      p &= (kRecWords == 8) ? 0xBFu : 0x3Fu;
       const uint32_t cls = shr_clamp(kProtoLut, 3u * p);
       // a row is built unless the class says "payload parser decides" and the parser said no (bit 30 of mw)
       act[u] = live[u] && (cls & 1u) && !((cls & 2u) && (mw & ((uint32_t)ALZ_MF_PAYLOAD_REJECT << 24)));

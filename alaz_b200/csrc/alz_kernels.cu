@@ -436,8 +436,12 @@ __global__ void __launch_bounds__(256) compact_raw_kernel(const uint8_t* __restr
     const uint32_t sport = *reinterpret_cast<const uint16_t*>(p + 1080);
     const uint32_t daddr = *reinterpret_cast<const uint32_t*>(p + 1084);
     const uint32_t dport = *reinterpret_cast<const uint16_t*>(p + 1088);
-    const uint32_t protocol = pm & 0xFFu, method = (pm >> 8) & 0xFFu;
+    uint32_t protocol = pm & 0xFFu;
+    const uint32_t method = (pm >> 8) & 0xFFu;
     const uint32_t is_tls = (fl >> 16) & 0xFFu;
+    // the eBPF byte has no flag bits: one that would read as ALZ_PROTO_F_HOSTKEY (or anything else >= 0x40) is an
+    // undefined protocol and must stay one (alz_pack_l7 does the same)
+    if (protocol >= 0x40u) protocol = 0x3Fu;
     uint4 lo, hi;
     lo.x = saddr; lo.y = daddr; lo.z = sport | (dport << 16);
     lo.w = (status > 65535u ? 65535u : status) | (protocol << 16) |

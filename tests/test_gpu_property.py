@@ -13,7 +13,10 @@ pytestmark = pytest.mark.gpu
 
 IPS = [abi.ip("10.0.0.%d" % i) for i in range(1, 9)] + [0, 0xFFFFFFFF, abi.ip("8.8.8.8"), abi.ip("127.0.0.1")]
 ip_s = st.sampled_from(IPS)
-event_s = st.tuples(ip_s, ip_s, st.integers(0, 12), st.integers(0, 255),
+# protocol bytes: the defined ones and their neighbours, and any byte without ALZ_PROTO_F_HOSTKEY (bit 7 set, or
+# 9..63: no protocol, no row)
+proto_s = st.one_of(st.integers(0, 12), st.integers(0, 255).map(lambda p: p & ~abi.PROTO_F_HOSTKEY))
+event_s = st.tuples(ip_s, ip_s, proto_s, st.integers(0, 255),
                     st.sampled_from([0, 1, 2, 200, 404, 499, 500, 503, 599, 600, 65535]),
                     st.sampled_from([0, 1, 255, 256, 383, 384, 10**6, (1 << 40) - 1, 1 << 40, (1 << 64) - 1]))
 table_s = st.dictionaries(ip_s, st.integers(0, 50), max_size=8)
