@@ -432,6 +432,17 @@ static_assert(sizeof(EpPatch) == 32, "EpPatch layout");
 
 static int fold_locked(alz_handle* h);
 
+// time-cut windows: the records set aside for a later window, read from the device (the host copy h_ctr is only as
+// fresh as the last flush or alz_get_stats). *held counts past the buffer's capacity; *resolved <= min(held, cap).
+static int read_held(alz_handle* h, uint32_t* held, uint32_t* resolved) {
+  uint32_t v[2];
+  CK(cudaMemcpyAsync(v, &h->d_ctr->defer_count, sizeof(v), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  *held = v[0];
+  *resolved = std::min(v[1], std::min(v[0], h->defer_cap));
+  return ALZ_OK;
+}
+
 extern "C" int alz_table_commit(alz_handle* h) {
   if (!h) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
@@ -440,6 +451,17 @@ extern "C" int alz_table_commit(alz_handle* h) {
   // events already submitted are joined through the tables they arrived under
   int rc = fold_locked(h);
   if (rc != ALZ_OK) return rc;
+  // so are the records set aside for a later window (docs/SPEC.md §8): resolved now, before the patch
+  if (h->win_on) {
+    uint32_t held = 0, resolved = 0;
+    if ((rc = read_held(h, &held, &resolved)) != ALZ_OK) return rc;
+    const uint32_t n = std::min(held, h->defer_cap);
+    if (n > resolved) {
+      launch_defer_resolve(h->d_defer[h->defer_cur], resolved, n, h->d_ep, h->ep_cap - 1, h->d_ctr, h->sms, h->stream);
+      h->launches += 1;
+      CK(cudaGetLastError());
+    }
+  }
   for (uint32_t ip : h->ep_dirty_ips) {
     auto it = h->ep_host.find(ip);
     if (it == h->ep_host.end()) ep_mirror_del(h, ip); else ep_mirror_put(h, ip, it->second);
@@ -545,8 +567,7 @@ static int ingest_device(alz_handle* h, const void* d, uint64_t n, bool rec16, c
       launch_ingest_pairs_v1((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_ep, h->ep_cap - 1, h->sms, h->stream);
     } else if (h->win_on) {
       launch_ingest_pairs_windowed((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
-                                   h->d_bloom, h->d_win, h->win_off, h->d_defer[h->defer_cur], h->defer_cap, h->sms,
-                                   h->stream);
+                                   h->d_bloom, h->d_win, h->d_defer[h->defer_cur], h->defer_cap, h->sms, h->stream);
       h->launches += 1;
     } else {
       launch_ingest_pairs((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1, h->d_bloom,
@@ -792,19 +813,29 @@ static int finish_flush(alz_handle* h) {
 }
 
 // time-cut windows: the flushed epoch is closed; open the next one and submit the records that waited for it
-// (those of still later epochs are deferred again, into the other buffer)
+// (those of still later epochs are deferred again, into the other buffer). The buffer holds first the records a
+// table commit resolved, then raw ones: the first go straight into the edge accumulators, the rest are ingested.
 static int window_roll(alz_handle* h) {
   if (!h->win_on) return ALZ_OK;
   launch_window_advance(h->d_win, h->stream);
   h->launches += 1;
   const uint32_t n_def = std::min<uint32_t>(h->h_ctr->defer_count, h->defer_cap);   // read with the edge count
-  CK(cudaMemsetAsync(&h->d_ctr->defer_count, 0, 4, h->stream));
+  const uint32_t n_res = std::min<uint32_t>(h->h_ctr->defer_resolved, n_def);
+  CK(cudaMemsetAsync(&h->d_ctr->defer_count, 0, 2 * sizeof(uint32_t), h->stream));   // and defer_resolved
   h->deferred_last = 0;
   if (n_def == 0) return ALZ_OK;
   const alz_l7_rec* src = h->d_defer[h->defer_cur];
   h->defer_cur ^= 1;
+  if (n_res) {
+    launch_defer_roll(src, n_res, h->d_win, h->d_defer[h->defer_cur], h->defer_cap, h->edges, h->d_ctr, h->sms,
+                      h->stream);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    h->edges_dirty = true;
+  }
+  if (n_def == n_res) return ALZ_OK;
   const uint64_t before = h->events_in;
-  const int rc = ingest_device(h, src, n_def, false, nullptr);
+  const int rc = ingest_device(h, src + n_res, n_def - n_res, false, nullptr);
   h->events_in = before;   // they were counted when they were first submitted
   return rc;
 }
@@ -897,10 +928,12 @@ extern "C" int alz_get_stats(alz_handle* h, alz_stats* st) {
   CK(cudaStreamSynchronize(h->stream));
   memset(st, 0, sizeof(*st));
   const uint64_t lost = h->h_ctr->capacity_events + h->h_ctr->fold_lost_events;
+  // a record set aside past the buffer's capacity is in `lost` already, not waiting
+  const uint64_t held = std::min<uint64_t>(h->h_ctr->defer_count, h->defer_cap);
   st->events_in = h->events_in;
   st->not_request = h->h_ctr->not_request;
   st->src_unresolved = h->h_ctr->src_unresolved;   // complete once pending pairs are folded
-  st->rows_emitted = h->events_in - st->not_request - st->src_unresolved - lost - h->h_ctr->defer_count;   // waiting records are not rows yet
+  st->rows_emitted = h->events_in - st->not_request - st->src_unresolved - lost - held;   // waiting records are not rows yet
   st->pairs_live = h->h_ctr->pair_rows;
   st->edges_live = h->h_ctr->edge_rows;
   st->tcp_events_in = h->tcp_events_in;
@@ -908,7 +941,7 @@ extern "C" int alz_get_stats(alz_handle* h, alz_stats* st) {
   st->capacity_events = lost;
   st->windows = h->windows;
   st->late_events = h->h_ctr->late_events;
-  st->deferred_events = h->h_ctr->defer_count;
+  st->deferred_events = held;
   st->kernel_launches = h->launches;
   st->collective_bytes_last = h->collective_bytes_last;
   if (h->ev_t_valid) {   // the stream was synchronised above, so the events have completed
@@ -923,14 +956,17 @@ extern "C" int alz_window_clock(alz_handle* h, uint64_t first_kernel_ns, uint64_
   if (!h) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
   CK(cudaSetDevice(h->device));
-  if (h->pending_since_fold != 0 || h->h_ctr->defer_count != 0) return ALZ_E_STATE;   // only between windows
+  uint32_t held = 0, resolved = 0;
+  const int rc = read_held(h, &held, &resolved);
+  if (rc != ALZ_OK) return rc;
+  if (h->pending_since_fold != 0 || held != 0) return ALZ_E_STATE;   // only between windows
   if (window_ns == 0) { h->win_on = false; return ALZ_OK; }
   if (!h->d_win) {
-    CK(cudaMalloc(&h->d_win, 3 * sizeof(uint64_t)));
+    CK(cudaMalloc(&h->d_win, 5 * sizeof(uint64_t)));
     h->defer_cap = 2u * h->cfg.max_batch;
     for (int b = 0; b < 2; ++b) CK(cudaMalloc(&h->d_defer[b], (size_t)h->defer_cap * sizeof(alz_l7_rec)));
   }
-  const uint64_t init[3] = {0ull, window_ns, 0ull};
+  const uint64_t init[5] = {0ull, window_ns, 0ull, first_user_ns - first_kernel_ns, 0ull};   // WinClock
   CK(cudaMemcpyAsync(h->d_win, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   h->win_off = first_user_ns - first_kernel_ns;
@@ -943,11 +979,11 @@ extern "C" int alz_window_epoch(alz_handle* h, uint64_t* epoch) {
   std::lock_guard<std::mutex> g(h->mu);
   CK(cudaSetDevice(h->device));
   if (!h->win_on) return ALZ_E_STATE;
-  uint64_t w[3];
+  uint64_t w[5];   // WinClock
   CK(cudaMemcpyAsync(w, h->d_win, sizeof(w), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   if (!w[2]) return ALZ_E_STATE;
-  *epoch = (w[0] + h->win_off) / w[1];
+  *epoch = w[4];
   return ALZ_OK;
 }
 

@@ -342,7 +342,9 @@ struct Counters {
   unsigned long long capacity_events;   // events lost at ingest to an exhausted pair dictionary / row pool
   unsigned long long fold_lost_events;  // events lost at fold to an exhausted edge dictionary / row pool
   uint32_t pair_rows, edge_rows;            // row allocators of the two tables
-  uint32_t defer_count, pad1;               // time-cut windows: records waiting for their window (alz_ingest.cu)
+  // time-cut windows (alz_ingest.cu): records set aside for a later window, counted past the buffer's capacity too;
+  // the first defer_resolved of them were resolved by a table commit (defer_resolve_kernel)
+  uint32_t defer_count, defer_resolved;
   unsigned long long late_events;           // time-cut windows: records older than the open window (reduced into it)
   unsigned long long pad2;
 };

@@ -88,7 +88,7 @@ struct alz_handle {
   // time-cut windows (alz_window_clock)
   bool win_on = false;
   uint64_t win_off = 0, win_len = 0;      // first_user - first_kernel (mod 2^64), window length
-  uint64_t* d_win = nullptr;              // device WinClock {lo, len, ready}
+  uint64_t* d_win = nullptr;              // device WinClock {lo, len, ready, off, epoch} (alz_ingest.cu)
   alz_l7_rec* d_defer[2] = {nullptr, nullptr};   // records of later windows (ping-pong)
   uint32_t defer_cap = 0;
   int defer_cur = 0;

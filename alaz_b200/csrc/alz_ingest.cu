@@ -32,6 +32,8 @@
 //   slow  a cold event whose home slot does not hold its pair (new pair, collision) is queued once
 //         more and 32 of them at a time walk find_or_insert_pair.
 
+#include <algorithm>
+
 #include "alz_kernels.cuh"
 
 namespace alz {
@@ -467,8 +469,16 @@ __device__ __forceinline__ uint32_t preload_hot(const Shared& s, const HotState*
 struct WinClock {
   uint64_t lo;        // first kernel-time ns of the open window
   uint64_t len;       // window length, ns
-  uint64_t ready;     // lo is set (by win_init_kernel from the first record ever submitted)
+  uint64_t ready;     // 0: lo not set yet; 1: set (by win_init_kernel from the first record ever submitted);
+                      // 2: the open epoch starts at or past 2^64 in the user clock, so every record is late
+  uint64_t off;       // first_user_ns - first_kernel_ns (mod 2^64)
+  uint64_t epoch;     // epoch_open
 };
+// SPEC §8 orders epochs by user time, unsigned: a record is late iff its user time lies below the open window's
+// start (lo + off), and in the open window iff wt - lo < len. No division.
+__device__ __forceinline__ bool win_late(uint64_t wt, uint64_t lo, uint64_t off, bool past) {
+  return past || wt + off < lo + off;
+}
 
 // kRecWords = 8: alz_l7_rec (32 B). kRecWords = 4: alz_l7_rec16 (16 B; durations >= 2^32 ns sit in dur_ovf).
 // kWin (32-B records only): an event whose write_time lies beyond the open window is not reduced but appended
@@ -553,8 +563,9 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
   const uint32_t zero = (uint32_t)(n >> 63);   // n < 2^37
   uint32_t lost = 0, unresolved = 0, n_hit = 0, n_live = 0, n_cold = 0, n_late = 0;
   uint32_t probing = 0;                        // events at the head of the cold queue whose probes are in flight
-  uint64_t win_lo = 0, win_len = ~0ull;
-  if (kWin) { win_lo = win->lo; win_len = win->len; }
+  uint64_t win_lo = 0, win_len = ~0ull, win_off = 0;
+  bool win_past = false;
+  if (kWin) { win_lo = win->lo; win_len = win->len; win_off = win->off; win_past = win->ready > 1ull; }
   PROF_DECL;
   unsigned long long t_wait = 0, t_slow = 0;
   const long long p_begin = PROF_NOW();
@@ -598,9 +609,9 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
     for (int u = 0; u < kU; ++u) {
       live[u] = (uint32_t)u * 32u + lane < n_here;
       if constexpr (kWin && kRecWords == 8) {
-        const uint64_t rel = (((uint64_t)w[u][7] << 32) | w[u][6]) - win_lo;      // write_time relative to the window
-        const bool late = live[u] && (rel >> 63) != 0ull;                          // before the open window
-        const bool future = live[u] && !late && rel >= win_len;
+        const uint64_t wt = ((uint64_t)w[u][7] << 32) | w[u][6];
+        const bool late = live[u] && win_late(wt, win_lo, win_off, win_past);      // before the open window
+        const bool future = live[u] && !late && wt - win_lo >= win_len;
         n_late += late ? 1u : 0u;
         const uint32_t fm = __ballot_sync(0xFFFFFFFFu, future);
         if (fm != 0u) {   // warp-uniform and rare: only around a window boundary
@@ -747,15 +758,84 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
 
 // open the first window on the first record ever submitted: epoch = (write_time + off) / len, docs/SPEC.md §8
 // (off = FirstUserspaceTime - FirstKernelTime, aggregator/data.go:1740-1743)
-__global__ void win_init_kernel(const uint32_t* __restrict__ recs, uint64_t n, WinClock* win, uint64_t off) {
+__global__ void win_init_kernel(const uint32_t* __restrict__ recs, uint64_t n, WinClock* win) {
   if (threadIdx.x != 0 || blockIdx.x != 0 || n == 0 || win->ready) return;
   const uint64_t wt = ((uint64_t)recs[7] << 32) | recs[6];
-  const uint64_t e = (wt + off) / win->len;
-  win->lo = e * win->len - off;
+  const uint64_t e = (wt + win->off) / win->len;
+  win->lo = e * win->len - win->off;
+  win->epoch = e;
   win->ready = 1ull;
 }
 __global__ void win_advance_kernel(WinClock* win) {
-  if (threadIdx.x == 0 && blockIdx.x == 0 && win->ready) win->lo += win->len;
+  if (threadIdx.x != 0 || blockIdx.x != 0 || !win->ready) return;
+  const uint64_t start = win->lo + win->off;                  // user time where the closed epoch began
+  if (start + win->len < start) win->ready = 2ull;            // the next one would begin at 2^64 or later
+  win->lo += win->len;
+  win->epoch += 1ull;
+}
+
+// At a table commit: the set-aside records [lo, hi) are resolved under the tables they arrived under, before the
+// patch. A record that makes a row gets its edge key in place of saddr | daddr (kEmptyKey: its source is not a pod,
+// which no real edge key equals: the type-3 end is never reversed). A record that makes no row keeps its words.
+__global__ void __launch_bounds__(256) defer_resolve_kernel(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEntry* __restrict__ ep,
+                                                            uint32_t ep_mask, Counters* ctr) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) ctr->defer_resolved = hi;   // nothing reads it while this kernel runs
+  for (uint32_t i = lo + blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += gridDim.x * blockDim.x) {
+    Rec r;
+    for (int k = 0; k < 8; ++k) r.w[k] = reinterpret_cast<const uint32_t*>(buf + i)[k];
+    const uint32_t proto = rec_protocol(r), mf = rec_mflags(r);
+    if (!emits_request_row(proto, mf)) continue;
+    uint64_t ekey = kEmptyKey;
+    const bool ok = rec_hostkey(r) ? resolve_edge_hostkey(ep, ep_mask, rec_saddr(r), rec_daddr(r), &ekey)
+                                   : resolve_edge(ep, ep_mask, rec_saddr(r), rec_daddr(r), is_reversed(proto, mf), &ekey);
+    if (!ok) ekey = kEmptyKey;
+    buf[i].saddr = (uint32_t)ekey;
+    buf[i].daddr = (uint32_t)(ekey >> 32);
+  }
+}
+
+// At a flush, after the clock has advanced: the resolved set-aside records src[0, n) (defer_resolve_kernel). Those
+// of the window now open are reduced straight into the edge accumulators, as the eager plan does; those of a later
+// window are set aside again into dst, resolution kept, ahead of any raw record (the caller ingests those after).
+__global__ void __launch_bounds__(256) defer_roll_kernel(const alz_l7_rec* __restrict__ src, uint32_t n,
+                                                         const WinClock* __restrict__ win, alz_l7_rec* __restrict__ dst,
+                                                         uint32_t cap, AccTable edges, Counters* ctr) {
+  const uint64_t lo = win->lo, len = win->len, off = win->off;
+  const bool past = win->ready > 1ull;
+  uint32_t not_request = 0, unresolved = 0, lost = 0, late = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const Rec r = load_rec(src + i);
+    const uint64_t wt = ((uint64_t)r.w[7] << 32) | r.w[6];
+    const bool is_late = win_late(wt, lo, off, past);
+    if (!is_late && wt - lo >= len) {
+      const uint32_t at = atomicAdd(&ctr->defer_count, 1u);
+      atomicAdd(&ctr->defer_resolved, 1u);
+      if (at < cap) {
+        uint4* d = reinterpret_cast<uint4*>(dst + at);
+        d[0] = make_uint4(r.w[0], r.w[1], r.w[2], r.w[3]);
+        d[1] = make_uint4(r.w[4], r.w[5], r.w[6], r.w[7]);
+      } else {
+        ++lost;
+      }
+      continue;
+    }
+    late += is_late ? 1u : 0u;
+    const uint32_t proto = rec_protocol(r);
+    if (!emits_request_row(proto, rec_mflags(r))) { ++not_request; continue; }
+    const uint64_t ekey = ((uint64_t)r.w[1] << 32) | r.w[0];
+    if (ekey == kEmptyKey) { ++unresolved; continue; }
+    const uint32_t row = find_or_insert(edges, ekey);
+    if (row >= kLostRow) { ++lost; continue; }
+    const uint64_t dur = rec_duration(r);
+    atomicAdd(&edges.hist[(size_t)row * ALZ_NB + latency_bucket(dur)], 1u);
+    atomicAdd((unsigned long long*)&edges.lat_sum[row], (unsigned long long)dur);
+    if (is_5xx(proto, rec_status(r))) atomicAdd((unsigned long long*)&edges.err5xx[row], 1ull);
+    atomicAdd((unsigned long long*)&edges.count[row], 1ull);
+  }
+  if (not_request) atomicAdd(&ctr->not_request, (unsigned long long)not_request);
+  if (unresolved) atomicAdd(&ctr->src_unresolved, (unsigned long long)unresolved);
+  if (lost) atomicAdd(&ctr->capacity_events, (unsigned long long)lost);
+  if (late) atomicAdd(&ctr->late_events, (unsigned long long)late);
 }
 
 // ---- hot-pair feedback: after a fold, pick the pairs that took the most events -----
@@ -831,14 +911,23 @@ void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint6
 // time-cut windows: `win` = device WinClock {lo, len, ready}; records beyond the open window land in defer_buf
 void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
-                                  uint64_t* win, uint64_t off, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms,
-                                  cudaStream_t s) {
+                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s) {
   if (n == 0) return;
-  win_init_kernel<<<1, 32, 0, s>>>((const uint32_t*)recs, n, (WinClock*)win, off);
+  win_init_kernel<<<1, 32, 0, s>>>((const uint32_t*)recs, n, (WinClock*)win);
   launch_variant<kDefaultWarps, 8, true>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, s,
                                          (const WinClock*)win, defer_buf, defer_cap);
 }
 void launch_window_advance(uint64_t* win, cudaStream_t s) { win_advance_kernel<<<1, 32, 0, s>>>((WinClock*)win); }
+void launch_defer_resolve(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEntry* ep, uint32_t ep_mask, Counters* ctr,
+                          int sms, cudaStream_t s) {
+  const uint32_t grid = std::min<uint32_t>((uint32_t)sms * 4u, std::max<uint32_t>(1u, (hi - lo + 255u) / 256u));
+  defer_resolve_kernel<<<grid, 256, 0, s>>>(buf, lo, hi, ep, ep_mask, ctr);
+}
+void launch_defer_roll(const alz_l7_rec* src, uint32_t n, const uint64_t* win, alz_l7_rec* dst, uint32_t cap,
+                       const AccTable& edges, Counters* ctr, int sms, cudaStream_t s) {
+  const uint32_t grid = std::min<uint32_t>((uint32_t)sms * 4u, std::max<uint32_t>(1u, (n + 255u) / 256u));
+  defer_roll_kernel<<<grid, 256, 0, s>>>(src, n, (const WinClock*)win, dst, cap, edges, ctr);
+}
 
 // after fold_pairs_kernel / emit_edges_kernel filled hot->bins: choose next window's hot list
 void launch_hot_select(const AccTable& pairs, HotState* hot, int sms, cudaStream_t s) {

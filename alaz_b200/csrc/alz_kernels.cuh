@@ -14,9 +14,12 @@ void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint6
                                const uint32_t* bloom, int sms, cudaStream_t s);
 void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
-                                  uint64_t* win, uint64_t off, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms,
-                                  cudaStream_t s);
+                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s);
 void launch_window_advance(uint64_t* win, cudaStream_t s);
+void launch_defer_resolve(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEntry* ep, uint32_t ep_mask, Counters* ctr,
+                          int sms, cudaStream_t s);
+void launch_defer_roll(const alz_l7_rec* src, uint32_t n, const uint64_t* win, alz_l7_rec* dst, uint32_t cap,
+                       const AccTable& edges, Counters* ctr, int sms, cudaStream_t s);
 uint32_t ingest_table_rows();
 void launch_hot_select(const AccTable& pairs, HotState* hot, int sms, cudaStream_t s);
 void launch_ingest_eager(const alz_l7_rec* recs, uint64_t n, const EpEntry* ep, uint32_t ep_mask,
