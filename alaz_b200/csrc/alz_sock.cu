@@ -97,7 +97,7 @@ __device__ __forceinline__ const SockRec* get_value(SockRec* v, uint32_t len, ui
   while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (!(v[mid].ts < ts)) hi = mid; else lo = mid + 1; }
   const uint32_t idx = lo;
   if (idx == len) {                                                    // after the last entry, :94-105
-    atomicMax((unsigned long long*)&v[len - 1].lm, (unsigned long long)now);
+    v[len - 1].lm = now;                                               // every thread of a launch stores the same now
     if (!v[len - 1].open) {
       if (idx >= 2u && v[idx - 2].open && (ts - v[idx - 2].ts) < kOneMinuteNs) return &v[idx - 2];
       return nullptr;
@@ -111,7 +111,7 @@ __device__ __forceinline__ const SockRec* get_value(SockRec* v, uint32_t len, ui
       return (ts - v[idx - 2].ts < v[idx].ts - ts) ? &v[idx - 2] : &v[idx];
     return nullptr;
   }
-  atomicMax((unsigned long long*)&v[idx - 1].lm, (unsigned long long)now);   // :155-157
+  v[idx - 1].lm = now;                                                 // :155-157
   return &v[idx - 1];
 }
 

@@ -681,6 +681,16 @@ size_t orc_sockmaps_records(orc_sockmaps* m) {
   for (size_t i = 0; i < m->cap; i++) if (m->e[i].used) n += m->e[i].line->len;
   return n;
 }
+/* every line's (pid, fd) and length, in table order; returns the number of lines (the first `cap` are written) */
+size_t orc_sockmaps_lines(orc_sockmaps* m, uint32_t* pid, uint64_t* fd, uint64_t* len, size_t cap) {
+  size_t n = 0;
+  for (size_t i = 0; i < m->cap; i++) {
+    if (!m->e[i].used) continue;
+    if (n < cap) { pid[n] = m->e[i].pid; fd[n] = m->e[i].fd; len[n] = m->e[i].line->len; }
+    n++;
+  }
+  return n;
+}
 
 /* L7 events with an empty 5-tuple take the socket of (pid, fd) at WriteTimeNs (findRelatedSocket,
  * data.go:1407-1429); a miss leaves the record as it is */

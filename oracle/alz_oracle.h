@@ -96,6 +96,7 @@ void orc_sockmaps_lookup(orc_sockmaps* m, const alz_sock_query* q, size_t n,
 void orc_sockmaps_lookup_at(orc_sockmaps* m, const alz_sock_query* q, size_t n, uint64_t now, alz_sock_result* out);
 void orc_sockmaps_gc(orc_sockmaps* m);
 size_t orc_sockmaps_records(orc_sockmaps* m);
+size_t orc_sockmaps_lines(orc_sockmaps* m, uint32_t* pid, uint64_t* fd, uint64_t* len, size_t cap);
 void orc_sockmaps_join(orc_sockmaps* m, alz_l7_rec* recs, const alz_sock_query* keys, size_t n, uint64_t now,
                        uint64_t* joined);
 size_t orc_sockmaps_alive(orc_sockmaps* m, const orc* o, alz_alive_conn* out, size_t cap);

@@ -125,6 +125,7 @@ import bisect  # noqa: E402
 
 ONE_MINUTE_NS = 60 * 10**9
 FIVE_MINUTES_NS = 5 * ONE_MINUTE_NS
+MASK64 = (1 << 64) - 1
 
 
 class SocketLine:
@@ -187,7 +188,8 @@ class SocketLine:
                 last_matched = x[2]
         i = len(v) - 1
         while i >= 1:
-            if v[i][1] is None and v[i - 1][1] is not None and v[i - 1][2] + FIVE_MINUTES_NS < last_matched:
+            # uint64 in Go: a stamp within five minutes of 2^64 wraps to a small sum
+            if v[i][1] is None and v[i - 1][1] is not None and ((v[i - 1][2] + FIVE_MINUTES_NS) & MASK64) < last_matched:
                 v = v[:i - 1] + v[i + 1:]
                 i -= 1
             i -= 1

@@ -73,6 +73,8 @@ def lib():
         L.orc_sockmaps_gc.argtypes = [vp]
         L.orc_sockmaps_records.argtypes = [vp]
         L.orc_sockmaps_records.restype = sz
+        L.orc_sockmaps_lines.argtypes = [vp, vp, vp, vp, sz]
+        L.orc_sockmaps_lines.restype = sz
         L.orc_sockmaps_join.argtypes = [vp, vp, vp, sz, u64, C.POINTER(u64)]
         L.orc_sockmaps_alive.argtypes = [vp, vp, vp, sz]
         L.orc_sockmaps_alive.restype = sz
@@ -295,6 +297,14 @@ class SockMaps:
 
     def records(self):
         return int(self.L.orc_sockmaps_records(self.h))
+
+    def lines(self):
+        """{(pid, fd): number of values} of every line, including lines emptied by the GC."""
+        n = int(self.L.orc_sockmaps_lines(self.h, None, None, None, 0))
+        pid, fd, ln = np.zeros(n, np.uint32), np.zeros(n, np.uint64), np.zeros(n, np.uint64)
+        if n:
+            self.L.orc_sockmaps_lines(self.h, _ptr(pid), _ptr(fd), _ptr(ln), n)
+        return {(int(p), int(f)): int(k) for p, f, k in zip(pid, fd, ln)}
 
     def join(self, recs, keys, now_ns=1):
         """recs with empty 5-tuples filled from the timelines (a copy) and the number filled."""
