@@ -74,12 +74,7 @@ static int alloc_table(alz_handle* h, AccTable* t, uint32_t max_rows, uint32_t* 
   } else {
     CK(cudaMalloc(&t->sect, rows * kSectPerRow * 32));
     CK(cudaMemsetAsync(t->sect, 0, rows * kSectPerRow * 32, h->stream));
-    // reversed rows are a few per cent of the traffic: a quarter-size dictionary is ample, and both
-    // dictionaries draw rows from the one pool
-    const uint32_t rev_cap = std::max<uint32_t>(1024u, dict_cap >> 2);
-    t->dict_rev_mask = rev_cap - 1;
-    CK(cudaMalloc(&t->dict_rev, (size_t)rev_cap * sizeof(DictEnt)));
-    CK(cudaMemsetAsync(t->dict_rev, 0xFF, (size_t)rev_cap * sizeof(DictEnt), h->stream));
+    // reversed rows share the socket pair's slot in `dict`; both dictionaries draw rows from the one pool
     const uint32_t host_cap = std::max<uint32_t>(1024u, dict_cap >> 3);   // host-keyed outbound pairs: rarer still
     t->dict_host_mask = host_cap - 1;
     CK(cudaMalloc(&t->dict_host, (size_t)host_cap * sizeof(DictEnt)));
@@ -96,14 +91,13 @@ static int alloc_table(alz_handle* h, AccTable* t, uint32_t max_rows, uint32_t* 
   return ALZ_OK;
 }
 static void free_table(AccTable* t) {
-  cudaFree(t->dict); cudaFree(t->dict_rev); cudaFree(t->dict_host); cudaFree(t->row_key); cudaFree(t->row_kind); cudaFree(t->lat_sum);
+  cudaFree(t->dict); cudaFree(t->dict_host); cudaFree(t->row_key); cudaFree(t->row_kind); cudaFree(t->lat_sum);
   cudaFree(t->err5xx); cudaFree(t->count); cudaFree(t->row_cnt); cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->hist); cudaFree(t->sect);
   memset(t, 0, sizeof(*t));
 }
 // all keys out of the dictionaries; the rows keep their indices until clear_dict resets the allocator
 static int clear_keys(alz_handle* h, AccTable* t) {
   CK(cudaMemsetAsync(t->dict, 0xFF, ((size_t)t->dict_mask + 1) * sizeof(DictEnt), h->stream));
-  if (t->dict_rev) CK(cudaMemsetAsync(t->dict_rev, 0xFF, ((size_t)t->dict_rev_mask + 1) * sizeof(DictEnt), h->stream));
   if (t->dict_host) CK(cudaMemsetAsync(t->dict_host, 0xFF, ((size_t)t->dict_host_mask + 1) * sizeof(DictEnt), h->stream));
   return ALZ_OK;
 }

@@ -120,32 +120,30 @@ __device__ __forceinline__ uint32_t latency_bucket(uint64_t d) {
 // by an atomic counter, so the accumulators of the live keys stay contiguous
 // however large the dictionary was sized. v1 indexed the accumulators by
 // dictionary slot and nearly every reduction missed L2.
+// In the pair table one slot serves both directions of a socket pair: row[kPairFwd] is the row of its forward
+// events, row[kPairRev] the row of its reversed ones (AMQP DELIVER, REDIS PUSHED_EVENT), each allocated on first use.
+// The edge table and the host-keyed dictionary use row[0] only.
 struct __align__(16) DictEnt {
-  uint64_t key;   // kEmptyKey = free
-  uint32_t row;   // kNoRow until the inserting thread has published it
-  uint32_t pad;
+  uint64_t key;     // kEmptyKey = free
+  uint32_t row[2];  // kNoRow = none yet, kClaimRow = being allocated, then the row (or kLostRow)
 };
 constexpr uint32_t kNoRow = 0xFFFFFFFFu;
 constexpr uint32_t kLostRow = 0xFFFFFFFEu;  // dictionary or row pool exhausted
+constexpr uint32_t kClaimRow = 0xFFFFFFFCu; // pair table: a thread is allocating this row word's row; every row
+                                            // word from kClaimRow up names no row
 
 constexpr uint32_t kPairFwd = 0u, kPairRev = 1u, kPairHost = 2u, kPairKinds = 3u;
 
 struct AccTable {
-  DictEnt* dict;      // [dict_mask + 1]   (= dicts[kPairFwd])
+  DictEnt* dict;      // [dict_mask + 1]; pair table: socket pairs, forward and reversed rows in one slot
   uint32_t dict_mask;
-  // pair table only: further dictionaries for the socket pairs of reversed rows (kind 1: AMQP DELIVER, REDIS
-  // PUSHED_EVENT) and for host-keyed outbound events (kind 2: the key's high word is a Host-header id, not a
-  // daddr; ALZ_PROTO_F_HOSTKEY). All dictionaries hand out rows of the same pool; row_kind[row] says which one.
-  DictEnt* dict_rev;
-  uint32_t dict_rev_mask;
+  // pair table only: the dictionary of host-keyed outbound events (kind 2: the key's high word is a Host-header id,
+  // not a daddr; ALZ_PROTO_F_HOSTKEY), a key space of its own. Both dictionaries hand out rows of the same pool;
+  // row_kind[row] says which kind a row is.
   DictEnt* dict_host;
   uint32_t dict_host_mask;
-  __device__ __forceinline__ DictEnt* dict_of(uint32_t kind) const {
-    return kind == kPairFwd ? dict : kind == kPairRev ? dict_rev : dict_host;
-  }
-  __device__ __forceinline__ uint32_t mask_of(uint32_t kind) const {
-    return kind == kPairFwd ? dict_mask : kind == kPairRev ? dict_rev_mask : dict_host_mask;
-  }
+  __device__ __forceinline__ DictEnt* dict_of(uint32_t kind) const { return kind == kPairHost ? dict_host : dict; }
+  __device__ __forceinline__ uint32_t mask_of(uint32_t kind) const { return kind == kPairHost ? dict_host_mask : dict_mask; }
   uint32_t max_rows;  // rows [0, max_rows) are allocatable; rows max_rows + kind are the sentinel rows of the key that
                       // equals the free marker (one per kind); every per-row array has max_rows + kPairKinds entries
   uint32_t* n_rows;   // device counter of allocated rows
@@ -192,14 +190,14 @@ __device__ __forceinline__ uint32_t find_or_insert(const AccTable& t, uint64_t k
       if (old == kEmptyKey) {
         row = atomicAdd(t.n_rows, 1u);
         if (row >= t.max_rows) row = kLostRow; else t.row_key[row] = key;
-        *reinterpret_cast<volatile uint32_t*>(&t.dict[slot].row) = row;
+        *reinterpret_cast<volatile uint32_t*>(&t.dict[slot].row[0]) = row;
         return row;
       }
       k = old;
       row = kNoRow;
     }
     if (k == key) {
-      while (row == kNoRow) row = *reinterpret_cast<volatile uint32_t*>(&t.dict[slot].row);
+      while (row == kNoRow) row = *reinterpret_cast<volatile uint32_t*>(&t.dict[slot].row[0]);
       return row;
     }
     slot = (slot + 1u) & t.dict_mask;
@@ -223,7 +221,9 @@ __device__ __forceinline__ uint32_t ep_lookup(const EpEntry* __restrict__ tab, u
 // inserted if its source address is a pod right now (setFromToV2's first test, data.go:829-832).
 // Unresolvable traffic is often high-cardinality (every event a new pair); letting it into the
 // dictionary cost a CAS, a row and two DRAM-missing reductions per event.
-// Existing pairs are found without touching the endpoint table. Returns kDropRow for a rejected pair.
+// Existing rows are found without touching the endpoint table. Returns kDropRow for a rejected pair.
+// A forward and a reversed event of one socket pair share the slot; each kind's row is allocated the first time an
+// event of that kind comes, by the thread whose CAS takes that row word from kNoRow to kClaimRow.
 constexpr uint32_t kDropRow = 0xFFFFFFFDu;
 __device__ __forceinline__ uint32_t find_or_insert_pair(const AccTable& t, uint64_t key, uint32_t kind,
                                                         const EpEntry* __restrict__ ep, uint32_t ep_mask) {
@@ -231,32 +231,45 @@ __device__ __forceinline__ uint32_t find_or_insert_pair(const AccTable& t, uint6
   if (key == kEmptyKey) return t.max_rows + kind;
   DictEnt* const dict = t.dict_of(kind);
   const uint32_t mask = t.mask_of(kind);
+  const uint32_t w = kind == kPairRev ? 1u : 0u;   // the slot's row word of this kind
   uint32_t slot = pair_hash(key) & mask;
   bool checked = false;
+  auto is_pod = [&]() {
+    if (!checked) {
+      uint32_t pod, svc;
+      if ((ep_lookup(ep, ep_mask, pair_saddr(key), &pod, &svc) & kEpPod) == 0u) return false;
+      checked = true;
+    }
+    return true;
+  };
 #pragma unroll 1
   for (uint32_t p = 0; p < kMaxProbe; ++p) {
     const uint4 e = __ldcg(reinterpret_cast<const uint4*>(&dict[slot]));
     uint64_t k = ((uint64_t)e.y << 32) | e.x;
-    uint32_t row = e.z;
+    uint32_t row = w ? e.w : e.z;
     if (k == kEmptyKey) {
-      if (!checked) {
-        uint32_t pod, svc;
-        if ((ep_lookup(ep, ep_mask, pair_saddr(key), &pod, &svc) & kEpPod) == 0u) return kDropRow;
-        checked = true;
-      }
-      const uint64_t old = atomicCAS((unsigned long long*)&dict[slot].key, (unsigned long long)kEmptyKey,
-                                     (unsigned long long)key);
-      if (old == kEmptyKey) {
-        row = atomicAdd(t.n_rows, 1u);
-        if (row >= t.max_rows) row = kLostRow; else { t.row_key[row] = key; t.row_kind[row] = (uint8_t)kind; }
-        *reinterpret_cast<volatile uint32_t*>(&dict[slot].row) = row;
-        return row;
-      }
-      k = old;
-      row = kNoRow;
+      if (!is_pod()) return kDropRow;
+      k = atomicCAS((unsigned long long*)&dict[slot].key, (unsigned long long)kEmptyKey, (unsigned long long)key);
+      if (k == kEmptyKey) k = key;
+      row = *reinterpret_cast<volatile uint32_t*>(&dict[slot].row[w]);
     }
     if (k == key) {
-      while (row == kNoRow) row = *reinterpret_cast<volatile uint32_t*>(&dict[slot].row);
+      uint32_t* const rw = &dict[slot].row[w];
+#pragma unroll 1
+      while (row == kNoRow || row == kClaimRow) {
+        if (row == kNoRow) {
+          if (!is_pod()) return kDropRow;
+          row = atomicCAS(rw, kNoRow, kClaimRow);
+          if (row == kNoRow) {
+            row = atomicAdd(t.n_rows, 1u);
+            if (row >= t.max_rows) row = kLostRow; else { t.row_key[row] = key; t.row_kind[row] = (uint8_t)kind; }
+            *reinterpret_cast<volatile uint32_t*>(rw) = row;
+            return row;
+          }
+        } else {
+          row = *reinterpret_cast<volatile uint32_t*>(rw);
+        }
+      }
       return row;
     }
     slot = (slot + 1u) & mask;

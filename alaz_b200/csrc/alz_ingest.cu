@@ -17,8 +17,8 @@
 //         2-way bucket of the index (fingerprint | window | row per entry), one key load, two shared
 //         reductions. 16-bit cells stay exact: the lane that sees a cell at 0x7FFF spills 0x8000
 //         counts into the global table (bit 15 is head room for the increments racing with it).
-//   cold  everything else (a pair without a row, a latency outside its row's window, a reversed
-//         or host-keyed row) is NOT handled inline: the lane pushes the event onto its warp's
+//   cold  everything else (a pair without a row, a latency outside its row's window, a host-keyed
+//         row) is NOT handled inline: the lane pushes the event onto its warp's
 //         queue (ballot-compacted, no atomics) and the warp runs the cold path for 32 queued
 //         events at a time with all lanes busy — global dictionary probe of the home slot, then
 //         the reduction into the pair's row in L2: ONE red.u64 per event, a lane pair adding the
@@ -177,6 +177,15 @@ constexpr uint32_t kProtoLut = proto_class(0) | proto_class(1) << 3 | proto_clas
 __device__ __forceinline__ uint32_t table_hash(uint64_t key) {
   return (uint32_t)key * 0x9E3779B1u + (uint32_t)(key >> 32) * 0x85EBCA6Bu;
 }
+// Forward and reversed rows of one socket pair are separate rows of the table (the per-CTA table holds no host-keyed
+// rows). A reversed pair hashes to table_hash(key) ^ kRevSalt: another index bucket, and a fingerprint that differs
+// from the forward one of the same key in bit 17 (kRevSalt bit 1), so an entry whose row holds the event's key is
+// always of the event's kind.
+constexpr uint32_t kRevSalt = 0x5BD1E996u;
+static_assert((kRevSalt & 2u) != 0u, "the two kinds of one key must differ in a fingerprint bit");
+__device__ __forceinline__ uint32_t table_hash_kind(uint64_t key, uint32_t kind) {
+  return table_hash(key) ^ (kind == kPairRev ? kRevSalt : 0u);
+}
 // the key's two index slots are the two halves of one 8-byte bucket: one LDS.64 fetches both (two independent
 // 4-byte probes cost two instructions and, with 32 random addresses each, about twice the shared-memory passes)
 __device__ __forceinline__ uint32_t tab_idx1(uint32_t h) { return (h >> kTabShift) & ~1u; }
@@ -195,14 +204,15 @@ struct Shared {
   uint32_t* bloom;    // [ALZ_BLOOM_WORDS]
   uint64_t* rowkey;   // [kRows + 1], entry kRows = kEmptyKey (never a hit)
   uint32_t* rows;     // [(kRows + 1) * kRowWords]
-  uint8_t* rowbase;   // [kRows + 1] first bucket / 4 of the row's window (also in its index entry)
+  uint8_t* rowbase;   // [kRows + 1] first bucket / 4 of the row's window (also in its index entry) | pair kind << 4
   uint32_t* n_rows;   // rows handed out
 };
 
 // claim one of the key's two index slots and give it a row; false if both are taken or the rows are used up.
-// `publish_fenced`: other warps are probing concurrently, so the row's key must be visible before the entry
-__device__ __forceinline__ bool smem_admit(const Shared& s, uint64_t key, uint32_t h, uint32_t base4, uint32_t limit,
-                                           bool publish_fenced) {
+// h = table_hash_kind(key, kind). `publish_fenced`: other warps are probing concurrently, so the row's key must be
+// visible before the entry
+__device__ __forceinline__ bool smem_admit(const Shared& s, uint64_t key, uint32_t kind, uint32_t h, uint32_t base4,
+                                           uint32_t limit, bool publish_fenced) {
   uint32_t idx = tab_idx1(h);
   if (atomicCAS(&s.tab[idx], 0u, kBusy) != 0u) {
     idx = tab_idx2(h);
@@ -211,7 +221,7 @@ __device__ __forceinline__ bool smem_admit(const Shared& s, uint64_t key, uint32
   const uint32_t row = atomicAdd(s.n_rows, 1u);
   if (row >= limit) return false;                       // slot stays kBusy: reads as a miss for everyone
   s.rowkey[row] = key;
-  s.rowbase[row] = (uint8_t)base4;
+  s.rowbase[row] = (uint8_t)(base4 | (kind << 4));
   if (publish_fenced) __threadfence_block();
   *reinterpret_cast<volatile uint32_t*>(&s.tab[idx]) = tab_entry(h, base4, row);
   return true;
@@ -291,8 +301,8 @@ __device__ __forceinline__ void slow_one(uint64_t key, uint64_t dur, uint32_t bu
   if (row >= kDropRow) { if (row == kDropRow) *unresolved += 1u; else *lost += 1u; return; }
   global_add(t, row, bucket, dur, err);
   // a pair the per-CTA table does not hold: give it a private row while some are left (first-come)
-  if (kind == kPairFwd && key != kEmptyKey && *reinterpret_cast<volatile uint32_t*>(s.n_rows) < kRows)
-    smem_admit(s, key, table_hash(key), base4_around(bucket), kRows, true);
+  if (kind != kPairHost && key != kEmptyKey && *reinterpret_cast<volatile uint32_t*>(s.n_rows) < kRows)
+    smem_admit(s, key, kind, table_hash_kind(key, kind), base4_around(bucket), kRows, true);
 }
 template <uint32_t kRows>
 __device__ __forceinline__ void slow_batch(SlowQueue& q, uint32_t count, const AccTable& t, const Shared& s,
@@ -344,8 +354,10 @@ __device__ __forceinline__ void cold_consume(ColdQueue& q, uint32_t count, const
   uint4 e = make_uint4(0u, 0u, 0u, 0u), ent = make_uint4(0u, 0u, kNoRow, 0u);
   if (valid) { e = *q.at(lane); ent = probe[lane]; }
   const bool filtered = valid && ent.z == kDropRow && ent.w == 1u;
-  const bool home = valid && !filtered && ent.x == e.x && ent.y == e.y && ent.z < kDropRow && (e.x & e.y) != 0xFFFFFFFFu;
-  global_add_paired(t, home, ent.z, e.w, e.z);
+  // the row word of the event's kind; a slot that has the pair but no row of this kind yet goes to the slow queue
+  const uint32_t row = ((e.w >> 6) & 3u) == kPairRev ? ent.w : ent.z;
+  const bool home = valid && !filtered && ent.x == e.x && ent.y == e.y && row < kClaimRow && (e.x & e.y) != 0xFFFFFFFFu;
+  global_add_paired(t, home, row, e.w, e.z);
   if (filtered) *unresolved += 1u;
   slow.push(valid && !home && !filtered, ((uint64_t)e.y << 32) | e.x, e.z, e.w, lane_lt);
   __syncwarp();
@@ -376,7 +388,7 @@ __device__ __forceinline__ void drain_rows_and_count(const Shared& s, const AccT
 #pragma unroll
     for (int k = 0; k < (int)kRowWords; ++k) any |= row[k];
     uint32_t grow = kNoRow;                       // never hit in this launch: no global row needed
-    if (key != kEmptyKey && any != 0u) grow = find_or_insert_pair(pairs, key, kPairFwd, ep, ep_mask);
+    if (key != kEmptyKey && any != 0u) grow = find_or_insert_pair(pairs, key, s.rowbase[r] >> 4, ep, ep_mask);
     reinterpret_cast<uint32_t*>(&s.rowkey[r])[0] = grow;
   }
   __syncthreads();
@@ -397,7 +409,7 @@ __device__ __forceinline__ void drain_rows_and_count(const Shared& s, const AccT
     }
     // the window's 16 cells = 4 sectors of the global row, 4 lanes each; the row's latency and 5xx totals go to the
     // partials of the window's first sector (any sector of the row would do: the fold sums them)
-    const uint32_t base = (uint32_t)s.rowbase[r] * 4u;
+    const uint32_t base = ((uint32_t)s.rowbase[r] & 15u) * 4u;
     if (cnt) red_add_u32(pair_cell(pairs, grow, base + hl), cnt);
     if (hl == 0) {
       const uint64_t lat = (((uint64_t)row[10] << 32) + row[9]) + (((uint64_t)row[12] << 32) + row[11]);
@@ -432,18 +444,20 @@ __device__ __forceinline__ uint32_t preload_hot(const Shared& s, const HotState*
   if (hot == nullptr) return 0u;
   const uint32_t ns = min(hot->n_s, (uint32_t)kHotS);
   const uint32_t rep_rows = ns ? (uint32_t)(kHotS * kHotRep) : 0u;
+  // a hot-list base byte is the window's first bucket / 4 | pair kind << 4
   if (threadIdx.x < ns * kHotRep) {
-    const uint32_t i = threadIdx.x / kHotRep;
-    s.rowkey[threadIdx.x] = hot->skeys[i];
-    s.rowbase[threadIdx.x] = (uint8_t)min((uint32_t)hot->sbase[i], 12u);
+    const uint32_t b = hot->sbase[threadIdx.x / kHotRep];
+    s.rowkey[threadIdx.x] = hot->skeys[threadIdx.x / kHotRep];
+    s.rowbase[threadIdx.x] = (uint8_t)(min(b & 15u, 12u) | (b & 0x10u));
   }
   if (threadIdx.x < ns) {
     const uint64_t k = hot->skeys[threadIdx.x];
-    const uint32_t h = table_hash(k);
+    const uint32_t b = hot->sbase[threadIdx.x];
+    const uint32_t h = table_hash_kind(k, b >> 4);
     uint32_t idx = tab_idx1(h);
     bool got = atomicCAS(&s.tab[idx], 0u, kBusy) == 0u;
     if (!got) { idx = tab_idx2(h); got = atomicCAS(&s.tab[idx], 0u, kBusy) == 0u; }
-    if (got && k != kEmptyKey) s.tab[idx] = tab_entry(h, min((uint32_t)hot->sbase[threadIdx.x], 12u), threadIdx.x * kHotRep);
+    if (got && k != kEmptyKey) s.tab[idx] = tab_entry(h, min(b & 15u, 12u), threadIdx.x * kHotRep);
   }
   if (threadIdx.x == 0) *s.n_rows = rep_rows;
   __syncthreads();
@@ -452,12 +466,14 @@ __device__ __forceinline__ uint32_t preload_hot(const Shared& s, const HotState*
   const uint32_t nb = min(min(hot->n_b, (uint32_t)(kHotMax - kHotA)), room);
   for (uint32_t i = threadIdx.x; i < na; i += kThreads) {   // tier A before B: the hotter pairs cannot lose their slots
     const uint64_t k = hot->keys[i];
-    if (k != kEmptyKey) smem_admit(s, k, table_hash(k), min((uint32_t)hot->base[i], 12u), limit, false);
+    const uint32_t b = hot->base[i];
+    if (k != kEmptyKey) smem_admit(s, k, b >> 4, table_hash_kind(k, b >> 4), min(b & 15u, 12u), limit, false);
   }
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < nb; i += kThreads) {
     const uint64_t k = hot->keys[kHotA + i];
-    if (k != kEmptyKey) smem_admit(s, k, table_hash(k), min((uint32_t)hot->base[kHotA + i], 12u), limit, false);
+    const uint32_t b = hot->base[kHotA + i];
+    if (k != kEmptyKey) smem_admit(s, k, b >> 4, table_hash_kind(k, b >> 4), min(b & 15u, 12u), limit, false);
   }
   __syncthreads();
   if (threadIdx.x == 0 && *s.n_rows > limit) *s.n_rows = limit;   // failed claims past the limit
@@ -662,7 +678,7 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
       meta[u] = bucket | (kind << 6) | (err ? 0x100u : 0u) | ((uint32_t)(dur[u] >> 32) << 9);
 
       // per-CTA table: the key's bucket of two index entries, the matching one names the row and its histogram window
-      const uint32_t h = table_hash(key[u]);
+      const uint32_t h = table_hash(key[u]) ^ (rv ? kRevSalt : 0u);   // table_hash_kind; host-keyed: never a candidate
       const uint32_t fp = tab_fp(h);
       const uint2 t2 = *reinterpret_cast<const uint2*>(&s.tab[tab_idx1(h)]);
       const uint32_t x1 = t2.x ^ fp, x2 = t2.y ^ fp;
@@ -670,7 +686,7 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
       rowi[u] = min(x & kRowMask, kRows);
       rowi[u] += rowi[u] < rep_rows ? (lane & (uint32_t)(kHotRep - 1)) : 0u;   // tier S: this lane's row of the group
       cell[u] = bucket - ((x >> 12) & 15u) * 4u;                     // cell of this latency in the row's window
-      cand[u] = act[u] && kind == kPairFwd && x < 0x10000u && (x & kRowMask) < kRows && cell[u] < 16u;
+      cand[u] = act[u] && !hk && x < 0x10000u && (x & kRowMask) < kRows && cell[u] < 16u;
     }
     bool hit[kU];
 #pragma unroll
@@ -689,7 +705,7 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable p
         if (spill) {
           // this lane took the cell to 0x8000: move 0x8000 counts into the global table (rare: a pair with more
           // than 32767 events in one bucket within one launch of one CTA)
-          const uint32_t grow = find_or_insert_pair(pairs, key[u], kPairFwd, ep, ep_mask);
+          const uint32_t grow = find_or_insert_pair(pairs, key[u], (meta[u] >> 6) & 3u, ep, ep_mask);
           if (grow < kDropRow) red_add_u32(pair_cell(pairs, grow, meta[u] & 0x3Fu), 0x8000u);
           else if (grow == kDropRow) unresolved += 0x8000u; else lost += 0x8000u;
           atomicSub(cellp, 0x8000u << sh);
@@ -861,17 +877,19 @@ __global__ void __launch_bounds__(256) hot_emit_kernel(AccTable pairs, HotState*
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t row = blockIdx.x * blockDim.x + threadIdx.x; row < n_rows; row += stride) {
     const uint32_t c = pairs.row_cnt[row];
-    if (c == 0u || pairs.row_kind[row] != kPairFwd) continue;   // only forward pairs enter the per-CTA table
+    const uint32_t kind = pairs.row_kind[row];
+    if (c == 0u || kind == kPairHost) continue;   // host-keyed pairs do not enter the per-CTA table
     const uint32_t b = count_bin(c);
+    const uint8_t base = (uint8_t)(pairs.row_base[row] | (kind << 4));   // window base | kind, see preload_hot
     if (b >= thr_s) {
       const uint32_t p = atomicAdd(&hot->n_s, 1u);
-      if (p < (uint32_t)kHotS) { hot->skeys[p] = pairs.row_key[row]; hot->sbase[p] = pairs.row_base[row]; }
+      if (p < (uint32_t)kHotS) { hot->skeys[p] = pairs.row_key[row]; hot->sbase[p] = base; }
     } else if (b >= thr_a) {
       const uint32_t p = atomicAdd(&hot->n_a, 1u);
-      if (p < (uint32_t)kHotA) { hot->keys[p] = pairs.row_key[row]; hot->base[p] = pairs.row_base[row]; }
+      if (p < (uint32_t)kHotA) { hot->keys[p] = pairs.row_key[row]; hot->base[p] = base; }
     } else if (b >= thr_b) {
       const uint32_t p = atomicAdd(&hot->n_b, 1u);
-      if (p < (uint32_t)(kHotMax - kHotA)) { hot->keys[kHotA + p] = pairs.row_key[row]; hot->base[kHotA + p] = pairs.row_base[row]; }
+      if (p < (uint32_t)(kHotMax - kHotA)) { hot->keys[kHotA + p] = pairs.row_key[row]; hot->base[kHotA + p] = base; }
     }
   }
 }

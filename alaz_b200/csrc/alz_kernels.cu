@@ -186,6 +186,20 @@ __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const
 // (row_base, row_cnt and the count bin of a forward row), zeroes what was not zero and returns the row's event count,
 // the same in all eight lanes. Every lane of the group calls it; `valid` is uniform over the group.
 struct PairSlice { uint4 a, pa, b, pb; };
+// The count bins of the hot list are summed per block in shared memory and added to hot_bins once per block: the
+// counts of a window's rows fall into a few dozen bins, and one global atomic per row piles up on those few words.
+// block_bins_begin returns the bins take_pair_row adds to (nullptr when there is no hot list); every thread of the
+// block calls both.
+__device__ __forceinline__ uint32_t* block_bins_begin(uint32_t* s_bins, uint32_t* hot_bins) {
+  for (uint32_t b = threadIdx.x; b < 128u; b += blockDim.x) s_bins[b] = 0u;
+  __syncthreads();
+  return hot_bins != nullptr ? s_bins : nullptr;
+}
+__device__ __forceinline__ void block_bins_end(const uint32_t* s_bins, uint32_t* hot_bins) {
+  __syncthreads();
+  if (hot_bins == nullptr) return;
+  for (uint32_t b = threadIdx.x; b < 128u; b += blockDim.x) if (s_bins[b]) atomicAdd(&hot_bins[b], s_bins[b]);
+}
 __device__ __forceinline__ uint64_t take_pair_row(const AccTable& pairs, uint32_t row, bool valid, uint32_t gmask,
                                                   uint32_t* __restrict__ hot_bins, PairSlice& s) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
@@ -215,7 +229,7 @@ __device__ __forceinline__ uint64_t take_pair_row(const AccTable& pairs, uint32_
   if (sl == 0 && row < pairs.max_rows && pairs.row_cnt != nullptr) {    // feedback for the next ingest
     const uint32_t c32 = cnt > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cnt;
     pairs.row_cnt[row] = c32;
-    if (hot_bins != nullptr && pairs.row_kind[row] == kPairFwd) atomicAdd(&hot_bins[count_bin(c32)], 1u);
+    if (hot_bins != nullptr && pairs.row_kind[row] != kPairHost) atomicAdd(&hot_bins[count_bin(c32)], 1u);
   }
   // zero what was not zero: a pair's latencies fall into a few of its 16 sectors, the rest was never written
   const uint4 pa = s.pa, pb = s.pb;
@@ -246,12 +260,14 @@ __global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTabl
   const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
+  __shared__ uint32_t s_bins[128];
+  uint32_t* const bins = block_bins_begin(s_bins, hot_bins);
   uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3;
   // rows [0, n_rows) plus the sentinel rows (index n_rows + kind stands for row max_rows + kind)
   for (; i < n_rows + kPairKinds; i += groups_per_grid) {
     const uint32_t row = i >= n_rows ? pairs.max_rows + (i - n_rows) : i;
     PairSlice s;
-    const uint64_t cnt = take_pair_row(pairs, row, true, gmask, hot_bins, s);
+    const uint64_t cnt = take_pair_row(pairs, row, true, gmask, bins, s);
     if (cnt == 0) continue;
     uint64_t lat = lat_partial(s), e5 = err_partial(s);
     for (int o = 1; o < 8; o <<= 1) {
@@ -279,6 +295,7 @@ __global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTabl
       count_stray_events(ctr, erow, cnt);
     }
   }
+  block_bins_end(s_bins, hot_bins);
 }
 
 // ---------------------------------------------------------------------------
@@ -376,11 +393,13 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTabl
   const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_groups = n_live + (off != nullptr ? *n_stray : 0u);
+  __shared__ uint32_t s_bins[128];
+  uint32_t* const bins = block_bins_begin(s_bins, hot_bins);
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_groups; i += groups_per_grid) {
     if (i >= n_live) {
       const uint32_t row = row_list[list_cap - 1u - (i - n_live)];
       PairSlice s;
-      const uint64_t cnt = take_pair_row(pairs, row, true, gmask, hot_bins, s);
+      const uint64_t cnt = take_pair_row(pairs, row, true, gmask, bins, s);
       if (sl == 0 && cnt != 0) count_stray_events(ctr, pairs.row_aux[row], cnt);
       continue;
     }
@@ -402,7 +421,7 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTabl
       const uint32_t end = off[erow + 1u];
       for (uint32_t j = off[erow]; j < end; ++j) {
         PairSlice s;
-        count += take_pair_row(pairs, row_list[j], true, gmask, hot_bins, s);
+        count += take_pair_row(pairs, row_list[j], true, gmask, bins, s);
         c[0] += s.a.x; c[1] += s.a.y; c[2] += s.a.z; c[3] += s.a.w;
         c[4] += s.b.x; c[5] += s.b.y; c[6] += s.b.z; c[7] += s.b.w;
         lat += lat_partial(s);
@@ -415,6 +434,7 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTabl
     }
     store_edge_out(&out[i], sl, keys[i], c, count, e5, lat);
   }
+  block_bins_end(s_bins, hot_bins);
 }
 
 // ---------------------------------------------------------------------------
