@@ -834,14 +834,20 @@ static int window_roll(alz_handle* h) {
   return rc;
 }
 
+// Several ranks: *n_out is 0 and *dev_edges untouched unless the merge consumed the window; a failure the
+// ranks share (a peer's local error) keeps the window, and a lost event on any rank is ALZ_E_CAPACITY on all.
 static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, size_t* n_out) {
   bool overflow = false;
+  const bool ranks = h->comm_nranks > 1;
   CK(cudaEventRecord(h->ev_t[0], h->stream));
   int rc = prepare_flush(h, &overflow);
-  *n_out = h->n_live;
+  *n_out = ranks ? 0u : h->n_live;
   CK(cudaEventRecord(h->ev_t[1], h->stream));
-  int mrc = alz_internal_merge_ranks(h, rc);  // multi-GPU: one collective over the ranks' edge rows (alz_comm.cu)
-  if (mrc == ALZ_E_UNSUPPORTED) {             // single rank
+  int mrc;
+  if (ranks) {    // one collective over the ranks' edge rows (alz_comm.cu)
+    mrc = alz_internal_merge_ranks(h, rc, &overflow);
+    if (mrc != ALZ_OK && overflow && rc == ALZ_OK) h->lost_reported = ~0ull;   // window kept: report the loss again
+  } else {
     if (rc != ALZ_OK) return rc;
     mrc = finish_flush(h);
   }
@@ -891,11 +897,20 @@ extern "C" int alz_window_flush(alz_handle* h, alz_edge_out* out, size_t cap, si
   }
   // several ranks: the merge consumes the window on every rank, so a too-small buffer cannot keep it.
   // The merged rows stay on the device (alz_window_fetch) and *n_out says how many there are.
+  // Every rank returns the same status for the same window:
+  //  - ALZ_OK: *n_out merged rows in canonical order;
+  //  - ALZ_E_CAPACITY with rows: some rank lost events in its own tables, or the merged graph had more than
+  //    max_edges rows and the first max_edges in canonical order are returned (each rank counts the events of
+  //    its own rows past the cut in capacity_events, so the ranks' rows_emitted add up to the rows returned);
+  //  - ALZ_E_CAPACITY with *n_out = 0 rows after a merge of keys present on several ranks whose union, or R x the
+  //    largest rank's count, exceeds max_edges: the window is consumed and every event of it counted lost;
+  //  - ALZ_E_CAPACITY with *n_out > cap: the window is consumed, alz_window_fetch returns its rows;
+  //  - another error (a rank's local preparation failed): *n_out = 0, the window is kept on every rank.
   const alz_edge_out* d = nullptr;
   int rc = flush_device_locked(h, &d, n_out);
   if (rc != ALZ_OK && rc != ALZ_E_CAPACITY) return rc;
   if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, d, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  if (*n_out && d) CK(cudaMemcpyAsync(out, d, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return rc;
 }
@@ -921,7 +936,7 @@ extern "C" int alz_get_stats(alz_handle* h, alz_stats* st) {
   CK(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   memset(st, 0, sizeof(*st));
-  const uint64_t lost = h->h_ctr->capacity_events + h->h_ctr->fold_lost_events;
+  const uint64_t lost = h->h_ctr->capacity_events + h->h_ctr->fold_lost_events + h->merge_lost_events;
   // a record set aside past the buffer's capacity is in `lost` already, not waiting
   const uint64_t held = std::min<uint64_t>(h->h_ctr->defer_count, h->defer_cap);
   st->events_in = h->events_in;

@@ -11,17 +11,22 @@
 //   3. every rank merges the R sorted, disjoint lists: a row's place in the canonical
 //      (ascending packed key) order is its index in its own list plus its lower bounds
 //      in the other lists. The same kernel notices a key present on two ranks, a rank
-//      whose rows did not fit its block, or a rank that reported a local error — all
-//      ranks see the same headers, so all ranks take the same decision.
+//      whose rows did not fit its block, a rank that reported a local error, or a rank
+//      that lost events in its own tables — all ranks see the same headers, so all ranks
+//      take the same decision and return the same status.
 //   4. one device->host read of {total, flags}: the only synchronisation, and the one the
 //      API needs anyway to return the edge count.
 // A block that was too small (traffic grew by more than 25 % in one window) is sent
 // again, larger; the local rows are only reset after a successful merge.
+// A merged graph larger than max_edges is cut in canonical order: every rank keeps the
+// first max_edges rows, consumes its window and counts the events of its own rows past
+// the cut as lost, so the ranks' rows_emitted still add up to the rows returned.
 //
 // General path (a key present on several ranks: the caller did not partition by
 // alz_owner_rank): canonical dictionary by all-gather + sort + unique, local rows
 // scattered into a zeroed canonical array, ONE ncclAllReduce(sum) on the accumulators.
-// Integer sums either way, so bit-exact for any rank count.
+// Integer sums either way, so bit-exact for any rank count. When the gathered keys or
+// their union do not fit max_edges, every rank drops its window and counts its events lost.
 //
 // NCCL is loaded lazily with dlopen so that single-GPU users (and the Go agent
 // on a box without NCCL) never need libnccl.so.2.
@@ -85,12 +90,14 @@ constexpr uint32_t kHdrMagic = 0xA1A2C0DEu;
 struct BlockHeader {      // first row of a rank's block
   uint32_t magic, count;
   int32_t status;
-  uint32_t pad;
+  uint32_t lost;          // 1: this rank's pair or edge table lost events in this window
 };
 struct MergeInfo {        // written by the merge kernel, read by the host
   uint32_t total, dup, overflow, max_count;
   int32_t peer_status;
-  uint32_t pad[3];
+  uint32_t lost;          // some rank's header has lost = 1
+  uint32_t pad[2];
+  unsigned long long lost_events;   // counts of this rank's rows that fell at or past max_edges in the merged order
 };
 
 // out[i] = keys[i] for i < n, kEmptyKey padding up to n_pad
@@ -204,10 +211,11 @@ __device__ __forceinline__ uint32_t lower_bound_rows(const alz_edge_out* rows, u
 }
 
 // Merge of the gathered blocks: block q = header row + cap rows, of which header.count are live and sorted.
-// Eight lanes per row: the lanes split the other ranks' binary searches among them, then copy the row.
+// Eight lanes per row: the lanes split the other ranks' binary searches among them, then copy the row. Rows whose
+// place is at or past out_cap are not written; those of rank `me` add their counts to info->lost_events.
 __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* __restrict__ recv, uint32_t cap, uint32_t R,
-                                                           alz_edge_out* __restrict__ out, uint32_t out_cap,
-                                                           MergeInfo* __restrict__ info) {
+                                                           uint32_t me, alz_edge_out* __restrict__ out,
+                                                           uint32_t out_cap, MergeInfo* __restrict__ info) {
   __shared__ uint32_t s_cnt[64];
   __shared__ uint32_t s_bad;
   const size_t stride_rows = (size_t)cap + 1;
@@ -223,13 +231,14 @@ __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* _
     }
     if (cnt > cap) { atomicOr(&s_bad, 2u); if (blockIdx.x == 0) { info->overflow = 1u; atomicMax(&info->max_count, cnt); } }
     if (blockIdx.x == 0) atomicMax(&info->max_count, cnt);
+    if (blockIdx.x == 0 && hd->lost != 0u) info->lost = 1u;
     s_cnt[threadIdx.x] = cnt;
   }
   __syncthreads();
   uint32_t total = 0;
   for (uint32_t q = 0; q < R; ++q) total += s_cnt[q];
   if (blockIdx.x == 0 && threadIdx.x == 0) info->total = total;
-  if (s_bad != 0u || total > out_cap) { if (blockIdx.x == 0 && threadIdx.x == 0 && total > out_cap) info->overflow = 2u; return; }
+  if (s_bad != 0u) return;
   const uint32_t sl = threadIdx.x & 7u;
   const uint32_t groups = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_iter = (total + groups - 1) / groups;
@@ -254,6 +263,10 @@ __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* _
     part += __shfl_xor_sync(0xFFFFFFFFu, part, 4);
     if (dup) info->dup = 1u;
     if (!valid) continue;
+    if (i + part >= out_cap) {   // past the cut: the owner counts the row's events as lost
+      if (q == me && sl == 0u) atomicAdd(&info->lost_events, (unsigned long long)src->count);
+      continue;
+    }
     const uint64_t* s64 = reinterpret_cast<const uint64_t*>(src);
     uint64_t* d64 = reinterpret_cast<uint64_t*>(out + (i + part));
     for (uint32_t w = sl; w < kRowWords64; w += 8u) d64[w] = s64[w];
@@ -280,6 +293,15 @@ __global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __
     cells[1] = make_uint4(0u, 0u, 0u, 0u);
     if (sl == 0) { edges.count[row] = 0ull; edges.err5xx[row] = 0ull; edges.lat_sum[row] = 0ull; }
   }
+}
+
+// info->lost_events += the counts of n rows (the general path's dropped window)
+__global__ void __launch_bounds__(256) sum_counts_kernel(const alz_edge_out* __restrict__ rows, uint32_t n,
+                                                         MergeInfo* __restrict__ info) {
+  unsigned long long s = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) s += rows[i].count;
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, o);
+  if ((threadIdx.x & 31u) == 0u && s) atomicAdd(&info->lost_events, s);
 }
 
 }  // namespace
@@ -344,6 +366,7 @@ static uint32_t block_rows_for(uint64_t max_count) {   // +25 % head room, in st
 
 extern "C" int alz_comm_init(alz_handle* h, int nranks, int rank, const void* id_bytes) {
   if (!h || !id_bytes || nranks < 1 || rank < 0 || rank >= nranks) return ALZ_E_INVAL;
+  if (nranks > 64) return ALZ_E_UNSUPPORTED;   // the merge kernel keeps one block count per rank in 64 shared words
   std::lock_guard<std::mutex> g(h->mu);
   if (h->comm) return ALZ_E_STATE;
   if (!load_nccl()) { h->last_err = "dlopen(libnccl.so.2) failed"; return ALZ_E_NCCL; }
@@ -395,8 +418,34 @@ void alz_internal_free_comm(alz_handle* h) {
   h->comm = nullptr;
 }
 
+// The general path's keys do not fit max_edges: this rank's window is consumed without a merge, its events are
+// counted lost and the flush returns no rows. Every rank decides this from the same gathered counts or keys.
+// The local rows are in d_send (gathered before the block exchange).
+static int drop_window(alz_handle* h, bool* lost) {
+  alz_comm_state* c = h->comm;
+  cudaStream_t s = h->stream;
+  const unsigned grid = (unsigned)h->sms * 4;
+  CK(cudaMemsetAsync(c->d_info, 0, sizeof(MergeInfo), s));
+  if (h->n_live) {
+    sum_counts_kernel<<<grid, 256, 0, s>>>(c->d_send + 1, h->n_live, c->d_info);
+    consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], h->n_live);
+    h->launches += 2;
+  } else {
+    CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
+    CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(c->h_info, c->d_info, sizeof(MergeInfo), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  h->merge_lost_events += c->h_info->lost_events;
+  *lost = true;
+  h->last_n_edges = 0;
+  h->windows++;
+  return ALZ_OK;
+}
+
 // General path: keys may live on several ranks. Local live edges are sorted in d_keys[1] / d_rows[1].
-static int merge_allreduce(alz_handle* h) {
+static int merge_allreduce(alz_handle* h, bool* lost) {
   alz_comm_state* c = h->comm;
   const int R = h->comm_nranks;
   cudaStream_t s = h->stream;
@@ -417,7 +466,7 @@ static int merge_allreduce(alz_handle* h) {
     CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
     return ALZ_OK;
   }
-  if ((uint64_t)pad * R > c->gather_cap) return ALZ_E_CAPACITY;
+  if ((uint64_t)pad * R > c->gather_cap) return drop_window(h, lost);
   const uint32_t n_g = pad * (uint32_t)R;
 
   // 2. keys: pad, all-gather, merge. Each rank's list is sorted and, when the caller partitioned by
@@ -444,7 +493,7 @@ static int merge_allreduce(alz_handle* h) {
     CK(cudaStreamSynchronize(s));
     n_can = last[0] + last[1];
   }
-  if (n_can > h->cfg.max_edges) return ALZ_E_CAPACITY;
+  if (n_can > h->cfg.max_edges) return drop_window(h, lost);
 
   // 3. scatter local rows into the zeroed canonical array
   const size_t can_bytes = (size_t)n_can * kCanWords * 8;
@@ -467,13 +516,13 @@ static int merge_allreduce(alz_handle* h) {
 }
 
 // Called by the flush after prepare_flush(): local live edges are sorted in d_keys[1] (keys) / d_rows[1]
-// (rows), h->n_live of them; local_rc is this rank's status so far. Every rank enters the collective whatever
-// its own status, so nobody is left waiting in NCCL, and all ranks return the same failure.
-int alz_internal_merge_ranks(alz_handle* h, int local_rc) {
+// (rows), h->n_live of them; local_rc is this rank's status so far, *lost whether it lost events. Every rank
+// enters the collective whatever its own status, so nobody is left waiting in NCCL, and all ranks return the
+// same status.
+int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost) {
   alz_comm_state* c = h->comm;
-  if (!c || h->comm_nranks <= 1) return ALZ_E_UNSUPPORTED;
   const int R = h->comm_nranks;
-  if (R > 64) return ALZ_E_UNSUPPORTED;
+  if (!c || R <= 1 || R > 64) return ALZ_E_STATE;   // alz_comm_init admits 2..64 ranks here
   cudaStream_t s = h->stream;
   const unsigned grid = (unsigned)h->sms * 4;
   const uint32_t n_local = local_rc == ALZ_OK ? h->n_live : 0u;
@@ -496,6 +545,7 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc) {
   for (int attempt = 0; attempt < 4; ++attempt) {
     memset(c->h_hdr, 0, sizeof(alz_edge_out));
     c->h_hdr->magic = kHdrMagic; c->h_hdr->count = n_local; c->h_hdr->status = local_rc;
+    c->h_hdr->lost = *lost ? 1u : 0u;
     CK(cudaMemcpyAsync(c->d_send, c->h_hdr, sizeof(alz_edge_out), cudaMemcpyHostToDevice, s));
     const size_t block_rows = (size_t)c->cap_r + 1;
     if (block_rows * R > c->recv_rows) {
@@ -509,7 +559,8 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc) {
     // the single exchange step: every rank's header + its first cap_r rows
     NK(g_nccl.AllGather(c->d_send, c->d_recv, block_rows * kRowWords64, ncclUint64, c->comm, s));
     h->collective_bytes_last += (uint64_t)block_rows * R * kRowBytes;
-    merge_blocks_kernel<<<grid, 256, 0, s>>>(c->d_recv, c->cap_r, (uint32_t)R, h->d_out, h->cfg.max_edges, c->d_info);
+    merge_blocks_kernel<<<grid, 256, 0, s>>>(c->d_recv, c->cap_r, (uint32_t)R, (uint32_t)h->comm_rank, h->d_out,
+                                             h->cfg.max_edges, c->d_info);
     consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], n_local);
     h->launches += 2;
     CK(cudaGetLastError());
@@ -517,12 +568,13 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc) {
     CK(cudaStreamSynchronize(s));   // the flush's one synchronisation: the caller needs the edge count
     const MergeInfo inf = *c->h_info;
     if (inf.peer_status != ALZ_OK) return local_rc != ALZ_OK ? local_rc : inf.peer_status;   // the window stays intact
-    if (inf.overflow == 1u) { c->cap_r = block_rows_for(inf.max_count); continue; }   // every rank sees the same headers
-    if (inf.overflow == 2u) return ALZ_E_CAPACITY;                                    // merged graph larger than max_edges
+    if (inf.overflow != 0u) { c->cap_r = block_rows_for(inf.max_count); continue; }   // every rank sees the same headers
     c->cap_r = block_rows_for(inf.max_count);                                         // next window's block size
-    if (inf.dup) return merge_allreduce(h);                                           // not partitioned by owner: general path
-    // success: consume_window_kernel has consumed the window
-    h->last_n_edges = inf.total;
+    *lost = inf.lost != 0u;                                                           // some rank lost events
+    if (inf.dup) return merge_allreduce(h, lost);                                     // not partitioned by owner: general path
+    // success: consume_window_kernel has consumed the window; rows past max_edges were left out
+    if (inf.total > h->cfg.max_edges) { *lost = true; h->merge_lost_events += inf.lost_events; }
+    h->last_n_edges = std::min<uint32_t>(inf.total, h->cfg.max_edges);
     h->windows++;
     return ALZ_OK;
   }

@@ -103,6 +103,7 @@ struct alz_handle {
 
   int comm_nranks = 1, comm_rank = 0;
   alz_comm_state* comm = nullptr;
+  uint64_t merge_lost_events = 0;         // events of this rank's rows that a merge left out (merged graph > max_edges)
   alz_gnn_state* gnn = nullptr;
   alz_sock_state* sock = nullptr;
 };
@@ -110,10 +111,12 @@ struct alz_handle {
 int alz_internal_fold(alz_handle* h);
 // device records -> the ingest kernel of the current mode; caller holds h->mu and has set the device
 int alz_internal_ingest(alz_handle* h, const alz_l7_rec* d_recs, size_t n);
-// multi-GPU merge of the prepared (sorted) live edges; ALZ_E_UNSUPPORTED = single rank,
-// caller finishes the flush locally. local_rc: this rank's own status so far (every rank enters the
-// collectives even when its local preparation failed, and all ranks return the same failure)
-int alz_internal_merge_ranks(alz_handle* h, int local_rc);
+// multi-GPU merge of the prepared (sorted) live edges of a handle with comm_nranks > 1. local_rc: this rank's
+// own status so far (every rank enters the collectives even when its local preparation failed, and all ranks
+// return the same failure). *lost: in, this rank lost events in this window; out, some rank did or the merged
+// graph was cut at max_edges (the same answer on every rank). ALZ_OK: the window is consumed, h->last_n_edges
+// merged rows are in h->d_out; any other status: the window is kept.
+int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

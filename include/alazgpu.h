@@ -340,6 +340,7 @@ int alz_sock_stats(alz_handle* h, alz_sock_stats_t* st);
 /* ---- multi-GPU: one rank per GPU, events pre-partitioned by alz_owner_rank ---- */
 #define ALZ_COMM_ID_BYTES 128
 int alz_comm_unique_id(void* out_id /* ALZ_COMM_ID_BYTES */);
+/* nranks 1..64 (more: ALZ_E_UNSUPPORTED, before any NCCL call); a second init on a handle: ALZ_E_STATE */
 int alz_comm_init(alz_handle* h, int nranks, int rank, const void* id);
 /* rank that owns an event: hash of the source address only, so every event of
  * an edge lands on one rank before any resolve (From is the pod at saddr,
