@@ -217,7 +217,10 @@ int alz_sync(alz_handle* h);
  * each event is resolved by the tables in force when it was submitted. */
 int alz_table_upsert(alz_handle* h, int table, uint32_t ipv4, uint32_t id);
 int alz_table_erase(alz_handle* h, int table, uint32_t ipv4);
-/* n upserts in one call (informer resync / initial list: k8s/informer.go hands the whole cluster at start) */
+/* n upserts in one call (informer resync / initial list: k8s/informer.go hands the whole cluster at start).
+ * Not atomic: the upserts are applied in order and the call stops at the first that fails, returning
+ * ALZ_E_INVAL (ids[i] >= 2^29) or ALZ_E_CAPACITY (a new address with max_endpoints already in the table).
+ * The upserts before it stay staged and take effect at the next alz_table_commit; the rest are not applied. */
 int alz_table_upsert_batch(alz_handle* h, int table, const uint32_t* ipv4, const uint32_t* ids, size_t n);
 int alz_table_commit(alz_handle* h);
 
