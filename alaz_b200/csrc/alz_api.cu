@@ -844,8 +844,9 @@ static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, si
   *n_out = ranks ? 0u : h->n_live;
   CK(cudaEventRecord(h->ev_t[1], h->stream));
   int mrc;
+  bool roll = true;
   if (ranks) {    // one collective over the ranks' edge rows (alz_comm.cu)
-    mrc = alz_internal_merge_ranks(h, rc, &overflow);
+    mrc = alz_internal_merge_ranks(h, rc, &overflow, &roll);
     if (mrc != ALZ_OK && overflow && rc == ALZ_OK) h->lost_reported = ~0ull;   // window kept: report the loss again
   } else {
     if (rc != ALZ_OK) return rc;
@@ -854,7 +855,7 @@ static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, si
   CK(cudaEventRecord(h->ev_t[2], h->stream));
   h->ev_t_valid = true;
   if (mrc != ALZ_OK) return mrc;
-  if ((mrc = window_roll(h)) != ALZ_OK) return mrc;
+  if (roll && (mrc = window_roll(h)) != ALZ_OK) return mrc;
   *n_out = h->last_n_edges;
   if (dev_edges) *dev_edges = h->d_out;
   return overflow ? ALZ_E_CAPACITY : ALZ_OK;

@@ -91,14 +91,34 @@ struct BlockHeader {      // first row of a rank's block
   uint32_t magic, count;
   int32_t status;
   uint32_t lost;          // 1: this rank's pair or edge table lost events in this window
+  uint32_t clk_on, pad;   // 1: the rank has a window clock, copied into clk on the device; 0: clk is all zero
+  WinClock clk;
+};
+// What a merge does to this rank's window (docs/SPEC.md §8 "Several ranks"): E is the smallest open epoch of the
+// ranks, the past state after every epoch. Clockless ranks are always at E.
+enum : uint32_t {
+  kAtE = 0,        // the rank's rows are E's: merged, consumed, and the clock advances
+  kKeep = 1,       // the rank is ahead of E, or no rank has an epoch: nothing sent, nothing changes
+  kOpenNext = 2,   // the rank has no epoch: it opens E + 1 (info->clk is E's clock, advanced by the roll)
 };
 struct MergeInfo {        // written by the merge kernel, read by the host
   uint32_t total, dup, overflow, max_count;
   int32_t peer_status;
-  uint32_t lost;          // some rank's header has lost = 1
-  uint32_t pad[2];
+  uint32_t lost;          // some rank at E has lost = 1
+  uint32_t roll;          // kAtE, kKeep or kOpenNext for this rank
+  uint32_t pad;
   unsigned long long lost_events;   // counts of this rank's rows that fell at or past max_edges in the merged order
+  WinClock clk;           // the clock of the first rank at E
 };
+
+// the order of open epochs across ranks: the past state (ready 2) after every epoch, and all past states equal
+__device__ __forceinline__ bool clk_before(const WinClock& a, const WinClock& b) {
+  const bool pa = a.ready > 1ull, pb = b.ready > 1ull;
+  return pa != pb ? pb : (!pa && a.epoch < b.epoch);
+}
+__device__ __forceinline__ bool clk_same(const WinClock& a, const WinClock& b) {
+  return !clk_before(a, b) && !clk_before(b, a);
+}
 
 // out[i] = keys[i] for i < n, kEmptyKey padding up to n_pad
 __global__ void pad_keys_kernel(const uint64_t* __restrict__ keys, uint32_t n, uint64_t* __restrict__ out,
@@ -213,25 +233,54 @@ __device__ __forceinline__ uint32_t lower_bound_rows(const alz_edge_out* rows, u
 // Merge of the gathered blocks: block q = header row + cap rows, of which header.count are live and sorted.
 // Eight lanes per row: the lanes split the other ranks' binary searches among them, then copy the row. Rows whose
 // place is at or past out_cap are not written; those of rank `me` add their counts to info->lost_events.
+// Under a window clock only the ranks at the merged epoch E take part: another rank counts as 0 rows.
 __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* __restrict__ recv, uint32_t cap, uint32_t R,
                                                            uint32_t me, alz_edge_out* __restrict__ out,
                                                            uint32_t out_cap, MergeInfo* __restrict__ info) {
   __shared__ uint32_t s_cnt[64];
   __shared__ uint32_t s_bad;
+  __shared__ uint32_t s_clk, s_open;
+  __shared__ WinClock s_e;
   const size_t stride_rows = (size_t)cap + 1;
-  if (threadIdx.x == 0) s_bad = 0u;
+  auto header = [&](uint32_t q) { return reinterpret_cast<const BlockHeader*>(recv + q * stride_rows); };
+  if (threadIdx.x == 0) {
+    s_bad = 0u;
+    // the clock must be the same on every rank (length and offset); E = the smallest open epoch
+    const BlockHeader* h0 = header(0);
+    uint32_t open = 0u, mismatch = 0u;
+    WinClock e{};
+    for (uint32_t q = 0; q < R; ++q) {
+      const BlockHeader* hq = header(q);
+      mismatch |= (hq->clk_on != h0->clk_on || hq->clk.len != h0->clk.len || hq->clk.off != h0->clk.off) ? 1u : 0u;
+      if (hq->clk.ready != 0ull && (!open || clk_before(hq->clk, e))) { e = hq->clk; open = 1u; }
+    }
+    s_clk = h0->clk_on;
+    s_open = open;
+    s_e = e;
+    if (mismatch) {
+      s_bad = 1u;
+      if (blockIdx.x == 0) info->peer_status = (int32_t)ALZ_E_STATE;
+    }
+    if (blockIdx.x == 0) {
+      const WinClock& mine = header(me)->clk;
+      info->roll = !s_clk ? kAtE : !open ? kKeep : mine.ready == 0ull ? kOpenNext : clk_same(mine, e) ? kAtE : kKeep;
+      info->clk = e;
+    }
+  }
   __syncthreads();
   if (threadIdx.x < R) {
-    const BlockHeader* hd = reinterpret_cast<const BlockHeader*>(recv + threadIdx.x * stride_rows);
+    const BlockHeader* hd = header(threadIdx.x);
     uint32_t cnt = hd->count;
     if (hd->magic != kHdrMagic || hd->status != ALZ_OK) {
       atomicOr(&s_bad, 1u);
       if (blockIdx.x == 0) info->peer_status = hd->magic != kHdrMagic ? (int32_t)ALZ_E_STATE : hd->status;
       cnt = 0;
     }
-    if (cnt > cap) { atomicOr(&s_bad, 2u); if (blockIdx.x == 0) { info->overflow = 1u; atomicMax(&info->max_count, cnt); } }
-    if (blockIdx.x == 0) atomicMax(&info->max_count, cnt);
-    if (blockIdx.x == 0 && hd->lost != 0u) info->lost = 1u;
+    if (blockIdx.x == 0) atomicMax(&info->max_count, cnt);   // block sizing: every rank's rows, at E or not
+    const bool at_e = !s_clk || (s_open && hd->clk.ready != 0ull && clk_same(hd->clk, s_e));
+    if (!at_e) cnt = 0;
+    if (cnt > cap) { atomicOr(&s_bad, 2u); if (blockIdx.x == 0) info->overflow = 1u; }
+    if (blockIdx.x == 0 && hd->lost != 0u && at_e) info->lost = 1u;   // an ahead rank's loss waits for its window
     s_cnt[threadIdx.x] = cnt;
   }
   __syncthreads();
@@ -278,7 +327,7 @@ __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* _
 // the end, instead of synchronising in the middle of the flush to decide whether to launch this.
 __global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __restrict__ info, AccTable edges,
                                                              const uint32_t* __restrict__ rows, uint32_t n) {
-  if (info->peer_status != ALZ_OK || info->overflow != 0u || info->dup != 0u) return;
+  if (info->peer_status != ALZ_OK || info->overflow != 0u || info->dup != 0u || info->roll != kAtE) return;
   const uint32_t sl = threadIdx.x & 7u;
   const uint32_t groups = (gridDim.x * blockDim.x) >> 3;
   const size_t dict_words = ((size_t)edges.dict_mask + 1u) * (sizeof(DictEnt) / 16u);
@@ -420,17 +469,18 @@ void alz_internal_free_comm(alz_handle* h) {
 
 // The general path's keys do not fit max_edges: this rank's window is consumed without a merge, its events are
 // counted lost and the flush returns no rows. Every rank decides this from the same gathered counts or keys.
-// The local rows are in d_send (gathered before the block exchange).
-static int drop_window(alz_handle* h, bool* lost) {
+// The local rows are in d_send (gathered before the block exchange). A rank that is not at the merged epoch
+// (at_e false) keeps its window.
+static int drop_window(alz_handle* h, bool* lost, bool at_e) {
   alz_comm_state* c = h->comm;
   cudaStream_t s = h->stream;
   const unsigned grid = (unsigned)h->sms * 4;
   CK(cudaMemsetAsync(c->d_info, 0, sizeof(MergeInfo), s));
-  if (h->n_live) {
+  if (at_e && h->n_live) {
     sum_counts_kernel<<<grid, 256, 0, s>>>(c->d_send + 1, h->n_live, c->d_info);
     consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], h->n_live);
     h->launches += 2;
-  } else {
+  } else if (at_e) {
     CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
     CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
   }
@@ -444,15 +494,17 @@ static int drop_window(alz_handle* h, bool* lost) {
   return ALZ_OK;
 }
 
-// General path: keys may live on several ranks. Local live edges are sorted in d_keys[1] / d_rows[1].
-static int merge_allreduce(alz_handle* h, bool* lost) {
+// General path: keys may live on several ranks. Local live edges are sorted in d_keys[1] / d_rows[1]. A rank that
+// is not at the merged epoch (at_e false) contributes no rows and keeps its window.
+static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   alz_comm_state* c = h->comm;
   const int R = h->comm_nranks;
   cudaStream_t s = h->stream;
   const unsigned grid = (unsigned)h->sms * 4;
+  const uint32_t n_local = at_e ? h->n_live : 0u;
 
   // 1. counts
-  CK(cudaMemcpyAsync(c->d_counts + h->comm_rank, &h->n_live, 4, cudaMemcpyHostToDevice, s));
+  CK(cudaMemcpyAsync(c->d_counts + h->comm_rank, &n_local, 4, cudaMemcpyHostToDevice, s));
   NK(g_nccl.AllGather(c->d_counts + h->comm_rank, c->d_counts, 1, ncclUint32, c->comm, s));
   CK(cudaMemcpyAsync(c->h_counts, c->d_counts, 4 * R, cudaMemcpyDeviceToHost, s));
   CK(cudaStreamSynchronize(s));
@@ -462,18 +514,20 @@ static int merge_allreduce(alz_handle* h, bool* lost) {
   if (total == 0) {
     h->last_n_edges = 0;
     h->windows++;
-    CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
-    CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+    if (at_e) {
+      CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
+      CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+    }
     return ALZ_OK;
   }
-  if ((uint64_t)pad * R > c->gather_cap) return drop_window(h, lost);
+  if ((uint64_t)pad * R > c->gather_cap) return drop_window(h, lost, at_e);
   const uint32_t n_g = pad * (uint32_t)R;
 
   // 2. keys: pad, all-gather, merge. Each rank's list is sorted and, when the caller partitioned by
   //    alz_owner_rank, the lists are disjoint: a key's place in the union is then the sum of its lower
   //    bounds in the R lists - no sort. A key found on two ranks (caller routed one source to two ranks)
   //    raises a flag and the general path (sort + unique) runs instead; the sums are right either way.
-  pad_keys_kernel<<<grid, 256, 0, s>>>(h->d_keys[1], h->n_live, c->d_sorted, pad);
+  pad_keys_kernel<<<grid, 256, 0, s>>>(h->d_keys[1], n_local, c->d_sorted, pad);
   NK(g_nccl.AllGather(c->d_sorted, c->d_gather, pad, ncclUint64, c->comm, s));
   CK(cudaMemsetAsync(c->d_flags, 0, 4, s));
   merge_disjoint_kernel<<<grid, 256, 0, s>>>(c->d_gather, pad, (uint32_t)R, c->d_counts, c->d_can_keys, c->d_flags);
@@ -493,13 +547,13 @@ static int merge_allreduce(alz_handle* h, bool* lost) {
     CK(cudaStreamSynchronize(s));
     n_can = last[0] + last[1];
   }
-  if (n_can > h->cfg.max_edges) return drop_window(h, lost);
+  if (n_can > h->cfg.max_edges) return drop_window(h, lost, at_e);
 
   // 3. scatter local rows into the zeroed canonical array
   const size_t can_bytes = (size_t)n_can * kCanWords * 8;
   CK(cudaMemsetAsync(c->d_can, 0, can_bytes, s));
-  if (h->n_live)
-    scatter_canonical_kernel<<<grid * 2, 256, 0, s>>>(h->edges, h->d_keys[1], h->d_rows[1], h->n_live,
+  if (n_local)
+    scatter_canonical_kernel<<<grid * 2, 256, 0, s>>>(h->edges, h->d_keys[1], h->d_rows[1], n_local,
                                                       c->d_can_keys, n_can, c->d_can);
   // 4. the single exchange step
   NK(g_nccl.AllReduce(c->d_can, c->d_can, (size_t)n_can * kCanWords, ncclUint64, ncclSum, c->comm, s));
@@ -508,8 +562,10 @@ static int merge_allreduce(alz_handle* h, bool* lost) {
   // 5. unpack; local edge table back to empty
   unpack_canonical_kernel<<<grid * 2, 256, 0, s>>>(c->d_can_keys, c->d_can, n_can, h->d_out);
   CK(cudaGetLastError());
-  CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
-  CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+  if (at_e) {
+    CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
+    CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+  }
   h->last_n_edges = n_can;
   h->windows++;
   return ALZ_OK;
@@ -518,15 +574,18 @@ static int merge_allreduce(alz_handle* h, bool* lost) {
 // Called by the flush after prepare_flush(): local live edges are sorted in d_keys[1] (keys) / d_rows[1]
 // (rows), h->n_live of them; local_rc is this rank's status so far, *lost whether it lost events. Every rank
 // enters the collective whatever its own status, so nobody is left waiting in NCCL, and all ranks return the
-// same status.
-int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost) {
+// same status. Under a window clock the header carries the rank's clock, and *roll says whether the flush closes
+// this rank's window (see kAtE / kKeep / kOpenNext).
+int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost, bool* roll) {
   alz_comm_state* c = h->comm;
   const int R = h->comm_nranks;
   if (!c || R <= 1 || R > 64) return ALZ_E_STATE;   // alz_comm_init admits 2..64 ranks here
   cudaStream_t s = h->stream;
   const unsigned grid = (unsigned)h->sms * 4;
   const uint32_t n_local = local_rc == ALZ_OK ? h->n_live : 0u;
+  const bool lost_here = *lost;
   h->collective_bytes_last = 0;
+  *roll = true;
 
   if (c->cap_r == 0) {   // first window: nothing to size the blocks from, exchange the counts once
     CK(cudaMemcpyAsync(c->d_counts + h->comm_rank, &n_local, 4, cudaMemcpyHostToDevice, s));
@@ -545,8 +604,12 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost) {
   for (int attempt = 0; attempt < 4; ++attempt) {
     memset(c->h_hdr, 0, sizeof(alz_edge_out));
     c->h_hdr->magic = kHdrMagic; c->h_hdr->count = n_local; c->h_hdr->status = local_rc;
-    c->h_hdr->lost = *lost ? 1u : 0u;
+    c->h_hdr->lost = lost_here ? 1u : 0u;
+    c->h_hdr->clk_on = h->win_on ? 1u : 0u;
     CK(cudaMemcpyAsync(c->d_send, c->h_hdr, sizeof(alz_edge_out), cudaMemcpyHostToDevice, s));
+    if (h->win_on)   // the clock as the device has it: win_init_kernel may have opened it in this window
+      CK(cudaMemcpyAsync(&reinterpret_cast<BlockHeader*>(c->d_send)->clk, h->d_win, sizeof(WinClock),
+                         cudaMemcpyDeviceToDevice, s));
     const size_t block_rows = (size_t)c->cap_r + 1;
     if (block_rows * R > c->recv_rows) {
       CK(cudaStreamSynchronize(s));
@@ -570,8 +633,12 @@ int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost) {
     if (inf.peer_status != ALZ_OK) return local_rc != ALZ_OK ? local_rc : inf.peer_status;   // the window stays intact
     if (inf.overflow != 0u) { c->cap_r = block_rows_for(inf.max_count); continue; }   // every rank sees the same headers
     c->cap_r = block_rows_for(inf.max_count);                                         // next window's block size
-    *lost = inf.lost != 0u;                                                           // some rank lost events
-    if (inf.dup) return merge_allreduce(h, lost);                                     // not partitioned by owner: general path
+    *lost = inf.lost != 0u;                                                           // some rank at E lost events
+    *roll = inf.roll != kKeep;
+    if (inf.roll == kKeep && lost_here) h->lost_reported = ~0ull;   // the window is kept: report its loss with it
+    if (inf.roll == kOpenNext)   // E's clock; the flush's roll advances it to E + 1
+      CK(cudaMemcpyAsync(h->d_win, &c->d_info->clk, sizeof(WinClock), cudaMemcpyDeviceToDevice, s));
+    if (inf.dup) return merge_allreduce(h, lost, inf.roll == kAtE);                   // not partitioned by owner: general path
     // success: consume_window_kernel has consumed the window; rows past max_edges were left out
     if (inf.total > h->cfg.max_edges) { *lost = true; h->merge_lost_events += inf.lost_events; }
     h->last_n_edges = std::min<uint32_t>(inf.total, h->cfg.max_edges);

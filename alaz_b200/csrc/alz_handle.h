@@ -115,8 +115,9 @@ int alz_internal_ingest(alz_handle* h, const alz_l7_rec* d_recs, size_t n);
 // own status so far (every rank enters the collectives even when its local preparation failed, and all ranks
 // return the same failure). *lost: in, this rank lost events in this window; out, some rank did or the merged
 // graph was cut at max_edges (the same answer on every rank). ALZ_OK: the window is consumed, h->last_n_edges
-// merged rows are in h->d_out; any other status: the window is kept.
-int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost);
+// merged rows are in h->d_out; any other status: the window is kept. *roll (with ALZ_OK): the flush closes this
+// rank's time-cut window; false: the rank is ahead of the ranks' merged epoch, or no rank has one, and keeps it.
+int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost, bool* roll);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -481,15 +481,6 @@ __device__ __forceinline__ uint32_t preload_hot(const Shared& s, const HotState*
   return rep_rows;
 }
 
-// time-cut windows (SURVEY §8 row R13, docs/SPEC.md §8): the open window in the records' own (kernel) clock
-struct WinClock {
-  uint64_t lo;        // first kernel-time ns of the open window
-  uint64_t len;       // window length, ns
-  uint64_t ready;     // 0: lo not set yet; 1: set (by win_init_kernel from the first record ever submitted);
-                      // 2: the open epoch starts at or past 2^64 in the user clock, so every record is late
-  uint64_t off;       // first_user_ns - first_kernel_ns (mod 2^64)
-  uint64_t epoch;     // epoch_open
-};
 // SPEC §8 orders epochs by user time, unsigned: a record is late iff its user time lies below the open window's
 // start (lo + off), and in the open window iff wt - lo < len. No division.
 __device__ __forceinline__ bool win_late(uint64_t wt, uint64_t lo, uint64_t off, bool past) {

@@ -4,6 +4,17 @@
 #include "../synth/alz_synth.h"
 
 namespace alz {
+// time-cut windows (SURVEY §8 row R13, docs/SPEC.md §8): the open window in the records' own (kernel) clock.
+// The ingest reads it; a multi-rank merge copies it into the rank's block header (alz_comm.cu).
+struct WinClock {
+  uint64_t lo;        // first kernel-time ns of the open window
+  uint64_t len;       // window length, ns
+  uint64_t ready;     // 0: lo not set yet; 1: set (by win_init_kernel from the first record ever submitted, or by a
+                      // merge that opened it after the ranks' agreed epoch); 2: the open epoch starts at or past 2^64
+                      // in the user clock, so every record is late
+  uint64_t off;       // first_user_ns - first_kernel_ns (mod 2^64)
+  uint64_t epoch;     // epoch_open
+};
 void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
                             const EpEntry* ep, uint32_t ep_mask, int sms, cudaStream_t s);
 void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,

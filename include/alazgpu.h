@@ -271,7 +271,13 @@ int alz_get_stats(alz_handle* h, alz_stats* out);
  * window; a record of an earlier epoch is late: it is reduced into the open window and counted
  * (alz_stats.late_events). Each alz_window_flush* closes the open epoch and opens the next one. Only 32-byte
  * records carry a write time: packed submits return ALZ_E_STATE while the clock is set. window_ns = 0 turns
- * the clock off again. */
+ * the clock off again.
+ * Several ranks (alz_comm_init): every rank must set the same clock, the same window_ns and the same offset
+ * first_user_ns - first_kernel_ns; otherwise the next flush returns ALZ_E_STATE on every rank and every rank
+ * keeps its window. Each rank opens at its own first record; a flush merges epoch E, the smallest open epoch of
+ * the ranks (the past state after every epoch). A rank at E is flushed and advances; a rank ahead of E keeps its
+ * window, its set-aside records and any loss it recorded until E reaches it; a rank with no epoch yet opens E + 1.
+ * After one merge at E the ranks agree and advance together (docs/SPEC.md §8 "Several ranks"). */
 int alz_window_clock(alz_handle* h, uint64_t first_kernel_ns, uint64_t first_user_ns, uint64_t window_ns);
 /* epoch of the open window; ALZ_E_STATE until the first record has been submitted */
 int alz_window_epoch(alz_handle* h, uint64_t* epoch);
@@ -343,7 +349,8 @@ int alz_sock_stats(alz_handle* h, alz_sock_stats_t* st);
 /* ---- multi-GPU: one rank per GPU, events pre-partitioned by alz_owner_rank ---- */
 #define ALZ_COMM_ID_BYTES 128
 int alz_comm_unique_id(void* out_id /* ALZ_COMM_ID_BYTES */);
-/* nranks 1..64 (more: ALZ_E_UNSUPPORTED, before any NCCL call); a second init on a handle: ALZ_E_STATE */
+/* nranks 1..64 (more: ALZ_E_UNSUPPORTED, before any NCCL call); a second init on a handle: ALZ_E_STATE.
+ * Time-cut windows on several ranks need the same alz_window_clock on every rank (see there). */
 int alz_comm_init(alz_handle* h, int nranks, int rank, const void* id);
 /* rank that owns an event: hash of the source address only, so every event of
  * an edge lands on one rank before any resolve (From is the pod at saddr,
