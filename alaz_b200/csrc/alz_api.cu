@@ -26,15 +26,6 @@
 
 using namespace alz;
 
-#define CK(expr)                                                                       \
-  do {                                                                                 \
-    cudaError_t _e = (expr);                                                           \
-    if (_e != cudaSuccess) {                                                           \
-      h->last_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                \
-      return ALZ_E_CUDA;                                                               \
-    }                                                                                  \
-  } while (0)
-
 static uint32_t next_pow2(uint64_t x) {
   uint64_t p = 1;
   while (p < x) p <<= 1;
@@ -53,59 +44,76 @@ static bool is_lib_pinned(const void* p, size_t bytes) {
   return false;
 }
 
-static int alloc_table(alz_handle* h, AccTable* t, uint32_t max_rows, uint32_t* n_rows_dev, bool pair_table) {
+// a dictionary of `cap` free slots
+static int alloc_dict(alz_handle* h, DictEnt** dict, uint32_t cap) {
+  CK(cudaMalloc(dict, (size_t)cap * sizeof(DictEnt)));
+  CK(cudaMemsetAsync(*dict, 0xFF, (size_t)cap * sizeof(DictEnt), h->stream));
+  return ALZ_OK;
+}
+static int alloc_table(alz_handle* h, PairTable* t, uint32_t max_rows, uint32_t* n_rows_dev) {
   memset(t, 0, sizeof(*t));
   t->max_rows = max_rows;
   t->n_rows = n_rows_dev;
   const uint32_t dict_cap = next_pow2(2ull * max_rows);
   t->dict_mask = dict_cap - 1;
+  // reversed rows share the socket pair's slot in `dict`; both dictionaries draw rows from the one pool
+  const uint32_t host_cap = std::max<uint32_t>(1024u, dict_cap >> 3);   // host-keyed outbound pairs: rarer still
+  t->dict_host_mask = host_cap - 1;
+  int rc;
+  if ((rc = alloc_dict(h, &t->dict, dict_cap)) != ALZ_OK || (rc = alloc_dict(h, &t->dict_host, host_cap)) != ALZ_OK) return rc;
   const size_t rows = (size_t)max_rows + kPairKinds;
-  CK(cudaMalloc(&t->dict, (size_t)dict_cap * sizeof(DictEnt)));
   CK(cudaMalloc(&t->row_key, rows * 8));
-  if (!pair_table) {
-    CK(cudaMalloc(&t->lat_sum, rows * 8));
-    CK(cudaMalloc(&t->err5xx, rows * 8));
-    CK(cudaMalloc(&t->count, rows * 8));
-    CK(cudaMalloc(&t->hist, rows * ALZ_NB * 4));
-    CK(cudaMemsetAsync(t->count, 0, rows * 8, h->stream));
-    CK(cudaMemsetAsync(t->lat_sum, 0, rows * 8, h->stream));
-    CK(cudaMemsetAsync(t->err5xx, 0, rows * 8, h->stream));
-    CK(cudaMemsetAsync(t->hist, 0, rows * ALZ_NB * 4, h->stream));
-  } else {
-    CK(cudaMalloc(&t->sect, rows * kSectPerRow * 32));
-    CK(cudaMemsetAsync(t->sect, 0, rows * kSectPerRow * 32, h->stream));
-    // reversed rows share the socket pair's slot in `dict`; both dictionaries draw rows from the one pool
-    const uint32_t host_cap = std::max<uint32_t>(1024u, dict_cap >> 3);   // host-keyed outbound pairs: rarer still
-    t->dict_host_mask = host_cap - 1;
-    CK(cudaMalloc(&t->dict_host, (size_t)host_cap * sizeof(DictEnt)));
-    CK(cudaMemsetAsync(t->dict_host, 0xFF, (size_t)host_cap * sizeof(DictEnt), h->stream));
-    CK(cudaMalloc(&t->row_kind, rows));
-    CK(cudaMemsetAsync(t->row_kind, 0, rows, h->stream));
-    CK(cudaMemsetAsync(t->row_kind + max_rows + kPairRev, (int)kPairRev, 1, h->stream));   // sentinel rows of the free-marker key
-    CK(cudaMemsetAsync(t->row_kind + max_rows + kPairHost, (int)kPairHost, 1, h->stream));
-    CK(cudaMalloc(&t->row_cnt, rows * 4)); CK(cudaMemsetAsync(t->row_cnt, 0, rows * 4, h->stream));
-    CK(cudaMalloc(&t->row_base, rows)); CK(cudaMemsetAsync(t->row_base, 0, rows, h->stream));
-    CK(cudaMalloc(&t->row_aux, rows * 4));
-  }
-  CK(cudaMemsetAsync(t->dict, 0xFF, (size_t)dict_cap * sizeof(DictEnt), h->stream));
+  CK(cudaMalloc(&t->sect, rows * kSectPerRow * 32));
+  CK(cudaMemsetAsync(t->sect, 0, rows * kSectPerRow * 32, h->stream));
+  CK(cudaMalloc(&t->row_kind, rows));
+  CK(cudaMemsetAsync(t->row_kind, 0, rows, h->stream));
+  CK(cudaMemsetAsync(t->row_kind + max_rows + kPairRev, (int)kPairRev, 1, h->stream));   // sentinel rows of the free-marker key
+  CK(cudaMemsetAsync(t->row_kind + max_rows + kPairHost, (int)kPairHost, 1, h->stream));
+  CK(cudaMalloc(&t->row_cnt, rows * 4)); CK(cudaMemsetAsync(t->row_cnt, 0, rows * 4, h->stream));
+  CK(cudaMalloc(&t->row_base, rows)); CK(cudaMemsetAsync(t->row_base, 0, rows, h->stream));
+  CK(cudaMalloc(&t->row_aux, rows * 4));
   return ALZ_OK;
 }
-static void free_table(AccTable* t) {
-  cudaFree(t->dict); cudaFree(t->dict_host); cudaFree(t->row_key); cudaFree(t->row_kind); cudaFree(t->lat_sum);
-  cudaFree(t->err5xx); cudaFree(t->count); cudaFree(t->row_cnt); cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->hist); cudaFree(t->sect);
+static int alloc_table(alz_handle* h, EdgeTable* t, uint32_t max_rows, uint32_t* n_rows_dev) {
+  memset(t, 0, sizeof(*t));
+  t->max_rows = max_rows;
+  t->n_rows = n_rows_dev;
+  const uint32_t dict_cap = next_pow2(2ull * max_rows);
+  t->dict_mask = dict_cap - 1;
+  const int rc = alloc_dict(h, &t->dict, dict_cap);
+  if (rc != ALZ_OK) return rc;
+  const size_t rows = (size_t)max_rows + 1;   // row max_rows: the free-marker key's
+  CK(cudaMalloc(&t->row_key, rows * 8));
+  CK(cudaMalloc(&t->count, rows * 8));
+  CK(cudaMalloc(&t->lat_sum, rows * 8));
+  CK(cudaMalloc(&t->err5xx, rows * 8));
+  CK(cudaMalloc(&t->hist, rows * ALZ_NB * 4));
+  CK(cudaMemsetAsync(t->count, 0, rows * 8, h->stream));
+  CK(cudaMemsetAsync(t->lat_sum, 0, rows * 8, h->stream));
+  CK(cudaMemsetAsync(t->err5xx, 0, rows * 8, h->stream));
+  CK(cudaMemsetAsync(t->hist, 0, rows * ALZ_NB * 4, h->stream));
+  return ALZ_OK;
+}
+static void free_table(PairTable* t) {
+  cudaFree(t->dict); cudaFree(t->dict_host); cudaFree(t->row_key); cudaFree(t->row_kind); cudaFree(t->row_cnt);
+  cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->sect);
   memset(t, 0, sizeof(*t));
 }
-// all keys out of the dictionaries; the rows keep their indices until clear_dict resets the allocator
-static int clear_keys(alz_handle* h, AccTable* t) {
-  CK(cudaMemsetAsync(t->dict, 0xFF, ((size_t)t->dict_mask + 1) * sizeof(DictEnt), h->stream));
-  if (t->dict_host) CK(cudaMemsetAsync(t->dict_host, 0xFF, ((size_t)t->dict_host_mask + 1) * sizeof(DictEnt), h->stream));
+static void free_table(EdgeTable* t) {
+  cudaFree(t->dict); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->lat_sum); cudaFree(t->err5xx); cudaFree(t->hist);
+  memset(t, 0, sizeof(*t));
+}
+// all keys out of the pair dictionaries; the rows keep their indices until clear_dict resets the allocator
+static int clear_keys(alz_handle* h, const PairTable& t) {
+  CK(cudaMemsetAsync(t.dict, 0xFF, ((size_t)t.dict_mask + 1) * sizeof(DictEnt), h->stream));
+  CK(cudaMemsetAsync(t.dict_host, 0xFF, ((size_t)t.dict_host_mask + 1) * sizeof(DictEnt), h->stream));
   return ALZ_OK;
 }
-// all keys out of the dictionaries, row allocator back to zero (rows were zeroed by fold / emit)
-static int clear_dict(alz_handle* h, AccTable* t) {
+// all keys out of the pair dictionaries, row allocator back to zero (rows were zeroed by fold / emit)
+static int clear_dict(alz_handle* h, const PairTable& t) {
   int rc = clear_keys(h, t);
   if (rc != ALZ_OK) return rc;
-  CK(cudaMemsetAsync(t->n_rows, 0, 4, h->stream));
+  CK(cudaMemsetAsync(t.n_rows, 0, 4, h->stream));
   return ALZ_OK;
 }
 
@@ -183,9 +191,9 @@ extern "C" int alz_create(const alz_config* cfg, alz_handle** out) {
   CKC(cudaMemsetAsync(h->d_hot, 0, sizeof(HotState), h->stream));
   int rc;
   if (!(h->cfg.flags & ALZ_CFG_EAGER_JOIN)) {
-    if ((rc = alloc_table(h, &h->pairs, h->cfg.max_pairs, &h->d_ctr->pair_rows, true)) != ALZ_OK) return fail(rc);
+    if ((rc = alloc_table(h, &h->pairs, h->cfg.max_pairs, &h->d_ctr->pair_rows)) != ALZ_OK) return fail(rc);
   }
-  if ((rc = alloc_table(h, &h->edges, h->cfg.max_edges, &h->d_ctr->edge_rows, false)) != ALZ_OK) return fail(rc);
+  if ((rc = alloc_table(h, &h->edges, h->cfg.max_edges, &h->d_ctr->edge_rows)) != ALZ_OK) return fail(rc);
   CKC(cudaMallocHost(&h->h_ctr, sizeof(Counters)));
   memset(h->h_ctr, 0, sizeof(Counters));
   for (int b = 0; b < 2; ++b) {
@@ -507,7 +515,7 @@ extern "C" int alz_table_commit(alz_handle* h) {
 // It also leaves per-pair counts behind, from which the next ingest launches learn which pairs are hot
 // (alz_ingest.cu). Split in two so that a flush can read the edge count between the halves.
 static int fold_first_half(alz_handle* h) {
-  launch_fold_resolve(h->pairs, h->d_ep, h->ep_cap - 1, h->edges, h->d_ctr, h->d_hot, h->sms, h->stream);
+  launch_fold_resolve(h->pairs, h->d_ep, h->ep_cap - 1, h->edges, h->d_hot, h->sms, h->stream);
   h->launches += 1;
   CK(cudaGetLastError());
   return ALZ_OK;
@@ -517,7 +525,7 @@ static int fold_second_half(alz_handle* h) {
   launch_hot_select(h->pairs, h->d_hot, h->sms, h->stream);
   h->launches += 2;
   CK(cudaGetLastError());
-  int rc = clear_dict(h, &h->pairs);
+  int rc = clear_dict(h, h->pairs);
   h->pending_since_fold = 0;
   h->edges_dirty = true;
   return rc;
@@ -751,7 +759,7 @@ static int prepare_flush(alz_handle* h, bool* overflow) {
     launch_bucket_count(h->pairs, h->cfg.max_edges, h->bk, h->sms, h->stream);
     h->launches += 1;
     CK(cudaGetLastError());
-    if ((rc = clear_keys(h, &h->pairs)) != ALZ_OK) return rc;
+    if ((rc = clear_keys(h, h->pairs)) != ALZ_OK) return rc;
     h->bucketed = true;
   } else if (fold && (rc = fold_second_half(h)) != ALZ_OK) {
     return rc;
@@ -798,8 +806,7 @@ static int finish_flush(alz_handle* h) {
     h->bucketed = false;
     h->pending_since_fold = 0;
   }
-  int rc = clear_dict(h, &h->edges);
-  if (rc != ALZ_OK) return rc;
+  CK(edge_table_clear(h->edges, h->stream));
   h->edges_dirty = false;
   h->last_n_edges = h->n_live;
   h->windows++;

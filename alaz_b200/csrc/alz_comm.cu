@@ -128,27 +128,6 @@ __global__ void pad_keys_kernel(const uint64_t* __restrict__ keys, uint32_t n, u
     out[i] = i < n ? keys[i] : kEmptyKey;
 }
 
-// unique of the sorted gathered keys: flag run heads, exclusive-scan the flags, scatter the heads
-__global__ void flag_heads_kernel(const uint64_t* __restrict__ sorted, uint32_t n, uint32_t* __restrict__ flags) {
-  const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const uint64_t k = sorted[i];
-    flags[i] = (k != kEmptyKey && (i == 0 || sorted[i - 1] != k)) ? 1u : 0u;
-  }
-}
-__global__ void scatter_heads_kernel(const uint64_t* __restrict__ sorted, const uint32_t* __restrict__ flags,
-                                     const uint32_t* __restrict__ pos, uint32_t n, uint64_t* __restrict__ out) {
-  const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    if (flags[i]) out[pos[i]] = sorted[i];
-}
-
-__device__ __forceinline__ uint32_t lower_bound_u64(const uint64_t* __restrict__ a, uint32_t n, uint64_t k) {
-  uint32_t lo = 0, hi = n;
-  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < k) lo = mid + 1; else hi = mid; }
-  return lo;
-}
-
 // union of R sorted, pairwise disjoint key lists (segment r = gathered[r * pad .. + counts[r])):
 // out[sum of lower bounds] = key. *dup is set if a key occurs in two lists.
 __global__ void __launch_bounds__(256) merge_disjoint_kernel(const uint64_t* __restrict__ gathered, uint32_t pad,
@@ -171,25 +150,22 @@ __global__ void __launch_bounds__(256) merge_disjoint_kernel(const uint64_t* __r
   }
 }
 
-// local live rows -> canonical array (zeroed beforehand); a warp per local edge; rows are zeroed
-__global__ void __launch_bounds__(256) scatter_canonical_kernel(AccTable edges, const uint64_t* __restrict__ keys,
+// local live rows -> canonical array (zeroed beforehand); eight lanes per local edge; rows are zeroed
+__global__ void __launch_bounds__(256) scatter_canonical_kernel(EdgeTable edges, const uint64_t* __restrict__ keys,
                                                                 const uint32_t* __restrict__ rows, uint32_t n_local,
                                                                 const uint64_t* __restrict__ can_keys, uint32_t n_can,
                                                                 uint64_t* __restrict__ can) {
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t warps_per_grid = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n_local; i += warps_per_grid) {
+  const uint32_t sl = threadIdx.x & 7u;
+  const uint32_t groups = (gridDim.x * blockDim.x) >> 3;
+  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_local; i += groups) {
     const uint32_t row = rows[i];
-    const uint32_t pos = lower_bound_u64(can_keys, n_can, keys[i]);   // always present
-    uint64_t* dst = can + (size_t)pos * kCanWords;
-    dst[3 + lane] = edges.hist[(size_t)row * ALZ_NB + lane];
-    dst[3 + 32 + lane] = edges.hist[(size_t)row * ALZ_NB + 32 + lane];
-    edges.hist[(size_t)row * ALZ_NB + lane] = 0u;
-    edges.hist[(size_t)row * ALZ_NB + 32 + lane] = 0u;
-    if (lane == 0) {
-      dst[0] = edges.count[row]; dst[1] = edges.err5xx[row]; dst[2] = edges.lat_sum[row];
-      edges.count[row] = 0ull; edges.err5xx[row] = 0ull; edges.lat_sum[row] = 0ull;
-    }
+    uint32_t c[8];
+    uint64_t count, lat, e5;
+    edge_row_load(edges, row, sl, c, count, lat, e5);
+    edge_row_zero(edges, row, sl);
+    uint64_t* dst = can + (size_t)lower_bound_u64(can_keys, n_can, keys[i]) * kCanWords;   // always present
+    for (int k = 0; k < 8; ++k) dst[3 + sl * 8u + k] = c[k];
+    if (sl == 0) { dst[0] = count; dst[1] = e5; dst[2] = lat; }
   }
 }
 
@@ -325,7 +301,7 @@ __global__ void __launch_bounds__(256) merge_blocks_kernel(const alz_edge_out* _
 // a successful merge consumes the window: zero the local edge rows that were sent, empty the edge dictionary, reset
 // the row allocator. Decided on the device from the merge kernel's verdict, so the host reads that verdict once, at
 // the end, instead of synchronising in the middle of the flush to decide whether to launch this.
-__global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __restrict__ info, AccTable edges,
+__global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __restrict__ info, EdgeTable edges,
                                                              const uint32_t* __restrict__ rows, uint32_t n) {
   if (info->peer_status != ALZ_OK || info->overflow != 0u || info->dup != 0u || info->roll != kAtE) return;
   const uint32_t sl = threadIdx.x & 7u;
@@ -335,13 +311,7 @@ __global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dict_words; i += (size_t)gridDim.x * blockDim.x)
     dict[i] = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
   if (blockIdx.x == 0 && threadIdx.x == 0) *edges.n_rows = 0u;
-  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n; i += groups) {
-    const uint32_t row = rows[i];
-    uint4* cells = reinterpret_cast<uint4*>(edges.hist + (size_t)row * ALZ_NB + sl * 8u);
-    cells[0] = make_uint4(0u, 0u, 0u, 0u);
-    cells[1] = make_uint4(0u, 0u, 0u, 0u);
-    if (sl == 0) { edges.count[row] = 0ull; edges.err5xx[row] = 0ull; edges.lat_sum[row] = 0ull; }
-  }
+  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n; i += groups) edge_row_zero(edges, rows[i], sl);
 }
 
 // info->lost_events += the counts of n rows (the general path's dropped window)
@@ -380,14 +350,6 @@ struct alz_comm_state {
   MergeInfo* h_info = nullptr;    // pinned
 };
 
-#define CK(expr)                                                                       \
-  do {                                                                                 \
-    cudaError_t _e = (expr);                                                           \
-    if (_e != cudaSuccess) {                                                           \
-      h->last_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                \
-      return ALZ_E_CUDA;                                                               \
-    }                                                                                  \
-  } while (0)
 #define NK(expr)                                                                       \
   do {                                                                                 \
     ncclResult_t _r = (expr);                                                          \
@@ -481,8 +443,7 @@ static int drop_window(alz_handle* h, bool* lost, bool at_e) {
     consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], h->n_live);
     h->launches += 2;
   } else if (at_e) {
-    CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
-    CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
+    CK(edge_table_clear(h->edges, s));
   }
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(c->h_info, c->d_info, sizeof(MergeInfo), cudaMemcpyDeviceToHost, s));
@@ -514,10 +475,7 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   if (total == 0) {
     h->last_n_edges = 0;
     h->windows++;
-    if (at_e) {
-      CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
-      CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
-    }
+    if (at_e) CK(edge_table_clear(h->edges, s));
     return ALZ_OK;
   }
   if ((uint64_t)pad * R > c->gather_cap) return drop_window(h, lost, at_e);
@@ -538,9 +496,7 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   if (dup) {
     launch_iota(c->d_iota, n_g, h->sms, s);
     sort_pairs(c->d_tmp, c->tmp_bytes, c->d_gather, c->d_sorted, c->d_iota, c->d_vals, n_g, s);
-    flag_heads_kernel<<<grid, 256, 0, s>>>(c->d_sorted, n_g, c->d_flags);
-    exclusive_scan_u32(c->d_tmp, c->tmp_bytes, c->d_flags, c->d_pos, n_g, s);
-    scatter_heads_kernel<<<grid, 256, 0, s>>>(c->d_sorted, c->d_flags, c->d_pos, n_g, c->d_can_keys);
+    launch_unique_sorted(c->d_sorted, n_g, c->d_flags, c->d_pos, c->d_can_keys, c->d_tmp, c->tmp_bytes, h->sms, s);
     uint32_t last[2];
     CK(cudaMemcpyAsync(&last[0], c->d_pos + (n_g - 1), 4, cudaMemcpyDeviceToHost, s));
     CK(cudaMemcpyAsync(&last[1], c->d_flags + (n_g - 1), 4, cudaMemcpyDeviceToHost, s));
@@ -562,10 +518,7 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   // 5. unpack; local edge table back to empty
   unpack_canonical_kernel<<<grid * 2, 256, 0, s>>>(c->d_can_keys, c->d_can, n_can, h->d_out);
   CK(cudaGetLastError());
-  if (at_e) {
-    CK(cudaMemsetAsync(h->edges.dict, 0xFF, ((size_t)h->edges.dict_mask + 1) * sizeof(DictEnt), s));
-    CK(cudaMemsetAsync(h->edges.n_rows, 0, 4, s));
-  }
+  if (at_e) CK(edge_table_clear(h->edges, s));
   h->last_n_edges = n_can;
   h->windows++;
   return ALZ_OK;

@@ -134,13 +134,14 @@ constexpr uint32_t kClaimRow = 0xFFFFFFFCu; // pair table: a thread is allocatin
 
 constexpr uint32_t kPairFwd = 0u, kPairRev = 1u, kPairHost = 2u, kPairKinds = 3u;
 
-struct AccTable {
-  DictEnt* dict;      // [dict_mask + 1]; pair table: socket pairs, forward and reversed rows in one slot
+// The pair table: socket pairs -> rows of the sectored layout below. One dictionary slot serves both directions of
+// a pair (kPairFwd, kPairRev); the host-keyed outbound events (kind kPairHost: the key's high word is a Host-header
+// id, not a daddr; ALZ_PROTO_F_HOSTKEY) have a dictionary of their own, a key space of its own. Both dictionaries
+// hand out rows of the same pool; row_kind[row] says which kind a row is.
+struct PairTable {
+  DictEnt* dict;      // [dict_mask + 1] socket pairs, forward and reversed rows in one slot
   uint32_t dict_mask;
-  // pair table only: the dictionary of host-keyed outbound events (kind 2: the key's high word is a Host-header id,
-  // not a daddr; ALZ_PROTO_F_HOSTKEY), a key space of its own. Both dictionaries hand out rows of the same pool;
-  // row_kind[row] says which kind a row is.
-  DictEnt* dict_host;
+  DictEnt* dict_host; // [dict_host_mask + 1] host-keyed outbound pairs
   uint32_t dict_host_mask;
   __device__ __forceinline__ DictEnt* dict_of(uint32_t kind) const { return kind == kPairHost ? dict_host : dict; }
   __device__ __forceinline__ uint32_t mask_of(uint32_t kind) const { return kind == kPairHost ? dict_host_mask : dict_mask; }
@@ -148,16 +149,12 @@ struct AccTable {
                       // equals the free marker (one per kind); every per-row array has max_rows + kPairKinds entries
   uint32_t* n_rows;   // device counter of allocated rows
   uint64_t* row_key;  // [max_rows + 3]
-  uint8_t* row_kind;  // [max_rows + 3] (pair table only) kPairFwd / kPairRev / kPairHost
-  uint64_t* lat_sum;  // [max_rows + 3]
-  uint64_t* err5xx;   // [max_rows + 3]
-  uint64_t* count;    // [max_rows + 3] (edge table only; the pair table derives it from hist)
-  uint32_t* row_cnt;  // [max_rows + 3] (pair table only) events of the row at the last fold, saturated
-  uint8_t* row_base;  // [max_rows + 3] (pair table only) first bucket / 4 of the 16-bucket window that held most of
-                      // the row's events at the last fold (the per-CTA table keeps only such a window per pair)
-  uint32_t* row_aux;  // [max_rows + 3] (pair table only) edge row found by fold_resolve_kernel
-  uint32_t* hist;     // [(max_rows + 3) * ALZ_NB] (edge table only)
-  // Pair table rows are kept in 32-byte SECTORS, 16 per row (512 B): sector g = { cells 4g, 4g+1 | cells 4g+2, 4g+3 |
+  uint8_t* row_kind;  // [max_rows + 3] kPairFwd / kPairRev / kPairHost
+  uint32_t* row_cnt;  // [max_rows + 3] events of the row at the last fold, saturated
+  uint8_t* row_base;  // [max_rows + 3] first bucket / 4 of the 16-bucket window that held most of the row's events at
+                      // the last fold (the per-CTA table keeps only such a window per pair)
+  uint32_t* row_aux;  // [max_rows + 3] edge row found by fold_resolve_kernel
+  // Rows are kept in 32-byte SECTORS, 16 per row (512 B): sector g = { cells 4g, 4g+1 | cells 4g+2, 4g+3 |
   // latency partial u64 | 5xx partial u64 }. A global reduction costs the SM one LSU pass per distinct sector an
   // instruction touches, not per lane (scripts/micro/red_merge.cu: a histogram increment and a latency add as
   // two instructions = 93 G events/s chip-wide whether or not they share a sector; as ONE red.u64 instruction with two
@@ -165,18 +162,61 @@ struct AccTable {
   // in one sector and are added by a lane pair of one instruction; a row's latency / 5xx totals are the sums of its 16
   // partials (take_pair_row, alz_kernels.cu). A cell pair is added to as a u64: cells are u32 and a fold runs before any cell
   // could reach 2^31 (alz_api.cu), so nothing carries from the low cell into the high one.
-  uint64_t* sect;     // [(max_rows + 3) * kSectPerRow * 4] (pair table only; hist / lat_sum / err5xx are null there)
+  uint64_t* sect;     // [(max_rows + 3) * kSectPerRow * 4]
 };
 constexpr uint32_t kSectPerRow = 16;
-__device__ __forceinline__ uint64_t* pair_sect(const AccTable& t, uint32_t row, uint32_t bucket) {
+__device__ __forceinline__ uint64_t* pair_sect(const PairTable& t, uint32_t row, uint32_t bucket) {
   return t.sect + ((size_t)row * kSectPerRow + (bucket >> 2)) * 4u;
 }
-__device__ __forceinline__ uint32_t* pair_cell(const AccTable& t, uint32_t row, uint32_t bucket) {
+__device__ __forceinline__ uint32_t* pair_cell(const PairTable& t, uint32_t row, uint32_t bucket) {
   return reinterpret_cast<uint32_t*>(pair_sect(t, row, bucket)) + (bucket & 3u);
 }
 
+// The edge table: packed edge keys -> dense rows of a window's sums (docs/SPEC.md §3), one dictionary (row[0] only).
+struct EdgeTable {
+  DictEnt* dict;      // [dict_mask + 1]
+  uint32_t dict_mask;
+  uint32_t max_rows;  // rows [0, max_rows) are allocatable; row max_rows is the sentinel row of the key that equals
+                      // the free marker, which no flush emits; every per-row array has max_rows + 1 entries
+  uint32_t* n_rows;   // device counter of allocated rows
+  uint64_t* row_key;  // [max_rows + 1]
+  uint64_t* count;    // [max_rows + 1]
+  uint64_t* lat_sum;  // [max_rows + 1]
+  uint64_t* err5xx;   // [max_rows + 1]
+  uint32_t* hist;     // [(max_rows + 1) * ALZ_NB]
+};
+
+// one event into an edge row
+__device__ __forceinline__ void edge_add(const EdgeTable& t, uint32_t row, uint32_t bucket, uint64_t dur, bool err) {
+  atomicAdd(&t.hist[(size_t)row * ALZ_NB + bucket], 1u);
+  atomicAdd((unsigned long long*)&t.lat_sum[row], (unsigned long long)dur);
+  if (err) atomicAdd((unsigned long long*)&t.err5xx[row], 1ull);
+  atomicAdd((unsigned long long*)&t.count[row], 1ull);
+}
+// An edge row taken by an 8-lane group: lane sl (0..7) holds histogram cells 8sl..8sl+7 (two 16-byte accesses),
+// lane 0 also the row's count, latency and 5xx sums (0 in the other lanes).
+__device__ __forceinline__ void edge_row_load(const EdgeTable& t, uint32_t row, uint32_t sl, uint32_t (&c)[8],
+                                              uint64_t& count, uint64_t& lat, uint64_t& e5) {
+  const uint4* cells = reinterpret_cast<const uint4*>(t.hist + (size_t)row * ALZ_NB + sl * 8u);
+  const uint4 a = cells[0], b = cells[1];
+  c[0] = a.x; c[1] = a.y; c[2] = a.z; c[3] = a.w; c[4] = b.x; c[5] = b.y; c[6] = b.z; c[7] = b.w;
+  count = 0; lat = 0; e5 = 0;
+  if (sl == 0) { count = t.count[row]; lat = t.lat_sum[row]; e5 = t.err5xx[row]; }
+}
+__device__ __forceinline__ void edge_row_zero(const EdgeTable& t, uint32_t row, uint32_t sl) {
+  uint4* cells = reinterpret_cast<uint4*>(t.hist + (size_t)row * ALZ_NB + sl * 8u);
+  cells[0] = make_uint4(0u, 0u, 0u, 0u);
+  cells[1] = make_uint4(0u, 0u, 0u, 0u);
+  if (sl == 0) { t.count[row] = 0ull; t.lat_sum[row] = 0ull; t.err5xx[row] = 0ull; }
+}
+// all keys out of the dictionary and the row allocator back to zero, in stream order (whoever took the rows zeroed them)
+inline cudaError_t edge_table_clear(const EdgeTable& t, cudaStream_t s) {
+  const cudaError_t e = cudaMemsetAsync(t.dict, 0xFF, ((size_t)t.dict_mask + 1) * sizeof(DictEnt), s);
+  return e != cudaSuccess ? e : cudaMemsetAsync(t.n_rows, 0, 4, s);
+}
+
 // row of `key`, inserting it if absent; >= kLostRow when capacity is exhausted
-__device__ __forceinline__ uint32_t find_or_insert(const AccTable& t, uint64_t key) {
+__device__ __forceinline__ uint32_t find_or_insert(const EdgeTable& t, uint64_t key) {
   if (key == kEmptyKey) return t.max_rows;  // the one key that collides with the free marker
   uint32_t slot = (uint32_t)hash64(key) & t.dict_mask;
 #pragma unroll 1
@@ -225,7 +265,7 @@ __device__ __forceinline__ uint32_t ep_lookup(const EpEntry* __restrict__ tab, u
 // A forward and a reversed event of one socket pair share the slot; each kind's row is allocated the first time an
 // event of that kind comes, by the thread whose CAS takes that row word from kNoRow to kClaimRow.
 constexpr uint32_t kDropRow = 0xFFFFFFFDu;
-__device__ __forceinline__ uint32_t find_or_insert_pair(const AccTable& t, uint64_t key, uint32_t kind,
+__device__ __forceinline__ uint32_t find_or_insert_pair(const PairTable& t, uint64_t key, uint32_t kind,
                                                         const EpEntry* __restrict__ ep, uint32_t ep_mask) {
   // the one key that collides with the free marker has a fixed row per kind
   if (key == kEmptyKey) return t.max_rows + kind;
@@ -277,30 +317,32 @@ __device__ __forceinline__ uint32_t find_or_insert_pair(const AccTable& t, uint6
   return kLostRow;
 }
 
-// setFromToV2 on integers: false = "error finding pod with sockets saddr" (drop)
-__device__ __forceinline__ bool resolve_edge(const EpEntry* __restrict__ tab, uint32_t mask, uint32_t saddr,
-                                             uint32_t daddr, bool rev, uint64_t* edge_key) {
+// setFromToV2 on integers for a socket pair of kind kPairFwd / kPairRev / kPairHost: false = "error finding pod with
+// sockets saddr" (drop). A host-keyed pair (ALZ_PROTO_F_HOSTKEY) has its Host-header id where daddr would be: the
+// caller has already established that the destination is neither service nor pod, and HTTP rows are never
+// reversed; only the drop rule is left (data.go:851-854).
+__device__ __forceinline__ bool resolve_pair(const EpEntry* __restrict__ tab, uint32_t mask, uint64_t key, uint32_t kind,
+                                             uint64_t* edge_key) {
   uint32_t pod, svc;
-  const uint32_t s = ep_lookup(tab, mask, saddr, &pod, &svc);
+  const uint32_t s = ep_lookup(tab, mask, pair_saddr(key), &pod, &svc);
   if ((s & kEpPod) == 0u) return false;                 // data.go:829-832
   const uint32_t from_pod = pod;
-  const uint32_t d = ep_lookup(tab, mask, daddr, &pod, &svc);
-  uint32_t ot, ov;
-  if (d & kEpSvc) { ot = ALZ_NODE_SVC; ov = svc; }       // :840-843 service first
-  else if (d & kEpPod) { ot = ALZ_NODE_POD; ov = pod; }  // :845-849
-  else { ot = ALZ_NODE_OUTBOUND; ov = daddr; }           // :862 raw daddr
-  *edge_key = make_edge_key(from_pod, ot, ov, rev);
+  uint32_t ot = ALZ_NODE_OUTBOUND_HOST, ov = pair_daddr(key);
+  if (kind != kPairHost) {
+    const uint32_t d = ep_lookup(tab, mask, ov, &pod, &svc);
+    if (d & kEpSvc) { ot = ALZ_NODE_SVC; ov = svc; }       // :840-843 service first
+    else if (d & kEpPod) { ot = ALZ_NODE_POD; ov = pod; }  // :845-849
+    else ot = ALZ_NODE_OUTBOUND;                           // :862 raw daddr
+  }
+  *edge_key = make_edge_key(from_pod, ot, ov, kind == kPairRev);
   return true;
 }
 
-// host-keyed outbound pair (ALZ_PROTO_F_HOSTKEY): the caller has already established that the destination is
-// neither service nor pod, and HTTP rows are never reversed; only the drop rule is left (data.go:829-832, :851-854)
-__device__ __forceinline__ bool resolve_edge_hostkey(const EpEntry* __restrict__ tab, uint32_t mask, uint32_t saddr,
-                                                     uint32_t host_id, uint64_t* edge_key) {
-  uint32_t pod, svc;
-  if ((ep_lookup(tab, mask, saddr, &pod, &svc) & kEpPod) == 0u) return false;
-  *edge_key = make_edge_key(pod, ALZ_NODE_OUTBOUND_HOST, host_id, false);
-  return true;
+// first index of a sorted array whose element is not below k
+__device__ __forceinline__ uint32_t lower_bound_u64(const uint64_t* __restrict__ a, uint32_t n, uint64_t k) {
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < k) lo = mid + 1; else hi = mid; }
+  return lo;
 }
 
 // 32-byte record, two 128-bit loads (the widest global load on sm_90a), streaming: bypass L1
@@ -330,7 +372,7 @@ struct HotState {
   uint32_t thr_a, thr_b;       // lowest bin of tier A (hottest, listed first) / of tier B
   uint32_t n_a, n_b;           // tier A occupies keys[0, n_a), tier B keys[kHotA, kHotA + n_b)
   uint64_t keys[kHotMax];
-  uint8_t base[kHotMax];       // the pair's histogram window (first bucket / 4), see AccTable::row_base
+  uint8_t base[kHotMax];       // the pair's histogram window (first bucket / 4), see PairTable::row_base
   // tier S: the (at most) kHotS hottest pairs of all. The per-CTA table gives each of them kHotRep rows and a lane
   // uses row (lane % kHotRep) of the group: when one pair is most of a GPU's traffic — the rank that owns the
   // hottest pair of a sharded stream sees it in every second event — its reductions would otherwise pile up on

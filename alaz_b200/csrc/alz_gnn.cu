@@ -21,6 +21,7 @@
 #include <vector>
 
 #include "alz_handle.h"
+#include "alz_mbar.cuh"
 
 using namespace alz;
 
@@ -74,22 +75,6 @@ __global__ void edge_node_keys_kernel(const alz_edge_out* __restrict__ e, uint32
     out[2 * i] = node_key(e[i].from_type, e[i].from);
     out[2 * i + 1] = node_key(e[i].to_type, e[i].to);
   }
-}
-__global__ void flag_heads_kernel(const uint64_t* __restrict__ sorted, uint32_t n, uint32_t* __restrict__ flags) {
-  const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    flags[i] = (i == 0 || sorted[i - 1] != sorted[i]) ? 1u : 0u;
-}
-__global__ void scatter_heads_kernel(const uint64_t* __restrict__ sorted, const uint32_t* __restrict__ flags,
-                                     const uint32_t* __restrict__ pos, uint32_t n, uint64_t* __restrict__ out) {
-  const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
-    if (flags[i]) out[pos[i]] = sorted[i];
-}
-__device__ __forceinline__ uint32_t lower_bound_u64(const uint64_t* __restrict__ a, uint32_t n, uint64_t k) {
-  uint32_t lo = 0, hi = n;
-  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < k) lo = mid + 1; else hi = mid; }
-  return lo;
 }
 
 // per node: [out_count, in_count, out_err, in_err, out_lat, in_lat, out_deg, in_deg]
@@ -228,7 +213,6 @@ __device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo, 
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(sbo >> 4) << 32);
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ uint32_t to_tf32(float x) {
   uint32_t u;
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
@@ -259,19 +243,6 @@ __device__ __forceinline__ void wgmma_tf32(float* d, uint64_t da, uint64_t db) {
 constexpr uint32_t RING_ROWS = 8, RING_BYTES = RING_ROWS * 256;
 constexpr uint32_t SMEM_TC = 2 * A_BYTES + 2 * B_BYTES + 8 * 2 * RING_BYTES + 256;
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  } while (!ok);
-}
 __device__ __forceinline__ void tma_row(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
@@ -518,15 +489,6 @@ struct alz_gnn_state {
   uint32_t* d_nv = nullptr;      // node count of the last pass, on the device
 };
 
-#define CK(expr)                                                                       \
-  do {                                                                                 \
-    cudaError_t _e = (expr);                                                           \
-    if (_e != cudaSuccess) {                                                           \
-      h->last_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                \
-      return ALZ_E_CUDA;                                                               \
-    }                                                                                  \
-  } while (0)
-
 static int gnn_init_impl(alz_handle* h) {
   alz_gnn_state* g = new alz_gnn_state();
   h->gnn = g;
@@ -630,9 +592,7 @@ static int gnn_run(alz_handle* h) {
   edge_node_keys_kernel<<<grid, 256, 0, s>>>(h->d_out, n_e, g->d_nk);
   launch_iota(g->d_iota, n2, h->sms, s);
   sort_pairs(g->d_tmp, g->tmp_bytes, g->d_nk, g->d_nk_sorted, g->d_iota, g->d_vals, n2, s, 34);
-  flag_heads_kernel<<<grid, 256, 0, s>>>(g->d_nk_sorted, n2, g->d_flags);
-  exclusive_scan_u32(g->d_tmp, g->tmp_bytes, g->d_flags, g->d_pos, n2, s);
-  scatter_heads_kernel<<<grid, 256, 0, s>>>(g->d_nk_sorted, g->d_flags, g->d_pos, n2, g->d_nodes);
+  launch_unique_sorted(g->d_nk_sorted, n2, g->d_flags, g->d_pos, g->d_nodes, g->d_tmp, g->tmp_bytes, h->sms, s);
   node_count_kernel<<<1, 32, 0, s>>>(g->d_pos, g->d_flags, n2, g->d_nv);
   // stats + CSR by destination (destination index < n2)
   CK(cudaMemsetAsync(g->d_stats, 0, (size_t)n2 * 64, s));

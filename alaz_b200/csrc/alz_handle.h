@@ -16,6 +16,16 @@ struct HostEp {
   uint32_t pod = 0, svc = 0;
 };
 
+// return ALZ_E_CUDA from a function of the handle `h` when a CUDA call fails, the call and its error in h->last_err
+#define CK(expr)                                                                       \
+  do {                                                                                 \
+    cudaError_t _e = (expr);                                                           \
+    if (_e != cudaSuccess) {                                                           \
+      h->last_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                \
+      return ALZ_E_CUDA;                                                               \
+    }                                                                                  \
+  } while (0)
+
 struct alz_gnn_state;   // alz_gnn.cu
 struct alz_sock_state;  // alz_sock.cu
 struct alz_comm_state;  // alz_comm.cu
@@ -68,7 +78,8 @@ struct alz_handle {
   cudaEvent_t ev_patch = nullptr;
 
   // accumulators
-  alz::AccTable pairs{}, edges{};
+  alz::PairTable pairs{};                 // not with ALZ_CFG_EAGER_JOIN
+  alz::EdgeTable edges{};
   alz::Counters* d_ctr = nullptr;
   alz::Counters* h_ctr = nullptr;  // pinned
   alz::HotState* d_hot = nullptr;

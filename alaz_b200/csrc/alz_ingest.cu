@@ -35,6 +35,7 @@
 #include <algorithm>
 
 #include "alz_kernels.cuh"
+#include "alz_mbar.cuh"
 
 namespace alz {
 
@@ -125,21 +126,7 @@ __device__ __forceinline__ uint32_t shr_clamp(uint32_t v, uint32_t by) {   // PT
   asm("shr.b32 %0, %1, %2;" : "=r"(r) : "r"(v), "r"(by));
   return r;
 }
-// ---- TMA / mbarrier / cp.async (PTX) ----------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-  } while (!ok);
-}
+// ---- TMA / cp.async (PTX; the mbarrier helpers are in alz_mbar.cuh) ----------------------------
 // global -> shared bulk copy, completion counted on the mbarrier; L2 evict-first so that the stream does not
 // push the accumulator rows out of L2
 __device__ __forceinline__ void tma_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t policy) {
@@ -258,7 +245,7 @@ __device__ __forceinline__ uint64_t keep_policy() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-__device__ __forceinline__ void global_add(const AccTable& t, uint32_t row, uint32_t bucket, uint64_t dur, bool err) {
+__device__ __forceinline__ void global_add(const PairTable& t, uint32_t row, uint32_t bucket, uint64_t dur, bool err) {
   const uint64_t pol = keep_policy();
   uint64_t* sc = pair_sect(t, row, bucket);
   red_add_u32_keep(reinterpret_cast<uint32_t*>(sc) + (bucket & 3u), 1u, pol);
@@ -267,9 +254,9 @@ __device__ __forceinline__ void global_add(const AccTable& t, uint32_t row, uint
 }
 // The same for up to 32 events held one per lane (`on`, row, meta = bucket | ... | err << 8 | dur_hi << 9, dur_lo), as
 // ONE red.u64 instruction per 16 events: lane pair (2j, 2j+1) takes one event, the even lane adds to the cell pair,
-// the odd lane the duration, both in the event's sector, which the LSU serves in one pass (alz_device.cuh, AccTable).
+// the odd lane the duration, both in the event's sector, which the LSU serves in one pass (alz_device.cuh, PairTable).
 // Round r takes the events of lanes 16r..16r+15. All lanes must call this.
-__device__ __forceinline__ void global_add_paired(const AccTable& t, bool on, uint32_t row, uint32_t meta, uint32_t dlo) {
+__device__ __forceinline__ void global_add_paired(const PairTable& t, bool on, uint32_t row, uint32_t meta, uint32_t dlo) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t have = __ballot_sync(0xFFFFFFFFu, on);
   if (have == 0u) return;
@@ -295,7 +282,7 @@ __device__ __forceinline__ void global_add_paired(const AccTable& t, bool on, ui
 // pair, or its source is no pod (dropped like the reference does, aggregator/data.go:829-832)
 template <uint32_t kRows>
 __device__ __forceinline__ void slow_one(uint64_t key, uint64_t dur, uint32_t bucket, uint32_t kind, bool err,
-                                         const AccTable& t, const Shared& s, const EpEntry* __restrict__ ep,
+                                         const PairTable& t, const Shared& s, const EpEntry* __restrict__ ep,
                                          uint32_t ep_mask, uint32_t* lost, uint32_t* unresolved) {
   const uint32_t row = find_or_insert_pair(t, key, kind, ep, ep_mask);
   if (row >= kDropRow) { if (row == kDropRow) *unresolved += 1u; else *lost += 1u; return; }
@@ -305,7 +292,7 @@ __device__ __forceinline__ void slow_one(uint64_t key, uint64_t dur, uint32_t bu
     smem_admit(s, key, kind, table_hash_kind(key, kind), base4_around(bucket), kRows, true);
 }
 template <uint32_t kRows>
-__device__ __forceinline__ void slow_batch(SlowQueue& q, uint32_t count, const AccTable& t, const Shared& s,
+__device__ __forceinline__ void slow_batch(SlowQueue& q, uint32_t count, const PairTable& t, const Shared& s,
                                            const EpEntry* __restrict__ ep, uint32_t ep_mask, uint32_t* lost,
                                            uint32_t* unresolved) {
   const uint32_t lane = threadIdx.x & 31u;
@@ -325,7 +312,7 @@ __device__ __forceinline__ void slow_batch(SlowQueue& q, uint32_t count, const A
 // (cp.async): nothing waits on them until the batch is consumed, which happens when the NEXT batch is ready to be
 // requested. (Holding the probes in registers did not work: handing them from one loop trip to the next needs a
 // move, and the move waits for the load.)
-__device__ __forceinline__ void cold_issue(const ColdQueue& q, uint32_t count, const AccTable& t, const Shared& s,
+__device__ __forceinline__ void cold_issue(const ColdQueue& q, uint32_t count, const PairTable& t, const Shared& s,
                                            uint4* probe, uint32_t probe_a) {
   const uint32_t lane = threadIdx.x & 31u;
   if (lane < count) {
@@ -343,7 +330,7 @@ __device__ __forceinline__ void cold_issue(const ColdQueue& q, uint32_t count, c
 // counted, anything else joins the slow queue.
 template <uint32_t kRows>
 __device__ __forceinline__ void cold_consume(ColdQueue& q, uint32_t count, const uint4* probe, SlowQueue& slow,
-                                             const AccTable& t, const Shared& s, const EpEntry* __restrict__ ep,
+                                             const PairTable& t, const Shared& s, const EpEntry* __restrict__ ep,
                                              uint32_t ep_mask, uint32_t lane_lt, uint32_t* lost, uint32_t* unresolved,
                                              unsigned long long* t_wait, unsigned long long* t_slow) {
   const uint32_t lane = threadIdx.x & 31u;
@@ -372,7 +359,7 @@ __device__ __forceinline__ void cold_consume(ColdQueue& q, uint32_t count, const
 // End of a launch, all warps (after a __syncthreads): drain the private rows into the global table and publish
 // the launch's counters.
 template <int kWarps, uint32_t kRows, bool kWin>
-__device__ __forceinline__ void drain_rows_and_count(const Shared& s, const AccTable& pairs, Counters* ctr,
+__device__ __forceinline__ void drain_rows_and_count(const Shared& s, const PairTable& pairs, Counters* ctr,
                                                      const EpEntry* __restrict__ ep, uint32_t ep_mask, uint32_t lost,
                                                      uint32_t unresolved, uint32_t n_hit, uint32_t n_live,
                                                      uint32_t n_cold, uint32_t n_late) {
@@ -493,7 +480,7 @@ __device__ __forceinline__ bool win_late(uint64_t wt, uint64_t lo, uint64_t off,
 // the open window and counted.
 template <int kWarps, int kRecWords, bool kWin>
 __global__ void __launch_bounds__(kWarps * 32, 1)
-ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, AccTable pairs, Counters* ctr,
+ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable pairs, Counters* ctr,
                        const HotState* __restrict__ hot, const EpEntry* __restrict__ ep, uint32_t ep_mask,
                        const uint32_t* __restrict__ bloom_g, const uint64_t* __restrict__ dur_ovf,
                        const WinClock* __restrict__ win, uint4* __restrict__ defer_buf, uint32_t defer_cap) {
@@ -793,9 +780,8 @@ __global__ void __launch_bounds__(256) defer_resolve_kernel(alz_l7_rec* buf, uin
     const uint32_t proto = rec_protocol(r), mf = rec_mflags(r);
     if (!emits_request_row(proto, mf)) continue;
     uint64_t ekey = kEmptyKey;
-    const bool ok = rec_hostkey(r) ? resolve_edge_hostkey(ep, ep_mask, rec_saddr(r), rec_daddr(r), &ekey)
-                                   : resolve_edge(ep, ep_mask, rec_saddr(r), rec_daddr(r), is_reversed(proto, mf), &ekey);
-    if (!ok) ekey = kEmptyKey;
+    const uint32_t kind = rec_hostkey(r) ? kPairHost : is_reversed(proto, mf) ? kPairRev : kPairFwd;
+    if (!resolve_pair(ep, ep_mask, make_pair_key(rec_saddr(r), rec_daddr(r)), kind, &ekey)) ekey = kEmptyKey;
     buf[i].saddr = (uint32_t)ekey;
     buf[i].daddr = (uint32_t)(ekey >> 32);
   }
@@ -806,7 +792,7 @@ __global__ void __launch_bounds__(256) defer_resolve_kernel(alz_l7_rec* buf, uin
 // window are set aside again into dst, resolution kept, ahead of any raw record (the caller ingests those after).
 __global__ void __launch_bounds__(256) defer_roll_kernel(const alz_l7_rec* __restrict__ src, uint32_t n,
                                                          const WinClock* __restrict__ win, alz_l7_rec* __restrict__ dst,
-                                                         uint32_t cap, AccTable edges, Counters* ctr) {
+                                                         uint32_t cap, EdgeTable edges, Counters* ctr) {
   const uint64_t lo = win->lo, len = win->len, off = win->off;
   const bool past = win->ready > 1ull;
   uint32_t not_request = 0, unresolved = 0, lost = 0, late = 0;
@@ -834,10 +820,7 @@ __global__ void __launch_bounds__(256) defer_roll_kernel(const alz_l7_rec* __res
     const uint32_t row = find_or_insert(edges, ekey);
     if (row >= kLostRow) { ++lost; continue; }
     const uint64_t dur = rec_duration(r);
-    atomicAdd(&edges.hist[(size_t)row * ALZ_NB + latency_bucket(dur)], 1u);
-    atomicAdd((unsigned long long*)&edges.lat_sum[row], (unsigned long long)dur);
-    if (is_5xx(proto, rec_status(r))) atomicAdd((unsigned long long*)&edges.err5xx[row], 1ull);
-    atomicAdd((unsigned long long*)&edges.count[row], 1ull);
+    edge_add(edges, row, latency_bucket(dur), dur, is_5xx(proto, rec_status(r)));
   }
   if (not_request) atomicAdd(&ctr->not_request, (unsigned long long)not_request);
   if (unresolved) atomicAdd(&ctr->src_unresolved, (unsigned long long)unresolved);
@@ -849,7 +832,7 @@ __global__ void __launch_bounds__(256) defer_roll_kernel(const alz_l7_rec* __res
 // the fold (fold_pairs_kernel, or emit_edges_kernel at a single-rank flush) left row_cnt[row], row_base[row] and a 128-bin (quarter-octave) histogram of the counts of
 // the forward rows; thresholds = the lowest bins that keep tier A <= kHotA and A+B <= target. Every block derives
 // the same two thresholds from the bins itself (128 adds) instead of a separate launch.
-__global__ void __launch_bounds__(256) hot_emit_kernel(AccTable pairs, HotState* hot, uint32_t target_total) {
+__global__ void __launch_bounds__(256) hot_emit_kernel(PairTable pairs, HotState* hot, uint32_t target_total) {
   __shared__ uint32_t s_thr[3];
   if (threadIdx.x == 0) {
     uint32_t cum = 0, thr_s = 128, thr_a = 128, thr_b = 128;
@@ -886,7 +869,7 @@ __global__ void __launch_bounds__(256) hot_emit_kernel(AccTable pairs, HotState*
 }
 
 template <int kWarps, int kRecWords, bool kWin = false>
-void launch_variant(const void* recs, uint64_t n, const AccTable& pairs, Counters* ctr, const HotState* hot,
+void launch_variant(const void* recs, uint64_t n, const PairTable& pairs, Counters* ctr, const HotState* hot,
                     const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, const uint64_t* dur_ovf, int sms,
                     cudaStream_t s, const WinClock* win = nullptr, void* defer_buf = nullptr, uint32_t defer_cap = 0) {
   using L = Layout<kWarps, kRecWords>;
@@ -903,14 +886,14 @@ constexpr int kDefaultWarps = 16;
 
 uint32_t ingest_table_rows() { return Layout<kDefaultWarps, 8>::kRows; }
 
-void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                          const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, int sms,
                          cudaStream_t s) {
   if (n == 0) return;
   launch_variant<kDefaultWarps, 8>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, s);
 }
 
-void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const AccTable& pairs,
+void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const PairTable& pairs,
                                Counters* ctr, const HotState* hot, const EpEntry* ep, uint32_t ep_mask,
                                const uint32_t* bloom, int sms, cudaStream_t s) {
   if (n == 0) return;
@@ -918,7 +901,7 @@ void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint6
 }
 
 // time-cut windows: `win` = device WinClock {lo, len, ready}; records beyond the open window land in defer_buf
-void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
                                   uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s) {
   if (n == 0) return;
@@ -933,13 +916,13 @@ void launch_defer_resolve(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEnt
   defer_resolve_kernel<<<grid, 256, 0, s>>>(buf, lo, hi, ep, ep_mask, ctr);
 }
 void launch_defer_roll(const alz_l7_rec* src, uint32_t n, const uint64_t* win, alz_l7_rec* dst, uint32_t cap,
-                       const AccTable& edges, Counters* ctr, int sms, cudaStream_t s) {
+                       const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s) {
   const uint32_t grid = std::min<uint32_t>((uint32_t)sms * 4u, std::max<uint32_t>(1u, (n + 255u) / 256u));
   defer_roll_kernel<<<grid, 256, 0, s>>>(src, n, (const WinClock*)win, dst, cap, edges, ctr);
 }
 
 // after fold_pairs_kernel / emit_edges_kernel filled hot->bins: choose next window's hot list
-void launch_hot_select(const AccTable& pairs, HotState* hot, int sms, cudaStream_t s) {
+void launch_hot_select(const PairTable& pairs, HotState* hot, int sms, cudaStream_t s) {
   hot_emit_kernel<<<(unsigned)sms * 2, 256, 0, s>>>(pairs, hot, Layout<kDefaultWarps, 8>::kPreload);
 }
 

@@ -42,15 +42,8 @@ __device__ __forceinline__ Ev decode(const Rec& r, bool live) {
   return e;
 }
 
-__device__ __forceinline__ void global_accumulate(const AccTable& t, uint32_t row, uint32_t bucket, uint64_t dur,
-                                                  bool err) {
-  atomicAdd(&t.hist[(size_t)row * ALZ_NB + bucket], 1u);
-  atomicAdd((unsigned long long*)&t.lat_sum[row], (unsigned long long)dur);
-  if (err) atomicAdd((unsigned long long*)&t.err5xx[row], 1ull);
-}
-
-// the same into a pair row (sectored layout, alz_device.cuh); v1 plan: one lane per event, three instructions
-__device__ __forceinline__ void pair_accumulate(const AccTable& t, uint32_t row, uint32_t bucket, uint64_t dur, bool err) {
+// one event into a pair row (sectored layout, alz_device.cuh); v1 plan: one lane per event, three instructions
+__device__ __forceinline__ void pair_accumulate(const PairTable& t, uint32_t row, uint32_t bucket, uint64_t dur, bool err) {
   uint64_t* sc = pair_sect(t, row, bucket);
   atomicAdd(reinterpret_cast<uint32_t*>(sc) + (bucket & 3u), 1u);
   atomicAdd((unsigned long long*)(sc + 2), (unsigned long long)dur);
@@ -76,7 +69,7 @@ __device__ __forceinline__ void flush_thread_counters(Counters* ctr, uint32_t no
 // ---------------------------------------------------------------------------
 template <int UNROLL>
 __global__ void __launch_bounds__(256) ingest_pairs_kernel(const alz_l7_rec* __restrict__ recs, uint64_t n,
-                                                           AccTable pairs, Counters* ctr, const EpEntry* __restrict__ ep,
+                                                           PairTable pairs, Counters* ctr, const EpEntry* __restrict__ ep,
                                                            uint32_t ep_mask) {
   uint32_t not_request = 0, lost = 0, unresolved = 0;
   const uint32_t lane = threadIdx.x & 31u;
@@ -112,7 +105,7 @@ __global__ void __launch_bounds__(256) ingest_pairs_kernel(const alz_l7_rec* __r
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) ingest_eager_kernel(const alz_l7_rec* __restrict__ recs, uint64_t n,
                                                            const EpEntry* __restrict__ ep, uint32_t ep_mask,
-                                                           AccTable edges, Counters* ctr) {
+                                                           EdgeTable edges, Counters* ctr) {
   uint32_t not_request = 0, unresolved = 0, lost = 0;
   const uint32_t lane = threadIdx.x & 31u;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -125,8 +118,7 @@ __global__ void __launch_bounds__(256) ingest_eager_kernel(const alz_l7_rec* __r
     not_request += (live && !e.act) ? 1u : 0u;
     uint64_t ekey = 0;
     bool ok = false;
-    if (e.act) ok = e.hostkey ? resolve_edge_hostkey(ep, ep_mask, pair_saddr(e.key), pair_daddr(e.key), &ekey)
-                              : resolve_edge(ep, ep_mask, pair_saddr(e.key), pair_daddr(e.key), e.rev, &ekey);
+    if (e.act) ok = resolve_pair(ep, ep_mask, e.key, e.hostkey ? kPairHost : e.rev ? kPairRev : kPairFwd, &ekey);
     __syncwarp();
     unresolved += (e.act && !ok) ? 1u : 0u;
     uint32_t row = kLostRow;
@@ -134,10 +126,7 @@ __global__ void __launch_bounds__(256) ingest_eager_kernel(const alz_l7_rec* __r
     __syncwarp();
     if (ok) {
       if (row >= kLostRow) ++lost;
-      else {
-        global_accumulate(edges, row, e.bucket, e.dur, e.err);
-        atomicAdd((unsigned long long*)&edges.count[row], 1ull);
-      }
+      else edge_add(edges, row, e.bucket, e.dur, e.err);
     }
   }
   flush_thread_counters(ctr, not_request, unresolved, lost);
@@ -151,11 +140,11 @@ __global__ void __launch_bounds__(256) ingest_eager_kernel(const alz_l7_rec* __r
 // pass 1, a thread per pair row: resolve and find the edge row. All the dependent
 // table/dictionary probes of a pair sit in one thread, 32 pairs per warp in flight
 // (the one-warp-per-row version spent its time in lane 0's probe chain).
-__global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const EpEntry* __restrict__ ep,
-                                                           uint32_t ep_mask, AccTable edges, HotState* hot) {
+__global__ void __launch_bounds__(256) fold_resolve_kernel(PairTable pairs, const EpEntry* __restrict__ ep,
+                                                           uint32_t ep_mask, EdgeTable edges, HotState* hot) {
   // the hot-list bookkeeping of this fold starts from zero (fold_pairs_kernel or emit_edges_kernel fills the bins, hot_emit
   // the list; both run after this kernel, the ingest launches that read the list ran before it)
-  if (blockIdx.x == 0 && hot != nullptr) {
+  if (blockIdx.x == 0) {
     if (threadIdx.x < 128) hot->bins[threadIdx.x] = 0u;
     if (threadIdx.x == 0) { hot->n_a = 0u; hot->n_b = 0u; hot->n_s = 0u; }
   }
@@ -174,9 +163,7 @@ __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const
     }
     uint64_t ekey = 0;
     uint32_t erow = kDropRow;                                  // source is not a pod: data.go:829-832
-    const bool ok = kind == kPairHost ? resolve_edge_hostkey(ep, ep_mask, pair_saddr(key), pair_daddr(key), &ekey)
-                                      : resolve_edge(ep, ep_mask, pair_saddr(key), pair_daddr(key), kind == kPairRev, &ekey);
-    if (ok) erow = find_or_insert(edges, ekey);
+    if (resolve_pair(ep, ep_mask, key, kind, &ekey)) erow = find_or_insert(edges, ekey);
     pairs.row_aux[row] = erow;
   }
 }
@@ -188,19 +175,16 @@ __global__ void __launch_bounds__(256) fold_resolve_kernel(AccTable pairs, const
 struct PairSlice { uint4 a, pa, b, pb; };
 // The count bins of the hot list are summed per block in shared memory and added to hot_bins once per block: the
 // counts of a window's rows fall into a few dozen bins, and one global atomic per row piles up on those few words.
-// block_bins_begin returns the bins take_pair_row adds to (nullptr when there is no hot list); every thread of the
-// block calls both.
-__device__ __forceinline__ uint32_t* block_bins_begin(uint32_t* s_bins, uint32_t* hot_bins) {
+// take_pair_row adds to the block's bins in between; every thread of the block calls both.
+__device__ __forceinline__ void block_bins_begin(uint32_t* s_bins) {
   for (uint32_t b = threadIdx.x; b < 128u; b += blockDim.x) s_bins[b] = 0u;
   __syncthreads();
-  return hot_bins != nullptr ? s_bins : nullptr;
 }
 __device__ __forceinline__ void block_bins_end(const uint32_t* s_bins, uint32_t* hot_bins) {
   __syncthreads();
-  if (hot_bins == nullptr) return;
   for (uint32_t b = threadIdx.x; b < 128u; b += blockDim.x) if (s_bins[b]) atomicAdd(&hot_bins[b], s_bins[b]);
 }
-__device__ __forceinline__ uint64_t take_pair_row(const AccTable& pairs, uint32_t row, bool valid, uint32_t gmask,
+__device__ __forceinline__ uint64_t take_pair_row(const PairTable& pairs, uint32_t row, bool valid, uint32_t gmask,
                                                   uint32_t* __restrict__ hot_bins, PairSlice& s) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
   uint4* cells = reinterpret_cast<uint4*>(pairs.sect + ((size_t)row * kSectPerRow + sl * 2u) * 4u);
@@ -211,25 +195,23 @@ __device__ __forceinline__ uint64_t take_pair_row(const AccTable& pairs, uint32_
   cnt += __shfl_xor_sync(gmask, cnt, 1);
   cnt += __shfl_xor_sync(gmask, cnt, 2);
   cnt += __shfl_xor_sync(gmask, cnt, 4);
-  if (pairs.row_base != nullptr) {   // every lane of the group takes part in the shuffles (uniform branch)
-    // the 16-bucket window (aligned to 4 buckets) that holds most of the row's events: group sums of 4 cells,
-    // two candidates per lane, arg-max over the row's eight lanes
-    const uint64_t g0 = (uint64_t)a.x + a.y + a.z + a.w, g1 = (uint64_t)b.x + b.y + b.z + b.w;   // groups 2sl, 2sl+1
-    const uint32_t seg = lane & ~7u;
-    const uint64_t n0 = __shfl_sync(gmask, g0, seg | ((sl + 1u) & 7u)), n1 = __shfl_sync(gmask, g1, seg | ((sl + 1u) & 7u));
-    const uint64_t m0 = __shfl_sync(gmask, g0, seg | ((sl + 2u) & 7u));
-    // candidate j covers groups j..j+3 (j <= 12); lanes past the end contribute nothing
-    uint64_t c0 = sl <= 6u ? g0 + g1 + n0 + n1 : 0ull;                    // j = 2 sl       (sl = 6 -> j = 12)
-    uint64_t c1 = sl <= 5u ? g1 + n0 + n1 + m0 : 0ull;                    // j = 2 sl + 1   (sl = 5 -> j = 11)
-    uint64_t best = c0 >= c1 ? (c0 << 4) | (2u * sl) : (c1 << 4) | (2u * sl + 1u);   // counts < 2^37: room for 4 index bits
-    for (int o = 1; o < 8; o <<= 1) { const uint64_t x = __shfl_xor_sync(gmask, best, o); best = x > best ? x : best; }
-    if (sl == 0 && valid && row < pairs.max_rows) pairs.row_base[row] = (uint8_t)(best & 15u);
-  }
+  // the 16-bucket window (aligned to 4 buckets) that holds most of the row's events: group sums of 4 cells,
+  // two candidates per lane, arg-max over the row's eight lanes
+  const uint64_t g0 = (uint64_t)a.x + a.y + a.z + a.w, g1 = (uint64_t)b.x + b.y + b.z + b.w;   // groups 2sl, 2sl+1
+  const uint32_t seg = lane & ~7u;
+  const uint64_t n0 = __shfl_sync(gmask, g0, seg | ((sl + 1u) & 7u)), n1 = __shfl_sync(gmask, g1, seg | ((sl + 1u) & 7u));
+  const uint64_t m0 = __shfl_sync(gmask, g0, seg | ((sl + 2u) & 7u));
+  // candidate j covers groups j..j+3 (j <= 12); lanes past the end contribute nothing
+  uint64_t c0 = sl <= 6u ? g0 + g1 + n0 + n1 : 0ull;                    // j = 2 sl       (sl = 6 -> j = 12)
+  uint64_t c1 = sl <= 5u ? g1 + n0 + n1 + m0 : 0ull;                    // j = 2 sl + 1   (sl = 5 -> j = 11)
+  uint64_t best = c0 >= c1 ? (c0 << 4) | (2u * sl) : (c1 << 4) | (2u * sl + 1u);   // counts < 2^37: room for 4 index bits
+  for (int o = 1; o < 8; o <<= 1) { const uint64_t x = __shfl_xor_sync(gmask, best, o); best = x > best ? x : best; }
+  if (sl == 0 && valid && row < pairs.max_rows) pairs.row_base[row] = (uint8_t)(best & 15u);
   if (!valid || cnt == 0) return cnt;  // unused sentinel row (allocated rows always hold >= 1 event)
-  if (sl == 0 && row < pairs.max_rows && pairs.row_cnt != nullptr) {    // feedback for the next ingest
+  if (sl == 0 && row < pairs.max_rows) {    // feedback for the next ingest
     const uint32_t c32 = cnt > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)cnt;
     pairs.row_cnt[row] = c32;
-    if (hot_bins != nullptr && pairs.row_kind[row] != kPairHost) atomicAdd(&hot_bins[count_bin(c32)], 1u);
+    if (pairs.row_kind[row] != kPairHost) atomicAdd(&hot_bins[count_bin(c32)], 1u);
   }
   // zero what was not zero: a pair's latencies fall into a few of its 16 sectors, the rest was never written
   const uint4 pa = s.pa, pb = s.pb;
@@ -254,20 +236,20 @@ __device__ __forceinline__ void count_stray_events(Counters* ctr, uint32_t erow,
 // eight lanes per pair row (four rows per warp in flight): add the row into its edge row and zero it. Each lane
 // owns 8 histogram cells = two 16-byte loads; the one-warp-per-row version was bound by its chain of dependent L2
 // round trips.
-__global__ void __launch_bounds__(256) fold_pairs_kernel(AccTable pairs, AccTable edges, Counters* ctr,
+__global__ void __launch_bounds__(256) fold_pairs_kernel(PairTable pairs, EdgeTable edges, Counters* ctr,
                                                          uint32_t* __restrict__ hot_bins) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
   const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
   __shared__ uint32_t s_bins[128];
-  uint32_t* const bins = block_bins_begin(s_bins, hot_bins);
+  block_bins_begin(s_bins);
   uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3;
   // rows [0, n_rows) plus the sentinel rows (index n_rows + kind stands for row max_rows + kind)
   for (; i < n_rows + kPairKinds; i += groups_per_grid) {
     const uint32_t row = i >= n_rows ? pairs.max_rows + (i - n_rows) : i;
     PairSlice s;
-    const uint64_t cnt = take_pair_row(pairs, row, true, gmask, bins, s);
+    const uint64_t cnt = take_pair_row(pairs, row, true, gmask, s_bins, s);
     if (cnt == 0) continue;
     uint64_t lat = lat_partial(s), e5 = err_partial(s);
     for (int o = 1; o < 8; o <<= 1) {
@@ -307,6 +289,23 @@ __global__ void __launch_bounds__(256) iota_kernel(uint32_t* out, uint32_t n) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = i;
 }
 
+// unique of a sorted key array (the merge's canonical keys, the GNN's node set): flag the run heads, exclusive-scan
+// the flags, scatter the heads. kEmptyKey is never a head: the merge pads its gathered key lists with it, and no GNN
+// node key equals it (node_key, alz_gnn.cu, puts a node type, below 4, in the high word).
+__global__ void flag_heads_kernel(const uint64_t* __restrict__ sorted, uint32_t n, uint32_t* __restrict__ flags) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const uint64_t k = sorted[i];
+    flags[i] = (k != kEmptyKey && (i == 0 || sorted[i - 1] != k)) ? 1u : 0u;
+  }
+}
+__global__ void scatter_heads_kernel(const uint64_t* __restrict__ sorted, const uint32_t* __restrict__ flags,
+                                     const uint32_t* __restrict__ pos, uint32_t n, uint64_t* __restrict__ out) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    if (flags[i]) out[pos[i]] = sorted[i];
+}
+
 // the fixed part of an output row and the lane's 8 histogram cells (hist sits at byte 40 of a 296-byte row:
 // 8-byte aligned only)
 __device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uint64_t key, const uint32_t (&c)[8],
@@ -328,19 +327,16 @@ __device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uin
 
 // multi-rank flush: the live edge rows, as they are, into the send buffer (the window stays in the table until
 // every rank has taken part in the merge, alz_comm.cu)
-__global__ void __launch_bounds__(256) gather_edges_kernel(AccTable edges, const uint64_t* __restrict__ keys,
+__global__ void __launch_bounds__(256) gather_edges_kernel(EdgeTable edges, const uint64_t* __restrict__ keys,
                                                            const uint32_t* __restrict__ rows, uint32_t n_live,
                                                            alz_edge_out* __restrict__ out) {
   // eight lanes per edge, four edges per warp in flight; a lane moves 8 histogram cells (2 x 16 bytes)
   const uint32_t sl = threadIdx.x & 7u;
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_live; i += groups_per_grid) {
-    const uint32_t row = rows[i];
-    const uint4* cells = reinterpret_cast<const uint4*>(edges.hist + (size_t)row * ALZ_NB + sl * 8u);
-    const uint4 a = cells[0], b = cells[1];
-    const uint32_t c[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-    uint64_t count = 0, e5 = 0, lat = 0;
-    if (sl == 0) { count = edges.count[row]; e5 = edges.err5xx[row]; lat = edges.lat_sum[row]; }
+    uint32_t c[8];
+    uint64_t count, lat, e5;
+    edge_row_load(edges, rows[i], sl, c, count, lat, e5);
     store_edge_out(&out[i], sl, keys[i], c, count, e5, lat);
   }
 }
@@ -353,7 +349,7 @@ __global__ void __launch_bounds__(256) gather_edges_kernel(AccTable edges, const
 // ---------------------------------------------------------------------------
 // pair rows per edge row into cnt[]; a row that reaches no edge row (unresolved source, full edge table, the
 // free-marker edge key) goes to the back of row_list, *n_stray of them
-__global__ void __launch_bounds__(256) bucket_count_kernel(AccTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
+__global__ void __launch_bounds__(256) bucket_count_kernel(PairTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
                                                            uint32_t* __restrict__ row_list, uint32_t list_cap,
                                                            uint32_t* __restrict__ n_stray) {
   const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
@@ -366,7 +362,7 @@ __global__ void __launch_bounds__(256) bucket_count_kernel(AccTable pairs, uint3
   }
 }
 // each row to its place in its edge's bucket; counts cnt[] back down to zero for the next flush
-__global__ void __launch_bounds__(256) bucket_fill_kernel(AccTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
+__global__ void __launch_bounds__(256) bucket_fill_kernel(PairTable pairs, uint32_t max_edges, uint32_t* __restrict__ cnt,
                                                           const uint32_t* __restrict__ off, uint32_t* __restrict__ row_list) {
   const uint32_t n_rows = min(*pairs.n_rows, pairs.max_rows);
   const uint32_t stride = gridDim.x * blockDim.x;
@@ -382,7 +378,7 @@ __global__ void __launch_bounds__(256) bucket_fill_kernel(AccTable pairs, uint32
 // Eight lanes per output row as in fold_pairs_kernel, plain stores only. The n_stray pair rows at the back of
 // row_list follow as groups n_live.. : they leave their feedback and their events in the counters. off == nullptr:
 // no pair rows to take (nothing was ingested since the last fold, or ALZ_CFG_EAGER_JOIN).
-__global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTable edges, Counters* ctr,
+__global__ void __launch_bounds__(256) emit_edges_kernel(PairTable pairs, EdgeTable edges, Counters* ctr,
                                                          uint32_t* __restrict__ hot_bins, const uint64_t* __restrict__ keys,
                                                          const uint32_t* __restrict__ rows, uint32_t n_live,
                                                          const uint32_t* __restrict__ off,
@@ -394,12 +390,12 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTabl
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
   const uint32_t n_groups = n_live + (off != nullptr ? *n_stray : 0u);
   __shared__ uint32_t s_bins[128];
-  uint32_t* const bins = block_bins_begin(s_bins, hot_bins);
+  block_bins_begin(s_bins);
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n_groups; i += groups_per_grid) {
     if (i >= n_live) {
       const uint32_t row = row_list[list_cap - 1u - (i - n_live)];
       PairSlice s;
-      const uint64_t cnt = take_pair_row(pairs, row, true, gmask, bins, s);
+      const uint64_t cnt = take_pair_row(pairs, row, true, gmask, s_bins, s);
       if (sl == 0 && cnt != 0) count_stray_events(ctr, pairs.row_aux[row], cnt);
       continue;
     }
@@ -407,21 +403,14 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(AccTable pairs, AccTabl
     uint32_t c[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
     uint64_t count = 0, lat = 0, e5 = 0;   // lane partials of the latency and 5xx sums; count in lane 0
     if (with_edges) {
-      uint4* cells = reinterpret_cast<uint4*>(edges.hist + (size_t)erow * ALZ_NB + sl * 8u);
-      const uint4 a = cells[0], b = cells[1];
-      c[0] = a.x; c[1] = a.y; c[2] = a.z; c[3] = a.w; c[4] = b.x; c[5] = b.y; c[6] = b.z; c[7] = b.w;
-      cells[0] = make_uint4(0u, 0u, 0u, 0u);
-      cells[1] = make_uint4(0u, 0u, 0u, 0u);
-      if (sl == 0) {
-        count = edges.count[erow]; lat = edges.lat_sum[erow]; e5 = edges.err5xx[erow];
-        edges.count[erow] = 0ull; edges.lat_sum[erow] = 0ull; edges.err5xx[erow] = 0ull;
-      }
+      edge_row_load(edges, erow, sl, c, count, lat, e5);
+      edge_row_zero(edges, erow, sl);
     }
     if (off != nullptr) {
       const uint32_t end = off[erow + 1u];
       for (uint32_t j = off[erow]; j < end; ++j) {
         PairSlice s;
-        count += take_pair_row(pairs, row_list[j], true, gmask, bins, s);
+        count += take_pair_row(pairs, row_list[j], true, gmask, s_bins, s);
         c[0] += s.a.x; c[1] += s.a.y; c[2] += s.a.z; c[3] += s.a.w;
         c[4] += s.b.x; c[5] += s.b.y; c[6] += s.b.z; c[7] += s.b.w;
         lat += lat_partial(s);
@@ -513,24 +502,23 @@ __global__ void __launch_bounds__(256) synth_owned_kernel(alz_synth_view v, uint
 // ---------------------------------------------------------------------------
 static inline unsigned grid_for(int sms, int per_sm) { return (unsigned)(sms * per_sm); }
 
-void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                             const EpEntry* ep, uint32_t ep_mask, int sms, cudaStream_t s) {
   if (n == 0) return;   // global reductions only (ALZ_CFG_NO_SMEM_CACHE; kept for the ncu comparison)
   ingest_pairs_kernel<4><<<grid_for(sms, 8), 256, 0, s>>>(recs, n, pairs, ctr, ep, ep_mask);
 }
 void launch_ingest_eager(const alz_l7_rec* recs, uint64_t n, const EpEntry* ep, uint32_t ep_mask,
-                         const AccTable& edges, Counters* ctr, int sms, cudaStream_t s) {
+                         const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s) {
   if (n == 0) return;
   ingest_eager_kernel<<<grid_for(sms, 8), 256, 0, s>>>(recs, n, ep, ep_mask, edges, ctr);
 }
-void launch_fold_resolve(const AccTable& pairs, const EpEntry* ep, uint32_t ep_mask, const AccTable& edges,
-                         Counters* ctr, HotState* hot, int sms, cudaStream_t s) {
-  (void)ctr;
+void launch_fold_resolve(const PairTable& pairs, const EpEntry* ep, uint32_t ep_mask, const EdgeTable& edges,
+                         HotState* hot, int sms, cudaStream_t s) {
   fold_resolve_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, ep, ep_mask, edges, hot);
 }
-void launch_fold_add(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, int sms,
+void launch_fold_add(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, int sms,
                      cudaStream_t s) {
-  fold_pairs_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot ? hot->bins : nullptr);
+  fold_pairs_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot->bins);
 }
 // changed slots of the endpoint table (alz_table_commit): patch[i] = {slot, pad x3, entry}
 __global__ void __launch_bounds__(256) ep_patch_kernel(EpEntry* __restrict__ tab, const uint4* __restrict__ patch, uint32_t n) {
@@ -549,21 +537,27 @@ void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s) {
   if (n == 0) return;
   iota_kernel<<<grid_for(sms, 4), 256, 0, s>>>(out, n);
 }
-void launch_gather_edges(const AccTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
+void launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
+                          void* temp, size_t temp_bytes, int sms, cudaStream_t s) {
+  flag_heads_kernel<<<grid_for(sms, 4), 256, 0, s>>>(sorted, n, flags);
+  exclusive_scan_u32(temp, temp_bytes, flags, pos, n, s);
+  scatter_heads_kernel<<<grid_for(sms, 4), 256, 0, s>>>(sorted, flags, pos, n, out);
+}
+void launch_gather_edges(const EdgeTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
                          alz_edge_out* out, int sms, cudaStream_t s) {
   if (n_live == 0) return;
   gather_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(edges, keys, rows, n_live, out);
 }
-void launch_bucket_count(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
+void launch_bucket_count(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
   bucket_count_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, max_edges, b.cnt, b.rows, b.cap, b.n_stray);
 }
-void launch_bucket_fill(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
+void launch_bucket_fill(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s) {
   bucket_fill_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, max_edges, b.cnt, b.off, b.rows);
 }
-void launch_emit_edges(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
+void launch_emit_edges(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
                        const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
                        int sms, cudaStream_t s) {
-  emit_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot ? hot->bins : nullptr, keys, rows, n_live,
+  emit_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot->bins, keys, rows, n_live,
                                                      b ? b->off : nullptr, b ? b->rows : nullptr, b ? b->cap : 0u,
                                                      b ? b->n_stray : nullptr, with_edges, out);
 }

@@ -15,33 +15,36 @@ struct WinClock {
   uint64_t off;       // first_user_ns - first_kernel_ns (mod 2^64)
   uint64_t epoch;     // epoch_open
 };
-void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                             const EpEntry* ep, uint32_t ep_mask, int sms, cudaStream_t s);
-void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                          const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, int sms,
                          cudaStream_t s);
-void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const AccTable& pairs,
+void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const PairTable& pairs,
                                Counters* ctr, const HotState* hot, const EpEntry* ep, uint32_t ep_mask,
                                const uint32_t* bloom, int sms, cudaStream_t s);
-void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const AccTable& pairs, Counters* ctr,
+void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
                                   uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s);
 void launch_window_advance(uint64_t* win, cudaStream_t s);
 void launch_defer_resolve(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEntry* ep, uint32_t ep_mask, Counters* ctr,
                           int sms, cudaStream_t s);
 void launch_defer_roll(const alz_l7_rec* src, uint32_t n, const uint64_t* win, alz_l7_rec* dst, uint32_t cap,
-                       const AccTable& edges, Counters* ctr, int sms, cudaStream_t s);
+                       const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s);
 uint32_t ingest_table_rows();
-void launch_hot_select(const AccTable& pairs, HotState* hot, int sms, cudaStream_t s);
+void launch_hot_select(const PairTable& pairs, HotState* hot, int sms, cudaStream_t s);
 void launch_ingest_eager(const alz_l7_rec* recs, uint64_t n, const EpEntry* ep, uint32_t ep_mask,
-                         const AccTable& edges, Counters* ctr, int sms, cudaStream_t s);
-void launch_fold_resolve(const AccTable& pairs, const EpEntry* ep, uint32_t ep_mask, const AccTable& edges,
-                         Counters* ctr, HotState* hot, int sms, cudaStream_t s);
-void launch_fold_add(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, int sms,
+                         const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s);
+void launch_fold_resolve(const PairTable& pairs, const EpEntry* ep, uint32_t ep_mask, const EdgeTable& edges,
+                         HotState* hot, int sms, cudaStream_t s);
+void launch_fold_add(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, int sms,
                      cudaStream_t s);
 void launch_ep_patch(EpEntry* tab, const void* patch, uint32_t n, int sms, cudaStream_t s);
 void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s);
-void launch_gather_edges(const AccTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
+// the distinct keys of sorted[0, n) into out, in order: out has pos[n - 1] + flags[n - 1] entries (alz_kernels.cu)
+void launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
+                          void* temp, size_t temp_bytes, int sms, cudaStream_t s);
+void launch_gather_edges(const EdgeTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
                          alz_edge_out* out, int sms, cudaStream_t s);
 // single-rank flush scratch: pair rows bucketed by edge row (alz_kernels.cu, emit_edges_kernel)
 struct FlushBuckets {
@@ -51,10 +54,10 @@ struct FlushBuckets {
   uint32_t cap;        // max_pairs + kPairKinds
   uint32_t* n_stray;   // rows at the back of `rows`
 };
-void launch_bucket_count(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
-void launch_bucket_fill(const AccTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
+void launch_bucket_count(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
+void launch_bucket_fill(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
 // b == nullptr: no pair rows to take
-void launch_emit_edges(const AccTable& pairs, const AccTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
+void launch_emit_edges(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
                        const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
                        int sms, cudaStream_t s);
 void launch_compact_raw(const uint8_t* raw, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s);

@@ -264,15 +264,6 @@ struct alz_sock_state {
   uint64_t syncs = 0, sync_ops = 0, sync_bytes = 0, repools = 0;
 };
 
-#define CK(expr)                                                                       \
-  do {                                                                                 \
-    cudaError_t _e = (expr);                                                           \
-    if (_e != cudaSuccess) {                                                           \
-      h->last_err = std::string(#expr) + ": " + cudaGetErrorString(_e);                \
-      return ALZ_E_CUDA;                                                               \
-    }                                                                                  \
-  } while (0)
-
 static alz_sock_state* state_of(alz_handle* h) {
   if (!h->sock) h->sock = new alz_sock_state();
   return h->sock;
