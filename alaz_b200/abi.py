@@ -97,6 +97,18 @@ class Stats(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_ if not n.startswith("_")}
 
 
+class RollupInfo(C.Structure):
+    """alz_rollup_info."""
+    _fields_ = [
+        ("windows", C.c_uint32), ("clocked", C.c_uint32),
+        ("window_first", C.c_uint64), ("window_last", C.c_uint64),
+        ("epoch_first", C.c_uint64), ("epoch_last", C.c_uint64), ("rows_in", C.c_uint64),
+    ]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SockStats(C.Structure):
     """alz_sock_stats_t."""
     _fields_ = [(n, C.c_uint64) for n in ("lines", "pool_records", "pool_garbage", "syncs", "sync_ops", "sync_bytes",

@@ -23,7 +23,8 @@ EXPORTS = [
     "alz_table_upsert", "alz_table_upsert_batch", "alz_table_erase", "alz_table_commit", "alz_submit_l7", "alz_submit_l7_device",
     "alz_submit_l7_packed", "alz_submit_l7_packed_device", "alz_pack_l7",
     "alz_submit_l7_raw", "alz_window_flush", "alz_window_flush_device", "alz_window_fetch", "alz_get_stats",
-    "alz_window_clock", "alz_window_epoch", "alz_gnn_score",
+    "alz_window_clock", "alz_window_epoch", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
+    "alz_gnn_score",
     "alz_gnn_score_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -61,6 +62,9 @@ def load(rebuild=False):
         "alz_window_fetch": ([vp, vp, sz, C.POINTER(sz)], i),
         "alz_window_clock": ([vp, u64, u64, u64], i),
         "alz_window_epoch": ([vp, C.POINTER(u64)], i),
+        "alz_window_history": ([vp, u32, u64], i),
+        "alz_window_rollup": ([vp, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
+        "alz_window_rollup_device": ([vp, u32, pp, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
         "alz_pinned_alloc_local": ([vp, sz, pp], i),
         "alz_window_flush": ([vp, vp, sz, C.POINTER(sz)], i),
         "alz_window_flush_device": ([vp, pp, C.POINTER(sz)], i),
@@ -99,7 +103,7 @@ def load(rebuild=False):
         for k in ("alz_submit_l7_packed", "alz_submit_l7_packed_device", "alz_pack_l7", "alz_window_fetch",
                   "alz_pinned_alloc_local", "alz_table_upsert_batch", "alz_window_clock", "alz_window_epoch",
                   "alz_sock_lookup_at", "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats",
-                  "alz_submit_tcp_raw"):
+                  "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -294,6 +298,32 @@ class Handle:
         e = C.c_uint64(0)
         self._ck(self.L.alz_window_epoch(self.h, C.byref(e)), "alz_window_epoch")
         return e.value
+
+    # ---- rolling windows (alz_rollup.cu)
+    def window_history(self, depth, arena_rows):
+        self._ck(self.L.alz_window_history(self.h, int(depth), int(arena_rows)), "alz_window_history")
+
+    def rollup(self, k, cap=None):
+        """alz_window_rollup: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
+        info = abi.RollupInfo()
+        n = C.c_size_t(0)
+        if cap is None:
+            if self._ck(self.L.alz_window_rollup(self.h, int(k), None, 0, C.byref(n), C.byref(info)),
+                        "alz_window_rollup", allow=(abi.E_CAPACITY,)) == 0:
+                return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
+            cap = n.value
+        out = np.zeros(cap, dtype=abi.EDGE_OUT)
+        self._ck(self.L.alz_window_rollup(self.h, int(k), _ptr(out), cap, C.byref(n), C.byref(info)), "alz_window_rollup")
+        return out[: n.value].copy(), info.as_dict()
+
+    def rollup_device(self, k):
+        """alz_window_rollup_device: (device pointer, rows, info dict)."""
+        info = abi.RollupInfo()
+        p = C.c_void_p()
+        n = C.c_size_t(0)
+        self._ck(self.L.alz_window_rollup_device(self.h, int(k), C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_window_rollup_device")
+        return p.value, n.value, info.as_dict()
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -236,6 +236,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_comm(h);
   alz_internal_free_gnn(h);
   alz_internal_free_sock(h);
+  alz_internal_free_rollup(h);
   free_table(&h->pairs); free_table(&h->edges);
   cudaFree(h->d_ep); cudaFree(h->d_ctr); cudaFree(h->d_hot); cudaFree(h->d_patch);
   cudaFree(h->d_win); cudaFree(h->d_defer[0]); cudaFree(h->d_defer[1]); cudaFree(h->d_bloom);
@@ -862,6 +863,8 @@ static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, si
   CK(cudaEventRecord(h->ev_t[2], h->stream));
   h->ev_t_valid = true;
   if (mrc != ALZ_OK) return mrc;
+  const uint64_t* closed = !h->win_on ? nullptr : ranks ? alz_internal_merged_clock(h) : h->d_win;
+  if ((mrc = alz_internal_history_append(h, closed)) != ALZ_OK) return mrc;
   if (roll && (mrc = window_roll(h)) != ALZ_OK) return mrc;
   *n_out = h->last_n_edges;
   if (dev_edges) *dev_edges = h->d_out;
@@ -899,6 +902,7 @@ extern "C" int alz_window_flush(alz_handle* h, alz_edge_out* out, size_t cap, si
     if (rc != ALZ_OK) return rc;
     if (h->n_live) CK(cudaMemcpyAsync(out, h->d_out, (size_t)h->n_live * sizeof(alz_edge_out),
                                       cudaMemcpyDeviceToHost, h->stream));
+    if ((rc = alz_internal_history_append(h, h->win_on ? h->d_win : nullptr)) != ALZ_OK) return rc;
     if ((rc = window_roll(h)) != ALZ_OK) return rc;
     CK(cudaStreamSynchronize(h->stream));
     return overflow ? ALZ_E_CAPACITY : ALZ_OK;

@@ -34,6 +34,7 @@
 #include <nccl.h>
 
 #include <algorithm>
+#include <cstddef>
 #include <cstdio>
 #include <cstring>
 #include <mutex>
@@ -190,15 +191,6 @@ __global__ void __launch_bounds__(256) unpack_canonical_kernel(const uint64_t* _
   }
 }
 
-// packed edge key of an output row (inverse of unpack_edge_key)
-__device__ __forceinline__ uint64_t row_key_of(const alz_edge_out* r) {
-  // rows are 296 bytes apart: 8-byte aligned only
-  const uint2 ty = reinterpret_cast<const uint2*>(r)[0];   // from_type, to_type, pad | pad
-  const uint2 ft_ = reinterpret_cast<const uint2*>(r)[1];  // from | to
-  const uint32_t ft = ty.x & 0xFFu, tt = (ty.x >> 8) & 0xFFu;
-  if (ft == ALZ_NODE_POD) return ((uint64_t)tt << 61) | ((uint64_t)(ft_.x & 0x1FFFFFFFu) << 32) | ft_.y;
-  return (1ull << 63) | ((uint64_t)ft << 61) | ((uint64_t)(ft_.y & 0x1FFFFFFFu) << 32) | ft_.x;
-}
 __device__ __forceinline__ uint32_t lower_bound_rows(const alz_edge_out* rows, uint32_t n, uint64_t k, bool* equal) {
   uint32_t lo = 0, hi = n;
   while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (row_key_of(rows + mid) < k) lo = mid + 1; else hi = mid; }
@@ -437,7 +429,7 @@ static int drop_window(alz_handle* h, bool* lost, bool at_e) {
   alz_comm_state* c = h->comm;
   cudaStream_t s = h->stream;
   const unsigned grid = (unsigned)h->sms * 4;
-  CK(cudaMemsetAsync(c->d_info, 0, sizeof(MergeInfo), s));
+  CK(cudaMemsetAsync(c->d_info, 0, offsetof(MergeInfo, clk), s));   // E's clock stays (alz_internal_merged_clock)
   if (at_e && h->n_live) {
     sum_counts_kernel<<<grid, 256, 0, s>>>(c->d_send + 1, h->n_live, c->d_info);
     consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], h->n_live);
@@ -529,6 +521,8 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
 // enters the collective whatever its own status, so nobody is left waiting in NCCL, and all ranks return the
 // same status. Under a window clock the header carries the rank's clock, and *roll says whether the flush closes
 // this rank's window (see kAtE / kKeep / kOpenNext).
+const uint64_t* alz_internal_merged_clock(alz_handle* h) { return reinterpret_cast<const uint64_t*>(&h->comm->d_info->clk); }
+
 int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost, bool* roll) {
   alz_comm_state* c = h->comm;
   const int R = h->comm_nranks;

@@ -86,6 +86,45 @@ __host__ __device__ __forceinline__ void unpack_edge_key(uint64_t k, uint8_t* fr
   else      { *from_type = ot; *from = other; *to_type = ALZ_NODE_POD; *to = pod; }
 }
 
+// packed edge key of an output row (inverse of unpack_edge_key)
+__device__ __forceinline__ uint64_t row_key_of(const alz_edge_out* r) {
+  // rows are 296 bytes apart: 8-byte aligned only
+  const uint2 ty = reinterpret_cast<const uint2*>(r)[0];   // from_type, to_type, pad | pad
+  const uint2 ft_ = reinterpret_cast<const uint2*>(r)[1];  // from | to
+  const uint32_t ft = ty.x & 0xFFu, tt = (ty.x >> 8) & 0xFFu;
+  if (ft == ALZ_NODE_POD) return ((uint64_t)tt << 61) | ((uint64_t)(ft_.x & 0x1FFFFFFFu) << 32) | ft_.y;
+  return (1ull << 63) | ((uint64_t)ft << 61) | ((uint64_t)(ft_.y & 0x1FFFFFFFu) << 32) | ft_.x;
+}
+// the fixed part of an output row and the lane's 8 histogram cells (hist sits at byte 40 of a 296-byte row:
+// 8-byte aligned only)
+__device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uint64_t key, const uint32_t (&c)[8],
+                                               uint64_t count, uint64_t err5xx, uint64_t lat_sum) {
+  uint2* d2 = reinterpret_cast<uint2*>(&o->hist[sl * 8u]);
+  d2[0] = make_uint2(c[0], c[1]); d2[1] = make_uint2(c[2], c[3]);
+  d2[2] = make_uint2(c[4], c[5]); d2[3] = make_uint2(c[6], c[7]);
+  if (sl == 0) {
+    uint8_t ft, tt; uint32_t f, t;
+    unpack_edge_key(key, &ft, &f, &tt, &t);
+    o->from_type = ft; o->to_type = tt;
+    for (int k = 0; k < 6; ++k) o->_pad[k] = 0;
+    o->from = f; o->to = t;
+    o->count = count;
+    o->err5xx = err5xx;
+    o->lat_sum_ns = lat_sum;
+  }
+}
+
+// the lane's part of an output row, the layout edge_row_load gives an edge-table row: 8 histogram cells, and in lane 0
+// the row's count, latency and 5xx sums (0 in the other lanes)
+__device__ __forceinline__ void load_edge_out(const alz_edge_out* r, uint32_t sl, uint32_t (&c)[8], uint64_t& count,
+                                              uint64_t& lat, uint64_t& e5) {
+  const uint2* s2 = reinterpret_cast<const uint2*>(&r->hist[sl * 8u]);
+  const uint2 a = s2[0], b = s2[1], d = s2[2], e = s2[3];
+  c[0] = a.x; c[1] = a.y; c[2] = b.x; c[3] = b.y; c[4] = d.x; c[5] = d.y; c[6] = e.x; c[7] = e.y;
+  count = 0; lat = 0; e5 = 0;
+  if (sl == 0) { count = r->count; lat = r->lat_sum_ns; e5 = r->err5xx; }
+}
+
 // ---- per-record rules ------------------------------------------------------------
 // Does processL7 hand a row to PersistRequest for this record (before resolve)?
 __host__ __device__ __forceinline__ bool emits_request_row(uint32_t protocol, uint32_t method_flags) {

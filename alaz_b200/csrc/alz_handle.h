@@ -29,6 +29,7 @@ struct HostEp {
 struct alz_gnn_state;   // alz_gnn.cu
 struct alz_sock_state;  // alz_sock.cu
 struct alz_comm_state;  // alz_comm.cu
+struct alz_rollup_state;  // alz_rollup.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -117,6 +118,7 @@ struct alz_handle {
   uint64_t merge_lost_events = 0;         // events of this rank's rows that a merge left out (merged graph > max_edges)
   alz_gnn_state* gnn = nullptr;
   alz_sock_state* sock = nullptr;
+  alz_rollup_state* roll = nullptr;       // rolling windows (alz_window_history); null = off
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -129,6 +131,13 @@ int alz_internal_ingest(alz_handle* h, const alz_l7_rec* d_recs, size_t n);
 // merged rows are in h->d_out; any other status: the window is kept. *roll (with ALZ_OK): the flush closes this
 // rank's time-cut window; false: the rank is ahead of the ranks' merged epoch, or no rank has one, and keeps it.
 int alz_internal_merge_ranks(alz_handle* h, int local_rc, bool* lost, bool* roll);
+// device WinClock of the epoch E the last merge closed (ready 0 when no rank had an epoch); valid after a merge
+const uint64_t* alz_internal_merged_clock(alz_handle* h);
+// Rolling windows: the window a flush has just consumed (h->last_n_edges rows in h->d_out, h->windows counted) becomes
+// the newest entry of the history. d_clk: the device WinClock of the epoch it closed, read in stream order, so before
+// the flush's roll advances it; null without a window clock. Nothing happens with the history off. Caller holds h->mu.
+int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk);
+void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -306,25 +306,6 @@ __global__ void scatter_heads_kernel(const uint64_t* __restrict__ sorted, const 
     if (flags[i]) out[pos[i]] = sorted[i];
 }
 
-// the fixed part of an output row and the lane's 8 histogram cells (hist sits at byte 40 of a 296-byte row:
-// 8-byte aligned only)
-__device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uint64_t key, const uint32_t (&c)[8],
-                                               uint64_t count, uint64_t err5xx, uint64_t lat_sum) {
-  uint2* d2 = reinterpret_cast<uint2*>(&o->hist[sl * 8u]);
-  d2[0] = make_uint2(c[0], c[1]); d2[1] = make_uint2(c[2], c[3]);
-  d2[2] = make_uint2(c[4], c[5]); d2[3] = make_uint2(c[6], c[7]);
-  if (sl == 0) {
-    uint8_t ft, tt; uint32_t f, t;
-    unpack_edge_key(key, &ft, &f, &tt, &t);
-    o->from_type = ft; o->to_type = tt;
-    for (int k = 0; k < 6; ++k) o->_pad[k] = 0;
-    o->from = f; o->to = t;
-    o->count = count;
-    o->err5xx = err5xx;
-    o->lat_sum_ns = lat_sum;
-  }
-}
-
 // multi-rank flush: the live edge rows, as they are, into the send buffer (the window stays in the table until
 // every rank has taken part in the merge, alz_comm.cu)
 __global__ void __launch_bounds__(256) gather_edges_kernel(EdgeTable edges, const uint64_t* __restrict__ keys,

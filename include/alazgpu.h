@@ -282,6 +282,39 @@ int alz_window_clock(alz_handle* h, uint64_t first_kernel_ns, uint64_t first_use
 /* epoch of the open window; ALZ_E_STATE until the first record has been submitted */
 int alz_window_epoch(alz_handle* h, uint64_t* epoch);
 
+/* ---- rolling windows (docs/SPEC.md §12) -------------------------------------------
+ * Keep the rows of the last `depth` flushed windows on the device, in an arena of `arena_rows` alz_edge_out
+ * rows (296 B each). depth = 0 turns the history off and frees it. A call with other values than the current
+ * ones drops what is retained; a call with the current values changes nothing. Off by default.
+ * Every flush that consumes its window appends that window's rows (what alz_window_fetch would return), also a
+ * window of 0 rows and one returned with ALZ_E_CAPACITY; a flush that keeps its window appends nothing. Appending
+ * evicts the oldest windows until at most `depth` remain and the rows fit; a window with more rows than the
+ * arena clears the history and is not retained. arena_rows >= 2^31 (or 0 with depth > 0): ALZ_E_INVAL; no
+ * memory: ALZ_E_NOMEM and the history is off. */
+int alz_window_history(alz_handle* h, uint32_t depth, uint64_t arena_rows);
+
+typedef struct alz_rollup_info {
+  uint32_t windows;        /* windows summed: min(k, retained) */
+  uint32_t clocked;        /* 1: every summed window was cut by alz_window_clock and the epochs below are set */
+  uint64_t window_first;   /* alz_stats.windows as it was after the oldest / newest summed window's flush */
+  uint64_t window_last;
+  uint64_t epoch_first;    /* the epochs those flushes closed (several ranks: the merged epoch E) */
+  uint64_t epoch_last;
+  uint64_t rows_in;        /* rows read: the sum of the summed windows' row counts */
+} alz_rollup_info;
+
+/* The last k retained windows added up per edge: count, err5xx, lat_sum_ns mod 2^64, hist cells mod 2^32, in
+ * ascending packed-key order: what one window holding those windows' events would have returned. Rows are
+ * matched by (from_type, from, to_type, to), that is by the CALLER'S ids: a pod or service id that was given
+ * to another UID inside the retained span merges the two nodes into one. The number of rows is not bounded by
+ * max_edges. Reads only: the open window, the last flushed window (alz_window_fetch, alz_gnn_score) and the
+ * history are unchanged. *n_out = rows of the sum; cap too small: ALZ_E_CAPACITY, nothing written, call again.
+ * ALZ_E_STATE without a history; ALZ_E_INVAL for k = 0. info may be NULL. */
+int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, size_t cap, size_t* n_out, alz_rollup_info* info);
+/* same, rows left on the device; valid until the next rollup or alz_window_history on this handle */
+int alz_window_rollup_device(alz_handle* h, uint32_t k, const alz_edge_out** dev_rows, size_t* n_out,
+                             alz_rollup_info* info);
+
 /* ---- GNN anomaly pass over the last flushed window (docs/SPEC.md §6) -------- */
 int alz_gnn_score(alz_handle* h, float* edge_scores, size_t cap, size_t* n_out);
 /* same, scores left on the device (valid until the next call on this handle) */
