@@ -109,6 +109,22 @@ class RollupInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+MAX_TIERS = 4
+
+
+class HistoryTier(C.Structure):
+    """alz_history_tier."""
+    _fields_ = [("factor", C.c_uint32), ("depth", C.c_uint32), ("arena_rows", C.c_uint64), ("block_rows", C.c_uint64)]
+
+
+class TierState(C.Structure):
+    """alz_tier_state."""
+    _fields_ = [("entries", C.c_uint32), ("open_windows", C.c_uint32), ("dropped", C.c_uint64)]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SockStats(C.Structure):
     """alz_sock_stats_t."""
     _fields_ = [(n, C.c_uint64) for n in ("lines", "pool_records", "pool_garbage", "syncs", "sync_ops", "sync_bytes",

@@ -24,6 +24,7 @@ EXPORTS = [
     "alz_submit_l7_packed", "alz_submit_l7_packed_device", "alz_pack_l7",
     "alz_submit_l7_raw", "alz_window_flush", "alz_window_flush_device", "alz_window_fetch", "alz_get_stats",
     "alz_window_clock", "alz_window_epoch", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
+    "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device", "alz_window_tier_state",
     "alz_gnn_score",
     "alz_gnn_score_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
@@ -65,6 +66,10 @@ def load(rebuild=False):
         "alz_window_history": ([vp, u32, u64], i),
         "alz_window_rollup": ([vp, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
         "alz_window_rollup_device": ([vp, u32, pp, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
+        "alz_window_history_tiers": ([vp, C.POINTER(abi.HistoryTier), u32], i),
+        "alz_window_rollup_tier": ([vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
+        "alz_window_rollup_tier_device": ([vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
+        "alz_window_tier_state": ([vp, u32, C.POINTER(abi.TierState)], i),
         "alz_pinned_alloc_local": ([vp, sz, pp], i),
         "alz_window_flush": ([vp, vp, sz, C.POINTER(sz)], i),
         "alz_window_flush_device": ([vp, pp, C.POINTER(sz)], i),
@@ -103,7 +108,9 @@ def load(rebuild=False):
         for k in ("alz_submit_l7_packed", "alz_submit_l7_packed_device", "alz_pack_l7", "alz_window_fetch",
                   "alz_pinned_alloc_local", "alz_table_upsert_batch", "alz_window_clock", "alz_window_epoch",
                   "alz_sock_lookup_at", "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats",
-                  "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device"):
+                  "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
+                  "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device",
+                  "alz_window_tier_state"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -324,6 +331,40 @@ class Handle:
         self._ck(self.L.alz_window_rollup_device(self.h, int(k), C.byref(p), C.byref(n), C.byref(info)),
                  "alz_window_rollup_device")
         return p.value, n.value, info.as_dict()
+
+    # ---- tiered history (alz_rollup.cu, docs/SPEC.md §13)
+    def window_history_tiers(self, tiers):
+        """tiers: a list of (factor, depth, arena_rows, block_rows), tier 1 first; [] turns the tiers off."""
+        arr = (abi.HistoryTier * max(len(tiers), 1))(*[abi.HistoryTier(*map(int, t)) for t in tiers])
+        self._ck(self.L.alz_window_history_tiers(self.h, arr, len(tiers)), "alz_window_history_tiers")
+
+    def rollup_tier(self, tier, k, cap=None):
+        """alz_window_rollup_tier: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
+        info = abi.RollupInfo()
+        n = C.c_size_t(0)
+        if cap is None:
+            if self._ck(self.L.alz_window_rollup_tier(self.h, int(tier), int(k), None, 0, C.byref(n), C.byref(info)),
+                        "alz_window_rollup_tier", allow=(abi.E_CAPACITY,)) == 0:
+                return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
+            cap = n.value
+        out = np.zeros(cap, dtype=abi.EDGE_OUT)
+        self._ck(self.L.alz_window_rollup_tier(self.h, int(tier), int(k), _ptr(out), cap, C.byref(n), C.byref(info)),
+                 "alz_window_rollup_tier")
+        return out[: n.value].copy(), info.as_dict()
+
+    def rollup_tier_device(self, tier, k):
+        """alz_window_rollup_tier_device: (device pointer, rows, info dict)."""
+        info = abi.RollupInfo()
+        p = C.c_void_p()
+        n = C.c_size_t(0)
+        self._ck(self.L.alz_window_rollup_tier_device(self.h, int(tier), int(k), C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_window_rollup_tier_device")
+        return p.value, n.value, info.as_dict()
+
+    def tier_state(self, tier):
+        st = abi.TierState()
+        self._ck(self.L.alz_window_tier_state(self.h, int(tier), C.byref(st)), "alz_window_tier_state")
+        return st.as_dict()
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -30,6 +30,7 @@ struct alz_gnn_state;   // alz_gnn.cu
 struct alz_sock_state;  // alz_sock.cu
 struct alz_comm_state;  // alz_comm.cu
 struct alz_rollup_state;  // alz_rollup.cu
+struct alz_tier_set;      // alz_rollup.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -119,6 +120,7 @@ struct alz_handle {
   alz_gnn_state* gnn = nullptr;
   alz_sock_state* sock = nullptr;
   alz_rollup_state* roll = nullptr;       // rolling windows (alz_window_history); null = off
+  alz_tier_set* tiers = nullptr;          // tiered history (alz_window_history_tiers); null = off
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -136,8 +138,10 @@ const uint64_t* alz_internal_merged_clock(alz_handle* h);
 // Rolling windows: the window a flush has just consumed (h->last_n_edges rows in h->d_out, h->windows counted) becomes
 // the newest entry of the history. d_clk: the device WinClock of the epoch it closed, read in stream order, so before
 // the flush's roll advances it; null without a window clock. Nothing happens with the history off. Caller holds h->mu.
+// With tiers configured the window is also the next input of tier 1 (docs/SPEC.md §13).
 int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk);
 void alz_internal_free_rollup(alz_handle* h);
+void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -1,5 +1,6 @@
 // alz_rollup.cu — rolling windows (docs/SPEC.md §12): the rows of the last flushed windows kept on the device, and
-// the sum of the last k of them as one edge list.
+// the sum of the last k of them as one edge list; and tiered history (docs/SPEC.md §13): every consumed window merged
+// into coarser blocks on the device, each closed block retained as an entry of its tier.
 //
 // Every accumulator of an output row is an integer sum (docs/SPEC.md §3), so the sum of k windows' rows per edge
 // is what one window holding those windows' events would have returned. The flush is left as it is: a flush that
@@ -7,6 +8,11 @@
 // A rollup has the shape of the single-rank flush (DESIGN.md §5.3) applied to output rows instead of pair rows:
 // packed key of every retained row -> radix sort of (key, arena row) -> the distinct keys -> eight lanes per output
 // row add up the key's run of source rows in registers and store the row once.
+//
+// A tier's open block is a sorted row list. Both it and its input (a flushed window, or a closed block of the tier
+// below) are strictly ascending by packed key, so feeding it is a 2-way merge that adds matching keys (DESIGN.md
+// §5.6): tier_match_kernel, an exclusive scan of the unmatched input rows, tier_merge_kernel. The block's row count
+// and overflow flag stay on the device; only a block that closes (once per `factor` inputs) is waited for.
 #include <algorithm>
 #include <deque>
 #include <new>
@@ -17,11 +23,55 @@
 using namespace alz;
 
 namespace {
-struct Entry {            // one retained window; host-side record of rows [first_row, first_row + n) of the arena
+struct Entry {            // one retained entry; host-side record of rows [first_row, first_row + n) of an arena
   uint64_t first_row, n;
-  uint64_t window;        // alz_stats.windows after its flush
-  uint32_t slot;          // its clock in d_clk
-  bool clocked;           // a window clock was set when it was flushed
+  uint64_t window_first;  // alz_stats.windows after the flush of the oldest / newest window it covers
+  uint64_t window_last;
+  uint32_t windows;       // flushed windows it covers (1 in the window history)
+  uint32_t slot;          // its clock(s) in the arena's clock array
+  bool clocked;           // a window clock was set at every covered window's flush
+};
+
+// The ring rule of docs/SPEC.md §12: where an entry of n rows goes in an arena of arena_rows rows that keeps at most
+// depth entries; evicts the oldest entries until it fits. The caller has checked n <= arena_rows.
+uint64_t ring_place(std::deque<Entry>& entries, uint32_t depth, uint64_t arena_rows, uint64_t n) {
+  // The entry goes behind the newest one, or to row 0 when it would pass the end (the rows skipped there are free
+  // again once the entries before them have gone). The oldest entries are evicted until at most depth - 1 remain
+  // and the place overlaps none of the rest.
+  for (;;) {
+    while (entries.size() >= depth) entries.pop_front();
+    uint64_t at = entries.empty() ? 0 : entries.back().first_row + entries.back().n;
+    if (at + n > arena_rows) at = 0;
+    bool overlaps = false;
+    for (const Entry& e : entries) overlaps |= at < e.first_row + e.n && e.first_row < at + n;
+    if (!overlaps) return at;
+    entries.pop_front();
+  }
+}
+
+// sort-based rollup scratch, sized by the number of source rows (which max_edges does not bound), grown on demand
+struct RollupScratch {
+  uint32_t cap_rows = 0;
+  uint64_t* d_keys[2] = {nullptr, nullptr};   // [cap_rows] packed keys of the source rows, unsorted / sorted
+  uint32_t* d_src[2] = {nullptr, nullptr};    // [cap_rows] their arena rows
+  uint64_t* d_ukeys = nullptr;                // [cap_rows] the distinct keys in order
+  void* d_tmp = nullptr;                      // CUB scratch of the sort, then of the scan
+  size_t tmp_bytes = 0;
+  alz_edge_out* d_sum = nullptr;              // the last rollup's rows
+  size_t sum_rows = 0;
+};
+
+// the clock of a tier's open block and of each of its entries: the oldest and newest covered window's clocks
+struct TierClk {
+  WinClock first, last;
+  uint64_t unready;   // some covered window's clock was not ready (no open epoch)
+};
+// device state of a tier's open block
+struct TierOpen {
+  TierClk clk;
+  uint32_t count[2];  // rows in block buffer 0 / 1
+  uint32_t overflow;  // the open block would have passed block_rows: it is dropped when it closes
+  uint32_t _pad;
 };
 }  // namespace
 
@@ -33,15 +83,42 @@ struct alz_rollup_state {
   std::vector<WinClock> h_clk;
   std::deque<Entry> entries;          // oldest first: a contiguous run of the most recent consumed windows
   uint64_t appended = 0;              // entries ever appended: the next one's clock slot is appended % depth
-  // rollup scratch, sized by the number of source rows (which max_edges does not bound), grown on demand
-  uint32_t cap_rows = 0;
-  uint64_t* d_keys[2] = {nullptr, nullptr};   // [cap_rows] packed keys of the source rows, unsorted / sorted
-  uint32_t* d_src[2] = {nullptr, nullptr};    // [cap_rows] their arena rows
-  uint64_t* d_ukeys = nullptr;                // [cap_rows] the distinct keys in order
-  void* d_tmp = nullptr;                      // CUB scratch of the sort, then of the scan
+  RollupScratch sc;
+};
+
+namespace {
+struct Tier {
+  alz_history_tier cfg{};
+  alz_edge_out* d_arena = nullptr;    // [arena_rows] the retained entries, a ring in rows
+  TierClk* d_clk = nullptr;           // [depth] each entry's clocks
+  std::vector<TierClk> h_clk;
+  std::deque<Entry> entries;
+  uint64_t appended = 0;
+  alz_edge_out* d_block[2] = {nullptr, nullptr};   // [block_rows] the open block, ping-pong
+  uint64_t* d_bkeys[2] = {nullptr, nullptr};       // [block_rows] its packed keys
+  int cur = 0;                        // the buffer that holds the open block
+  uint32_t inputs = 0;                // inputs merged into the open block
+  uint64_t window_first = 0;          // alz_stats.windows of the open block's oldest window
+  bool clocked = true;                // every input so far was clocked
+  bool poisoned = false;              // the open block would contain a dropped block of a tier below
+  uint64_t dropped = 0;
+  uint32_t windows_per_input = 1;     // flushed windows one input covers
+};
+}  // namespace
+
+struct alz_tier_set {
+  std::vector<Tier> tiers;            // tiers 1..n
+  TierOpen* d_open = nullptr;         // [n]
+  // merge scratch, for an input of up to max_in rows
+  uint32_t max_in = 0;
+  uint64_t* d_ikeys = nullptr;        // [max_in] packed keys of the input rows
+  uint32_t* d_pos = nullptr;          // [max_in] insertion point of each input row in the block
+  uint32_t* d_unm = nullptr;          // [max_in + 1] 1: the input row's key is not in the block
+  uint32_t* d_scan = nullptr;         // [max_in + 1] exclusive scan of d_unm
+  void* d_tmp = nullptr;
   size_t tmp_bytes = 0;
-  alz_edge_out* d_sum = nullptr;              // the last rollup's rows
-  size_t sum_rows = 0;
+  TierOpen h_open{};                  // host copy of the closing tier's TierOpen
+  RollupScratch sc;
 };
 
 // keys[i], src[i] = packed edge key and arena row of source row first_row + i (16 of the row's 296 bytes are read)
@@ -87,19 +164,101 @@ __global__ void __launch_bounds__(256) rollup_emit_kernel(const alz_edge_out* __
   }
 }
 
-static void free_scratch(alz_rollup_state* st) {
-  cudaFree(st->d_keys[0]); cudaFree(st->d_tmp);
-  st->d_keys[0] = st->d_keys[1] = st->d_ukeys = nullptr;
-  st->d_src[0] = st->d_src[1] = nullptr;
-  st->d_tmp = nullptr;
-  st->cap_rows = 0; st->tmp_bytes = 0;
+// Step 1 of merging n input rows into a tier's open block (bkeys, open->count[cur] rows): for every input row j its
+// packed key, its insertion point in the block and whether the block lacks its key (unm[n] = 0 closes the scan).
+// Thread 0 also carries the input's clocks into the open block's: clk_first / clk_last are the input's oldest and
+// newest window clock, clk_unready its unready flag (null: the input is one window, unready when its clock is not).
+__global__ void __launch_bounds__(256) tier_match_kernel(const alz_edge_out* __restrict__ in,
+                                                         const uint64_t* __restrict__ in_keys, uint32_t n,
+                                                         const uint64_t* __restrict__ bkeys, TierOpen* open, int cur,
+                                                         uint64_t* __restrict__ ikeys, uint32_t* __restrict__ pos,
+                                                         uint32_t* __restrict__ unm, const WinClock* clk_first,
+                                                         const WinClock* clk_last, const uint64_t* clk_unready,
+                                                         bool first_input) {
+  const uint32_t n_b = open->count[cur];
+  const uint32_t stride = gridDim.x * blockDim.x;
+  const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t j = t0; j < n; j += stride) {
+    const uint64_t key = in_keys ? in_keys[j] : row_key_of(in + j);
+    const uint32_t p = lower_bound_u64(bkeys, n_b, key);
+    ikeys[j] = key;
+    pos[j] = p;
+    unm[j] = (p < n_b && bkeys[p] == key) ? 0u : 1u;
+  }
+  if (t0 == 0) {
+    unm[n] = 0u;
+    if (clk_first) {
+      const uint64_t u = clk_unready ? *clk_unready : (uint64_t)(clk_last->ready == 0ull);
+      if (first_input) { open->clk.first = *clk_first; open->clk.unready = 0ull; }
+      open->clk.last = *clk_last;
+      open->clk.unready |= u;
+    }
+  }
+}
+
+// Step 2: the merged block into the other buffer, each output row written once by eight lanes. scan = exclusive scan
+// of unm, so scan[n] input rows are new. Block row i goes to i + (new input rows before its key), and adds the input
+// row with its key if there is one; new input row j goes to pos[j] + scan[j]. A block that would pass block_rows is
+// flagged and left empty: it is dropped when it closes. Bounds come from the device; the grid from the host's bound.
+__global__ void __launch_bounds__(256) tier_merge_kernel(const alz_edge_out* __restrict__ blk,
+                                                         const uint64_t* __restrict__ bkeys, TierOpen* open, int cur,
+                                                         const alz_edge_out* __restrict__ in,
+                                                         const uint64_t* __restrict__ ikeys,
+                                                         const uint32_t* __restrict__ pos,
+                                                         const uint32_t* __restrict__ unm,
+                                                         const uint32_t* __restrict__ scan, uint32_t n,
+                                                         uint32_t block_rows, alz_edge_out* __restrict__ out,
+                                                         uint64_t* __restrict__ okeys) {
+  const uint32_t n_b = open->count[cur];
+  const uint32_t total = n_b + scan[n];
+  const bool over = open->overflow != 0u || total > block_rows;
+  const uint32_t t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  if (over) {
+    if (t0 == 0) { open->overflow = 1u; open->count[cur ^ 1] = 0u; }
+    return;
+  }
+  if (t0 == 0) open->count[cur ^ 1] = total;
+  const uint32_t sl = threadIdx.x & 7u;
+  const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
+  for (uint32_t g = t0 >> 3; g < n_b + n; g += groups_per_grid) {
+    uint32_t c[8];
+    uint64_t count, lat, e5, key;
+    uint32_t o;
+    if (g < n_b) {
+      key = bkeys[g];
+      const uint32_t p = lower_bound_u64(ikeys, n, key);
+      o = g + scan[p];
+      load_edge_out(blk + g, sl, c, count, lat, e5);
+      if (p < n && ikeys[p] == key) {
+        uint32_t rc[8];
+        uint64_t r_count, r_lat, r_e5;
+        load_edge_out(in + p, sl, rc, r_count, r_lat, r_e5);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) c[q] += rc[q];
+        count += r_count; lat += r_lat; e5 += r_e5;
+      }
+    } else {
+      const uint32_t j = g - n_b;
+      if (!unm[j]) continue;
+      key = ikeys[j];
+      o = pos[j] + scan[j];
+      load_edge_out(in + j, sl, c, count, lat, e5);
+    }
+    store_edge_out(&out[o], sl, key, c, count, e5, lat);
+    if (sl == 0) okeys[o] = key;
+  }
+}
+
+static void free_scratch(RollupScratch& sc) {
+  cudaFree(sc.d_keys[0]); cudaFree(sc.d_tmp); cudaFree(sc.d_sum);
+  sc = RollupScratch{};
 }
 
 void alz_internal_free_rollup(alz_handle* h) {
   alz_rollup_state* st = h->roll;
   if (!st) return;
-  free_scratch(st);
-  cudaFree(st->d_arena); cudaFree(st->d_clk); cudaFree(st->d_sum);
+  free_scratch(st->sc);
+  cudaFree(st->d_arena); cudaFree(st->d_clk);
   delete st;
   h->roll = nullptr;
 }
@@ -127,90 +286,90 @@ extern "C" int alz_window_history(alz_handle* h, uint32_t depth, uint64_t arena_
   return ALZ_OK;
 }
 
-int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk) {
+static int tiers_input_window(alz_handle* h, const uint64_t* d_clk);
+
+// the window a flush has just consumed becomes the newest entry of the window history (docs/SPEC.md §12)
+static int window_history_append(alz_handle* h, const uint64_t* d_clk) {
   alz_rollup_state* st = h->roll;
-  if (!st) return ALZ_OK;
   const uint64_t n = h->last_n_edges;
   if (n > st->arena_rows) { st->entries.clear(); return ALZ_OK; }   // not retained, and the run would have a gap
-  // The arena is a ring in rows: the entry goes behind the newest one, or to row 0 when it would pass the end (the
-  // rows skipped there are free again once the entries before them have gone). The oldest entries are evicted
-  // until at most depth - 1 remain and the place overlaps none of the rest.
-  uint64_t at = 0;
-  for (;;) {
-    while (st->entries.size() >= st->depth) st->entries.pop_front();
-    at = st->entries.empty() ? 0 : st->entries.back().first_row + st->entries.back().n;
-    if (at + n > st->arena_rows) at = 0;
-    bool overlaps = false;
-    for (const Entry& e : st->entries) overlaps |= at < e.first_row + e.n && e.first_row < at + n;
-    if (!overlaps) break;
-    st->entries.pop_front();
-  }
+  const uint64_t at = ring_place(st->entries, st->depth, st->arena_rows, n);
   const uint32_t slot = (uint32_t)(st->appended++ % st->depth);
   if (n) CK(cudaMemcpyAsync(st->d_arena + at, h->d_out, (size_t)n * sizeof(alz_edge_out), cudaMemcpyDeviceToDevice, h->stream));
   if (d_clk) CK(cudaMemcpyAsync(st->d_clk + slot, d_clk, sizeof(WinClock), cudaMemcpyDeviceToDevice, h->stream));
-  st->entries.push_back(Entry{at, n, h->windows, slot, d_clk != nullptr});
+  st->entries.push_back(Entry{at, n, h->windows, h->windows, 1u, slot, d_clk != nullptr});
   return ALZ_OK;
 }
 
-// scratch for n source rows
-static int ensure_scratch(alz_handle* h, alz_rollup_state* st, uint32_t n) {
-  if (n <= st->cap_rows) return ALZ_OK;
+// The window history and the tiers each take the window whatever happens to the other.
+int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk) {
+  const int rc0 = h->roll ? window_history_append(h, d_clk) : ALZ_OK;
+  const int rc1 = h->tiers ? tiers_input_window(h, d_clk) : ALZ_OK;
+  return rc0 != ALZ_OK ? rc0 : rc1;
+}
+
+// scratch for n source rows of an arena of arena_rows rows
+static int ensure_scratch(alz_handle* h, RollupScratch& sc, uint64_t arena_rows, uint32_t n) {
+  if (n <= sc.cap_rows) return ALZ_OK;
   CK(cudaStreamSynchronize(h->stream));
-  free_scratch(st);
-  const uint32_t cap = (uint32_t)std::min<uint64_t>(st->arena_rows + 63u, ((uint64_t)n + n / 2u + 63u)) & ~63u;   // regions stay 256-byte aligned
+  cudaFree(sc.d_keys[0]); cudaFree(sc.d_tmp);
+  sc.d_keys[0] = sc.d_keys[1] = sc.d_ukeys = nullptr;
+  sc.d_src[0] = sc.d_src[1] = nullptr;
+  sc.d_tmp = nullptr;
+  sc.cap_rows = 0; sc.tmp_bytes = 0;
+  const uint32_t cap = (uint32_t)std::min<uint64_t>(arena_rows + 63u, ((uint64_t)n + n / 2u + 63u)) & ~63u;   // regions stay 256-byte aligned
   const size_t tmp = std::max(sort_pairs_temp_bytes(cap), scan_temp_bytes(cap));
   char* base = nullptr;
-  if (cudaMalloc(&base, (size_t)cap * 32u) != cudaSuccess || cudaMalloc(&st->d_tmp, tmp) != cudaSuccess) {
+  if (cudaMalloc(&base, (size_t)cap * 32u) != cudaSuccess || cudaMalloc(&sc.d_tmp, tmp) != cudaSuccess) {
     h->last_err = std::string("alz_window_rollup scratch: ") + cudaGetErrorString(cudaGetLastError());
     cudaFree(base);
-    st->d_tmp = nullptr;
+    sc.d_tmp = nullptr;
     return ALZ_E_NOMEM;
   }
-  st->d_keys[0] = (uint64_t*)base;
-  st->d_keys[1] = st->d_keys[0] + cap;
-  st->d_ukeys = st->d_keys[1] + cap;
-  st->d_src[0] = (uint32_t*)(st->d_ukeys + cap);
-  st->d_src[1] = st->d_src[0] + cap;
-  st->cap_rows = cap;
-  st->tmp_bytes = tmp;
+  sc.d_keys[0] = (uint64_t*)base;
+  sc.d_keys[1] = sc.d_keys[0] + cap;
+  sc.d_ukeys = sc.d_keys[1] + cap;
+  sc.d_src[0] = (uint32_t*)(sc.d_ukeys + cap);
+  sc.d_src[1] = sc.d_src[0] + cap;
+  sc.cap_rows = cap;
+  sc.tmp_bytes = tmp;
   return ALZ_OK;
 }
 
-// The sum of the last k entries into st->d_sum; *n_out rows. Caller holds h->mu and has set the device.
-static int rollup_locked(alz_handle* h, uint32_t k, size_t* n_out, alz_rollup_info* info) {
-  alz_rollup_state* st = h->roll;
-  if (!st) return ALZ_E_STATE;
-  if (k == 0) return ALZ_E_INVAL;
+// The sum of entries [first, end) of an arena into sc.d_sum; *n_out rows. The host clocks are copied from d_clk
+// (clk_bytes) into h_clk in stream order, so they are read when this returns. Caller holds h->mu and has set the
+// device.
+static int sum_entries(alz_handle* h, RollupScratch& sc, const alz_edge_out* d_arena, uint64_t arena_rows,
+                       const std::deque<Entry>& entries, size_t first, void* h_clk, const void* d_clk,
+                       size_t clk_bytes, size_t* n_out) {
   cudaStream_t s = h->stream;
-  const size_t m = std::min<size_t>(k, st->entries.size());
-  const size_t first = st->entries.size() - m;
   uint64_t n_src = 0;
-  for (size_t i = first; i < st->entries.size(); ++i) n_src += st->entries[i].n;
+  for (size_t i = first; i < entries.size(); ++i) n_src += entries[i].n;
   const uint32_t n = (uint32_t)n_src;   // at most arena_rows: the entries do not overlap
   uint32_t n_sum = 0;
-  CK(cudaMemcpyAsync(st->h_clk.data(), st->d_clk, (size_t)st->depth * sizeof(WinClock), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(h_clk, d_clk, clk_bytes, cudaMemcpyDeviceToHost, s));
   if (n) {
-    int rc = ensure_scratch(h, st, n);
+    int rc = ensure_scratch(h, sc, arena_rows, n);
     if (rc != ALZ_OK) return rc;
     // entries that follow one another in the arena (all of them, or all but one jump back to row 0) take one launch
     const unsigned grid = (unsigned)h->sms * 4u;
     uint32_t done = 0;
-    for (size_t i = first; i < st->entries.size();) {
-      const uint64_t run_first = st->entries[i].first_row;
+    for (size_t i = first; i < entries.size();) {
+      const uint64_t run_first = entries[i].first_row;
       uint64_t run_n = 0;
-      for (; i < st->entries.size() && st->entries[i].first_row == run_first + run_n; ++i) run_n += st->entries[i].n;
+      for (; i < entries.size() && entries[i].first_row == run_first + run_n; ++i) run_n += entries[i].n;
       if (run_n == 0) continue;
-      rollup_keys_kernel<<<grid, 256, 0, s>>>(st->d_arena, (uint32_t)run_first, (uint32_t)run_n, st->d_keys[0] + done,
-                                              st->d_src[0] + done);
+      rollup_keys_kernel<<<grid, 256, 0, s>>>(d_arena, (uint32_t)run_first, (uint32_t)run_n, sc.d_keys[0] + done,
+                                              sc.d_src[0] + done);
       h->launches += 1;
       done += (uint32_t)run_n;
     }
-    sort_pairs(st->d_tmp, st->tmp_bytes, st->d_keys[0], st->d_keys[1], st->d_src[0], st->d_src[1], n, s);
+    sort_pairs(sc.d_tmp, sc.tmp_bytes, sc.d_keys[0], sc.d_keys[1], sc.d_src[0], sc.d_src[1], n, s);
     // the unsorted keys are done with: their buffer takes the head flags and their scan. No row of a flush has the
     // key that equals the free marker (alz_device.cuh, EdgeTable), which launch_unique_sorted never takes as a head.
-    uint32_t* flags = reinterpret_cast<uint32_t*>(st->d_keys[0]);
-    uint32_t* pos = flags + st->cap_rows;
-    launch_unique_sorted(st->d_keys[1], n, flags, pos, st->d_ukeys, st->d_tmp, st->tmp_bytes, h->sms, s);
+    uint32_t* flags = reinterpret_cast<uint32_t*>(sc.d_keys[0]);
+    uint32_t* pos = flags + sc.cap_rows;
+    launch_unique_sorted(sc.d_keys[1], n, flags, pos, sc.d_ukeys, sc.d_tmp, sc.tmp_bytes, h->sms, s);
     h->launches += 2;
     CK(cudaGetLastError());
     uint32_t last[2];
@@ -218,41 +377,61 @@ static int rollup_locked(alz_handle* h, uint32_t k, size_t* n_out, alz_rollup_in
     CK(cudaMemcpyAsync(&last[1], flags + (n - 1), 4, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));   // the one count the host needs, as a flush needs its edge count
     n_sum = last[0] + last[1];
-    if (n_sum > st->sum_rows) {
-      cudaFree(st->d_sum);
-      st->d_sum = nullptr;
-      st->sum_rows = 0;
-      const size_t want = std::min<size_t>(st->arena_rows, (size_t)n_sum + n_sum / 2u);
-      if (cudaMalloc(&st->d_sum, want * sizeof(alz_edge_out)) != cudaSuccess) {
+    if (n_sum > sc.sum_rows) {
+      cudaFree(sc.d_sum);
+      sc.d_sum = nullptr;
+      sc.sum_rows = 0;
+      const size_t want = std::min<size_t>(arena_rows, (size_t)n_sum + n_sum / 2u);
+      if (cudaMalloc(&sc.d_sum, want * sizeof(alz_edge_out)) != cudaSuccess) {
         h->last_err = std::string("alz_window_rollup rows: ") + cudaGetErrorString(cudaGetLastError());
         return ALZ_E_NOMEM;
       }
-      st->sum_rows = want;
+      sc.sum_rows = want;
     }
-    rollup_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(st->d_arena, st->d_keys[1], st->d_src[1], n, st->d_ukeys,
-                                                             n_sum, st->d_sum);
+    rollup_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(d_arena, sc.d_keys[1], sc.d_src[1], n, sc.d_ukeys,
+                                                             n_sum, sc.d_sum);
     h->launches += 1;
     CK(cudaGetLastError());
   } else {
     CK(cudaStreamSynchronize(s));
   }
   *n_out = n_sum;
+  return ALZ_OK;
+}
+
+// what a rollup of entries [first, end) covers, apart from the epochs
+static void fill_info(const std::deque<Entry>& entries, size_t first, alz_rollup_info* info) {
+  *info = alz_rollup_info{};
+  for (size_t i = first; i < entries.size(); ++i) {
+    info->windows += entries[i].windows;
+    info->rows_in += entries[i].n;
+  }
+  if (first < entries.size()) {
+    info->window_first = entries[first].window_first;
+    info->window_last = entries.back().window_last;
+  }
+}
+
+// The sum of the last k window-history entries into st->sc.d_sum; *n_out rows. Caller holds h->mu and has set the device.
+static int rollup_locked(alz_handle* h, uint32_t k, size_t* n_out, alz_rollup_info* info) {
+  alz_rollup_state* st = h->roll;
+  if (!st) return ALZ_E_STATE;
+  if (k == 0) return ALZ_E_INVAL;
+  const size_t m = std::min<size_t>(k, st->entries.size());
+  const size_t first = st->entries.size() - m;
+  const int rc = sum_entries(h, st->sc, st->d_arena, st->arena_rows, st->entries, first, st->h_clk.data(), st->d_clk,
+                             (size_t)st->depth * sizeof(WinClock), n_out);
+  if (rc != ALZ_OK) return rc;
   if (info) {
-    *info = alz_rollup_info{};
-    info->windows = (uint32_t)m;
-    info->rows_in = n_src;
+    fill_info(st->entries, first, info);
     if (m) {
-      const Entry& a = st->entries[first];
-      const Entry& b = st->entries.back();
-      info->window_first = a.window;
-      info->window_last = b.window;
       bool clocked = true;
       for (size_t i = first; i < st->entries.size(); ++i)
         clocked &= st->entries[i].clocked && st->h_clk[st->entries[i].slot].ready != 0ull;
       if (clocked) {
         info->clocked = 1u;
-        info->epoch_first = st->h_clk[a.slot].epoch;
-        info->epoch_last = st->h_clk[b.slot].epoch;
+        info->epoch_first = st->h_clk[st->entries[first].slot].epoch;
+        info->epoch_last = st->h_clk[st->entries.back().slot].epoch;
       }
     }
   }
@@ -265,7 +444,7 @@ extern "C" int alz_window_rollup_device(alz_handle* h, uint32_t k, const alz_edg
   std::lock_guard<std::mutex> g(h->mu);
   CK(cudaSetDevice(h->device));
   const int rc = rollup_locked(h, k, n_out, info);
-  if (rc == ALZ_OK && dev_rows) *dev_rows = h->roll->d_sum;
+  if (rc == ALZ_OK && dev_rows) *dev_rows = h->roll->sc.d_sum;
   return rc;
 }
 
@@ -277,7 +456,245 @@ extern "C" int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, s
   const int rc = rollup_locked(h, k, n_out, info);
   if (rc != ALZ_OK) return rc;
   if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, h->roll->d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  if (*n_out) CK(cudaMemcpyAsync(out, h->roll->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
+  return ALZ_OK;
+}
+
+// ---- tiered history (docs/SPEC.md §13) ------------------------------------------------------------------------------
+
+void alz_internal_free_tiers(alz_handle* h) {
+  alz_tier_set* ts = h->tiers;
+  if (!ts) return;
+  for (Tier& t : ts->tiers) {
+    cudaFree(t.d_arena); cudaFree(t.d_clk); cudaFree(t.d_block[0]); cudaFree(t.d_block[1]);
+    cudaFree(t.d_bkeys[0]); cudaFree(t.d_bkeys[1]);
+  }
+  cudaFree(ts->d_open); cudaFree(ts->d_ikeys); cudaFree(ts->d_tmp);
+  free_scratch(ts->sc);
+  delete ts;
+  h->tiers = nullptr;
+}
+
+static bool same_tiers(const alz_tier_set* ts, const alz_history_tier* tiers, uint32_t n) {
+  if (!ts) return n == 0;
+  if (ts->tiers.size() != n) return false;
+  for (uint32_t i = 0; i < n; ++i) {
+    const alz_history_tier& a = ts->tiers[i].cfg;
+    if (a.factor != tiers[i].factor || a.depth != tiers[i].depth || a.arena_rows != tiers[i].arena_rows ||
+        a.block_rows != tiers[i].block_rows)
+      return false;
+  }
+  return true;
+}
+
+extern "C" int alz_window_history_tiers(alz_handle* h, const alz_history_tier* tiers, uint32_t n) {
+  if (!h || n > ALZ_MAX_TIERS || (n && !tiers)) return ALZ_E_INVAL;
+  uint64_t span = 1;                   // flushed windows one entry of tier i covers
+  for (uint32_t i = 0; i < n; ++i) {   // rows are indexed by u32, counted by int
+    const alz_history_tier& t = tiers[i];
+    if (t.factor < 2 || t.depth == 0 || t.arena_rows == 0 || t.arena_rows >= (1ull << 31) || t.block_rows == 0 ||
+        t.block_rows >= (1ull << 31))
+      return ALZ_E_INVAL;
+    // windows are counted in u32 (alz_rollup_info.windows, alz_tier_state.open_windows): the windows of all
+    // retained entries of a tier must stay below 2^32 (both factors are below 2^32, so the products fit in u64)
+    span *= t.factor;
+    if (span >= (1ull << 32) || span * t.depth >= (1ull << 32)) return ALZ_E_INVAL;
+  }
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  if (same_tiers(h->tiers, tiers, n)) return ALZ_OK;
+  CK(cudaStreamSynchronize(h->stream));   // merges, copies into the arenas and a rollup may still be running
+  alz_internal_free_tiers(h);
+  if (n == 0) return ALZ_OK;
+  alz_tier_set* ts = new (std::nothrow) alz_tier_set();
+  if (!ts) return ALZ_E_NOMEM;
+  h->tiers = ts;
+  ts->tiers.resize(n);
+  // an input of tier 1 is a flushed window (at most max_edges rows); of tier t + 1, a block of tier t
+  uint64_t max_in = h->cfg.max_edges;
+  uint32_t wpi = 1;
+  for (uint32_t i = 0; i < n; ++i) {
+    ts->tiers[i].cfg = tiers[i];
+    ts->tiers[i].windows_per_input = wpi;
+    wpi *= tiers[i].factor;
+    if (i + 1 < n) max_in = std::max<uint64_t>(max_in, tiers[i].block_rows);
+  }
+  ts->max_in = (uint32_t)max_in;
+  ts->tmp_bytes = scan_temp_bytes(ts->max_in + 1);
+  bool ok = cudaMalloc(&ts->d_open, n * sizeof(TierOpen)) == cudaSuccess &&
+            cudaMalloc(&ts->d_ikeys, (size_t)(max_in + 1) * 8u + 3u * (size_t)(max_in + 1) * 4u) == cudaSuccess &&
+            cudaMalloc(&ts->d_tmp, ts->tmp_bytes) == cudaSuccess;
+  for (Tier& t : ts->tiers) {
+    if (!ok) break;
+    t.h_clk.resize(t.cfg.depth);
+    ok = cudaMalloc(&t.d_arena, (size_t)t.cfg.arena_rows * sizeof(alz_edge_out)) == cudaSuccess &&
+         cudaMalloc(&t.d_clk, (size_t)t.cfg.depth * sizeof(TierClk)) == cudaSuccess;
+    for (int b = 0; b < 2 && ok; ++b)
+      ok = cudaMalloc(&t.d_block[b], (size_t)t.cfg.block_rows * sizeof(alz_edge_out)) == cudaSuccess &&
+           cudaMalloc(&t.d_bkeys[b], (size_t)t.cfg.block_rows * 8u) == cudaSuccess;
+  }
+  if (!ok) {
+    h->last_err = std::string("alz_window_history_tiers: ") + cudaGetErrorString(cudaGetLastError());
+    alz_internal_free_tiers(h);
+    return ALZ_E_NOMEM;
+  }
+  ts->d_pos = reinterpret_cast<uint32_t*>(ts->d_ikeys + max_in + 1);
+  ts->d_unm = ts->d_pos + max_in + 1;
+  ts->d_scan = ts->d_unm + max_in + 1;
+  CK(cudaMemsetAsync(ts->d_open, 0, n * sizeof(TierOpen), h->stream));
+  return ALZ_OK;
+}
+
+// Merge n rows (in, with their keys in_keys or null) into tier ti's open block. clocks: see tier_match_kernel.
+static int tier_merge(alz_handle* h, uint32_t ti, const alz_edge_out* in, const uint64_t* in_keys, uint32_t n,
+                      const WinClock* clk_first, const WinClock* clk_last, const uint64_t* clk_unready) {
+  alz_tier_set* ts = h->tiers;
+  Tier& t = ts->tiers[ti];
+  TierOpen* open = ts->d_open + ti;
+  cudaStream_t s = h->stream;
+  const int c = t.cur;
+  const unsigned match_grid = (unsigned)std::min<uint64_t>((uint64_t)h->sms * 4u, (n + 255u) / 256u + 1u);
+  tier_match_kernel<<<match_grid, 256, 0, s>>>(in, in_keys, n, t.d_bkeys[c], open, c, ts->d_ikeys, ts->d_pos,
+                                               ts->d_unm, clk_first, clk_last, clk_unready, t.inputs == 0);
+  exclusive_scan_u32(ts->d_tmp, ts->tmp_bytes, ts->d_unm, ts->d_scan, n + 1, s);
+  const uint64_t groups = (uint64_t)t.cfg.block_rows + n;   // the block has at most block_rows rows
+  const unsigned merge_grid = (unsigned)std::min<uint64_t>((uint64_t)h->sms * 8u, (groups * 8u + 255u) / 256u);
+  tier_merge_kernel<<<merge_grid, 256, 0, s>>>(t.d_block[c], t.d_bkeys[c], open, c, in, ts->d_ikeys, ts->d_pos,
+                                               ts->d_unm, ts->d_scan, n, (uint32_t)t.cfg.block_rows,
+                                               t.d_block[c ^ 1], t.d_bkeys[c ^ 1]);
+  h->launches += 3;
+  CK(cudaGetLastError());
+  t.cur = c ^ 1;
+  return ALZ_OK;
+}
+
+static int tier_input(alz_handle* h, uint32_t ti, const alz_edge_out* in, const uint64_t* in_keys, uint32_t n,
+                      const WinClock* clk_first, const WinClock* clk_last, const uint64_t* clk_unready,
+                      uint64_t window_first, bool clocked, bool poisoned);
+
+// Tier ti's open block has its factor-th input: retain it as the tier's newest entry, or drop it, and feed it to the
+// tier above. One wait, for the block's count and overflow flag.
+static int tier_close(alz_handle* h, uint32_t ti) {
+  alz_tier_set* ts = h->tiers;
+  Tier& t = ts->tiers[ti];
+  TierOpen* open = ts->d_open + ti;
+  cudaStream_t s = h->stream;
+  CK(cudaMemcpyAsync(&ts->h_open, open, sizeof(TierOpen), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  const uint32_t n = ts->h_open.count[t.cur];
+  const bool drop = t.poisoned || ts->h_open.overflow != 0u || n > t.cfg.arena_rows;
+  const uint64_t window_first = t.window_first, window_last = h->windows;
+  const bool clocked = t.clocked;
+  if (drop) {
+    t.entries.clear();   // not retained, and the run would have a gap
+    t.dropped += 1;
+  } else {
+    const uint64_t at = ring_place(t.entries, t.cfg.depth, t.cfg.arena_rows, n);
+    const uint32_t slot = (uint32_t)(t.appended++ % t.cfg.depth);
+    if (n) CK(cudaMemcpyAsync(t.d_arena + at, t.d_block[t.cur], (size_t)n * sizeof(alz_edge_out),
+                              cudaMemcpyDeviceToDevice, s));
+    if (clocked) CK(cudaMemcpyAsync(t.d_clk + slot, &open->clk, sizeof(TierClk), cudaMemcpyDeviceToDevice, s));
+    t.entries.push_back(Entry{at, n, window_first, window_last, t.inputs * t.windows_per_input, slot, clocked});
+  }
+  // the next input of the tier above reads this block before it is emptied (stream order)
+  int rc = ALZ_OK;
+  if (ti + 1 < ts->tiers.size())
+    rc = tier_input(h, ti + 1, t.d_block[t.cur], t.d_bkeys[t.cur], drop ? 0u : n, &open->clk.first, &open->clk.last,
+                    &open->clk.unready, window_first, clocked, drop);
+  t.inputs = 0;
+  t.poisoned = false;
+  t.clocked = true;
+  if (rc == ALZ_OK) {
+    CK(cudaMemsetAsync(&open->count[t.cur], 0, sizeof(uint32_t), s));
+    CK(cudaMemsetAsync(&open->overflow, 0, sizeof(uint32_t), s));
+  }
+  return rc;
+}
+
+static int tier_input(alz_handle* h, uint32_t ti, const alz_edge_out* in, const uint64_t* in_keys, uint32_t n,
+                      const WinClock* clk_first, const WinClock* clk_last, const uint64_t* clk_unready,
+                      uint64_t window_first, bool clocked, bool poisoned) {
+  Tier& t = h->tiers->tiers[ti];
+  if (t.inputs == 0) t.window_first = window_first;
+  t.clocked &= clocked;
+  t.poisoned |= poisoned;
+  if (!t.poisoned) {   // a poisoned block is dropped when it closes: what it holds does not matter
+    const int rc = tier_merge(h, ti, in, in_keys, n, clocked ? clk_first : nullptr, clk_last, clk_unready);
+    if (rc != ALZ_OK) return rc;
+  }
+  t.inputs += 1;
+  return t.inputs == t.cfg.factor ? tier_close(h, ti) : ALZ_OK;
+}
+
+// the window a flush has just consumed (h->last_n_edges rows in h->d_out) is the next input of tier 1
+static int tiers_input_window(alz_handle* h, const uint64_t* d_clk) {
+  const WinClock* clk = reinterpret_cast<const WinClock*>(d_clk);
+  return tier_input(h, 0, h->d_out, nullptr, h->last_n_edges, clk, clk, nullptr, h->windows, d_clk != nullptr, false);
+}
+
+// The sum of the last k entries of tier `tier` (1..n) into ts->sc.d_sum. Caller holds h->mu and has set the device.
+static int rollup_tier_locked(alz_handle* h, uint32_t tier, uint32_t k, size_t* n_out, alz_rollup_info* info) {
+  alz_tier_set* ts = h->tiers;
+  if (!ts) return ALZ_E_STATE;
+  if (k == 0 || tier > ts->tiers.size()) return ALZ_E_INVAL;
+  Tier& t = ts->tiers[tier - 1];
+  const size_t m = std::min<size_t>(k, t.entries.size());
+  const size_t first = t.entries.size() - m;
+  const int rc = sum_entries(h, ts->sc, t.d_arena, t.cfg.arena_rows, t.entries, first, t.h_clk.data(), t.d_clk,
+                             (size_t)t.cfg.depth * sizeof(TierClk), n_out);
+  if (rc != ALZ_OK) return rc;
+  if (info) {
+    fill_info(t.entries, first, info);
+    if (m) {
+      bool clocked = true;
+      for (size_t i = first; i < t.entries.size(); ++i)
+        clocked &= t.entries[i].clocked && t.h_clk[t.entries[i].slot].unready == 0ull;
+      if (clocked) {
+        info->clocked = 1u;
+        info->epoch_first = t.h_clk[t.entries[first].slot].first.epoch;
+        info->epoch_last = t.h_clk[t.entries.back().slot].last.epoch;
+      }
+    }
+  }
+  return ALZ_OK;
+}
+
+extern "C" int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
+                                             size_t* n_out, alz_rollup_info* info) {
+  if (tier == 0) return alz_window_rollup_device(h, k, dev_rows, n_out, info);
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  const int rc = rollup_tier_locked(h, tier, k, n_out, info);
+  if (rc == ALZ_OK && dev_rows) *dev_rows = h->tiers->sc.d_sum;
+  return rc;
+}
+
+extern "C" int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap,
+                                      size_t* n_out, alz_rollup_info* info) {
+  if (tier == 0) return alz_window_rollup(h, k, out, cap, n_out, info);
+  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  const int rc = rollup_tier_locked(h, tier, k, n_out, info);
+  if (rc != ALZ_OK) return rc;
+  if (*n_out > cap) return ALZ_E_CAPACITY;
+  if (*n_out) CK(cudaMemcpyAsync(out, h->tiers->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return ALZ_OK;
+}
+
+extern "C" int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_state* out) {
+  if (!h || !out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const alz_tier_set* ts = h->tiers;
+  if (!ts) return ALZ_E_STATE;
+  if (tier == 0 || tier > ts->tiers.size()) return ALZ_E_INVAL;
+  const Tier& t = ts->tiers[tier - 1];
+  *out = alz_tier_state{};
+  out->entries = (uint32_t)t.entries.size();
+  out->open_windows = t.inputs * t.windows_per_input;
+  out->dropped = t.dropped;
   return ALZ_OK;
 }

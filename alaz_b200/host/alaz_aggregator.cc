@@ -1,6 +1,7 @@
 // alaz_aggregator.cc — see alaz_aggregator.hpp. Plain C++ over the C ABI; no CUDA here.
 #include "alaz_aggregator.hpp"
 
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 
@@ -111,30 +112,36 @@ uint32_t Aggregator::Interner::Acquire(const std::string& uid) {
   if (it != ids.end()) return it->second;
   uint32_t id;
   if (!free_ids.empty()) { id = free_ids.back(); free_ids.pop_back(); names[id] = uid; }
-  else { id = (uint32_t)names.size(); names.push_back(uid); refs.push_back(0); }
+  else { id = (uint32_t)names.size(); names.push_back(uid); refs.push_back(0); unmapped_in.push_back(0); }
   ids.emplace(uid, id);
   return id;
 }
-void Aggregator::Interner::Map(uint32_t ip, uint32_t id) {
+void Aggregator::Interner::Map(uint32_t ip, uint32_t id, uint64_t open_window) {
   auto it = ip_to_id.find(ip);
-  if (it != ip_to_id.end()) { if (it->second == id) return; Unmap(ip); }
+  if (it != ip_to_id.end()) { if (it->second == id) return; Unmap(ip, open_window); }
   ip_to_id[ip] = id;
   refs[id]++;
 }
-void Aggregator::Interner::Unmap(uint32_t ip) {
+void Aggregator::Interner::Unmap(uint32_t ip, uint64_t open_window) {
   auto it = ip_to_id.find(ip);
   if (it == ip_to_id.end()) return;
   const uint32_t id = it->second;
   ip_to_id.erase(it);
-  // no IP resolves to the id any more: edges of the open window may still carry it, so it is recycled one
-  // window later (a UID whose stale IP entry is still in the table keeps its id, like the reference keeps the
-  // map entry: ADD/UPDATE never delete the old IP, aggregator/persist.go:55-65)
-  if (--refs[id] == 0) pending_free.push_back(id);
+  // no IP resolves to the id any more: edges of the open window, and the retained entries and open blocks that
+  // will cover it, may still carry it, so it is recycled later (a UID whose stale IP entry is still in the table
+  // keeps its id, like the reference keeps the map entry: ADD/UPDATE never delete the old IP, persist.go:55-65)
+  if (--refs[id] == 0) { unmapped_in[id] = open_window; pending_free.push_back(id); }
 }
-void Aggregator::Interner::EndWindow() {
-  for (uint32_t id : pending_free)
-    if (refs[id] == 0) { ids.erase(names[id]); free_ids.push_back(id); }
-  pending_free.clear();
+void Aggregator::Interner::EndWindow(uint64_t flushed, uint64_t hold) {
+  size_t keep = 0;
+  for (uint32_t id : pending_free) {
+    auto it = ids.find(names[id]);
+    if (refs[id] != 0 || it == ids.end() || it->second != id) continue;   // mapped again, or freed already
+    if (unmapped_in[id] + hold > flushed) { pending_free[keep++] = id; continue; }   // inside the retained span
+    ids.erase(it);
+    free_ids.push_back(id);
+  }
+  pending_free.resize(keep);
 }
 
 // processPod / processSvc: ADD and UPDATE write map[ip] = uid, DELETE removes (persist.go:55-71, 114-130)
@@ -155,10 +162,10 @@ void Aggregator::ProcessK8s(const K8sResourceMessage& m) {
     const uint32_t id = in.Acquire(m.UID);
     const int rc = alz_table_upsert(h_, table, ip, id);
     if (rc != ALZ_OK) { err_ = std::string("alz_table_upsert: ") + alz_strerror(rc); return; }
-    in.Map(ip, id);
+    in.Map(ip, id, windows_ + 1);
   } else if (m.EventType == "Delete") {
     alz_table_erase(h_, table, ip);
-    in.Unmap(ip);
+    in.Unmap(ip, windows_ + 1);
   } else {
     return;
   }
@@ -246,9 +253,17 @@ int Aggregator::Flush(bool with_scores) {
     rc = alz_gnn_score(h_, scores_.data(), n, &ns);
     if (rc != ALZ_OK) return rc;
   }
+  std::vector<EdgeWindow> edges = ToEdges(out_.data(), n, with_scores ? scores_.data() : nullptr);
+  windows_ += 1;
+  pods_.EndWindow(windows_, hold_);
+  svcs_.EndWindow(windows_, hold_);
+  return ds_ ? ds_->PersistEdgeWindow(edges) : ALZ_OK;
+}
+
+std::vector<EdgeWindow> Aggregator::ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const {
   std::vector<EdgeWindow> edges(n);
   for (size_t i = 0; i < n; ++i) {
-    const alz_edge_out& o = out_[i];
+    const alz_edge_out& o = rows[i];
     EdgeWindow& w = edges[i];
     auto uid = [&](uint8_t t, uint32_t v) -> std::string {
       if (t == ALZ_NODE_POD) return v < pods_.names.size() ? pods_.names[v] : std::string("?");
@@ -260,11 +275,40 @@ int Aggregator::Flush(bool with_scores) {
     w.ToType = NodeTypeName(o.to_type);     w.ToUID = uid(o.to_type, o.to);
     w.Count = o.count; w.Err5xx = o.err5xx; w.LatSumNs = o.lat_sum_ns;
     memcpy(w.Hist, o.hist, sizeof w.Hist);
-    if (with_scores) w.Score = scores_[i];
+    if (scores) w.Score = scores[i];
   }
-  pods_.EndWindow();
-  svcs_.EndWindow();
-  return ds_ ? ds_->PersistEdgeWindow(edges) : ALZ_OK;
+  return edges;
+}
+
+int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  // The longest span, in flushed windows, that a retained entry or an open block can reach back: depth windows in
+  // the window history; in tier t, depth_t closed entries and the open block, each of factor_1 x ... x factor_t
+  // windows (the library keeps that product times depth_t below 2^32). The hold only grows: entries retained under
+  // an earlier configuration may still be there.
+  uint64_t hold = depth, span = 1;
+  for (const alz_history_tier& t : tiers) {
+    span = std::min<uint64_t>(span * t.factor, 1ull << 32);
+    hold = std::max<uint64_t>(hold, span * ((uint64_t)t.depth + 1u));
+  }
+  hold_ = std::max(hold_, hold);
+  const int rc = alz_window_history(h_, depth, arena_rows);
+  if (rc != ALZ_OK) return rc;
+  return alz_window_history_tiers(h_, tiers.empty() ? nullptr : tiers.data(), (uint32_t)tiers.size());
+}
+
+int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  size_t n = 0;
+  int rc = alz_window_rollup_tier(h_, tier, k, roll_.data(), roll_.size(), &n, info);
+  if (rc == ALZ_E_CAPACITY) {   // n = the rows there are; nothing was written
+    roll_.resize(n + n / 4);
+    rc = alz_window_rollup_tier(h_, tier, k, roll_.data(), roll_.size(), &n, info);
+  }
+  if (rc != ALZ_OK) return rc;
+  return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
 }
 
 int Aggregator::Stats(alz_stats* out) { return h_ ? alz_get_stats(h_, out) : ALZ_E_STATE; }

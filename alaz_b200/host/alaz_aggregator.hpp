@@ -105,6 +105,14 @@ class Aggregator {
   void ProcessTcpConnect(const TcpConnectEvent& e);
   // close the window: rows grouped by edge go to ds->PersistEdgeWindow. Returns 0 or an alz_status.
   int Flush(bool with_scores = false);
+  // Rolling windows and tiered history (docs/SPEC.md §12, §13): keep the last `depth` flushed windows (depth 0: off)
+  // and the tiers (empty: off) on the device. Rows are summed by id, so from here on a freed pod or service id is
+  // not handed to another UID while a retained entry or an open block can still contain it.
+  // Returns 0 or the status of the call that refused its part (alz_window_history, alz_window_history_tiers).
+  int SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers = {});
+  // the last k entries of `tier` (0: flushed windows, 1..n: the tiers) added up per edge go to
+  // ds->PersistEdgeWindow, as a flush's rows do. info may be null. Returns 0 or an alz_status.
+  int Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -118,16 +126,22 @@ class Aggregator {
 
  private:
   int SubmitBatch();   // requires mu_
-  struct Interner {     // UID <-> dense id (< 2^29), ids recycled one window after their last IP mapping went away
+  // rows -> EdgeWindow with the UIDs the interners hold (scores: one per row, or null)
+  std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
+  // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by
+  // window w, and by every retained entry and open block that covers w: it is recycled once `hold` more windows
+  // have been flushed after w (hold 0: when w is flushed).
+  struct Interner {
     std::unordered_map<std::string, uint32_t> ids;
     std::vector<std::string> names;
     std::vector<uint32_t> refs;                       // IP entries currently mapping to the id
     std::unordered_map<uint32_t, uint32_t> ip_to_id;  // mirror of the device table's value per IP
+    std::vector<uint64_t> unmapped_in;                // the window that was open when refs last fell to 0
     std::vector<uint32_t> free_ids, pending_free;
     uint32_t Acquire(const std::string& uid);
-    void Map(uint32_t ip, uint32_t id);
-    void Unmap(uint32_t ip);
-    void EndWindow();
+    void Map(uint32_t ip, uint32_t id, uint64_t open_window);
+    void Unmap(uint32_t ip, uint64_t open_window);
+    void EndWindow(uint64_t flushed, uint64_t hold);
   };
 
   DataStore* ds_;
@@ -139,10 +153,13 @@ class Aggregator {
   bool tables_dirty_ = false;
   std::mutex mu_;
   uint64_t dropped_events_ = 0;
+  uint64_t windows_ = 0;          // windows flushed through Flush
+  uint64_t hold_ = 0;             // windows a retained entry or open block can reach back (SetHistory)
   Interner pods_, svcs_;
   std::unordered_map<std::string, uint32_t> host_ids_;   // Host header text -> dense id (ALZ_NODE_OUTBOUND_HOST)
   std::vector<std::string> host_names_;
   std::vector<alz_edge_out> out_;
+  std::vector<alz_edge_out> roll_;   // rows of the last Rollup
   std::vector<float> scores_;
   std::vector<alz_alive_conn> alive_;
 };

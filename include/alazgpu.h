@@ -315,6 +315,47 @@ int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, size_t cap, 
 int alz_window_rollup_device(alz_handle* h, uint32_t k, const alz_edge_out** dev_rows, size_t* n_out,
                              alz_rollup_info* info);
 
+/* ---- tiered history (docs/SPEC.md §13) ---------------------------------------------
+ * Tier 1 sums `factor` consecutive consumed windows into one entry, tier t + 1 sums `factor` consecutive entries of
+ * tier t, so a few retained entries span minutes, hours or days. The windows that enter tier 1 are exactly those
+ * that enter the window history (§12), whether or not that is on. Block boundaries are counted from the configuring
+ * call and never move. A block with more distinct rows than block_rows, or more rows than its arena, is not
+ * retained: it clears its tier, and the blocks of the tiers above that would contain it are dropped when they close
+ * (each drop counted in alz_tier_state.dropped). The open block of each tier lives on the device; a flush that closes
+ * no block adds no host synchronisation. */
+#define ALZ_MAX_TIERS 4
+typedef struct alz_history_tier {
+  uint32_t factor;         /* entries of the tier below that one entry of this tier sums (>= 2) */
+  uint32_t depth;          /* entries retained (>= 1) */
+  uint64_t arena_rows;     /* rows of the ring the retained entries live in (1 .. 2^31 - 1), as in §12 */
+  uint64_t block_rows;     /* distinct rows the open block can hold (1 .. 2^31 - 1) */
+} alz_history_tier;
+
+/* Configure tiers 1..n (n <= ALZ_MAX_TIERS; n = 0 frees them). The current values change nothing; other values drop
+ * every retained entry and open block. Bad values, among them tiers whose retained entries would cover 2^32
+ * flushed windows or more (factor_1 x ... x factor_t x depth_t): ALZ_E_INVAL; no memory: ALZ_E_NOMEM and the tiers
+ * are off.
+ * alz_window_history never touches the tiers and this call never touches the window history. Off by default. */
+int alz_window_history_tiers(alz_handle* h, const alz_history_tier* tiers, uint32_t n);
+
+/* The last k closed entries of tier `tier` added up per edge, as alz_window_rollup does (tier 0 is
+ * alz_window_rollup). The open blocks are never included; the call reads only. info->windows counts flushed windows
+ * covered, window_* / epoch_* refer to the oldest and newest of them, rows_in counts entry rows read.
+ * ALZ_E_STATE without tiers; ALZ_E_INVAL for k = 0 or a tier above the configured ones. */
+int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap, size_t* n_out,
+                           alz_rollup_info* info);
+/* same, rows left on the device; valid until the next tier rollup or alz_window_history_tiers on this handle */
+int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
+                                  size_t* n_out, alz_rollup_info* info);
+
+typedef struct alz_tier_state {
+  uint32_t entries;        /* entries retained */
+  uint32_t open_windows;   /* flushed windows in the open block */
+  uint64_t dropped;        /* blocks not retained since the configuring call */
+} alz_tier_state;
+/* tier 1..n: ALZ_E_INVAL otherwise; ALZ_E_STATE without tiers */
+int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_state* st);
+
 /* ---- GNN anomaly pass over the last flushed window (docs/SPEC.md §6) -------- */
 int alz_gnn_score(alz_handle* h, float* edge_scores, size_t cap, size_t* n_out);
 /* same, scores left on the device (valid until the next call on this handle) */
