@@ -125,6 +125,19 @@ class TierState(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+SPAN_AT_MOST, SPAN_AT_LEAST = 0, 1
+
+
+class SpanInfo(C.Structure):
+    """alz_span_info."""
+    _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),
+                ("_reserved", C.c_uint32 * 2)]
+
+    def as_dict(self):
+        """alz_rollup_info's fields, `entries` as a list per tier (0 = window history), `open_blocks` as a bit mask"""
+        return dict(self.r.as_dict(), entries=[int(x) for x in self.entries], open_blocks=int(self.open_blocks))
+
+
 class SockStats(C.Structure):
     """alz_sock_stats_t."""
     _fields_ = [(n, C.c_uint64) for n in ("lines", "pool_records", "pool_garbage", "syncs", "sync_ops", "sync_bytes",

@@ -25,7 +25,7 @@ EXPORTS = [
     "alz_submit_l7_raw", "alz_window_flush", "alz_window_flush_device", "alz_window_fetch", "alz_get_stats",
     "alz_window_clock", "alz_window_epoch", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
     "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device", "alz_window_tier_state",
-    "alz_gnn_score",
+    "alz_window_rollup_span", "alz_window_rollup_span_device", "alz_gnn_score",
     "alz_gnn_score_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -70,6 +70,8 @@ def load(rebuild=False):
         "alz_window_rollup_tier": ([vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
         "alz_window_rollup_tier_device": ([vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.RollupInfo)], i),
         "alz_window_tier_state": ([vp, u32, C.POINTER(abi.TierState)], i),
+        "alz_window_rollup_span": ([vp, u64, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.SpanInfo)], i),
+        "alz_window_rollup_span_device": ([vp, u64, u32, pp, C.POINTER(sz), C.POINTER(abi.SpanInfo)], i),
         "alz_pinned_alloc_local": ([vp, sz, pp], i),
         "alz_window_flush": ([vp, vp, sz, C.POINTER(sz)], i),
         "alz_window_flush_device": ([vp, pp, C.POINTER(sz)], i),
@@ -110,7 +112,7 @@ def load(rebuild=False):
                   "alz_sock_lookup_at", "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats",
                   "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
                   "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device",
-                  "alz_window_tier_state"):
+                  "alz_window_tier_state", "alz_window_rollup_span", "alz_window_rollup_span_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -365,6 +367,31 @@ class Handle:
         st = abi.TierState()
         self._ck(self.L.alz_window_tier_state(self.h, int(tier), C.byref(st)), "alz_window_tier_state")
         return st.as_dict()
+
+    # ---- span rollups (alz_rollup.cu, docs/SPEC.md §14)
+    def rollup_span(self, windows, mode=abi.SPAN_AT_MOST, cap=None):
+        """alz_window_rollup_span: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
+        info = abi.SpanInfo()
+        n = C.c_size_t(0)
+        if cap is None:
+            if self._ck(self.L.alz_window_rollup_span(self.h, int(windows), int(mode), None, 0, C.byref(n),
+                                                      C.byref(info)),
+                        "alz_window_rollup_span", allow=(abi.E_CAPACITY,)) == 0:
+                return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
+            cap = n.value
+        out = np.zeros(cap, dtype=abi.EDGE_OUT)
+        self._ck(self.L.alz_window_rollup_span(self.h, int(windows), int(mode), _ptr(out), cap, C.byref(n),
+                                               C.byref(info)), "alz_window_rollup_span")
+        return out[: n.value].copy(), info.as_dict()
+
+    def rollup_span_device(self, windows, mode=abi.SPAN_AT_MOST):
+        """alz_window_rollup_span_device: (device pointer, rows, info dict)."""
+        info = abi.SpanInfo()
+        p = C.c_void_p()
+        n = C.c_size_t(0)
+        self._ck(self.L.alz_window_rollup_span_device(self.h, int(windows), int(mode), C.byref(p), C.byref(n),
+                                                      C.byref(info)), "alz_window_rollup_span_device")
+        return p.value, n.value, info.as_dict()
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -238,6 +238,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);
+  alz_internal_free_span(h);
   free_table(&h->pairs); free_table(&h->edges);
   cudaFree(h->d_ep); cudaFree(h->d_ctr); cudaFree(h->d_hot); cudaFree(h->d_patch);
   cudaFree(h->d_win); cudaFree(h->d_defer[0]); cudaFree(h->d_defer[1]); cudaFree(h->d_bloom);

@@ -31,6 +31,7 @@ struct alz_sock_state;  // alz_sock.cu
 struct alz_comm_state;  // alz_comm.cu
 struct alz_rollup_state;  // alz_rollup.cu
 struct alz_tier_set;      // alz_rollup.cu
+struct alz_span_state;    // alz_rollup.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -121,6 +122,7 @@ struct alz_handle {
   alz_sock_state* sock = nullptr;
   alz_rollup_state* roll = nullptr;       // rolling windows (alz_window_history); null = off
   alz_tier_set* tiers = nullptr;          // tiered history (alz_window_history_tiers); null = off
+  alz_span_state* span = nullptr;         // span rollup scratch (alz_window_rollup_span); null until the first one
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -142,6 +144,7 @@ const uint64_t* alz_internal_merged_clock(alz_handle* h);
 int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk);
 void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_tiers(alz_handle* h);
+void alz_internal_free_span(alz_handle* h);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

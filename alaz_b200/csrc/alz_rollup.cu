@@ -13,9 +13,13 @@
 // below) are strictly ascending by packed key, so feeding it is a 2-way merge that adds matching keys (DESIGN.md
 // §5.6): tier_match_kernel, an exclusive scan of the unmatched input rows, tier_merge_kernel. The block's row count
 // and overflow flag stay on the device; only a block that closes (once per `factor` inputs) is waited for.
+//
+// A span rollup (docs/SPEC.md §14) sums the last m windows from pieces of all of these: window-history entries, tier
+// entries and open blocks. The host plans the pieces; the sum is the rollup above over a table of source buffers.
 #include <algorithm>
 #include <deque>
 #include <new>
+#include <unordered_map>
 #include <vector>
 
 #include "alz_handle.h"
@@ -99,6 +103,7 @@ struct Tier {
   int cur = 0;                        // the buffer that holds the open block
   uint32_t inputs = 0;                // inputs merged into the open block
   uint64_t window_first = 0;          // alz_stats.windows of the open block's oldest window
+  uint64_t window_last = 0;           // and of its newest: that of the flush that fed its last input
   bool clocked = true;                // every input so far was clocked
   bool poisoned = false;              // the open block would contain a dropped block of a tier below
   uint64_t dropped = 0;
@@ -132,15 +137,15 @@ __global__ void __launch_bounds__(256) rollup_keys_kernel(const alz_edge_out* __
   }
 }
 
-// Output row u = the sum of the source rows src[b, e), the run of ukeys[u] in sorted[0, n). Eight lanes per output
-// row, a lane owning 8 histogram cells and lane 0 the three u64 sums as everywhere else (edge_row_load): lanes 0 and 1
-// find the two ends of the run, every source row is read once and the output row is written once with plain
+// Output row u = the sum of the source rows row_of(src[b, e)), the run of ukeys[u] in sorted[0, n). Eight lanes per
+// output row, a lane owning 8 histogram cells and lane 0 the three u64 sums as everywhere else (edge_row_load): lanes
+// 0 and 1 find the two ends of the run, every source row is read once and the output row is written once with plain
 // stores. All sums wrap (u64 sums mod 2^64, cells mod 2^32, docs/SPEC.md §3).
-__global__ void __launch_bounds__(256) rollup_emit_kernel(const alz_edge_out* __restrict__ arena,
-                                                          const uint64_t* __restrict__ sorted,
-                                                          const uint32_t* __restrict__ src, uint32_t n,
-                                                          const uint64_t* __restrict__ ukeys, uint32_t n_out,
-                                                          alz_edge_out* __restrict__ out) {
+template <class RowOf>
+__device__ __forceinline__ void emit_sums(RowOf row_of, const uint64_t* __restrict__ sorted,
+                                          const uint32_t* __restrict__ src, uint32_t n,
+                                          const uint64_t* __restrict__ ukeys, uint32_t n_out,
+                                          alz_edge_out* __restrict__ out) {
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
   const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
@@ -155,13 +160,74 @@ __global__ void __launch_bounds__(256) rollup_emit_kernel(const alz_edge_out* __
     for (uint32_t j = b; j < e; ++j) {
       uint32_t rc[8];
       uint64_t r_count, r_lat, r_e5;
-      load_edge_out(arena + src[j], sl, rc, r_count, r_lat, r_e5);
+      load_edge_out(row_of(src[j]), sl, rc, r_count, r_lat, r_e5);
 #pragma unroll
       for (int q = 0; q < 8; ++q) c[q] += rc[q];
       count += r_count; lat += r_lat; e5 += r_e5;
     }
     store_edge_out(&out[u], sl, key, c, count, e5, lat);
   }
+}
+
+// the sum of entries of one arena: src[] holds arena rows
+__global__ void __launch_bounds__(256) rollup_emit_kernel(const alz_edge_out* __restrict__ arena,
+                                                          const uint64_t* __restrict__ sorted,
+                                                          const uint32_t* __restrict__ src, uint32_t n,
+                                                          const uint64_t* __restrict__ ukeys, uint32_t n_out,
+                                                          alz_edge_out* __restrict__ out) {
+  emit_sums([arena](uint32_t r) { return arena + r; }, sorted, src, n, ukeys, n_out, out);
+}
+
+// ---- span rollups (docs/SPEC.md §14): pieces from several arenas and open blocks in one sum -----------------------
+// The source buffers of one span rollup: the window-history arena, each tier's arena and each tier's open block (the
+// buffer that holds it). Their rows are numbered in one virtual space, buffer b taking [vbase[b], vbase[b + 1]);
+// the keys pass writes virtual rows and the emit maps them back to a buffer and a row.
+constexpr int kSpanSources = 1 + 2 * ALZ_MAX_TIERS;
+struct SpanSources {
+  const alz_edge_out* buf[kSpanSources];
+  uint32_t vbase[kSpanSources + 1];
+  uint32_t n;
+};
+
+// keys[i], vrow[i] = packed key and virtual row of row i of a contiguous run (rows, virtual rows v0 + i); the keys
+// of an open block are read from its key array (bkeys) instead of its 296-byte rows
+__global__ void __launch_bounds__(256) span_keys_kernel(const alz_edge_out* __restrict__ rows,
+                                                        const uint64_t* __restrict__ bkeys, uint32_t n, uint32_t v0,
+                                                        uint64_t* __restrict__ keys, uint32_t* __restrict__ vrow) {
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    keys[i] = bkeys ? bkeys[i] : row_key_of(rows + i);
+    vrow[i] = v0 + i;
+  }
+}
+
+struct SpanRowOf {
+  const alz_edge_out* const* buf;
+  const uint32_t* vbase;
+  uint32_t n;
+  __device__ __forceinline__ const alz_edge_out* operator()(uint32_t v) const {
+    uint32_t lo = 0, hi = n;   // the last buffer b with vbase[b] <= v
+    while (hi - lo > 1u) {
+      const uint32_t mid = (lo + hi) >> 1;
+      if (vbase[mid] <= v) lo = mid; else hi = mid;
+    }
+    return buf[lo] + (v - vbase[lo]);
+  }
+};
+
+// the sum of a span's pieces: src[] holds virtual rows, each mapped to its buffer by a binary search over vbase,
+// which the block keeps in shared memory
+__global__ void __launch_bounds__(256) span_emit_kernel(const __grid_constant__ SpanSources sources,
+                                                        const uint64_t* __restrict__ sorted,
+                                                        const uint32_t* __restrict__ src, uint32_t n,
+                                                        const uint64_t* __restrict__ ukeys, uint32_t n_out,
+                                                        alz_edge_out* __restrict__ out) {
+  __shared__ const alz_edge_out* s_buf[kSpanSources];
+  __shared__ uint32_t s_vbase[kSpanSources + 1];
+  if (threadIdx.x < kSpanSources) s_buf[threadIdx.x] = sources.buf[threadIdx.x];
+  if (threadIdx.x <= kSpanSources) s_vbase[threadIdx.x] = sources.vbase[threadIdx.x];
+  __syncthreads();
+  emit_sums(SpanRowOf{s_buf, s_vbase, sources.n}, sorted, src, n, ukeys, n_out, out);
 }
 
 // Step 1 of merging n input rows into a tier's open block (bkeys, open->count[cur] rows): for every input row j its
@@ -336,6 +402,38 @@ static int ensure_scratch(alz_handle* h, RollupScratch& sc, uint64_t arena_rows,
   return ALZ_OK;
 }
 
+// The n >= 1 (key, source) pairs in sc.d_keys[0] / sc.d_src[0] sorted into sc.d_keys[1] / sc.d_src[1], their
+// distinct keys into sc.d_ukeys, *n_sum of them: the one count the host waits for. sc.d_sum is grown to hold them
+// (at most out_bound rows).
+static int sort_distinct(alz_handle* h, RollupScratch& sc, uint32_t n, uint64_t out_bound, uint32_t* n_sum) {
+  cudaStream_t s = h->stream;
+  sort_pairs(sc.d_tmp, sc.tmp_bytes, sc.d_keys[0], sc.d_keys[1], sc.d_src[0], sc.d_src[1], n, s);
+  // the unsorted keys are done with: their buffer takes the head flags and their scan. No row of a flush has the
+  // key that equals the free marker (alz_device.cuh, EdgeTable), which launch_unique_sorted never takes as a head.
+  uint32_t* flags = reinterpret_cast<uint32_t*>(sc.d_keys[0]);
+  uint32_t* pos = flags + sc.cap_rows;
+  launch_unique_sorted(sc.d_keys[1], n, flags, pos, sc.d_ukeys, sc.d_tmp, sc.tmp_bytes, h->sms, s);
+  h->launches += 2;
+  CK(cudaGetLastError());
+  uint32_t last[2];
+  CK(cudaMemcpyAsync(&last[0], pos + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(&last[1], flags + (n - 1), 4, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));   // the one count the host needs, as a flush needs its edge count
+  *n_sum = last[0] + last[1];
+  if (*n_sum > sc.sum_rows) {
+    cudaFree(sc.d_sum);
+    sc.d_sum = nullptr;
+    sc.sum_rows = 0;
+    const size_t want = std::min<size_t>(out_bound, (size_t)*n_sum + *n_sum / 2u);
+    if (cudaMalloc(&sc.d_sum, want * sizeof(alz_edge_out)) != cudaSuccess) {
+      h->last_err = std::string("alz_window_rollup rows: ") + cudaGetErrorString(cudaGetLastError());
+      return ALZ_E_NOMEM;
+    }
+    sc.sum_rows = want;
+  }
+  return ALZ_OK;
+}
+
 // The sum of entries [first, end) of an arena into sc.d_sum; *n_out rows. The host clocks are copied from d_clk
 // (clk_bytes) into h_clk in stream order, so they are read when this returns. Caller holds h->mu and has set the
 // device.
@@ -364,30 +462,8 @@ static int sum_entries(alz_handle* h, RollupScratch& sc, const alz_edge_out* d_a
       h->launches += 1;
       done += (uint32_t)run_n;
     }
-    sort_pairs(sc.d_tmp, sc.tmp_bytes, sc.d_keys[0], sc.d_keys[1], sc.d_src[0], sc.d_src[1], n, s);
-    // the unsorted keys are done with: their buffer takes the head flags and their scan. No row of a flush has the
-    // key that equals the free marker (alz_device.cuh, EdgeTable), which launch_unique_sorted never takes as a head.
-    uint32_t* flags = reinterpret_cast<uint32_t*>(sc.d_keys[0]);
-    uint32_t* pos = flags + sc.cap_rows;
-    launch_unique_sorted(sc.d_keys[1], n, flags, pos, sc.d_ukeys, sc.d_tmp, sc.tmp_bytes, h->sms, s);
-    h->launches += 2;
-    CK(cudaGetLastError());
-    uint32_t last[2];
-    CK(cudaMemcpyAsync(&last[0], pos + (n - 1), 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(&last[1], flags + (n - 1), 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));   // the one count the host needs, as a flush needs its edge count
-    n_sum = last[0] + last[1];
-    if (n_sum > sc.sum_rows) {
-      cudaFree(sc.d_sum);
-      sc.d_sum = nullptr;
-      sc.sum_rows = 0;
-      const size_t want = std::min<size_t>(arena_rows, (size_t)n_sum + n_sum / 2u);
-      if (cudaMalloc(&sc.d_sum, want * sizeof(alz_edge_out)) != cudaSuccess) {
-        h->last_err = std::string("alz_window_rollup rows: ") + cudaGetErrorString(cudaGetLastError());
-        return ALZ_E_NOMEM;
-      }
-      sc.sum_rows = want;
-    }
+    rc = sort_distinct(h, sc, n, arena_rows, &n_sum);
+    if (rc != ALZ_OK) return rc;
     rollup_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(d_arena, sc.d_keys[1], sc.d_src[1], n, sc.d_ukeys,
                                                              n_sum, sc.d_sum);
     h->launches += 1;
@@ -617,6 +693,7 @@ static int tier_input(alz_handle* h, uint32_t ti, const alz_edge_out* in, const 
                       uint64_t window_first, bool clocked, bool poisoned) {
   Tier& t = h->tiers->tiers[ti];
   if (t.inputs == 0) t.window_first = window_first;
+  t.window_last = h->windows;   // an input is the flushed window, or a block closed by this flush
   t.clocked &= clocked;
   t.poisoned |= poisoned;
   if (!t.poisoned) {   // a poisoned block is dropped when it closes: what it holds does not matter
@@ -696,5 +773,259 @@ extern "C" int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_stat
   out->entries = (uint32_t)t.entries.size();
   out->open_windows = t.inputs * t.windows_per_input;
   out->dropped = t.dropped;
+  return ALZ_OK;
+}
+
+// ---- span rollups (docs/SPEC.md §14) --------------------------------------------------------------------------------
+
+struct alz_span_state {
+  RollupScratch sc;                   // its own scratch: the rows of the other rollups stay valid
+  std::vector<TierOpen> h_open;       // host copy of every tier's TierOpen
+};
+
+void alz_internal_free_span(alz_handle* h) {
+  if (!h->span) return;
+  free_scratch(h->span->sc);
+  delete h->span;
+  h->span = nullptr;
+}
+
+namespace {
+// one retained piece: a window-history entry, a closed tier entry or a tier's open block
+struct SpanUnit {
+  uint64_t window_first, window_last;   // the consumed windows it covers, alz_stats.windows numbering
+  uint64_t first_row, n;                // its rows in its buffer
+  uint32_t level;                       // 0: the window history, t: tier t
+  bool open;                            // tier `level`'s open block
+  bool clocked;
+  uint64_t epoch_first, epoch_last;
+};
+
+// the best decomposition of the windows (p, W] found so far: its cost and its oldest unit, behind which comes the
+// best decomposition of (units[unit].window_last, W]
+struct SpanBest {
+  uint64_t rows, units;
+  int unit;
+};
+
+// a before b under the rule of docs/SPEC.md §14: fewer source rows, then fewer units; two decompositions of one
+// span with equal counts have their oldest units start at the same window, so the coarser oldest unit decides
+bool span_better(const SpanBest& a, const SpanBest& b, const std::vector<SpanUnit>& units) {
+  if (a.rows != b.rows) return a.rows < b.rows;
+  if (a.units != b.units) return a.units < b.units;
+  return units[a.unit].level > units[b.unit].level;
+}
+}  // namespace
+
+// Every retained piece, with what the host must read from the device for it: every tier's TierOpen and the clocks
+// of every arena, in one wait.
+static int span_units(alz_handle* h, alz_span_state* sp, std::vector<SpanUnit>& units) {
+  cudaStream_t s = h->stream;
+  alz_rollup_state* st = h->roll;
+  alz_tier_set* ts = h->tiers;
+  if (st) CK(cudaMemcpyAsync(st->h_clk.data(), st->d_clk, (size_t)st->depth * sizeof(WinClock), cudaMemcpyDeviceToHost, s));
+  if (ts) {
+    sp->h_open.resize(ts->tiers.size());
+    CK(cudaMemcpyAsync(sp->h_open.data(), ts->d_open, ts->tiers.size() * sizeof(TierOpen), cudaMemcpyDeviceToHost, s));
+    for (Tier& t : ts->tiers)
+      CK(cudaMemcpyAsync(t.h_clk.data(), t.d_clk, (size_t)t.cfg.depth * sizeof(TierClk), cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  units.clear();
+  if (st)
+    for (const Entry& e : st->entries) {
+      const WinClock& c = st->h_clk[e.slot];
+      const bool clocked = e.clocked && c.ready != 0ull;
+      units.push_back(SpanUnit{e.window_first, e.window_last, e.first_row, e.n, 0u, false, clocked,
+                               clocked ? c.epoch : 0, clocked ? c.epoch : 0});
+    }
+  if (ts)
+    for (uint32_t i = 0; i < ts->tiers.size(); ++i) {
+      const Tier& t = ts->tiers[i];
+      for (const Entry& e : t.entries) {
+        const TierClk& c = t.h_clk[e.slot];
+        const bool clocked = e.clocked && c.unready == 0ull;
+        units.push_back(SpanUnit{e.window_first, e.window_last, e.first_row, e.n, i + 1u, false, clocked,
+                                 clocked ? c.first.epoch : 0, clocked ? c.last.epoch : 0});
+      }
+      const TierOpen& o = sp->h_open[i];
+      if (t.inputs == 0 || t.poisoned || o.overflow != 0u) continue;   // nothing in it, or not what it covers
+      const bool clocked = t.clocked && o.clk.unready == 0ull;
+      units.push_back(SpanUnit{t.window_first, t.window_last, 0, o.count[t.cur], i + 1u, true, clocked,
+                               clocked ? o.clk.first.epoch : 0, clocked ? o.clk.last.epoch : 0});
+    }
+  return ALZ_OK;
+}
+
+// The plan: the span m the mode picks among the coverable ones, and the units that cover (W - m, W] (oldest first).
+static uint64_t span_plan(const std::vector<SpanUnit>& units, uint64_t W, uint64_t N, uint32_t mode,
+                          std::vector<int>& plan) {
+  // best[p]: the best decomposition of (p, W]. A unit [a, b] extends best[b] to best[a - 1]; taking units by
+  // descending b, best[b] is final when its units come (every unit that ends at b' > b came before).
+  std::vector<int> order(units.size());
+  for (size_t i = 0; i < units.size(); ++i) order[i] = (int)i;
+  std::sort(order.begin(), order.end(), [&](int a, int b) { return units[a].window_last > units[b].window_last; });
+  std::unordered_map<uint64_t, SpanBest> best;
+  best[W] = SpanBest{0, 0, -1};
+  for (int i : order) {
+    const SpanUnit& u = units[i];
+    const auto it = best.find(u.window_last);
+    if (it == best.end()) continue;
+    const SpanBest c{it->second.rows + u.n, it->second.units + 1u, i};
+    const auto at = best.find(u.window_first - 1u);
+    if (at == best.end()) best.emplace(u.window_first - 1u, c);
+    else if (span_better(c, at->second, units)) at->second = c;
+  }
+  // windows are counted in 32 bits (alz_rollup_info.windows): larger spans are not offered
+  uint64_t lo = 0, hi = 0;   // the largest coverable m <= N; the smallest >= N (0: none)
+  uint64_t top = 0;          // the largest coverable m
+  for (const auto& kv : best) {
+    const uint64_t m = W - kv.first;
+    if (m >= (1ull << 32)) continue;
+    top = std::max(top, m);
+    if (m <= N) lo = std::max(lo, m);
+    if (m >= N && (hi == 0 || m < hi)) hi = m;
+  }
+  const uint64_t m = mode == ALZ_SPAN_AT_MOST ? lo : (hi ? hi : top);
+  plan.clear();
+  for (uint64_t p = W - m; p != W;) {
+    const int i = best[p].unit;
+    plan.push_back(i);
+    p = units[i].window_last;
+  }
+  return m;
+}
+
+// Sums the units of the plan into sp->sc.d_sum, *n_out rows. Caller holds h->mu and has set the device.
+static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, alz_span_info* info) {
+  *n_out = 0;
+  if (!h->roll && !h->tiers) return ALZ_E_STATE;
+  if (N == 0 || (mode != ALZ_SPAN_AT_MOST && mode != ALZ_SPAN_AT_LEAST)) return ALZ_E_INVAL;
+  if (!h->span) {
+    h->span = new (std::nothrow) alz_span_state();
+    if (!h->span) return ALZ_E_NOMEM;
+  }
+  alz_span_state* sp = h->span;
+  std::vector<SpanUnit> units;
+  int rc = span_units(h, sp, units);
+  if (rc != ALZ_OK) return rc;
+  std::vector<int> plan;
+  const uint64_t m = span_plan(units, h->windows, N, mode, plan);
+
+  // the source buffers the plan reads, numbered in one virtual row space up to the end of their last used row
+  const alz_edge_out* bufs[kSpanSources] = {};
+  const uint64_t* bkeys[kSpanSources] = {};
+  uint64_t used[kSpanSources] = {};
+  auto buf_of = [](const SpanUnit& u) { return u.level == 0 ? 0 : (int)(u.open ? 2 * u.level : 2 * u.level - 1); };
+  uint64_t n_src = 0;
+  for (int i : plan) {
+    const SpanUnit& u = units[i];
+    const int b = buf_of(u);
+    if (u.level == 0) bufs[b] = h->roll->d_arena;
+    else {
+      const Tier& t = h->tiers->tiers[u.level - 1];
+      bufs[b] = u.open ? t.d_block[t.cur] : t.d_arena;
+      if (u.open) bkeys[b] = t.d_bkeys[t.cur];
+    }
+    used[b] = std::max(used[b], u.first_row + u.n);
+    n_src += u.n;
+  }
+  if (n_src > 0x7FFFFFFFull) return ALZ_E_CAPACITY;   // rows are indexed by u32, counted by int
+  SpanSources srcs{};
+  int slot[kSpanSources];
+  uint64_t vtop = 0;
+  for (int b = 0; b < kSpanSources; ++b) {
+    slot[b] = -1;
+    if (!used[b]) continue;
+    slot[b] = (int)srcs.n;
+    srcs.buf[srcs.n] = bufs[b];
+    srcs.vbase[srcs.n++] = (uint32_t)vtop;
+    vtop += used[b];
+  }
+  // the used buffers hold fewer than 2^32 rows on any device below 1.2 TB; a bound, never reached
+  if (vtop >= (1ull << 32)) return ALZ_E_CAPACITY;
+  srcs.vbase[srcs.n] = (uint32_t)vtop;
+
+  uint32_t n_sum = 0;
+  if (n_src) {
+    RollupScratch& sc = sp->sc;
+    rc = ensure_scratch(h, sc, n_src, (uint32_t)n_src);
+    if (rc != ALZ_OK) return rc;
+    // keys pass: one launch per contiguous run of rows of a buffer
+    std::vector<int> by_row(plan);
+    std::sort(by_row.begin(), by_row.end(), [&](int a, int b) {
+      const int ba = buf_of(units[a]), bb = buf_of(units[b]);
+      return ba != bb ? ba < bb : units[a].first_row < units[b].first_row;
+    });
+    cudaStream_t s = h->stream;
+    const unsigned grid = (unsigned)h->sms * 4u;
+    uint32_t done = 0;
+    for (size_t i = 0; i < by_row.size();) {
+      const int b = buf_of(units[by_row[i]]);
+      const uint64_t run_first = units[by_row[i]].first_row;
+      uint64_t run_n = 0;
+      for (; i < by_row.size() && buf_of(units[by_row[i]]) == b && units[by_row[i]].first_row == run_first + run_n; ++i)
+        run_n += units[by_row[i]].n;
+      if (run_n == 0) continue;
+      span_keys_kernel<<<grid, 256, 0, s>>>(bufs[b] + run_first, bkeys[b] ? bkeys[b] + run_first : nullptr,
+                                            (uint32_t)run_n, srcs.vbase[slot[b]] + (uint32_t)run_first,
+                                            sc.d_keys[0] + done, sc.d_src[0] + done);
+      h->launches += 1;
+      done += (uint32_t)run_n;
+    }
+    rc = sort_distinct(h, sc, (uint32_t)n_src, n_src, &n_sum);
+    if (rc != ALZ_OK) return rc;
+    span_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(srcs, sc.d_keys[1], sc.d_src[1], (uint32_t)n_src,
+                                                           sc.d_ukeys, n_sum, sc.d_sum);
+    h->launches += 1;
+    CK(cudaGetLastError());
+  }
+  *n_out = n_sum;
+  if (info) {
+    *info = alz_span_info{};
+    if (m) {
+      const SpanUnit& a = units[plan.front()];
+      const SpanUnit& z = units[plan.back()];
+      info->r.windows = (uint32_t)m;
+      info->r.window_first = a.window_first;
+      info->r.window_last = z.window_last;
+      bool clocked = true;
+      for (int i : plan) {
+        const SpanUnit& u = units[i];
+        clocked &= u.clocked;
+        info->r.rows_in += u.n;
+        if (u.open) info->open_blocks |= 1u << u.level;
+        else info->entries[u.level] += 1u;
+      }
+      if (clocked) {
+        info->r.clocked = 1u;
+        info->r.epoch_first = a.epoch_first;
+        info->r.epoch_last = z.epoch_last;
+      }
+    }
+  }
+  return ALZ_OK;
+}
+
+extern "C" int alz_window_rollup_span_device(alz_handle* h, uint64_t windows, uint32_t mode,
+                                             const alz_edge_out** dev_rows, size_t* n_out, alz_span_info* info) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  const int rc = span_locked(h, windows, mode, n_out, info);
+  if (rc == ALZ_OK && dev_rows) *dev_rows = h->span->sc.d_sum;
+  return rc;
+}
+
+extern "C" int alz_window_rollup_span(alz_handle* h, uint64_t windows, uint32_t mode, alz_edge_out* out, size_t cap,
+                                      size_t* n_out, alz_span_info* info) {
+  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  const int rc = span_locked(h, windows, mode, n_out, info);
+  if (rc != ALZ_OK) return rc;
+  if (*n_out > cap) return ALZ_E_CAPACITY;
+  if (*n_out) CK(cudaMemcpyAsync(out, h->span->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }

@@ -311,6 +311,21 @@ int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
   return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
 }
 
+// A span is made of retained entries and open blocks, each inside the span SetHistory's hold covers, so the ids it
+// carries are held as those of a tier rollup are.
+int Aggregator::RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  size_t n = 0;
+  int rc = alz_window_rollup_span(h_, windows, mode, roll_.data(), roll_.size(), &n, info);
+  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {   // n = the rows there are; nothing was written
+    roll_.resize(n + n / 4);
+    rc = alz_window_rollup_span(h_, windows, mode, roll_.data(), roll_.size(), &n, info);
+  }
+  if (rc != ALZ_OK) return rc;
+  return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
+}
+
 int Aggregator::Stats(alz_stats* out) { return h_ ? alz_get_stats(h_, out) : ALZ_E_STATE; }
 
 int Aggregator::ClearSocketLines(bool send_alive, int64_t check_time_ms) {

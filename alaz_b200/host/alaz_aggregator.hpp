@@ -113,6 +113,10 @@ class Aggregator {
   // the last k entries of `tier` (0: flushed windows, 1..n: the tiers) added up per edge go to
   // ds->PersistEdgeWindow, as a flush's rows do. info may be null. Returns 0 or an alz_status.
   int Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info = nullptr);
+  // the last `windows` flushed windows up to now (docs/SPEC.md §14: ALZ_SPAN_AT_MOST or ALZ_SPAN_AT_LEAST; the span
+  // covered is info->r.windows), summed from every retained piece, go to ds->PersistEdgeWindow as a flush's rows do.
+  // info may be null. Returns 0 or an alz_status.
+  int RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to

@@ -356,6 +356,31 @@ typedef struct alz_tier_state {
 /* tier 1..n: ALZ_E_INVAL otherwise; ALZ_E_STATE without tiers */
 int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_state* st);
 
+/* ---- span rollups (docs/SPEC.md §14) -----------------------------------------------
+ * The last N consumed windows up to now, added up from whatever is retained: window-history entries, closed tier
+ * entries and the open blocks of the tiers (a tier's open block counts when it has an input, is not poisoned by a
+ * dropped block below and has not overflowed). Of the spans m that disjoint retained pieces cover exactly (the last
+ * m windows), ALZ_SPAN_AT_MOST takes the largest m <= N (0: an empty result), ALZ_SPAN_AT_LEAST the smallest m >= N,
+ * or the largest m there is when none reaches N; info->r.windows == N means the answer is exact. Of the pieces that
+ * cover m, the fewest source rows are read (ties: fewer pieces, then the coarser piece, oldest first). Rows as
+ * alz_window_rollup returns them, not bounded by max_edges. Reads only: nothing retained, no open block and no
+ * earlier rollup's device rows change. ALZ_E_INVAL for N = 0 or an unknown mode; ALZ_E_STATE with neither the
+ * window history nor the tiers on; ALZ_E_CAPACITY with nothing written for more than 2^31 - 1 source rows, or
+ * (host call) for cap below *n_out. info may be NULL. */
+#define ALZ_SPAN_AT_MOST  0u
+#define ALZ_SPAN_AT_LEAST 1u
+typedef struct alz_span_info {
+  alz_rollup_info r;                     /* windows covered, window_ / epoch_ first / last, clocked, rows_in */
+  uint32_t entries[1 + ALZ_MAX_TIERS];   /* closed entries used per tier (0 = window history) */
+  uint32_t open_blocks;                  /* bit t: tier t's open block was used */
+  uint32_t _reserved[2];
+} alz_span_info;
+int alz_window_rollup_span(alz_handle* h, uint64_t windows, uint32_t mode, alz_edge_out* out, size_t cap,
+                           size_t* n_out, alz_span_info* info);
+/* same, rows left on the device; valid until the next span rollup on this handle */
+int alz_window_rollup_span_device(alz_handle* h, uint64_t windows, uint32_t mode, const alz_edge_out** dev_rows,
+                                  size_t* n_out, alz_span_info* info);
+
 /* ---- GNN anomaly pass over the last flushed window (docs/SPEC.md §6) -------- */
 int alz_gnn_score(alz_handle* h, float* edge_scores, size_t cap, size_t* n_out);
 /* same, scores left on the device (valid until the next call on this handle) */
