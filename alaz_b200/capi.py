@@ -312,27 +312,31 @@ class Handle:
     def window_history(self, depth, arena_rows):
         self._ck(self.L.alz_window_history(self.h, int(depth), int(arena_rows)), "alz_window_history")
 
-    def rollup(self, k, cap=None):
-        """alz_window_rollup: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
-        info = abi.RollupInfo()
-        n = C.c_size_t(0)
+    def _rollup(self, fn, args, info, cap):
+        """fn(h, *args, out, cap, &n, &info): (rows, info dict). cap=None sizes the buffer from a first call with
+        cap 0."""
+        f, n = getattr(self.L, fn), C.c_size_t(0)
         if cap is None:
-            if self._ck(self.L.alz_window_rollup(self.h, int(k), None, 0, C.byref(n), C.byref(info)),
-                        "alz_window_rollup", allow=(abi.E_CAPACITY,)) == 0:
+            if self._ck(f(self.h, *args, None, 0, C.byref(n), C.byref(info)), fn, allow=(abi.E_CAPACITY,)) == 0:
                 return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
             cap = n.value
         out = np.zeros(cap, dtype=abi.EDGE_OUT)
-        self._ck(self.L.alz_window_rollup(self.h, int(k), _ptr(out), cap, C.byref(n), C.byref(info)), "alz_window_rollup")
+        self._ck(f(self.h, *args, _ptr(out), cap, C.byref(n), C.byref(info)), fn)
         return out[: n.value].copy(), info.as_dict()
+
+    def _rollup_device(self, fn, args, info):
+        """fn(h, *args, &dev_rows, &n, &info): (device pointer, rows, info dict)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        self._ck(getattr(self.L, fn)(self.h, *args, C.byref(p), C.byref(n), C.byref(info)), fn)
+        return p.value, n.value, info.as_dict()
+
+    def rollup(self, k, cap=None):
+        """alz_window_rollup: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
+        return self._rollup("alz_window_rollup", (int(k),), abi.RollupInfo(), cap)
 
     def rollup_device(self, k):
         """alz_window_rollup_device: (device pointer, rows, info dict)."""
-        info = abi.RollupInfo()
-        p = C.c_void_p()
-        n = C.c_size_t(0)
-        self._ck(self.L.alz_window_rollup_device(self.h, int(k), C.byref(p), C.byref(n), C.byref(info)),
-                 "alz_window_rollup_device")
-        return p.value, n.value, info.as_dict()
+        return self._rollup_device("alz_window_rollup_device", (int(k),), abi.RollupInfo())
 
     # ---- tiered history (alz_rollup.cu, docs/SPEC.md §13)
     def window_history_tiers(self, tiers):
@@ -342,26 +346,11 @@ class Handle:
 
     def rollup_tier(self, tier, k, cap=None):
         """alz_window_rollup_tier: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
-        info = abi.RollupInfo()
-        n = C.c_size_t(0)
-        if cap is None:
-            if self._ck(self.L.alz_window_rollup_tier(self.h, int(tier), int(k), None, 0, C.byref(n), C.byref(info)),
-                        "alz_window_rollup_tier", allow=(abi.E_CAPACITY,)) == 0:
-                return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
-            cap = n.value
-        out = np.zeros(cap, dtype=abi.EDGE_OUT)
-        self._ck(self.L.alz_window_rollup_tier(self.h, int(tier), int(k), _ptr(out), cap, C.byref(n), C.byref(info)),
-                 "alz_window_rollup_tier")
-        return out[: n.value].copy(), info.as_dict()
+        return self._rollup("alz_window_rollup_tier", (int(tier), int(k)), abi.RollupInfo(), cap)
 
     def rollup_tier_device(self, tier, k):
         """alz_window_rollup_tier_device: (device pointer, rows, info dict)."""
-        info = abi.RollupInfo()
-        p = C.c_void_p()
-        n = C.c_size_t(0)
-        self._ck(self.L.alz_window_rollup_tier_device(self.h, int(tier), int(k), C.byref(p), C.byref(n), C.byref(info)),
-                 "alz_window_rollup_tier_device")
-        return p.value, n.value, info.as_dict()
+        return self._rollup_device("alz_window_rollup_tier_device", (int(tier), int(k)), abi.RollupInfo())
 
     def tier_state(self, tier):
         st = abi.TierState()
@@ -371,27 +360,11 @@ class Handle:
     # ---- span rollups (alz_rollup.cu, docs/SPEC.md §14)
     def rollup_span(self, windows, mode=abi.SPAN_AT_MOST, cap=None):
         """alz_window_rollup_span: (rows, info dict). cap=None sizes the buffer from a first call with cap 0."""
-        info = abi.SpanInfo()
-        n = C.c_size_t(0)
-        if cap is None:
-            if self._ck(self.L.alz_window_rollup_span(self.h, int(windows), int(mode), None, 0, C.byref(n),
-                                                      C.byref(info)),
-                        "alz_window_rollup_span", allow=(abi.E_CAPACITY,)) == 0:
-                return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
-            cap = n.value
-        out = np.zeros(cap, dtype=abi.EDGE_OUT)
-        self._ck(self.L.alz_window_rollup_span(self.h, int(windows), int(mode), _ptr(out), cap, C.byref(n),
-                                               C.byref(info)), "alz_window_rollup_span")
-        return out[: n.value].copy(), info.as_dict()
+        return self._rollup("alz_window_rollup_span", (int(windows), int(mode)), abi.SpanInfo(), cap)
 
     def rollup_span_device(self, windows, mode=abi.SPAN_AT_MOST):
         """alz_window_rollup_span_device: (device pointer, rows, info dict)."""
-        info = abi.SpanInfo()
-        p = C.c_void_p()
-        n = C.c_size_t(0)
-        self._ck(self.L.alz_window_rollup_span_device(self.h, int(windows), int(mode), C.byref(p), C.byref(n),
-                                                      C.byref(info)), "alz_window_rollup_span_device")
-        return p.value, n.value, info.as_dict()
+        return self._rollup_device("alz_window_rollup_span_device", (int(windows), int(mode)), abi.SpanInfo())
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

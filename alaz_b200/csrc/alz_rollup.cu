@@ -1,21 +1,23 @@
 // alz_rollup.cu — rolling windows (docs/SPEC.md §12): the rows of the last flushed windows kept on the device, and
-// the sum of the last k of them as one edge list; and tiered history (docs/SPEC.md §13): every consumed window merged
-// into coarser blocks on the device, each closed block retained as an entry of its tier.
+// the sum of the last k of them as one edge list; tiered history (docs/SPEC.md §13): every consumed window merged
+// into coarser blocks on the device, each closed block retained as an entry of its tier; and span rollups
+// (docs/SPEC.md §14): the last m windows summed from pieces of all of these.
 //
 // Every accumulator of an output row is an integer sum (docs/SPEC.md §3), so the sum of k windows' rows per edge
 // is what one window holding those windows' events would have returned. The flush is left as it is: a flush that
 // consumed its window copies its rows into the arena (one device-to-device copy, no kernel, no synchronisation).
-// A rollup has the shape of the single-rank flush (DESIGN.md §5.3) applied to output rows instead of pair rows:
-// packed key of every retained row -> radix sort of (key, arena row) -> the distinct keys -> eight lanes per output
-// row add up the key's run of source rows in registers and store the row once.
+//
+// The window history and each tier keep their retained entries in a Ring: an arena of rows, a clock per entry and
+// the host's list of entries. Every rollup is one sum over pieces (sum_pieces), a piece being a run of rows of one
+// buffer: a ring entry or a tier's open block. A window or tier rollup takes the last k entries of one ring; a span
+// takes the pieces the host plans. The sum has the shape of the single-rank flush (DESIGN.md §5.3) applied to output
+// rows instead of pair rows: packed key of every source row -> radix sort of (key, source row) -> the distinct keys
+// -> eight lanes per output row add up the key's run of source rows in registers and store the row once.
 //
 // A tier's open block is a sorted row list. Both it and its input (a flushed window, or a closed block of the tier
 // below) are strictly ascending by packed key, so feeding it is a 2-way merge that adds matching keys (DESIGN.md
 // §5.6): tier_match_kernel, an exclusive scan of the unmatched input rows, tier_merge_kernel. The block's row count
 // and overflow flag stay on the device; only a block that closes (once per `factor` inputs) is waited for.
-//
-// A span rollup (docs/SPEC.md §14) sums the last m windows from pieces of all of these: window-history entries, tier
-// entries and open blocks. The host plans the pieces; the sum is the rollup above over a table of source buffers.
 #include <algorithm>
 #include <deque>
 #include <new>
@@ -57,7 +59,7 @@ uint64_t ring_place(std::deque<Entry>& entries, uint32_t depth, uint64_t arena_r
 struct RollupScratch {
   uint32_t cap_rows = 0;
   uint64_t* d_keys[2] = {nullptr, nullptr};   // [cap_rows] packed keys of the source rows, unsorted / sorted
-  uint32_t* d_src[2] = {nullptr, nullptr};    // [cap_rows] their arena rows
+  uint32_t* d_src[2] = {nullptr, nullptr};    // [cap_rows] their virtual rows
   uint64_t* d_ukeys = nullptr;                // [cap_rows] the distinct keys in order
   void* d_tmp = nullptr;                      // CUB scratch of the sort, then of the scan
   size_t tmp_bytes = 0;
@@ -77,27 +79,87 @@ struct TierOpen {
   uint32_t overflow;  // the open block would have passed block_rows: it is dropped when it closes
   uint32_t _pad;
 };
+
+// The clock rule: a clock gives epochs when every covered window's clock was ready. *first / *last: the epochs of
+// the oldest and newest covered window.
+bool clock_epochs(const WinClock& c, uint64_t* first, uint64_t* last) {
+  *first = *last = c.epoch;
+  return c.ready != 0ull;
+}
+bool clock_epochs(const TierClk& c, uint64_t* first, uint64_t* last) {
+  *first = c.first.epoch;
+  *last = c.last.epoch;
+  return c.unready == 0ull;
+}
+
+// one piece of a rollup: a retained entry or a tier's open block
+struct Piece {
+  const alz_edge_out* buf;              // the buffer that holds its rows
+  const uint64_t* keys;                 // the buffer's packed keys (an open block's key array), or null: read the rows
+  uint64_t first_row, n;                // its rows in buf
+  uint64_t window_first, window_last;   // the consumed windows it covers, alz_stats.windows numbering
+  uint32_t windows;
+  uint32_t level;                       // 0: the window history, t: tier t
+  bool open;                            // tier `level`'s open block
+  bool clocked;                         // the clock rule holds: epoch_first / epoch_last are its epochs
+  uint64_t epoch_first, epoch_last;
+};
+
+// Retained entries (docs/SPEC.md §12): an arena of arena_rows rows holding at most depth entries, each with a clock
+// in slot appended % depth of the clock array. The window history's clock is the WinClock its flush closed, a tier
+// entry's the TierClk of its block.
+template <class Clk>
+struct Ring {
+  uint32_t depth = 0;
+  uint64_t arena_rows = 0;
+  alz_edge_out* d_arena = nullptr;    // [arena_rows]
+  Clk* d_clk = nullptr;               // [depth]
+  std::vector<Clk> h_clk;             // host copy of d_clk, read by rollups
+  std::deque<Entry> entries;          // oldest first: a contiguous run of the most recent inputs
+  uint64_t appended = 0;              // entries ever appended: the next one's clock slot is appended % depth
+
+  bool alloc(uint32_t d, uint64_t rows) {
+    depth = d;
+    arena_rows = rows;
+    h_clk.resize(d);
+    return cudaMalloc(&d_arena, (size_t)rows * sizeof(alz_edge_out)) == cudaSuccess &&
+           cudaMalloc(&d_clk, (size_t)d * sizeof(Clk)) == cudaSuccess;
+  }
+  void free() { cudaFree(d_arena); cudaFree(d_clk); }
+
+  // The newest entry: n rows copied from rows and its clock from d_c (null: not clocked), in stream order. An entry
+  // larger than the arena is not retained and clears the ring: the run would have a gap.
+  int append(alz_handle* h, const alz_edge_out* rows, uint64_t n, const Clk* d_c, uint64_t window_first,
+             uint64_t window_last, uint32_t windows) {
+    if (n > arena_rows) { entries.clear(); return ALZ_OK; }
+    const uint64_t at = ring_place(entries, depth, arena_rows, n);
+    const uint32_t slot = (uint32_t)(appended++ % depth);
+    if (n) CK(cudaMemcpyAsync(d_arena + at, rows, (size_t)n * sizeof(alz_edge_out), cudaMemcpyDeviceToDevice, h->stream));
+    if (d_c) CK(cudaMemcpyAsync(d_clk + slot, d_c, sizeof(Clk), cudaMemcpyDeviceToDevice, h->stream));
+    entries.push_back(Entry{at, n, window_first, window_last, windows, slot, d_c != nullptr});
+    return ALZ_OK;
+  }
+
+  Piece piece(const Entry& e, uint32_t level) const {   // its clock is left to clocked()
+    return Piece{d_arena, nullptr, e.first_row, e.n, e.window_first, e.window_last, e.windows, level, false, false, 0, 0};
+  }
+  // whether entry e is clocked, and the epochs of its oldest and newest window; from h_clk, which the caller has
+  // copied from the device
+  bool clocked(const Entry& e, uint64_t* first, uint64_t* last) const {
+    return e.clocked && clock_epochs(h_clk[e.slot], first, last);
+  }
+};
 }  // namespace
 
 struct alz_rollup_state {
-  uint32_t depth = 0;
-  uint64_t arena_rows = 0;
-  alz_edge_out* d_arena = nullptr;
-  WinClock* d_clk = nullptr;          // [depth] the clock of the epoch each entry's flush closed
-  std::vector<WinClock> h_clk;
-  std::deque<Entry> entries;          // oldest first: a contiguous run of the most recent consumed windows
-  uint64_t appended = 0;              // entries ever appended: the next one's clock slot is appended % depth
-  RollupScratch sc;
+  Ring<WinClock> ring;
+  RollupScratch sc;                   // window rollups' rows
 };
 
 namespace {
 struct Tier {
   alz_history_tier cfg{};
-  alz_edge_out* d_arena = nullptr;    // [arena_rows] the retained entries, a ring in rows
-  TierClk* d_clk = nullptr;           // [depth] each entry's clocks
-  std::vector<TierClk> h_clk;
-  std::deque<Entry> entries;
-  uint64_t appended = 0;
+  Ring<TierClk> ring;
   alz_edge_out* d_block[2] = {nullptr, nullptr};   // [block_rows] the open block, ping-pong
   uint64_t* d_bkeys[2] = {nullptr, nullptr};       // [block_rows] its packed keys
   int cur = 0;                        // the buffer that holds the open block
@@ -123,19 +185,13 @@ struct alz_tier_set {
   void* d_tmp = nullptr;
   size_t tmp_bytes = 0;
   TierOpen h_open{};                  // host copy of the closing tier's TierOpen
-  RollupScratch sc;
+  RollupScratch sc;                   // tier rollups' rows
 };
 
-// keys[i], src[i] = packed edge key and arena row of source row first_row + i (16 of the row's 296 bytes are read)
-__global__ void __launch_bounds__(256) rollup_keys_kernel(const alz_edge_out* __restrict__ arena, uint32_t first_row,
-                                                          uint32_t n, uint64_t* __restrict__ keys,
-                                                          uint32_t* __restrict__ src) {
-  const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    keys[i] = row_key_of(arena + first_row + i);
-    src[i] = first_row + i;
-  }
-}
+struct alz_span_state {
+  RollupScratch sc;                   // span rollups' rows
+  std::vector<TierOpen> h_open;       // host copy of every tier's TierOpen
+};
 
 // Output row u = the sum of the source rows row_of(src[b, e)), the run of ukeys[u] in sorted[0, n). Eight lanes per
 // output row, a lane owning 8 histogram cells and lane 0 the three u64 sums as everywhere else (edge_row_load): lanes
@@ -169,17 +225,7 @@ __device__ __forceinline__ void emit_sums(RowOf row_of, const uint64_t* __restri
   }
 }
 
-// the sum of entries of one arena: src[] holds arena rows
-__global__ void __launch_bounds__(256) rollup_emit_kernel(const alz_edge_out* __restrict__ arena,
-                                                          const uint64_t* __restrict__ sorted,
-                                                          const uint32_t* __restrict__ src, uint32_t n,
-                                                          const uint64_t* __restrict__ ukeys, uint32_t n_out,
-                                                          alz_edge_out* __restrict__ out) {
-  emit_sums([arena](uint32_t r) { return arena + r; }, sorted, src, n, ukeys, n_out, out);
-}
-
-// ---- span rollups (docs/SPEC.md §14): pieces from several arenas and open blocks in one sum -----------------------
-// The source buffers of one span rollup: the window-history arena, each tier's arena and each tier's open block (the
+// The source buffers of one rollup: the window-history arena, each tier's arena and each tier's open block (the
 // buffer that holds it). Their rows are numbered in one virtual space, buffer b taking [vbase[b], vbase[b + 1]);
 // the keys pass writes virtual rows and the emit maps them back to a buffer and a row.
 constexpr int kSpanSources = 1 + 2 * ALZ_MAX_TIERS;
@@ -189,8 +235,8 @@ struct SpanSources {
   uint32_t n;
 };
 
-// keys[i], vrow[i] = packed key and virtual row of row i of a contiguous run (rows, virtual rows v0 + i); the keys
-// of an open block are read from its key array (bkeys) instead of its 296-byte rows
+// keys[i], vrow[i] = packed key and virtual row of row i of a contiguous run (rows, virtual rows v0 + i); 16 of a
+// row's 296 bytes are read, and the keys of an open block are read from its key array (bkeys) instead
 __global__ void __launch_bounds__(256) span_keys_kernel(const alz_edge_out* __restrict__ rows,
                                                         const uint64_t* __restrict__ bkeys, uint32_t n, uint32_t v0,
                                                         uint64_t* __restrict__ keys, uint32_t* __restrict__ vrow) {
@@ -215,19 +261,25 @@ struct SpanRowOf {
   }
 };
 
-// the sum of a span's pieces: src[] holds virtual rows, each mapped to its buffer by a binary search over vbase,
-// which the block keeps in shared memory
+// the sum of the pieces: src[] holds virtual rows. With one buffer (kOneBuffer) a virtual row is a row of it;
+// otherwise each is mapped to its buffer by a binary search over vbase, which the block keeps in shared memory.
+template <bool kOneBuffer>
 __global__ void __launch_bounds__(256) span_emit_kernel(const __grid_constant__ SpanSources sources,
                                                         const uint64_t* __restrict__ sorted,
                                                         const uint32_t* __restrict__ src, uint32_t n,
                                                         const uint64_t* __restrict__ ukeys, uint32_t n_out,
                                                         alz_edge_out* __restrict__ out) {
-  __shared__ const alz_edge_out* s_buf[kSpanSources];
-  __shared__ uint32_t s_vbase[kSpanSources + 1];
-  if (threadIdx.x < kSpanSources) s_buf[threadIdx.x] = sources.buf[threadIdx.x];
-  if (threadIdx.x <= kSpanSources) s_vbase[threadIdx.x] = sources.vbase[threadIdx.x];
-  __syncthreads();
-  emit_sums(SpanRowOf{s_buf, s_vbase, sources.n}, sorted, src, n, ukeys, n_out, out);
+  if constexpr (kOneBuffer) {
+    const alz_edge_out* buf = sources.buf[0];
+    emit_sums([buf](uint32_t v) { return buf + v; }, sorted, src, n, ukeys, n_out, out);
+  } else {
+    __shared__ const alz_edge_out* s_buf[kSpanSources];
+    __shared__ uint32_t s_vbase[kSpanSources + 1];
+    if (threadIdx.x < kSpanSources) s_buf[threadIdx.x] = sources.buf[threadIdx.x];
+    if (threadIdx.x <= kSpanSources) s_vbase[threadIdx.x] = sources.vbase[threadIdx.x];
+    __syncthreads();
+    emit_sums(SpanRowOf{s_buf, s_vbase, sources.n}, sorted, src, n, ukeys, n_out, out);
+  }
 }
 
 // Step 1 of merging n input rows into a tier's open block (bkeys, open->count[cur] rows): for every input row j its
@@ -324,7 +376,7 @@ void alz_internal_free_rollup(alz_handle* h) {
   alz_rollup_state* st = h->roll;
   if (!st) return;
   free_scratch(st->sc);
-  cudaFree(st->d_arena); cudaFree(st->d_clk);
+  st->ring.free();
   delete st;
   h->roll = nullptr;
 }
@@ -333,18 +385,14 @@ extern "C" int alz_window_history(alz_handle* h, uint32_t depth, uint64_t arena_
   if (!h || arena_rows >= (1ull << 31) || (depth != 0 && arena_rows == 0)) return ALZ_E_INVAL;   // rows are indexed by u32, counted by int
   std::lock_guard<std::mutex> g(h->mu);
   CK(cudaSetDevice(h->device));
-  if (h->roll && h->roll->depth == depth && h->roll->arena_rows == arena_rows) return ALZ_OK;
+  if (h->roll && h->roll->ring.depth == depth && h->roll->ring.arena_rows == arena_rows) return ALZ_OK;
   CK(cudaStreamSynchronize(h->stream));   // copies into the arena and a rollup's kernels may still be running
   alz_internal_free_rollup(h);
   if (depth == 0) return ALZ_OK;
   alz_rollup_state* st = new (std::nothrow) alz_rollup_state();
   if (!st) return ALZ_E_NOMEM;
   h->roll = st;
-  st->depth = depth;
-  st->arena_rows = arena_rows;
-  st->h_clk.resize(depth);
-  if (cudaMalloc(&st->d_arena, (size_t)arena_rows * sizeof(alz_edge_out)) != cudaSuccess ||
-      cudaMalloc(&st->d_clk, (size_t)depth * sizeof(WinClock)) != cudaSuccess) {
+  if (!st->ring.alloc(depth, arena_rows)) {
     h->last_err = std::string("alz_window_history: ") + cudaGetErrorString(cudaGetLastError());
     alz_internal_free_rollup(h);
     return ALZ_E_NOMEM;
@@ -354,28 +402,18 @@ extern "C" int alz_window_history(alz_handle* h, uint32_t depth, uint64_t arena_
 
 static int tiers_input_window(alz_handle* h, const uint64_t* d_clk);
 
-// the window a flush has just consumed becomes the newest entry of the window history (docs/SPEC.md §12)
-static int window_history_append(alz_handle* h, const uint64_t* d_clk) {
-  alz_rollup_state* st = h->roll;
-  const uint64_t n = h->last_n_edges;
-  if (n > st->arena_rows) { st->entries.clear(); return ALZ_OK; }   // not retained, and the run would have a gap
-  const uint64_t at = ring_place(st->entries, st->depth, st->arena_rows, n);
-  const uint32_t slot = (uint32_t)(st->appended++ % st->depth);
-  if (n) CK(cudaMemcpyAsync(st->d_arena + at, h->d_out, (size_t)n * sizeof(alz_edge_out), cudaMemcpyDeviceToDevice, h->stream));
-  if (d_clk) CK(cudaMemcpyAsync(st->d_clk + slot, d_clk, sizeof(WinClock), cudaMemcpyDeviceToDevice, h->stream));
-  st->entries.push_back(Entry{at, n, h->windows, h->windows, 1u, slot, d_clk != nullptr});
-  return ALZ_OK;
-}
-
-// The window history and the tiers each take the window whatever happens to the other.
+// The window a flush has just consumed becomes the newest entry of the window history (docs/SPEC.md §12). The
+// window history and the tiers each take the window whatever happens to the other.
 int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk) {
-  const int rc0 = h->roll ? window_history_append(h, d_clk) : ALZ_OK;
+  const int rc0 = h->roll ? h->roll->ring.append(h, h->d_out, h->last_n_edges, reinterpret_cast<const WinClock*>(d_clk),
+                                                 h->windows, h->windows, 1u)
+                          : ALZ_OK;
   const int rc1 = h->tiers ? tiers_input_window(h, d_clk) : ALZ_OK;
   return rc0 != ALZ_OK ? rc0 : rc1;
 }
 
-// scratch for n source rows of an arena of arena_rows rows
-static int ensure_scratch(alz_handle* h, RollupScratch& sc, uint64_t arena_rows, uint32_t n) {
+// scratch for n source rows of at most row_bound
+static int ensure_scratch(alz_handle* h, RollupScratch& sc, uint64_t row_bound, uint32_t n) {
   if (n <= sc.cap_rows) return ALZ_OK;
   CK(cudaStreamSynchronize(h->stream));
   cudaFree(sc.d_keys[0]); cudaFree(sc.d_tmp);
@@ -383,7 +421,7 @@ static int ensure_scratch(alz_handle* h, RollupScratch& sc, uint64_t arena_rows,
   sc.d_src[0] = sc.d_src[1] = nullptr;
   sc.d_tmp = nullptr;
   sc.cap_rows = 0; sc.tmp_bytes = 0;
-  const uint32_t cap = (uint32_t)std::min<uint64_t>(arena_rows + 63u, ((uint64_t)n + n / 2u + 63u)) & ~63u;   // regions stay 256-byte aligned
+  const uint32_t cap = (uint32_t)std::min<uint64_t>(row_bound + 63u, ((uint64_t)n + n / 2u + 63u)) & ~63u;   // regions stay 256-byte aligned
   const size_t tmp = std::max(sort_pairs_temp_bytes(cap), scan_temp_bytes(cap));
   char* base = nullptr;
   if (cudaMalloc(&base, (size_t)cap * 32u) != cudaSuccess || cudaMalloc(&sc.d_tmp, tmp) != cudaSuccess) {
@@ -434,38 +472,66 @@ static int sort_distinct(alz_handle* h, RollupScratch& sc, uint32_t n, uint64_t 
   return ALZ_OK;
 }
 
-// The sum of entries [first, end) of an arena into sc.d_sum; *n_out rows. The host clocks are copied from d_clk
-// (clk_bytes) into h_clk in stream order, so they are read when this returns. Caller holds h->mu and has set the
+// The sum of the pieces' rows into sc.d_sum, *n_out rows; row_bound bounds the source rows of any call with this
+// scratch. Whatever the caller has enqueued before is complete when this returns. Caller holds h->mu and has set the
 // device.
-static int sum_entries(alz_handle* h, RollupScratch& sc, const alz_edge_out* d_arena, uint64_t arena_rows,
-                       const std::deque<Entry>& entries, size_t first, void* h_clk, const void* d_clk,
-                       size_t clk_bytes, size_t* n_out) {
+static int sum_pieces(alz_handle* h, RollupScratch& sc, std::vector<Piece> pieces, uint64_t row_bound,
+                      size_t* n_out) {
+  // by buffer (the window history, then tier by tier its arena and its open block), then by row
+  std::sort(pieces.begin(), pieces.end(), [](const Piece& a, const Piece& b) {
+    if (a.level != b.level) return a.level < b.level;
+    return a.open != b.open ? b.open : a.first_row < b.first_row;
+  });
+  // the buffers the pieces read, numbered in one virtual row space up to the end of their last used row
+  std::vector<uint32_t> vbase(pieces.size());   // of each piece's buffer
+  SpanSources srcs{};
+  uint64_t n_src = 0, vtop = 0;
+  for (size_t i = 0; i < pieces.size();) {
+    const alz_edge_out* buf = pieces[i].buf;
+    uint64_t used = 0;
+    for (; i < pieces.size() && pieces[i].buf == buf; ++i) {
+      used = std::max(used, pieces[i].first_row + pieces[i].n);
+      n_src += pieces[i].n;
+      vbase[i] = (uint32_t)vtop;
+    }
+    if (!used) continue;
+    srcs.buf[srcs.n] = buf;
+    srcs.vbase[srcs.n++] = (uint32_t)vtop;
+    vtop += used;
+  }
+  if (n_src > 0x7FFFFFFFull) return ALZ_E_CAPACITY;   // rows are indexed by u32, counted by int
+  // the used buffers hold fewer than 2^32 rows on any device below 1.2 TB; a bound, never reached
+  if (vtop >= (1ull << 32)) return ALZ_E_CAPACITY;
+  srcs.vbase[srcs.n] = (uint32_t)vtop;
+
   cudaStream_t s = h->stream;
-  uint64_t n_src = 0;
-  for (size_t i = first; i < entries.size(); ++i) n_src += entries[i].n;
-  const uint32_t n = (uint32_t)n_src;   // at most arena_rows: the entries do not overlap
   uint32_t n_sum = 0;
-  CK(cudaMemcpyAsync(h_clk, d_clk, clk_bytes, cudaMemcpyDeviceToHost, s));
-  if (n) {
-    int rc = ensure_scratch(h, sc, arena_rows, n);
+  if (n_src) {
+    int rc = ensure_scratch(h, sc, row_bound, (uint32_t)n_src);
     if (rc != ALZ_OK) return rc;
-    // entries that follow one another in the arena (all of them, or all but one jump back to row 0) take one launch
+    // keys pass: pieces that follow one another in a buffer take one launch
     const unsigned grid = (unsigned)h->sms * 4u;
     uint32_t done = 0;
-    for (size_t i = first; i < entries.size();) {
-      const uint64_t run_first = entries[i].first_row;
+    for (size_t i = 0; i < pieces.size();) {
+      const Piece& p = pieces[i];
+      const uint32_t v0 = vbase[i] + (uint32_t)p.first_row;
       uint64_t run_n = 0;
-      for (; i < entries.size() && entries[i].first_row == run_first + run_n; ++i) run_n += entries[i].n;
+      for (; i < pieces.size() && pieces[i].buf == p.buf && pieces[i].first_row == p.first_row + run_n; ++i)
+        run_n += pieces[i].n;
       if (run_n == 0) continue;
-      rollup_keys_kernel<<<grid, 256, 0, s>>>(d_arena, (uint32_t)run_first, (uint32_t)run_n, sc.d_keys[0] + done,
-                                              sc.d_src[0] + done);
+      span_keys_kernel<<<grid, 256, 0, s>>>(p.buf + p.first_row, p.keys ? p.keys + p.first_row : nullptr,
+                                            (uint32_t)run_n, v0, sc.d_keys[0] + done, sc.d_src[0] + done);
       h->launches += 1;
       done += (uint32_t)run_n;
     }
-    rc = sort_distinct(h, sc, n, arena_rows, &n_sum);
+    rc = sort_distinct(h, sc, (uint32_t)n_src, row_bound, &n_sum);
     if (rc != ALZ_OK) return rc;
-    rollup_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(d_arena, sc.d_keys[1], sc.d_src[1], n, sc.d_ukeys,
-                                                             n_sum, sc.d_sum);
+    if (srcs.n == 1)
+      span_emit_kernel<true><<<(unsigned)h->sms * 8u, 256, 0, s>>>(srcs, sc.d_keys[1], sc.d_src[1], (uint32_t)n_src,
+                                                                   sc.d_ukeys, n_sum, sc.d_sum);
+    else
+      span_emit_kernel<false><<<(unsigned)h->sms * 8u, 256, 0, s>>>(srcs, sc.d_keys[1], sc.d_src[1], (uint32_t)n_src,
+                                                                    sc.d_ukeys, n_sum, sc.d_sum);
     h->launches += 1;
     CK(cudaGetLastError());
   } else {
@@ -475,66 +541,107 @@ static int sum_entries(alz_handle* h, RollupScratch& sc, const alz_edge_out* d_a
   return ALZ_OK;
 }
 
-// what a rollup of entries [first, end) covers, apart from the epochs
-static void fill_info(const std::deque<Entry>& entries, size_t first, alz_rollup_info* info) {
+// What the pieces (oldest first, covering a contiguous run of windows) cover; epochs when every one is clocked.
+static void fill_info(const std::vector<Piece>& pieces, alz_rollup_info* info) {
   *info = alz_rollup_info{};
-  for (size_t i = first; i < entries.size(); ++i) {
-    info->windows += entries[i].windows;
-    info->rows_in += entries[i].n;
+  if (pieces.empty()) return;
+  bool clocked = true;
+  for (const Piece& p : pieces) {
+    info->windows += p.windows;
+    info->rows_in += p.n;
+    clocked &= p.clocked;
   }
-  if (first < entries.size()) {
-    info->window_first = entries[first].window_first;
-    info->window_last = entries.back().window_last;
+  info->window_first = pieces.front().window_first;
+  info->window_last = pieces.back().window_last;
+  if (clocked) {
+    info->clocked = 1u;
+    info->epoch_first = pieces.front().epoch_first;
+    info->epoch_last = pieces.back().epoch_last;
   }
 }
 
-// The sum of the last k window-history entries into st->sc.d_sum; *n_out rows. Caller holds h->mu and has set the device.
-static int rollup_locked(alz_handle* h, uint32_t k, size_t* n_out, alz_rollup_info* info) {
-  alz_rollup_state* st = h->roll;
-  if (!st) return ALZ_E_STATE;
-  if (k == 0) return ALZ_E_INVAL;
-  const size_t m = std::min<size_t>(k, st->entries.size());
-  const size_t first = st->entries.size() - m;
-  const int rc = sum_entries(h, st->sc, st->d_arena, st->arena_rows, st->entries, first, st->h_clk.data(), st->d_clk,
-                             (size_t)st->depth * sizeof(WinClock), n_out);
+// The sum of the last k entries of a ring into sc.d_sum; *n_out rows. The ring's clocks are copied to the host in
+// stream order, so they are read when the sum returns.
+template <class Clk>
+static int ring_rollup(alz_handle* h, Ring<Clk>& r, uint32_t level, uint32_t k, RollupScratch& sc, size_t* n_out,
+                       alz_rollup_info* info) {
+  CK(cudaMemcpyAsync(r.h_clk.data(), r.d_clk, (size_t)r.depth * sizeof(Clk), cudaMemcpyDeviceToHost, h->stream));
+  size_t first = r.entries.size() - std::min<size_t>(k, r.entries.size());
+  std::vector<Piece> pieces;
+  for (size_t i = first; i < r.entries.size(); ++i) pieces.push_back(r.piece(r.entries[i], level));
+  const int rc = sum_pieces(h, sc, pieces, r.arena_rows, n_out);
   if (rc != ALZ_OK) return rc;
   if (info) {
-    fill_info(st->entries, first, info);
-    if (m) {
-      bool clocked = true;
-      for (size_t i = first; i < st->entries.size(); ++i)
-        clocked &= st->entries[i].clocked && st->h_clk[st->entries[i].slot].ready != 0ull;
-      if (clocked) {
-        info->clocked = 1u;
-        info->epoch_first = st->h_clk[st->entries[first].slot].epoch;
-        info->epoch_last = st->h_clk[st->entries.back().slot].epoch;
-      }
-    }
+    for (Piece& p : pieces) p.clocked = r.clocked(r.entries[first++], &p.epoch_first, &p.epoch_last);
+    fill_info(pieces, info);
   }
+  return ALZ_OK;
+}
+
+// The sum of the last k entries of the window history (level 0) or of tier `level` into the scratch of that kind of
+// rollup, so that each one's rows stay valid until the next of its kind; *rows, *n_out. Caller holds h->mu and has
+// set the device.
+static int rollup_locked(alz_handle* h, uint32_t level, uint32_t k, size_t* n_out, alz_rollup_info* info,
+                         const alz_edge_out** rows) {
+  RollupScratch* sc = nullptr;
+  int rc;
+  if (level == 0) {
+    if (!h->roll) return ALZ_E_STATE;
+    if (k == 0) return ALZ_E_INVAL;
+    sc = &h->roll->sc;
+    rc = ring_rollup(h, h->roll->ring, 0, k, *sc, n_out, info);
+  } else {
+    alz_tier_set* ts = h->tiers;
+    if (!ts) return ALZ_E_STATE;
+    if (k == 0 || level > ts->tiers.size()) return ALZ_E_INVAL;
+    sc = &ts->sc;
+    rc = ring_rollup(h, ts->tiers[level - 1].ring, level, k, *sc, n_out, info);
+  }
+  *rows = sc->d_sum;
+  return rc;
+}
+
+// A rollup entry point: lock, set the device and run the rollup (run(&rows), which sets *n_out). Into out (to_host):
+// ALZ_E_CAPACITY when the rows do not fit, and nothing is written; else *dev_rows (when not null) = the device rows.
+template <class Run>
+static int rollup_call(alz_handle* h, bool to_host, alz_edge_out* out, size_t cap, const alz_edge_out** dev_rows,
+                       size_t* n_out, Run run) {
+  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  CK(cudaSetDevice(h->device));
+  const alz_edge_out* rows = nullptr;
+  const int rc = run(&rows);
+  if (rc != ALZ_OK) return rc;
+  if (!to_host) {
+    if (dev_rows) *dev_rows = rows;
+    return ALZ_OK;
+  }
+  if (*n_out > cap) return ALZ_E_CAPACITY;
+  if (*n_out) CK(cudaMemcpyAsync(out, rows, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }
 
 extern "C" int alz_window_rollup_device(alz_handle* h, uint32_t k, const alz_edge_out** dev_rows, size_t* n_out,
                                         alz_rollup_info* info) {
-  if (!h || !n_out) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = rollup_locked(h, k, n_out, info);
-  if (rc == ALZ_OK && dev_rows) *dev_rows = h->roll->sc.d_sum;
-  return rc;
+  return alz_window_rollup_tier_device(h, 0, k, dev_rows, n_out, info);
 }
 
 extern "C" int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, size_t cap, size_t* n_out,
                                  alz_rollup_info* info) {
-  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = rollup_locked(h, k, n_out, info);
-  if (rc != ALZ_OK) return rc;
-  if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, h->roll->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return ALZ_OK;
+  return alz_window_rollup_tier(h, 0, k, out, cap, n_out, info);
+}
+
+extern "C" int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
+                                             size_t* n_out, alz_rollup_info* info) {
+  return rollup_call(h, false, nullptr, 0, dev_rows, n_out,
+                     [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
+}
+
+extern "C" int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap,
+                                      size_t* n_out, alz_rollup_info* info) {
+  return rollup_call(h, true, out, cap, nullptr, n_out,
+                     [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
 }
 
 // ---- tiered history (docs/SPEC.md §13) ------------------------------------------------------------------------------
@@ -543,8 +650,8 @@ void alz_internal_free_tiers(alz_handle* h) {
   alz_tier_set* ts = h->tiers;
   if (!ts) return;
   for (Tier& t : ts->tiers) {
-    cudaFree(t.d_arena); cudaFree(t.d_clk); cudaFree(t.d_block[0]); cudaFree(t.d_block[1]);
-    cudaFree(t.d_bkeys[0]); cudaFree(t.d_bkeys[1]);
+    t.ring.free();
+    cudaFree(t.d_block[0]); cudaFree(t.d_block[1]); cudaFree(t.d_bkeys[0]); cudaFree(t.d_bkeys[1]);
   }
   cudaFree(ts->d_open); cudaFree(ts->d_ikeys); cudaFree(ts->d_tmp);
   free_scratch(ts->sc);
@@ -603,9 +710,7 @@ extern "C" int alz_window_history_tiers(alz_handle* h, const alz_history_tier* t
             cudaMalloc(&ts->d_tmp, ts->tmp_bytes) == cudaSuccess;
   for (Tier& t : ts->tiers) {
     if (!ok) break;
-    t.h_clk.resize(t.cfg.depth);
-    ok = cudaMalloc(&t.d_arena, (size_t)t.cfg.arena_rows * sizeof(alz_edge_out)) == cudaSuccess &&
-         cudaMalloc(&t.d_clk, (size_t)t.cfg.depth * sizeof(TierClk)) == cudaSuccess;
+    ok = t.ring.alloc(t.cfg.depth, t.cfg.arena_rows);
     for (int b = 0; b < 2 && ok; ++b)
       ok = cudaMalloc(&t.d_block[b], (size_t)t.cfg.block_rows * sizeof(alz_edge_out)) == cudaSuccess &&
            cudaMalloc(&t.d_bkeys[b], (size_t)t.cfg.block_rows * 8u) == cudaSuccess;
@@ -663,15 +768,12 @@ static int tier_close(alz_handle* h, uint32_t ti) {
   const uint64_t window_first = t.window_first, window_last = h->windows;
   const bool clocked = t.clocked;
   if (drop) {
-    t.entries.clear();   // not retained, and the run would have a gap
+    t.ring.entries.clear();   // not retained, and the run would have a gap
     t.dropped += 1;
   } else {
-    const uint64_t at = ring_place(t.entries, t.cfg.depth, t.cfg.arena_rows, n);
-    const uint32_t slot = (uint32_t)(t.appended++ % t.cfg.depth);
-    if (n) CK(cudaMemcpyAsync(t.d_arena + at, t.d_block[t.cur], (size_t)n * sizeof(alz_edge_out),
-                              cudaMemcpyDeviceToDevice, s));
-    if (clocked) CK(cudaMemcpyAsync(t.d_clk + slot, &open->clk, sizeof(TierClk), cudaMemcpyDeviceToDevice, s));
-    t.entries.push_back(Entry{at, n, window_first, window_last, t.inputs * t.windows_per_input, slot, clocked});
+    const int rc = t.ring.append(h, t.d_block[t.cur], n, clocked ? &open->clk : nullptr, window_first, window_last,
+                                 t.inputs * t.windows_per_input);
+    if (rc != ALZ_OK) return rc;
   }
   // the next input of the tier above reads this block before it is emptied (stream order)
   int rc = ALZ_OK;
@@ -710,58 +812,6 @@ static int tiers_input_window(alz_handle* h, const uint64_t* d_clk) {
   return tier_input(h, 0, h->d_out, nullptr, h->last_n_edges, clk, clk, nullptr, h->windows, d_clk != nullptr, false);
 }
 
-// The sum of the last k entries of tier `tier` (1..n) into ts->sc.d_sum. Caller holds h->mu and has set the device.
-static int rollup_tier_locked(alz_handle* h, uint32_t tier, uint32_t k, size_t* n_out, alz_rollup_info* info) {
-  alz_tier_set* ts = h->tiers;
-  if (!ts) return ALZ_E_STATE;
-  if (k == 0 || tier > ts->tiers.size()) return ALZ_E_INVAL;
-  Tier& t = ts->tiers[tier - 1];
-  const size_t m = std::min<size_t>(k, t.entries.size());
-  const size_t first = t.entries.size() - m;
-  const int rc = sum_entries(h, ts->sc, t.d_arena, t.cfg.arena_rows, t.entries, first, t.h_clk.data(), t.d_clk,
-                             (size_t)t.cfg.depth * sizeof(TierClk), n_out);
-  if (rc != ALZ_OK) return rc;
-  if (info) {
-    fill_info(t.entries, first, info);
-    if (m) {
-      bool clocked = true;
-      for (size_t i = first; i < t.entries.size(); ++i)
-        clocked &= t.entries[i].clocked && t.h_clk[t.entries[i].slot].unready == 0ull;
-      if (clocked) {
-        info->clocked = 1u;
-        info->epoch_first = t.h_clk[t.entries[first].slot].first.epoch;
-        info->epoch_last = t.h_clk[t.entries.back().slot].last.epoch;
-      }
-    }
-  }
-  return ALZ_OK;
-}
-
-extern "C" int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
-                                             size_t* n_out, alz_rollup_info* info) {
-  if (tier == 0) return alz_window_rollup_device(h, k, dev_rows, n_out, info);
-  if (!h || !n_out) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = rollup_tier_locked(h, tier, k, n_out, info);
-  if (rc == ALZ_OK && dev_rows) *dev_rows = h->tiers->sc.d_sum;
-  return rc;
-}
-
-extern "C" int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap,
-                                      size_t* n_out, alz_rollup_info* info) {
-  if (tier == 0) return alz_window_rollup(h, k, out, cap, n_out, info);
-  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = rollup_tier_locked(h, tier, k, n_out, info);
-  if (rc != ALZ_OK) return rc;
-  if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, h->tiers->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return ALZ_OK;
-}
-
 extern "C" int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_state* out) {
   if (!h || !out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
@@ -770,18 +820,13 @@ extern "C" int alz_window_tier_state(alz_handle* h, uint32_t tier, alz_tier_stat
   if (tier == 0 || tier > ts->tiers.size()) return ALZ_E_INVAL;
   const Tier& t = ts->tiers[tier - 1];
   *out = alz_tier_state{};
-  out->entries = (uint32_t)t.entries.size();
+  out->entries = (uint32_t)t.ring.entries.size();
   out->open_windows = t.inputs * t.windows_per_input;
   out->dropped = t.dropped;
   return ALZ_OK;
 }
 
 // ---- span rollups (docs/SPEC.md §14) --------------------------------------------------------------------------------
-
-struct alz_span_state {
-  RollupScratch sc;                   // its own scratch: the rows of the other rollups stay valid
-  std::vector<TierOpen> h_open;       // host copy of every tier's TierOpen
-};
 
 void alz_internal_free_span(alz_handle* h) {
   if (!h->span) return;
@@ -791,16 +836,6 @@ void alz_internal_free_span(alz_handle* h) {
 }
 
 namespace {
-// one retained piece: a window-history entry, a closed tier entry or a tier's open block
-struct SpanUnit {
-  uint64_t window_first, window_last;   // the consumed windows it covers, alz_stats.windows numbering
-  uint64_t first_row, n;                // its rows in its buffer
-  uint32_t level;                       // 0: the window history, t: tier t
-  bool open;                            // tier `level`'s open block
-  bool clocked;
-  uint64_t epoch_first, epoch_last;
-};
-
 // the best decomposition of the windows (p, W] found so far: its cost and its oldest unit, behind which comes the
 // best decomposition of (units[unit].window_last, W]
 struct SpanBest {
@@ -810,7 +845,7 @@ struct SpanBest {
 
 // a before b under the rule of docs/SPEC.md §14: fewer source rows, then fewer units; two decompositions of one
 // span with equal counts have their oldest units start at the same window, so the coarser oldest unit decides
-bool span_better(const SpanBest& a, const SpanBest& b, const std::vector<SpanUnit>& units) {
+bool span_better(const SpanBest& a, const SpanBest& b, const std::vector<Piece>& units) {
   if (a.rows != b.rows) return a.rows < b.rows;
   if (a.units != b.units) return a.units < b.units;
   return units[a.unit].level > units[b.unit].level;
@@ -819,46 +854,44 @@ bool span_better(const SpanBest& a, const SpanBest& b, const std::vector<SpanUni
 
 // Every retained piece, with what the host must read from the device for it: every tier's TierOpen and the clocks
 // of every arena, in one wait.
-static int span_units(alz_handle* h, alz_span_state* sp, std::vector<SpanUnit>& units) {
+static int span_units(alz_handle* h, alz_span_state* sp, std::vector<Piece>& units) {
   cudaStream_t s = h->stream;
   alz_rollup_state* st = h->roll;
   alz_tier_set* ts = h->tiers;
-  if (st) CK(cudaMemcpyAsync(st->h_clk.data(), st->d_clk, (size_t)st->depth * sizeof(WinClock), cudaMemcpyDeviceToHost, s));
+  if (st) CK(cudaMemcpyAsync(st->ring.h_clk.data(), st->ring.d_clk, (size_t)st->ring.depth * sizeof(WinClock),
+                             cudaMemcpyDeviceToHost, s));
   if (ts) {
     sp->h_open.resize(ts->tiers.size());
     CK(cudaMemcpyAsync(sp->h_open.data(), ts->d_open, ts->tiers.size() * sizeof(TierOpen), cudaMemcpyDeviceToHost, s));
     for (Tier& t : ts->tiers)
-      CK(cudaMemcpyAsync(t.h_clk.data(), t.d_clk, (size_t)t.cfg.depth * sizeof(TierClk), cudaMemcpyDeviceToHost, s));
+      CK(cudaMemcpyAsync(t.ring.h_clk.data(), t.ring.d_clk, (size_t)t.ring.depth * sizeof(TierClk),
+                         cudaMemcpyDeviceToHost, s));
   }
   CK(cudaStreamSynchronize(s));
   units.clear();
-  if (st)
-    for (const Entry& e : st->entries) {
-      const WinClock& c = st->h_clk[e.slot];
-      const bool clocked = e.clocked && c.ready != 0ull;
-      units.push_back(SpanUnit{e.window_first, e.window_last, e.first_row, e.n, 0u, false, clocked,
-                               clocked ? c.epoch : 0, clocked ? c.epoch : 0});
+  auto add_ring = [&units](const auto& r, uint32_t level) {
+    for (const Entry& e : r.entries) {
+      units.push_back(r.piece(e, level));
+      units.back().clocked = r.clocked(e, &units.back().epoch_first, &units.back().epoch_last);
     }
+  };
+  if (st) add_ring(st->ring, 0u);
   if (ts)
     for (uint32_t i = 0; i < ts->tiers.size(); ++i) {
       const Tier& t = ts->tiers[i];
-      for (const Entry& e : t.entries) {
-        const TierClk& c = t.h_clk[e.slot];
-        const bool clocked = e.clocked && c.unready == 0ull;
-        units.push_back(SpanUnit{e.window_first, e.window_last, e.first_row, e.n, i + 1u, false, clocked,
-                                 clocked ? c.first.epoch : 0, clocked ? c.last.epoch : 0});
-      }
+      add_ring(t.ring, i + 1u);
       const TierOpen& o = sp->h_open[i];
       if (t.inputs == 0 || t.poisoned || o.overflow != 0u) continue;   // nothing in it, or not what it covers
-      const bool clocked = t.clocked && o.clk.unready == 0ull;
-      units.push_back(SpanUnit{t.window_first, t.window_last, 0, o.count[t.cur], i + 1u, true, clocked,
-                               clocked ? o.clk.first.epoch : 0, clocked ? o.clk.last.epoch : 0});
+      Piece p{t.d_block[t.cur], t.d_bkeys[t.cur], 0, o.count[t.cur], t.window_first, t.window_last,
+              t.inputs * t.windows_per_input, i + 1u, true, false, 0, 0};
+      p.clocked = t.clocked && clock_epochs(o.clk, &p.epoch_first, &p.epoch_last);
+      units.push_back(p);
     }
   return ALZ_OK;
 }
 
 // The plan: the span m the mode picks among the coverable ones, and the units that cover (W - m, W] (oldest first).
-static uint64_t span_plan(const std::vector<SpanUnit>& units, uint64_t W, uint64_t N, uint32_t mode,
+static uint64_t span_plan(const std::vector<Piece>& units, uint64_t W, uint64_t N, uint32_t mode,
                           std::vector<int>& plan) {
   // best[p]: the best decomposition of (p, W]. A unit [a, b] extends best[b] to best[a - 1]; taking units by
   // descending b, best[b] is final when its units come (every unit that ends at b' > b came before).
@@ -868,7 +901,7 @@ static uint64_t span_plan(const std::vector<SpanUnit>& units, uint64_t W, uint64
   std::unordered_map<uint64_t, SpanBest> best;
   best[W] = SpanBest{0, 0, -1};
   for (int i : order) {
-    const SpanUnit& u = units[i];
+    const Piece& u = units[i];
     const auto it = best.find(u.window_last);
     if (it == best.end()) continue;
     const SpanBest c{it->second.rows + u.n, it->second.units + 1u, i};
@@ -896,8 +929,9 @@ static uint64_t span_plan(const std::vector<SpanUnit>& units, uint64_t W, uint64
   return m;
 }
 
-// Sums the units of the plan into sp->sc.d_sum, *n_out rows. Caller holds h->mu and has set the device.
-static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, alz_span_info* info) {
+// Sums the units of the plan into sp->sc.d_sum; *rows, *n_out. Caller holds h->mu and has set the device.
+static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, alz_span_info* info,
+                       const alz_edge_out** rows) {
   *n_out = 0;
   if (!h->roll && !h->tiers) return ALZ_E_STATE;
   if (N == 0 || (mode != ALZ_SPAN_AT_MOST && mode != ALZ_SPAN_AT_LEAST)) return ALZ_E_INVAL;
@@ -906,102 +940,24 @@ static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, 
     if (!h->span) return ALZ_E_NOMEM;
   }
   alz_span_state* sp = h->span;
-  std::vector<SpanUnit> units;
+  std::vector<Piece> units;
   int rc = span_units(h, sp, units);
   if (rc != ALZ_OK) return rc;
   std::vector<int> plan;
-  const uint64_t m = span_plan(units, h->windows, N, mode, plan);
-
-  // the source buffers the plan reads, numbered in one virtual row space up to the end of their last used row
-  const alz_edge_out* bufs[kSpanSources] = {};
-  const uint64_t* bkeys[kSpanSources] = {};
-  uint64_t used[kSpanSources] = {};
-  auto buf_of = [](const SpanUnit& u) { return u.level == 0 ? 0 : (int)(u.open ? 2 * u.level : 2 * u.level - 1); };
+  span_plan(units, h->windows, N, mode, plan);
+  std::vector<Piece> pieces;
+  for (int i : plan) pieces.push_back(units[i]);
   uint64_t n_src = 0;
-  for (int i : plan) {
-    const SpanUnit& u = units[i];
-    const int b = buf_of(u);
-    if (u.level == 0) bufs[b] = h->roll->d_arena;
-    else {
-      const Tier& t = h->tiers->tiers[u.level - 1];
-      bufs[b] = u.open ? t.d_block[t.cur] : t.d_arena;
-      if (u.open) bkeys[b] = t.d_bkeys[t.cur];
-    }
-    used[b] = std::max(used[b], u.first_row + u.n);
-    n_src += u.n;
-  }
-  if (n_src > 0x7FFFFFFFull) return ALZ_E_CAPACITY;   // rows are indexed by u32, counted by int
-  SpanSources srcs{};
-  int slot[kSpanSources];
-  uint64_t vtop = 0;
-  for (int b = 0; b < kSpanSources; ++b) {
-    slot[b] = -1;
-    if (!used[b]) continue;
-    slot[b] = (int)srcs.n;
-    srcs.buf[srcs.n] = bufs[b];
-    srcs.vbase[srcs.n++] = (uint32_t)vtop;
-    vtop += used[b];
-  }
-  // the used buffers hold fewer than 2^32 rows on any device below 1.2 TB; a bound, never reached
-  if (vtop >= (1ull << 32)) return ALZ_E_CAPACITY;
-  srcs.vbase[srcs.n] = (uint32_t)vtop;
-
-  uint32_t n_sum = 0;
-  if (n_src) {
-    RollupScratch& sc = sp->sc;
-    rc = ensure_scratch(h, sc, n_src, (uint32_t)n_src);
-    if (rc != ALZ_OK) return rc;
-    // keys pass: one launch per contiguous run of rows of a buffer
-    std::vector<int> by_row(plan);
-    std::sort(by_row.begin(), by_row.end(), [&](int a, int b) {
-      const int ba = buf_of(units[a]), bb = buf_of(units[b]);
-      return ba != bb ? ba < bb : units[a].first_row < units[b].first_row;
-    });
-    cudaStream_t s = h->stream;
-    const unsigned grid = (unsigned)h->sms * 4u;
-    uint32_t done = 0;
-    for (size_t i = 0; i < by_row.size();) {
-      const int b = buf_of(units[by_row[i]]);
-      const uint64_t run_first = units[by_row[i]].first_row;
-      uint64_t run_n = 0;
-      for (; i < by_row.size() && buf_of(units[by_row[i]]) == b && units[by_row[i]].first_row == run_first + run_n; ++i)
-        run_n += units[by_row[i]].n;
-      if (run_n == 0) continue;
-      span_keys_kernel<<<grid, 256, 0, s>>>(bufs[b] + run_first, bkeys[b] ? bkeys[b] + run_first : nullptr,
-                                            (uint32_t)run_n, srcs.vbase[slot[b]] + (uint32_t)run_first,
-                                            sc.d_keys[0] + done, sc.d_src[0] + done);
-      h->launches += 1;
-      done += (uint32_t)run_n;
-    }
-    rc = sort_distinct(h, sc, (uint32_t)n_src, n_src, &n_sum);
-    if (rc != ALZ_OK) return rc;
-    span_emit_kernel<<<(unsigned)h->sms * 8u, 256, 0, s>>>(srcs, sc.d_keys[1], sc.d_src[1], (uint32_t)n_src,
-                                                           sc.d_ukeys, n_sum, sc.d_sum);
-    h->launches += 1;
-    CK(cudaGetLastError());
-  }
-  *n_out = n_sum;
+  for (const Piece& p : pieces) n_src += p.n;
+  rc = sum_pieces(h, sp->sc, pieces, n_src, n_out);
+  if (rc != ALZ_OK) return rc;
+  *rows = sp->sc.d_sum;
   if (info) {
     *info = alz_span_info{};
-    if (m) {
-      const SpanUnit& a = units[plan.front()];
-      const SpanUnit& z = units[plan.back()];
-      info->r.windows = (uint32_t)m;
-      info->r.window_first = a.window_first;
-      info->r.window_last = z.window_last;
-      bool clocked = true;
-      for (int i : plan) {
-        const SpanUnit& u = units[i];
-        clocked &= u.clocked;
-        info->r.rows_in += u.n;
-        if (u.open) info->open_blocks |= 1u << u.level;
-        else info->entries[u.level] += 1u;
-      }
-      if (clocked) {
-        info->r.clocked = 1u;
-        info->r.epoch_first = a.epoch_first;
-        info->r.epoch_last = z.epoch_last;
-      }
+    fill_info(pieces, &info->r);
+    for (const Piece& p : pieces) {
+      if (p.open) info->open_blocks |= 1u << p.level;
+      else info->entries[p.level] += 1u;
     }
   }
   return ALZ_OK;
@@ -1009,23 +965,12 @@ static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, 
 
 extern "C" int alz_window_rollup_span_device(alz_handle* h, uint64_t windows, uint32_t mode,
                                              const alz_edge_out** dev_rows, size_t* n_out, alz_span_info* info) {
-  if (!h || !n_out) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = span_locked(h, windows, mode, n_out, info);
-  if (rc == ALZ_OK && dev_rows) *dev_rows = h->span->sc.d_sum;
-  return rc;
+  return rollup_call(h, false, nullptr, 0, dev_rows, n_out,
+                     [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
 }
 
 extern "C" int alz_window_rollup_span(alz_handle* h, uint64_t windows, uint32_t mode, alz_edge_out* out, size_t cap,
                                       size_t* n_out, alz_span_info* info) {
-  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
-  std::lock_guard<std::mutex> g(h->mu);
-  CK(cudaSetDevice(h->device));
-  const int rc = span_locked(h, windows, mode, n_out, info);
-  if (rc != ALZ_OK) return rc;
-  if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, h->span->sc.d_sum, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return ALZ_OK;
+  return rollup_call(h, true, out, cap, nullptr, n_out,
+                     [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
 }

@@ -298,17 +298,26 @@ int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vecto
   return alz_window_history_tiers(h_, tiers.empty() ? nullptr : tiers.data(), (uint32_t)tiers.size());
 }
 
-int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
-  if (!h_) return ALZ_E_STATE;
-  std::lock_guard<std::mutex> g(mu_);
+// call(out, cap, &n) into roll_, grown once when the rows do not fit (ALZ_E_CAPACITY with n = the rows there are;
+// nothing was written), then the rows to the data store
+template <class Call>
+int Aggregator::PersistRollup(Call call) {
   size_t n = 0;
-  int rc = alz_window_rollup_tier(h_, tier, k, roll_.data(), roll_.size(), &n, info);
-  if (rc == ALZ_E_CAPACITY) {   // n = the rows there are; nothing was written
+  int rc = call(roll_.data(), roll_.size(), &n);
+  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {
     roll_.resize(n + n / 4);
-    rc = alz_window_rollup_tier(h_, tier, k, roll_.data(), roll_.size(), &n, info);
+    rc = call(roll_.data(), roll_.size(), &n);
   }
   if (rc != ALZ_OK) return rc;
   return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
+}
+
+int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  return PersistRollup([&](alz_edge_out* out, size_t cap, size_t* n) {
+    return alz_window_rollup_tier(h_, tier, k, out, cap, n, info);
+  });
 }
 
 // A span is made of retained entries and open blocks, each inside the span SetHistory's hold covers, so the ids it
@@ -316,14 +325,9 @@ int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
 int Aggregator::RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);
-  size_t n = 0;
-  int rc = alz_window_rollup_span(h_, windows, mode, roll_.data(), roll_.size(), &n, info);
-  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {   // n = the rows there are; nothing was written
-    roll_.resize(n + n / 4);
-    rc = alz_window_rollup_span(h_, windows, mode, roll_.data(), roll_.size(), &n, info);
-  }
-  if (rc != ALZ_OK) return rc;
-  return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
+  return PersistRollup([&](alz_edge_out* out, size_t cap, size_t* n) {
+    return alz_window_rollup_span(h_, windows, mode, out, cap, n, info);
+  });
 }
 
 int Aggregator::Stats(alz_stats* out) { return h_ ? alz_get_stats(h_, out) : ALZ_E_STATE; }

@@ -130,6 +130,9 @@ class Aggregator {
 
  private:
   int SubmitBatch();   // requires mu_
+  // a rollup call(out, cap, &n) into roll_, then its rows to ds->PersistEdgeWindow; requires mu_
+  template <class Call>
+  int PersistRollup(Call call);
   // rows -> EdgeWindow with the UIDs the interners hold (scores: one per row, or null)
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
   // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by

@@ -250,8 +250,13 @@ def test_a_span_reads_only_against_a_twin_handle():
             r.flush(recs=recs)
         if i % 3 == 1:                                          # earlier rollups' device rows stay valid
             p0, n0, _ = a.h.rollup_device(3)
+            rows0 = a.h.d2h(p0, n0, abi.EDGE_OUT).tobytes()
             p1, n1, _ = a.h.rollup_tier_device(1, 2)
-            before = (a.h.d2h(p0, n0, abi.EDGE_OUT).tobytes(), a.h.d2h(p1, n1, abi.EDGE_OUT).tobytes())
+            assert a.h.d2h(p0, n0, abi.EDGE_OUT).tobytes() == rows0   # a tier rollup leaves the window rollup's
+            rows1 = a.h.d2h(p1, n1, abi.EDGE_OUT).tobytes()
+            p0, n0, _ = a.h.rollup_device(1)
+            assert a.h.d2h(p1, n1, abi.EDGE_OUT).tobytes() == rows1   # and a window rollup the tier rollup's
+            before = (a.h.d2h(p0, n0, abi.EDGE_OUT).tobytes(), rows1)
             a.check_all()
             assert (a.h.d2h(p0, n0, abi.EDGE_OUT).tobytes(), a.h.d2h(p1, n1, abi.EDGE_OUT).tobytes()) == before
     recs = spec_records([0, 5, 9], rng)
