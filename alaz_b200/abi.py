@@ -126,6 +126,7 @@ class TierState(C.Structure):
 
 
 SPAN_AT_MOST, SPAN_AT_LEAST = 0, 1
+ROLLUP_WINDOWS, ROLLUP_TIER, ROLLUP_SPAN = 0, 1, 2   # alz_gnn_score_rollup kinds
 
 
 class SpanInfo(C.Structure):

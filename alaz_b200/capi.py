@@ -26,7 +26,7 @@ EXPORTS = [
     "alz_window_clock", "alz_window_epoch", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
     "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device", "alz_window_tier_state",
     "alz_window_rollup_span", "alz_window_rollup_span_device", "alz_gnn_score",
-    "alz_gnn_score_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_gnn_score_device", "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -78,6 +78,8 @@ def load(rebuild=False):
         "alz_get_stats": ([vp, C.POINTER(abi.Stats)], i),
         "alz_gnn_score": ([vp, vp, sz, C.POINTER(sz)], i),
         "alz_gnn_score_device": ([vp, pp, C.POINTER(sz)], i),
+        "alz_gnn_score_rollup": ([vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_gnn_score_rollup_device": ([vp, u32, pp, C.POINTER(sz)], i),
         "alz_gnn_nodes": ([vp, vp, vp, sz, C.POINTER(sz)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
@@ -112,7 +114,8 @@ def load(rebuild=False):
                   "alz_sock_lookup_at", "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats",
                   "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
                   "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device",
-                  "alz_window_tier_state", "alz_window_rollup_span", "alz_window_rollup_span_device"):
+                  "alz_window_tier_state", "alz_window_rollup_span", "alz_window_rollup_span_device",
+                  "alz_gnn_score_rollup", "alz_gnn_score_rollup_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -365,6 +368,27 @@ class Handle:
     def rollup_span_device(self, windows, mode=abi.SPAN_AT_MOST):
         """alz_window_rollup_span_device: (device pointer, rows, info dict)."""
         return self._rollup_device("alz_window_rollup_span_device", (int(windows), int(mode)), abi.SpanInfo())
+
+    # ---- GNN anomaly pass over a rollup (alz_gnn.cu, docs/SPEC.md §15)
+    def gnn_score_rollup(self, kind, cap=None):
+        """alz_gnn_score_rollup: the scores of the rows the last rollup of `kind` (abi.ROLLUP_*) returned, one per
+        row. cap=None sizes the buffer from a first call with cap 0."""
+        n = C.c_size_t(0)
+        if cap is None:
+            if self._ck(self.L.alz_gnn_score_rollup(self.h, int(kind), None, 0, C.byref(n)), "alz_gnn_score_rollup",
+                        allow=(abi.E_CAPACITY,)) == 0:
+                return np.zeros(0, dtype=np.float32)
+            cap = n.value
+        out = np.zeros(cap, dtype=np.float32)
+        self._ck(self.L.alz_gnn_score_rollup(self.h, int(kind), _ptr(out), cap, C.byref(n)), "alz_gnn_score_rollup")
+        return out[: n.value].copy()
+
+    def gnn_score_rollup_device(self, kind):
+        """alz_gnn_score_rollup_device: (device pointer, scores)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        self._ck(self.L.alz_gnn_score_rollup_device(self.h, int(kind), C.byref(p), C.byref(n)),
+                 "alz_gnn_score_rollup_device")
+        return p.value, n.value
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -1,6 +1,7 @@
 // alz_gnn.cu — GNN anomaly pass over the flushed service graph (docs/SPEC.md §6;
 // not in the reference: north_star's extension). 2-layer GraphSAGE-mean, d = 64,
-// fixed seeded weights, per-edge score.
+// fixed seeded weights, per-edge score. The same pass scores a window, tier or span
+// rollup's rows (docs/SPEC.md §15): it is a function of the rows it is given.
 //
 //   nodes   : 2 node keys per edge -> sort -> unique (ascending (kind,value))
 //   stats   : per-node in/out count, 5xx, latency sum, degree  (u64 atomics: exact,
@@ -489,32 +490,58 @@ struct alz_gnn_state {
   uint32_t* d_nv = nullptr;      // node count of the last pass, on the device
 };
 
+// The buffers sized by rows (cap_e) and nodes (cap_v = 2 cap_e), and the CUB scratch of the sorts and scans over
+// up to cap_v + 1 items. The first failed allocation's status; what was allocated stays for free_row_buffers.
+static cudaError_t alloc_row_buffers(alz_gnn_state* g, uint32_t cap_e) {
+  g->cap_e = cap_e;
+  g->cap_v = 2 * cap_e;
+  const size_t E = g->cap_e, V = g->cap_v;
+  cudaError_t e = cudaSuccess;
+  auto get = [&e](auto** p, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(p, bytes); };
+  get(&g->d_nk, V * 8);
+  get(&g->d_nk_sorted, V * 8);
+  get(&g->d_nodes, V * 8);
+  get(&g->d_dst_key, E * 8);
+  get(&g->d_dst_sorted, E * 8);
+  get(&g->d_flags, V * 4);
+  get(&g->d_pos, V * 4);
+  get(&g->d_iota, V * 4);
+  get(&g->d_vals, V * 4);
+  get(&g->d_src_idx, E * 4);
+  get(&g->d_in_deg, (V + 1) * 4);
+  get(&g->d_rowptr, (V + 1) * 4);
+  get(&g->d_col, E * 4);
+  get(&g->d_sorted_edge, E * 4);
+  get(&g->d_stats, V * 8 * 8);
+  for (int i = 0; i < 3; ++i) get(&g->d_h[i], V * D * 4);
+  get(&g->d_scores, E * 4);
+  g->tmp_bytes = std::max(sort_pairs_temp_bytes((uint32_t)V), scan_temp_bytes((uint32_t)V + 1));
+  get(&g->d_tmp, g->tmp_bytes);
+  return e;
+}
+
+static void free_row_buffers(alz_gnn_state* g) {
+  cudaFree(g->d_nk); cudaFree(g->d_nk_sorted); cudaFree(g->d_nodes); cudaFree(g->d_dst_key); cudaFree(g->d_dst_sorted);
+  cudaFree(g->d_flags); cudaFree(g->d_pos); cudaFree(g->d_iota); cudaFree(g->d_vals); cudaFree(g->d_src_idx);
+  cudaFree(g->d_in_deg); cudaFree(g->d_rowptr); cudaFree(g->d_col); cudaFree(g->d_sorted_edge); cudaFree(g->d_stats);
+  for (int i = 0; i < 3; ++i) cudaFree(g->d_h[i]);
+  cudaFree(g->d_scores); cudaFree(g->d_tmp);
+  g->d_nk = g->d_nk_sorted = g->d_nodes = g->d_dst_key = g->d_dst_sorted = nullptr;
+  g->d_flags = g->d_pos = g->d_iota = g->d_vals = g->d_src_idx = nullptr;
+  g->d_in_deg = g->d_rowptr = g->d_col = g->d_sorted_edge = nullptr;
+  g->d_stats = nullptr;
+  g->d_h[0] = g->d_h[1] = g->d_h[2] = nullptr;
+  g->d_scores = nullptr;
+  g->d_tmp = nullptr;
+  g->cap_e = g->cap_v = 0;
+  g->tmp_bytes = 0;
+}
+
 static int gnn_init_impl(alz_handle* h) {
   alz_gnn_state* g = new alz_gnn_state();
   h->gnn = g;
-  g->cap_e = h->cfg.max_edges;
-  g->cap_v = 2 * h->cfg.max_edges;
-  const size_t E = g->cap_e, V = g->cap_v;
-  CK(cudaMalloc(&g->d_nk, V * 8));
-  CK(cudaMalloc(&g->d_nk_sorted, V * 8));
-  CK(cudaMalloc(&g->d_nodes, V * 8));
-  CK(cudaMalloc(&g->d_dst_key, E * 8));
-  CK(cudaMalloc(&g->d_dst_sorted, E * 8));
-  CK(cudaMalloc(&g->d_flags, V * 4));
-  CK(cudaMalloc(&g->d_pos, V * 4));
-  CK(cudaMalloc(&g->d_iota, V * 4));
-  CK(cudaMalloc(&g->d_vals, V * 4));
-  CK(cudaMalloc(&g->d_src_idx, E * 4));
-  CK(cudaMalloc(&g->d_in_deg, (V + 1) * 4));
-  CK(cudaMalloc(&g->d_rowptr, (V + 1) * 4));
-  CK(cudaMalloc(&g->d_col, E * 4));
-  CK(cudaMalloc(&g->d_sorted_edge, E * 4));
-  CK(cudaMalloc(&g->d_stats, V * 8 * 8));
-  for (int i = 0; i < 3; ++i) CK(cudaMalloc(&g->d_h[i], V * D * 4));
-  CK(cudaMalloc(&g->d_scores, E * 4));
+  CK(alloc_row_buffers(g, h->cfg.max_edges));
   CK(cudaMalloc(&g->d_nv, 4));
-  g->tmp_bytes = std::max(sort_pairs_temp_bytes((uint32_t)V), scan_temp_bytes((uint32_t)V + 1));
-  CK(cudaMalloc(&g->d_tmp, g->tmp_bytes));
   const Weights w = make_weights();
   for (int l = 0; l < 2; ++l) {
     CK(cudaMalloc(&g->d_W[l], 128 * D * 4));
@@ -560,49 +587,70 @@ static int gnn_init(alz_handle* h) {
 void alz_internal_free_gnn(alz_handle* h) {
   alz_gnn_state* g = h->gnn;
   if (!g) return;
-  cudaFree(g->d_nk); cudaFree(g->d_nk_sorted); cudaFree(g->d_nodes); cudaFree(g->d_dst_key); cudaFree(g->d_dst_sorted);
-  cudaFree(g->d_flags); cudaFree(g->d_pos); cudaFree(g->d_iota); cudaFree(g->d_vals); cudaFree(g->d_src_idx);
-  cudaFree(g->d_in_deg); cudaFree(g->d_rowptr); cudaFree(g->d_col); cudaFree(g->d_sorted_edge); cudaFree(g->d_stats);
-  for (int i = 0; i < 3; ++i) cudaFree(g->d_h[i]);
+  free_row_buffers(g);
   for (int l = 0; l < 2; ++l) { cudaFree(g->d_W[l]); cudaFree(g->d_b[l]); cudaFree(g->d_Wcan[l]); }
-  cudaFree(g->d_a); cudaFree(g->d_scores); cudaFree(g->d_tmp); cudaFree(g->d_nv);
+  cudaFree(g->d_a); cudaFree(g->d_nv);
   delete g;
   h->gnn = nullptr;
 }
 
-// CSR build + 2 layers + scoring over the last flushed window (h->d_out). Nothing here waits for the device:
-// the node count lives in device memory and every kernel reads it there; buffers and grids are sized by the
-// bound 2 * n_e the host knows. Sorts only cover the key bits that can differ.
+// The CUB calls take int item counts over 2 * n_e node keys: at most 2^30 - 1 rows per pass.
+constexpr uint32_t kMaxRows = (1u << 30) - 1u;
+
+// A rollup can have more rows than max_edges (docs/SPEC.md §12). The row- and node-sized buffers and the CUB scratch
+// then grow to n + n/2 rows; the weights, the layer path and the node count stay. The state never shrinks. A failed
+// growth frees the whole state, as a failed gnn_init does, and the next call rebuilds it at max_edges.
+static int gnn_grow(alz_handle* h, uint32_t n_e) {
+  alz_gnn_state* g = h->gnn;
+  CK(cudaStreamSynchronize(h->stream));   // the last pass may still read the buffers
+  free_row_buffers(g);
+  if (alloc_row_buffers(g, (uint32_t)std::min<uint64_t>(kMaxRows, (uint64_t)n_e + n_e / 2u)) != cudaSuccess) {
+    h->last_err = std::string("alz_gnn_score_rollup: ") + cudaGetErrorString(cudaGetLastError());
+    alz_internal_free_gnn(h);
+    return ALZ_E_NOMEM;
+  }
+  return ALZ_OK;
+}
+
+// CSR build + 2 layers + scoring over n_e edge rows in device memory: the last flushed window (h->d_out) or a
+// rollup's rows (docs/SPEC.md §15). Nothing here waits for the device unless the state grows: the node count lives
+// in device memory and every kernel reads it there; buffers and grids are sized by the bound 2 * n_e the host knows.
+// Sorts only cover the key bits that can differ.
 static int bits_for(uint64_t x) { int b = 1; while (b < 64 && (x >> b) != 0) ++b; return b; }
 
-static int gnn_run(alz_handle* h) {
+static int gnn_run(alz_handle* h, const alz_edge_out* rows, size_t n_rows) {
   int rc = gnn_init(h);
   if (rc != ALZ_OK) return rc;
+  if (n_rows > kMaxRows) return ALZ_E_CAPACITY;
+  if (n_rows > h->gnn->cap_e) {
+    rc = gnn_grow(h, (uint32_t)n_rows);
+    if (rc != ALZ_OK) return rc;
+  }
   alz_gnn_state* g = h->gnn;
   cudaStream_t s = h->stream;
-  const uint32_t n_e = h->last_n_edges;
+  const uint32_t n_e = (uint32_t)n_rows;
   g->n_e = n_e;
   g->n_v = 0;
   g->n_v_known = n_e == 0;
   if (n_e == 0) { CK(cudaMemsetAsync(g->d_nv, 0, 4, s)); return ALZ_OK; }
-  if (n_e > g->cap_e) return ALZ_E_CAPACITY;
   const unsigned grid = (unsigned)h->sms * 4;
   const uint32_t n2 = 2 * n_e;   // bound on the node count
   // nodes: (kind 2 bits << 32 | value 32 bits): 34 key bits
-  edge_node_keys_kernel<<<grid, 256, 0, s>>>(h->d_out, n_e, g->d_nk);
+  edge_node_keys_kernel<<<grid, 256, 0, s>>>(rows, n_e, g->d_nk);
   launch_iota(g->d_iota, n2, h->sms, s);
-  sort_pairs(g->d_tmp, g->tmp_bytes, g->d_nk, g->d_nk_sorted, g->d_iota, g->d_vals, n2, s, 34);
-  launch_unique_sorted(g->d_nk_sorted, n2, g->d_flags, g->d_pos, g->d_nodes, g->d_tmp, g->tmp_bytes, h->sms, s);
+  CK(sort_pairs(g->d_tmp, g->tmp_bytes, g->d_nk, g->d_nk_sorted, g->d_iota, g->d_vals, n2, s, 34));
+  CK(launch_unique_sorted(g->d_nk_sorted, n2, g->d_flags, g->d_pos, g->d_nodes, g->d_tmp, g->tmp_bytes, h->sms, s));
   node_count_kernel<<<1, 32, 0, s>>>(g->d_pos, g->d_flags, n2, g->d_nv);
   // stats + CSR by destination (destination index < n2)
   CK(cudaMemsetAsync(g->d_stats, 0, (size_t)n2 * 64, s));
   CK(cudaMemsetAsync(g->d_in_deg, 0, ((size_t)n2 + 1) * 4, s));
-  edge_stats_kernel<<<grid, 256, 0, s>>>(h->d_out, n_e, g->d_nodes, g->d_nv, g->d_src_idx, g->d_dst_key, g->d_stats,
+  edge_stats_kernel<<<grid, 256, 0, s>>>(rows, n_e, g->d_nodes, g->d_nv, g->d_src_idx, g->d_dst_key, g->d_stats,
                                          g->d_in_deg);
   launch_iota(g->d_iota, n_e, h->sms, s);
-  sort_pairs(g->d_tmp, g->tmp_bytes, g->d_dst_key, g->d_dst_sorted, g->d_iota, g->d_sorted_edge, n_e, s, bits_for(n2));
+  CK(sort_pairs(g->d_tmp, g->tmp_bytes, g->d_dst_key, g->d_dst_sorted, g->d_iota, g->d_sorted_edge, n_e, s,
+                bits_for(n2)));
   csr_cols_kernel<<<grid, 256, 0, s>>>(g->d_sorted_edge, g->d_src_idx, n_e, g->d_col);
-  exclusive_scan_u32(g->d_tmp, g->tmp_bytes, g->d_in_deg, g->d_rowptr, n2 + 1, s);
+  CK(exclusive_scan_u32(g->d_tmp, g->tmp_bytes, g->d_in_deg, g->d_rowptr, n2 + 1, s));
   // features, layers, scores
   node_features_kernel<<<grid, 256, 0, s>>>(g->d_nodes, g->d_stats, g->d_nv, g->d_h[0]);
   for (int l = 0; l < 2; ++l) {
@@ -614,41 +662,74 @@ static int gnn_run(alz_handle* h) {
       sage_layer_kernel<<<grid, 256, 0, s>>>(g->d_h[l], g->d_h[l + 1], g->d_rowptr, g->d_col, g->d_W[l], g->d_b[l], g->d_nv);
     }
   }
-  edge_score_kernel<<<grid, 256, 0, s>>>(h->d_out, n_e, g->d_src_idx, g->d_dst_key, g->d_h[2], g->d_a, g->c,
+  edge_score_kernel<<<grid, 256, 0, s>>>(rows, n_e, g->d_src_idx, g->d_dst_key, g->d_h[2], g->d_a, g->c,
                                          g->d_scores);
   h->launches += 12;
   CK(cudaGetLastError());
   return ALZ_OK;
 }
 
-static int gnn_score_device_locked(alz_handle* h, const float** dev_scores, size_t* n_out) {
+// the pass over rows; *n_out = its rows (0 without a GNN state). Caller holds h->mu.
+static int gnn_score_locked(alz_handle* h, const alz_edge_out* rows, size_t n_rows, const float** dev_scores,
+                            size_t* n_out) {
   CK(cudaSetDevice(h->device));
-  int rc = gnn_run(h);
-  *n_out = h->gnn ? h->gnn->n_e : 0;
+  int rc = gnn_run(h, rows, n_rows);
+  *n_out = h->gnn ? n_rows : 0;
   if (rc != ALZ_OK) return rc;
   if (dev_scores) *dev_scores = h->gnn->d_scores;
+  return ALZ_OK;
+}
+
+// the pass over the rows the last rollup of `kind` returned (docs/SPEC.md §15)
+static int gnn_score_rollup_locked(alz_handle* h, uint32_t kind, const float** dev_scores, size_t* n_out) {
+  *n_out = 0;
+  const alz_edge_out* rows = nullptr;
+  size_t n_rows = 0;
+  const int rc = alz_internal_rollup_rows(h, kind, &rows, &n_rows);
+  if (rc != ALZ_OK) return rc;
+  return gnn_score_locked(h, rows, n_rows, dev_scores, n_out);
+}
+
+// scores on the device into `scores` (cap of them) and a wait; the usual cap rule
+static int copy_scores(alz_handle* h, const float* d, float* scores, size_t cap, size_t n) {
+  if (n > cap) return ALZ_E_CAPACITY;
+  if (n) CK(cudaMemcpyAsync(scores, d, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }
 
 extern "C" int alz_gnn_score_device(alz_handle* h, const float** dev_scores, size_t* n_out) {
   if (!h || !n_out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
-  return gnn_score_device_locked(h, dev_scores, n_out);
+  return gnn_score_locked(h, h->d_out, h->last_n_edges, dev_scores, n_out);
 }
 
 extern "C" int alz_gnn_score(alz_handle* h, float* edge_scores, size_t cap, size_t* n_out) {
   if (!h || !n_out || (!edge_scores && cap)) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
   const float* d = nullptr;
-  int rc = gnn_score_device_locked(h, &d, n_out);
+  int rc = gnn_score_locked(h, h->d_out, h->last_n_edges, &d, n_out);
   if (rc != ALZ_OK) return rc;
-  if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(edge_scores, d, *n_out * 4, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return ALZ_OK;
+  return copy_scores(h, d, edge_scores, cap, *n_out);
 }
 
-// debug/test: node keys ((kind << 32) | value, ascending) and the layer-2 embeddings of the last alz_gnn_score
+extern "C" int alz_gnn_score_rollup_device(alz_handle* h, uint32_t kind, const float** dev_scores, size_t* n_out) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  return gnn_score_rollup_locked(h, kind, dev_scores, n_out);
+}
+
+extern "C" int alz_gnn_score_rollup(alz_handle* h, uint32_t kind, float* scores, size_t cap, size_t* n_out) {
+  if (!h || !n_out || (!scores && cap)) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const float* d = nullptr;
+  int rc = gnn_score_rollup_locked(h, kind, &d, n_out);
+  if (rc != ALZ_OK) return rc;
+  return copy_scores(h, d, scores, cap, *n_out);
+}
+
+// debug/test: node keys ((kind << 32) | value, ascending) and the layer-2 embeddings of the last GNN pass, over a
+// window or a rollup
 extern "C" int alz_gnn_nodes(alz_handle* h, uint64_t* node_keys, float* h2, size_t cap, size_t* n_out) {
   if (!h || !n_out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);

@@ -142,6 +142,9 @@ const uint64_t* alz_internal_merged_clock(alz_handle* h);
 // the flush's roll advances it; null without a window clock. Nothing happens with the history off. Caller holds h->mu.
 // With tiers configured the window is also the next input of tier 1 (docs/SPEC.md §13).
 int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk);
+// The rows the last rollup of `kind` (ALZ_ROLLUP_*) returned with ALZ_OK, on the device: *rows, *n (docs/SPEC.md
+// §15). ALZ_E_INVAL for an unknown kind; ALZ_E_STATE when there are none. Caller holds h->mu.
+int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n);
 void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_span(alz_handle* h);

@@ -518,11 +518,13 @@ void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s) {
   if (n == 0) return;
   iota_kernel<<<grid_for(sms, 4), 256, 0, s>>>(out, n);
 }
-void launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
-                          void* temp, size_t temp_bytes, int sms, cudaStream_t s) {
+cudaError_t launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
+                                 void* temp, size_t temp_bytes, int sms, cudaStream_t s) {
   flag_heads_kernel<<<grid_for(sms, 4), 256, 0, s>>>(sorted, n, flags);
-  exclusive_scan_u32(temp, temp_bytes, flags, pos, n, s);
+  const cudaError_t e = exclusive_scan_u32(temp, temp_bytes, flags, pos, n, s);
+  if (e != cudaSuccess) return e;
   scatter_heads_kernel<<<grid_for(sms, 4), 256, 0, s>>>(sorted, flags, pos, n, out);
+  return cudaSuccess;
 }
 void launch_gather_edges(const EdgeTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
                          alz_edge_out* out, int sms, cudaStream_t s) {

@@ -42,8 +42,8 @@ void launch_fold_add(const PairTable& pairs, const EdgeTable& edges, Counters* c
 void launch_ep_patch(EpEntry* tab, const void* patch, uint32_t n, int sms, cudaStream_t s);
 void launch_iota(uint32_t* out, uint32_t n, int sms, cudaStream_t s);
 // the distinct keys of sorted[0, n) into out, in order: out has pos[n - 1] + flags[n - 1] entries (alz_kernels.cu)
-void launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
-                          void* temp, size_t temp_bytes, int sms, cudaStream_t s);
+cudaError_t launch_unique_sorted(const uint64_t* sorted, uint32_t n, uint32_t* flags, uint32_t* pos, uint64_t* out,
+                                 void* temp, size_t temp_bytes, int sms, cudaStream_t s);   // the scan's status
 void launch_gather_edges(const EdgeTable& edges, const uint64_t* keys, const uint32_t* rows, uint32_t n_live,
                          alz_edge_out* out, int sms, cudaStream_t s);
 // single-rank flush scratch: pair rows bucketed by edge row (alz_kernels.cu, emit_edges_kernel)
@@ -66,8 +66,10 @@ void launch_synth_owned(const alz_synth_view& v, uint64_t first, uint64_t n, uin
                         alz_l7_rec* out, uint64_t cap, unsigned long long* n_written, int sms, cudaStream_t s);
 // radix sort of (edge key, row) pairs by key (alz_sort.cu)
 size_t sort_pairs_temp_bytes(uint32_t n);
-void sort_pairs(void* temp, size_t temp_bytes, const uint64_t* keys_in, uint64_t* keys_out,
-                const uint32_t* vals_in, uint32_t* vals_out, uint32_t n, cudaStream_t s, int end_bit = 64);
+// both return CUB's status: cudaErrorInvalidValue, with nothing enqueued, when temp_bytes is too small
+cudaError_t sort_pairs(void* temp, size_t temp_bytes, const uint64_t* keys_in, uint64_t* keys_out,
+                       const uint32_t* vals_in, uint32_t* vals_out, uint32_t n, cudaStream_t s, int end_bit = 64);
 size_t scan_temp_bytes(uint32_t n);
-void exclusive_scan_u32(void* temp, size_t temp_bytes, const uint32_t* in, uint32_t* out, uint32_t n, cudaStream_t s);
+cudaError_t exclusive_scan_u32(void* temp, size_t temp_bytes, const uint32_t* in, uint32_t* out, uint32_t n,
+                               cudaStream_t s);
 }  // namespace alz

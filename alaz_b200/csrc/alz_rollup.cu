@@ -65,6 +65,9 @@ struct RollupScratch {
   size_t tmp_bytes = 0;
   alz_edge_out* d_sum = nullptr;              // the last rollup's rows
   size_t sum_rows = 0;
+  // the last call of this kind returned ALZ_OK with held_rows rows in d_sum: what alz_gnn_score_rollup scores
+  bool held = false;
+  size_t held_rows = 0;
 };
 
 // the clock of a tier's open block and of each of its entries: the oldest and newest covered window's clocks
@@ -601,24 +604,51 @@ static int rollup_locked(alz_handle* h, uint32_t level, uint32_t k, size_t* n_ou
   return rc;
 }
 
-// A rollup entry point: lock, set the device and run the rollup (run(&rows), which sets *n_out). Into out (to_host):
-// ALZ_E_CAPACITY when the rows do not fit, and nothing is written; else *dev_rows (when not null) = the device rows.
+// The scratch of a kind of rollup (ALZ_ROLLUP_*), or null when it has none
+static RollupScratch* scratch_of(alz_handle* h, uint32_t kind) {
+  switch (kind) {
+    case ALZ_ROLLUP_WINDOWS: return h->roll ? &h->roll->sc : nullptr;
+    case ALZ_ROLLUP_TIER: return h->tiers ? &h->tiers->sc : nullptr;
+    case ALZ_ROLLUP_SPAN: return h->span ? &h->span->sc : nullptr;
+    default: return nullptr;
+  }
+}
+
+static uint32_t kind_of_tier(uint32_t tier) { return tier == 0 ? ALZ_ROLLUP_WINDOWS : ALZ_ROLLUP_TIER; }
+
+int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n) {
+  if (kind > ALZ_ROLLUP_SPAN) return ALZ_E_INVAL;
+  const RollupScratch* sc = scratch_of(h, kind);
+  if (!sc || !sc->held) return ALZ_E_STATE;
+  *rows = sc->d_sum;
+  *n = sc->held_rows;
+  return ALZ_OK;
+}
+
+// A rollup entry point of a kind (ALZ_ROLLUP_*): lock, set the device and run the rollup (run(&rows), which sets
+// *n_out). Into out (to_host): ALZ_E_CAPACITY when the rows do not fit, and nothing is written; else *dev_rows (when
+// not null) = the device rows. The kind's scratch holds rows to score only after a call that returns ALZ_OK.
 template <class Run>
-static int rollup_call(alz_handle* h, bool to_host, alz_edge_out* out, size_t cap, const alz_edge_out** dev_rows,
-                       size_t* n_out, Run run) {
-  if (!h || !n_out || (!out && cap)) return ALZ_E_INVAL;
+static int rollup_call(alz_handle* h, uint32_t kind, bool to_host, alz_edge_out* out, size_t cap,
+                       const alz_edge_out** dev_rows, size_t* n_out, Run run) {
+  if (!h) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
+  if (RollupScratch* sc = scratch_of(h, kind)) sc->held = false;
+  if (!n_out || (!out && cap)) return ALZ_E_INVAL;
   CK(cudaSetDevice(h->device));
   const alz_edge_out* rows = nullptr;
   const int rc = run(&rows);
   if (rc != ALZ_OK) return rc;
-  if (!to_host) {
-    if (dev_rows) *dev_rows = rows;
-    return ALZ_OK;
+  if (to_host) {
+    if (*n_out > cap) return ALZ_E_CAPACITY;
+    if (*n_out) CK(cudaMemcpyAsync(out, rows, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  } else if (dev_rows) {
+    *dev_rows = rows;
   }
-  if (*n_out > cap) return ALZ_E_CAPACITY;
-  if (*n_out) CK(cudaMemcpyAsync(out, rows, *n_out * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  RollupScratch* sc = scratch_of(h, kind);
+  sc->held = true;
+  sc->held_rows = *n_out;
   return ALZ_OK;
 }
 
@@ -634,13 +664,13 @@ extern "C" int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, s
 
 extern "C" int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
                                              size_t* n_out, alz_rollup_info* info) {
-  return rollup_call(h, false, nullptr, 0, dev_rows, n_out,
+  return rollup_call(h, kind_of_tier(tier), false, nullptr, 0, dev_rows, n_out,
                      [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
 }
 
 extern "C" int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap,
                                       size_t* n_out, alz_rollup_info* info) {
-  return rollup_call(h, true, out, cap, nullptr, n_out,
+  return rollup_call(h, kind_of_tier(tier), true, out, cap, nullptr, n_out,
                      [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
 }
 
@@ -965,12 +995,12 @@ static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, 
 
 extern "C" int alz_window_rollup_span_device(alz_handle* h, uint64_t windows, uint32_t mode,
                                              const alz_edge_out** dev_rows, size_t* n_out, alz_span_info* info) {
-  return rollup_call(h, false, nullptr, 0, dev_rows, n_out,
+  return rollup_call(h, ALZ_ROLLUP_SPAN, false, nullptr, 0, dev_rows, n_out,
                      [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
 }
 
 extern "C" int alz_window_rollup_span(alz_handle* h, uint64_t windows, uint32_t mode, alz_edge_out* out, size_t cap,
                                       size_t* n_out, alz_span_info* info) {
-  return rollup_call(h, true, out, cap, nullptr, n_out,
+  return rollup_call(h, ALZ_ROLLUP_SPAN, true, out, cap, nullptr, n_out,
                      [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
 }

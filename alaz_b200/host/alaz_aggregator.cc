@@ -299,9 +299,9 @@ int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vecto
 }
 
 // call(out, cap, &n) into roll_, grown once when the rows do not fit (ALZ_E_CAPACITY with n = the rows there are;
-// nothing was written), then the rows to the data store
+// nothing was written), with_scores the GNN pass over those rows, then the rows to the data store
 template <class Call>
-int Aggregator::PersistRollup(Call call) {
+int Aggregator::PersistRollup(uint32_t kind, bool with_scores, Call call) {
   size_t n = 0;
   int rc = call(roll_.data(), roll_.size(), &n);
   if (rc == ALZ_E_CAPACITY && n > roll_.size()) {
@@ -309,23 +309,30 @@ int Aggregator::PersistRollup(Call call) {
     rc = call(roll_.data(), roll_.size(), &n);
   }
   if (rc != ALZ_OK) return rc;
-  return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, nullptr)) : ALZ_OK;
+  if (with_scores && n) {
+    scores_.resize(n);
+    size_t ns = 0;
+    rc = alz_gnn_score_rollup(h_, kind, scores_.data(), n, &ns);
+    if (rc != ALZ_OK) return rc;
+  }
+  return ds_ ? ds_->PersistEdgeWindow(ToEdges(roll_.data(), n, with_scores ? scores_.data() : nullptr)) : ALZ_OK;
 }
 
-int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info) {
+int Aggregator::Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info, bool with_scores) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);
-  return PersistRollup([&](alz_edge_out* out, size_t cap, size_t* n) {
-    return alz_window_rollup_tier(h_, tier, k, out, cap, n, info);
-  });
+  return PersistRollup(tier == 0 ? ALZ_ROLLUP_WINDOWS : ALZ_ROLLUP_TIER, with_scores,
+                       [&](alz_edge_out* out, size_t cap, size_t* n) {
+                         return alz_window_rollup_tier(h_, tier, k, out, cap, n, info);
+                       });
 }
 
 // A span is made of retained entries and open blocks, each inside the span SetHistory's hold covers, so the ids it
 // carries are held as those of a tier rollup are.
-int Aggregator::RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info) {
+int Aggregator::RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info, bool with_scores) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);
-  return PersistRollup([&](alz_edge_out* out, size_t cap, size_t* n) {
+  return PersistRollup(ALZ_ROLLUP_SPAN, with_scores, [&](alz_edge_out* out, size_t cap, size_t* n) {
     return alz_window_rollup_span(h_, windows, mode, out, cap, n, info);
   });
 }

@@ -111,12 +111,14 @@ class Aggregator {
   // Returns 0 or the status of the call that refused its part (alz_window_history, alz_window_history_tiers).
   int SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers = {});
   // the last k entries of `tier` (0: flushed windows, 1..n: the tiers) added up per edge go to
-  // ds->PersistEdgeWindow, as a flush's rows do. info may be null. Returns 0 or an alz_status.
-  int Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info = nullptr);
+  // ds->PersistEdgeWindow, as a flush's rows do. info may be null. with_scores: each row's Score is the GNN anomaly
+  // score of the row in the rollup's graph (docs/SPEC.md §15), as Flush(true) scores a window. Returns 0 or an
+  // alz_status.
+  int Rollup(uint32_t tier, uint32_t k, alz_rollup_info* info = nullptr, bool with_scores = false);
   // the last `windows` flushed windows up to now (docs/SPEC.md §14: ALZ_SPAN_AT_MOST or ALZ_SPAN_AT_LEAST; the span
   // covered is info->r.windows), summed from every retained piece, go to ds->PersistEdgeWindow as a flush's rows do.
-  // info may be null. Returns 0 or an alz_status.
-  int RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info = nullptr);
+  // info may be null; with_scores as in Rollup. Returns 0 or an alz_status.
+  int RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info = nullptr, bool with_scores = false);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -130,9 +132,10 @@ class Aggregator {
 
  private:
   int SubmitBatch();   // requires mu_
-  // a rollup call(out, cap, &n) into roll_, then its rows to ds->PersistEdgeWindow; requires mu_
+  // a rollup call(out, cap, &n) of `kind` (ALZ_ROLLUP_*) into roll_, with_scores its GNN scores, then its rows to
+  // ds->PersistEdgeWindow; requires mu_
   template <class Call>
-  int PersistRollup(Call call);
+  int PersistRollup(uint32_t kind, bool with_scores, Call call);
   // rows -> EdgeWindow with the UIDs the interners hold (scores: one per row, or null)
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
   // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by

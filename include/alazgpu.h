@@ -388,6 +388,26 @@ int alz_gnn_score_device(alz_handle* h, const float** dev_scores, size_t* n_out)
 /* quantiles from the histogram, the same float64 interpolation the scores use */
 int alz_edge_quantiles(const alz_edge_out* e, const double* qs, size_t nq, double* out_ns);
 
+/* ---- GNN anomaly pass over a rollup (docs/SPEC.md §15) ---------------------------
+ * The pass of §6 over the rows that the last rollup call of a kind returned with ALZ_OK: nodes are the distinct edge
+ * ends of those rows, and scores[i] belongs to row i of the rollup (ascending packed-key order). The result is a
+ * function of the rows and their order alone, so a rollup of one window scores bit for bit as alz_gnn_score scored
+ * that window after its flush. The rows stay scorable until the next call of that kind; window rollups' rows also
+ * go with an alz_window_history call with other values, tier rollups' with an alz_window_history_tiers call with
+ * other values (span rows survive both). A call of that kind that does not return ALZ_OK (ALZ_E_CAPACITY of a host
+ * call, k = 0, ...) leaves nothing to score: ALZ_E_STATE, as before any such call. ALZ_E_INVAL for an unknown kind.
+ * A 0-row rollup scores to *n_out = 0. *n_out is always set; cap too small: ALZ_E_CAPACITY, nothing written. Reads
+ * only: the rollup's rows, every retained entry, the open blocks and the window are unchanged. A rollup above
+ * max_edges rows grows the GNN state (it never shrinks); no memory: ALZ_E_NOMEM. Scores and alz_gnn_nodes refer to
+ * the last GNN pass on the handle, window or rollup; device scores stay valid until the next GNN call. Several
+ * ranks hold the same rollup rows, so they get the same scores with no collective. */
+#define ALZ_ROLLUP_WINDOWS 0u   /* alz_window_rollup*, and alz_window_rollup_tier* with tier 0 */
+#define ALZ_ROLLUP_TIER    1u   /* alz_window_rollup_tier* with tier >= 1 */
+#define ALZ_ROLLUP_SPAN    2u   /* alz_window_rollup_span* */
+int alz_gnn_score_rollup(alz_handle* h, uint32_t kind, float* scores, size_t cap, size_t* n_out);
+/* same, scores left on the device (valid until the next GNN call on this handle) */
+int alz_gnn_score_rollup_device(alz_handle* h, uint32_t kind, const float** dev_scores, size_t* n_out);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces
