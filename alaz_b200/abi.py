@@ -129,6 +129,14 @@ SPAN_AT_MOST, SPAN_AT_LEAST = 0, 1
 ROLLUP_WINDOWS, ROLLUP_TIER, ROLLUP_SPAN = 0, 1, 2   # alz_gnn_score_rollup kinds
 
 
+class TopInfo(C.Structure):
+    """alz_top_info."""
+    _fields_ = [("scored", C.c_uint64), ("above", C.c_uint64)]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

@@ -26,7 +26,8 @@ EXPORTS = [
     "alz_window_clock", "alz_window_epoch", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
     "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device", "alz_window_tier_state",
     "alz_window_rollup_span", "alz_window_rollup_span_device", "alz_gnn_score",
-    "alz_gnn_score_device", "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_gnn_score_device", "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_gnn_top", "alz_gnn_top_device",
+    "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -80,7 +81,12 @@ def load(rebuild=False):
         "alz_gnn_score_device": ([vp, pp, C.POINTER(sz)], i),
         "alz_gnn_score_rollup": ([vp, u32, vp, sz, C.POINTER(sz)], i),
         "alz_gnn_score_rollup_device": ([vp, u32, pp, C.POINTER(sz)], i),
+        "alz_gnn_top": ([vp, u32, C.c_float, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_gnn_top_device": ([vp, u32, C.c_float, pp, pp, pp, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_gnn_top_rollup": ([vp, u32, u32, C.c_float, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_gnn_top_rollup_device": ([vp, u32, u32, C.c_float, pp, pp, pp, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
         "alz_gnn_nodes": ([vp, vp, vp, sz, C.POINTER(sz)], i),
+        "alz_debug_top_scores": ([vp, vp, sz, u32, C.c_float, vp, sz, C.POINTER(sz), C.POINTER(u64)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -115,7 +121,8 @@ def load(rebuild=False):
                   "alz_submit_tcp_raw", "alz_window_history", "alz_window_rollup", "alz_window_rollup_device",
                   "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device",
                   "alz_window_tier_state", "alz_window_rollup_span", "alz_window_rollup_span_device",
-                  "alz_gnn_score_rollup", "alz_gnn_score_rollup_device"):
+                  "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_gnn_top", "alz_gnn_top_device",
+                  "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_debug_top_scores"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -389,6 +396,48 @@ class Handle:
         self._ck(self.L.alz_gnn_score_rollup_device(self.h, int(kind), C.byref(p), C.byref(n)),
                  "alz_gnn_score_rollup_device")
         return p.value, n.value
+
+    # ---- top anomalous rows (alz_gnn.cu, docs/SPEC.md §16)
+    def _top(self, fn, args, k, min_score):
+        """fn(h, *args, k, min_score, rows, scores, index, cap, &n, &info): (rows, scores, index, info dict). The first
+        call offers room for min(k, 65536) results; when more came out, the call is repeated with room for all."""
+        f, n, info = getattr(self.L, fn), C.c_size_t(0), abi.TopInfo()
+        cap = min(int(k), 1 << 16)
+        while True:
+            rows = np.zeros(cap, dtype=abi.EDGE_OUT)
+            scores = np.zeros(cap, dtype=np.float32)
+            index = np.zeros(cap, dtype=np.uint32)
+            rc = self._ck(f(self.h, *args, int(k), float(min_score), _ptr(rows), _ptr(scores), _ptr(index), cap,
+                            C.byref(n), C.byref(info)), fn, allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                m = n.value
+                return rows[:m].copy(), scores[:m].copy(), index[:m].copy(), info.as_dict()
+            cap = n.value
+
+    def _top_device(self, fn, args, k, min_score):
+        """fn(h, *args, k, min_score, &rows, &scores, &index, &n, &info): (rows, scores, index device pointers, results,
+        info dict)."""
+        pr, ps, pi, n, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), abi.TopInfo()
+        self._ck(getattr(self.L, fn)(self.h, *args, int(k), float(min_score), C.byref(pr), C.byref(ps), C.byref(pi),
+                                     C.byref(n), C.byref(info)), fn)
+        return pr.value, ps.value, pi.value, n.value, info.as_dict()
+
+    def gnn_top(self, k, min_score=0.0):
+        """alz_gnn_top over the last flushed window: (rows, scores, index, info dict), rank order."""
+        return self._top("alz_gnn_top", (), k, min_score)
+
+    def gnn_top_device(self, k, min_score=0.0):
+        """alz_gnn_top_device: (rows, scores, index device pointers, results, info dict)."""
+        return self._top_device("alz_gnn_top_device", (), k, min_score)
+
+    def gnn_top_rollup(self, kind, k, min_score=0.0):
+        """alz_gnn_top_rollup over the rows the last rollup of `kind` (abi.ROLLUP_*) returned: (rows, scores, index,
+        info dict), rank order."""
+        return self._top("alz_gnn_top_rollup", (int(kind),), k, min_score)
+
+    def gnn_top_rollup_device(self, kind, k, min_score=0.0):
+        """alz_gnn_top_rollup_device: (rows, scores, index device pointers, results, info dict)."""
+        return self._top_device("alz_gnn_top_rollup_device", (int(kind),), k, min_score)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -21,6 +21,8 @@
 #include <mutex>
 #include <vector>
 
+#include <cub/block/block_scan.cuh>
+
 #include "alz_handle.h"
 #include "alz_mbar.cuh"
 
@@ -488,6 +490,11 @@ struct alz_gnn_state {
   uint32_t n_v = 0, n_e = 0;
   bool n_v_known = true;
   uint32_t* d_nv = nullptr;      // node count of the last pass, on the device
+  // top anomalous rows (docs/SPEC.md §16): the result of the last selection, top_cap rows each; grown on demand
+  alz_edge_out* d_top_rows = nullptr;
+  float* d_top_scores = nullptr;
+  uint32_t* d_top_index = nullptr;
+  size_t top_cap = 0;
 };
 
 // The buffers sized by rows (cap_e) and nodes (cap_v = 2 cap_e), and the CUB scratch of the sorts and scans over
@@ -590,6 +597,7 @@ void alz_internal_free_gnn(alz_handle* h) {
   free_row_buffers(g);
   for (int l = 0; l < 2; ++l) { cudaFree(g->d_W[l]); cudaFree(g->d_b[l]); cudaFree(g->d_Wcan[l]); }
   cudaFree(g->d_a); cudaFree(g->d_nv);
+  cudaFree(g->d_top_rows); cudaFree(g->d_top_scores); cudaFree(g->d_top_index);
   delete g;
   h->gnn = nullptr;
 }
@@ -618,14 +626,18 @@ static int gnn_grow(alz_handle* h, uint32_t n_e) {
 // Sorts only cover the key bits that can differ.
 static int bits_for(uint64_t x) { int b = 1; while (b < 64 && (x >> b) != 0) ++b; return b; }
 
-static int gnn_run(alz_handle* h, const alz_edge_out* rows, size_t n_rows) {
-  int rc = gnn_init(h);
+// a GNN state whose row-sized buffers hold at least n_rows rows
+static int gnn_reserve(alz_handle* h, size_t n_rows) {
+  const int rc = gnn_init(h);
   if (rc != ALZ_OK) return rc;
   if (n_rows > kMaxRows) return ALZ_E_CAPACITY;
-  if (n_rows > h->gnn->cap_e) {
-    rc = gnn_grow(h, (uint32_t)n_rows);
-    if (rc != ALZ_OK) return rc;
-  }
+  return n_rows > h->gnn->cap_e ? gnn_grow(h, (uint32_t)n_rows) : ALZ_OK;
+}
+
+// scratch_rows: the state holds at least that many rows as well (the top-row selection's scratch, below)
+static int gnn_run(alz_handle* h, const alz_edge_out* rows, size_t n_rows, size_t scratch_rows = 0) {
+  const int rc = gnn_reserve(h, std::max(n_rows, scratch_rows));
+  if (rc != ALZ_OK) return rc;
   alz_gnn_state* g = h->gnn;
   cudaStream_t s = h->stream;
   const uint32_t n_e = (uint32_t)n_rows;
@@ -666,6 +678,271 @@ static int gnn_run(alz_handle* h, const alz_edge_out* rows, size_t n_rows) {
                                          g->d_scores);
   h->launches += 12;
   CK(cudaGetLastError());
+  return ALZ_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Top anomalous rows (docs/SPEC.md §16): the min(k, above) best of n scores, ranked by the order key descending, then
+// by index ascending. Radix select on the inverted key ik = ~key (ascending ik = rank order), state on the device:
+//   hist<P>  digit P (11/11/10 bits from the top) of every item whose higher digits equal the prefix so far: a
+//            shared-memory histogram per CTA, added into one global histogram; pass 0 also counts the eligible items
+//            (ik <= ~key(min_score)) and takes the largest key
+//   pick<P>  one CTA: the digit the remaining rank falls into; prefix and remaining rank stay in device memory
+//   after pass 2 the threshold T is the m-th smallest ik and r of the items with ik == T are taken, lowest index first:
+//   ties     per tile of 4096 items, the items with ik == T; an exclusive scan gives each tile its first tie rank
+//   emit     every item with ik < T, and the ties of rank < r: m candidates (ik - ik_min) << ib | index, unordered
+// One wait reads m, T and ik_min; a radix sort of the m candidates over the bits that can differ orders them, and the
+// gather copies index, score and row of each. Scores are read five times; rows only for the m results. The scratch is
+// the pass's: histogram and control words in d_flags, tile counts in d_pos, candidates in d_nk / d_iota, sorted in
+// d_nk_sorted / d_vals, CUB in d_tmp. The node keys, h2, the node count and the scores are not touched.
+// ---------------------------------------------------------------------------
+namespace top {
+constexpr uint32_t kThreads = 256, kRounds = 16, kTile = kThreads * kRounds, kWarps = kThreads / 32;
+constexpr uint32_t kHistWords = 2048;                             // the widest digit: 11 bits
+enum Ctl : uint32_t { kAbove, kM, kPrefix, kRank, kKeyMax, kCand, kCtlWords = 16 };
+constexpr uint32_t kScratchRows = (kHistWords + kCtlWords + 1) / 2;   // d_flags holds 2 words per row
+// The rows of GNN state the selection of at most k of n scores needs: at most min(k, n) candidates, 2 words of d_pos
+// per tile, the histogram and the control words. A pass over n rows already holds n.
+inline size_t scratch_rows(size_t n, uint32_t k) {
+  return std::max<size_t>({std::min<size_t>(n, k), n / kTile + 1, kScratchRows});
+}
+
+__host__ __device__ __forceinline__ uint32_t order_key(uint32_t u) { return (u & 0x80000000u) ? ~u : u ^ 0x80000000u; }
+
+template <int P> struct Digit;   // pass P: digit = (ik >> kShift) & (kBins - 1), prefix = ik >> (kShift + kBits)
+template <> struct Digit<0> { static constexpr uint32_t kShift = 21, kBits = 11; };
+template <> struct Digit<1> { static constexpr uint32_t kShift = 10, kBits = 11; };
+template <> struct Digit<2> { static constexpr uint32_t kShift = 0, kBits = 10; };
+
+template <int P>
+__global__ void __launch_bounds__(kThreads) top_hist_kernel(const float* __restrict__ s, uint32_t n, uint32_t ik_elig,
+                                                            uint32_t* __restrict__ hist, uint32_t* __restrict__ ctl) {
+  constexpr uint32_t kShift = Digit<P>::kShift, kBins = 1u << Digit<P>::kBits;
+  constexpr uint32_t kHi = P == 0 ? 0u : kShift + Digit<P>::kBits;   // the prefix's bits: ik >> kHi (pass 0: none)
+  __shared__ uint32_t sh[kBins];
+  if (P > 0 && ctl[kM] == 0) return;
+  const uint32_t prefix = P > 0 ? ctl[kPrefix] : 0u;
+  for (uint32_t b = threadIdx.x; b < kBins; b += kThreads) sh[b] = 0;
+  __syncthreads();
+  const uint32_t lane = threadIdx.x & 31u;
+  uint32_t above = 0, key_max = 0;
+  // i0 is the same in every lane of a warp: the whole warp reaches the __match_any_sync
+  for (uint32_t i0 = blockIdx.x * kThreads + (threadIdx.x & ~31u); i0 < n; i0 += gridDim.x * kThreads) {
+    const uint32_t i = i0 + lane;
+    uint32_t d = 0xFFFFFFFFu;
+    if (i < n) {
+      const uint32_t key = order_key(__float_as_uint(s[i])), ik = ~key;
+      if (P == 0) {
+        above += ik <= ik_elig;
+        key_max = max(key_max, key);
+      }
+      if (P == 0 || (ik >> kHi) == prefix) d = (ik >> kShift) & (kBins - 1);
+    }
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);   // one shared atomic per distinct digit of the warp
+    if (d != 0xFFFFFFFFu && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(&sh[d], (uint32_t)__popc(peers));
+  }
+  if (P == 0) {
+    above = __reduce_add_sync(0xFFFFFFFFu, above);
+    key_max = __reduce_max_sync(0xFFFFFFFFu, key_max);
+    if (lane == 0) {
+      if (above) atomicAdd(&ctl[kAbove], above);
+      atomicMax(&ctl[kKeyMax], key_max);
+    }
+  }
+  __syncthreads();
+  for (uint32_t b = threadIdx.x; b < kBins; b += kThreads)
+    if (sh[b]) atomicAdd(&hist[b], sh[b]);
+}
+
+// one CTA of 1024 threads, 2 bins each: the digit whose bucket holds the remaining rank; the histogram is cleared for
+// the next pass
+template <int P>
+__global__ void __launch_bounds__(1024) top_pick_kernel(uint32_t k, uint32_t* __restrict__ hist,
+                                                        uint32_t* __restrict__ ctl) {
+  using Scan = cub::BlockScan<uint32_t, 1024>;
+  __shared__ typename Scan::TempStorage tmp;
+  const uint32_t t = threadIdx.x;
+  const uint32_t m = P == 0 ? min(k, ctl[kAbove]) : ctl[kM];
+  const uint32_t rank = P == 0 ? m : ctl[kRank];
+  const uint32_t prefix = P == 0 ? 0u : ctl[kPrefix];
+  const uint32_t a = hist[2 * t], b = hist[2 * t + 1];
+  hist[2 * t] = hist[2 * t + 1] = 0;
+  if (P == 0 && t == 0) ctl[kM] = m;
+  if (m == 0) return;                                  // the same in every thread
+  uint32_t ex;
+  Scan(tmp).ExclusiveSum(a + b, ex);
+  const uint32_t bits = Digit<P>::kBits;
+  if (ex < rank && rank <= ex + a) {
+    ctl[kPrefix] = (prefix << bits) | (2 * t);
+    ctl[kRank] = rank - ex;
+  } else if (ex + a < rank && rank <= ex + a + b) {
+    ctl[kPrefix] = (prefix << bits) | (2 * t + 1);
+    ctl[kRank] = rank - ex - a;
+  }
+}
+
+// per tile: the items with ik == T
+__global__ void __launch_bounds__(kThreads) top_ties_kernel(const float* __restrict__ s, uint32_t n,
+                                                            const uint32_t* __restrict__ ctl, uint32_t* __restrict__ eq) {
+  if (ctl[kM] == 0) return;
+  const uint32_t T = ctl[kPrefix];
+  __shared__ uint32_t total;
+  if (threadIdx.x == 0) total = 0;
+  __syncthreads();
+  uint32_t c = 0;
+  for (uint32_t j = 0; j < kRounds; ++j) {
+    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
+    c += i < n && ~order_key(__float_as_uint(s[i])) == T;
+  }
+  c = __reduce_add_sync(0xFFFFFFFFu, c);
+  if ((threadIdx.x & 31u) == 0 && c) atomicAdd(&total, c);
+  __syncthreads();
+  if (threadIdx.x == 0) eq[blockIdx.x] = total;
+}
+
+// per tile, in index order (round j, warp w, lane l holds item tile + 256 j + 32 w + l): the candidates, appended
+__global__ void __launch_bounds__(kThreads) top_emit_kernel(const float* __restrict__ s, uint32_t n, uint32_t ib,
+                                                            uint32_t* __restrict__ ctl,
+                                                            const uint32_t* __restrict__ tie_base,
+                                                            uint64_t* __restrict__ cand_key,
+                                                            uint32_t* __restrict__ cand_idx) {
+  if (ctl[kM] == 0) return;
+  const uint32_t T = ctl[kPrefix], r = ctl[kRank], ik_min = ~ctl[kKeyMax];
+  __shared__ uint32_t ties[kRounds * kWarps];          // ties per (round, warp), then their exclusive scan
+  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
+  uint32_t ik[kRounds], eq_mask[kRounds];
+#pragma unroll
+  for (uint32_t j = 0; j < kRounds; ++j) {
+    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
+    ik[j] = i < n ? ~order_key(__float_as_uint(s[i])) : 0xFFFFFFFFu;
+    eq_mask[j] = __ballot_sync(0xFFFFFFFFu, i < n && ik[j] == T);
+    if (lane == 0) ties[j * kWarps + warp] = __popc(eq_mask[j]);
+  }
+  __syncthreads();
+  if (warp == 0) {                                     // exclusive scan of the 128 counts, 4 per lane
+    uint32_t v[4], sum = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { v[q] = ties[lane * 4 + q]; sum += v[q]; }
+    uint32_t incl = sum;
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+      if ((int)lane >= o) incl += x;
+    }
+    uint32_t run = incl - sum;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) { ties[lane * 4 + q] = run; run += v[q]; }
+  }
+  __syncthreads();
+  const uint32_t base = tie_base[blockIdx.x];
+#pragma unroll
+  for (uint32_t j = 0; j < kRounds; ++j) {
+    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
+    const uint32_t tie_rank = base + ties[j * kWarps + warp] + __popc(eq_mask[j] & lt);
+    const bool keep = i < n && (ik[j] < T || (ik[j] == T && tie_rank < r));
+    const uint32_t keep_mask = __ballot_sync(0xFFFFFFFFu, keep);
+    if (!keep_mask) continue;
+    uint32_t pos = 0;
+    if (lane == 0) pos = atomicAdd(&ctl[kCand], (uint32_t)__popc(keep_mask));
+    pos = __shfl_sync(0xFFFFFFFFu, pos, 0) + __popc(keep_mask & lt);
+    if (keep) {
+      cand_key[pos] = ((uint64_t)(ik[j] - ik_min) << ib) | i;
+      cand_idx[pos] = i;
+    }
+  }
+}
+
+// result j: the index, score and (with rows) row of the j-th candidate in sorted order; a warp per result
+__global__ void __launch_bounds__(kThreads) top_gather_kernel(const uint32_t* __restrict__ sorted_idx, uint32_t m,
+                                                              const float* __restrict__ s,
+                                                              const alz_edge_out* __restrict__ rows,
+                                                              uint32_t* __restrict__ out_index, float* __restrict__ out_scores,
+                                                              alz_edge_out* __restrict__ out_rows) {
+  constexpr uint32_t kWords = sizeof(alz_edge_out) / 8;
+  const uint32_t lane = threadIdx.x & 31u;
+  const uint32_t warps_per_grid = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < m; j += warps_per_grid) {
+    const uint32_t i = sorted_idx[j];
+    if (lane == 0) { out_index[j] = i; out_scores[j] = s[i]; }
+    if (rows) {
+      const uint64_t* src = reinterpret_cast<const uint64_t*>(rows + i);
+      uint64_t* dst = reinterpret_cast<uint64_t*>(out_rows + j);
+      for (uint32_t w = lane; w < kWords; w += 32) dst[w] = src[w];
+    }
+  }
+}
+static_assert(sizeof(alz_edge_out) % 8 == 0, "rows are copied in 8-byte words");
+}  // namespace top
+
+// The result buffers hold at least m rows: grown on demand, never shrunk; freed with the GNN state
+static int top_reserve(alz_handle* h, size_t m) {
+  alz_gnn_state* g = h->gnn;
+  if (m <= g->top_cap) return ALZ_OK;
+  cudaFree(g->d_top_rows); cudaFree(g->d_top_scores); cudaFree(g->d_top_index);
+  g->d_top_rows = nullptr; g->d_top_scores = nullptr; g->d_top_index = nullptr;
+  g->top_cap = 0;
+  const size_t cap = std::max<size_t>(m, 64);
+  if (cudaMalloc(&g->d_top_rows, cap * sizeof(alz_edge_out)) != cudaSuccess ||
+      cudaMalloc(&g->d_top_scores, cap * 4) != cudaSuccess || cudaMalloc(&g->d_top_index, cap * 4) != cudaSuccess) {
+    h->last_err = std::string("top anomalous rows: ") + cudaGetErrorString(cudaGetLastError());
+    cudaFree(g->d_top_rows); cudaFree(g->d_top_scores); cudaFree(g->d_top_index);
+    g->d_top_rows = nullptr; g->d_top_scores = nullptr; g->d_top_index = nullptr;
+    return ALZ_E_NOMEM;
+  }
+  g->top_cap = cap;
+  return ALZ_OK;
+}
+
+// The selection over n scores on the device (rows: n rows to gather from, or null). The state holds at least
+// top::scratch_rows(n, k) rows. *m_out = results, *above = eligible scores. One wait, for m.
+static int top_select(alz_handle* h, const float* scores, uint32_t n, uint32_t k, float min_score,
+                      const alz_edge_out* rows, size_t* m_out, uint64_t* above) {
+  using namespace top;
+  alz_gnn_state* g = h->gnn;
+  cudaStream_t s = h->stream;
+  *m_out = 0;
+  *above = 0;
+  if (n == 0) return ALZ_OK;
+  uint32_t* hist = g->d_flags;
+  uint32_t* ctl = g->d_flags + kHistWords;
+  const uint32_t tiles = (n + kTile - 1) / kTile;
+  uint32_t* tie_eq = g->d_pos;
+  uint32_t* tie_base = g->d_pos + tiles;
+  uint32_t ik_elig;
+  {
+    uint32_t u;
+    memcpy(&u, &min_score, 4);
+    ik_elig = ~order_key(u);
+  }
+  const unsigned grid = std::min<unsigned>(tiles, (unsigned)h->sms * 2);
+  CK(cudaMemsetAsync(g->d_flags, 0, (kHistWords + kCtlWords) * 4, s));
+  top_hist_kernel<0><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
+  top_pick_kernel<0><<<1, 1024, 0, s>>>(k, hist, ctl);
+  top_hist_kernel<1><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
+  top_pick_kernel<1><<<1, 1024, 0, s>>>(k, hist, ctl);
+  top_hist_kernel<2><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
+  top_pick_kernel<2><<<1, 1024, 0, s>>>(k, hist, ctl);
+  top_ties_kernel<<<tiles, kThreads, 0, s>>>(scores, n, ctl, tie_eq);
+  CK(exclusive_scan_u32(g->d_tmp, g->tmp_bytes, tie_eq, tie_base, tiles, s));
+  const uint32_t ib = (uint32_t)bits_for(n - 1);
+  top_emit_kernel<<<tiles, kThreads, 0, s>>>(scores, n, ib, ctl, tie_base, g->d_nk, g->d_iota);
+  h->launches += 8;
+  CK(cudaGetLastError());
+  uint32_t c[kCtlWords];
+  CK(cudaMemcpyAsync(c, ctl, sizeof c, cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  *above = c[kAbove];
+  const uint32_t m = c[kM];
+  if (m == 0) return ALZ_OK;
+  const int rc = top_reserve(h, m);
+  if (rc != ALZ_OK) return rc;
+  const uint32_t ik_min = ~c[kKeyMax], T = c[kPrefix];
+  CK(sort_pairs(g->d_tmp, g->tmp_bytes, g->d_nk, g->d_nk_sorted, g->d_iota, g->d_vals, m, s,
+                (int)ib + bits_for(T - ik_min)));
+  top_gather_kernel<<<std::min<unsigned>((m + kWarps - 1) / kWarps, (unsigned)h->sms * 4), kThreads, 0, s>>>(
+      g->d_vals, m, scores, rows, g->d_top_index, g->d_top_scores, g->d_top_rows);
+  h->launches += 1;
+  CK(cudaGetLastError());
+  *m_out = m;
   return ALZ_OK;
 }
 
@@ -726,6 +1003,119 @@ extern "C" int alz_gnn_score_rollup(alz_handle* h, uint32_t kind, float* scores,
   int rc = gnn_score_rollup_locked(h, kind, &d, n_out);
   if (rc != ALZ_OK) return rc;
   return copy_scores(h, d, scores, cap, *n_out);
+}
+
+// ---- top anomalous rows (docs/SPEC.md §16) ------------------------------------------------------------------------
+// the pass over rows, then the selection; *n_out = results, on the device in the GNN state. Caller holds h->mu.
+static int gnn_top_locked(alz_handle* h, const alz_edge_out* rows, size_t n_rows, uint32_t k, float min_score,
+                          size_t* n_out, alz_top_info* info) {
+  CK(cudaSetDevice(h->device));
+  int rc = gnn_run(h, rows, n_rows, top::scratch_rows(n_rows, k));
+  if (rc != ALZ_OK) return rc;
+  uint64_t above = 0;
+  rc = top_select(h, h->gnn->d_scores, (uint32_t)n_rows, k, min_score, rows, n_out, &above);
+  if (rc != ALZ_OK) return rc;
+  if (info) { info->scored = n_rows; info->above = above; }
+  return ALZ_OK;
+}
+
+// the rows of the last flushed window (rollup false) or of the last rollup of `kind`
+static int gnn_top_call(alz_handle* h, bool rollup, uint32_t kind, uint32_t k, float min_score, size_t* n_out,
+                        alz_top_info* info) {
+  *n_out = 0;
+  if (info) *info = alz_top_info{};
+  if (k == 0 || std::isnan(min_score)) return ALZ_E_INVAL;
+  const alz_edge_out* rows = h->d_out;
+  size_t n_rows = h->last_n_edges;
+  if (rollup) {
+    const int rc = alz_internal_rollup_rows(h, kind, &rows, &n_rows);
+    if (rc != ALZ_OK) return rc;
+  }
+  return gnn_top_locked(h, rows, n_rows, k, min_score, n_out, info);
+}
+
+static void top_device_out(alz_handle* h, const alz_edge_out** dev_rows, const float** dev_scores,
+                           const uint32_t** dev_index) {
+  if (dev_rows) *dev_rows = h->gnn->d_top_rows;
+  if (dev_scores) *dev_scores = h->gnn->d_top_scores;
+  if (dev_index) *dev_index = h->gnn->d_top_index;
+}
+
+// the results into the caller's buffers (each may be null) and a wait; the usual cap rule
+static int top_host_out(alz_handle* h, size_t n, alz_edge_out* rows, float* scores, uint32_t* index, size_t cap) {
+  if (n > cap) return ALZ_E_CAPACITY;
+  alz_gnn_state* g = h->gnn;
+  if (n && rows) CK(cudaMemcpyAsync(rows, g->d_top_rows, n * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, h->stream));
+  if (n && scores) CK(cudaMemcpyAsync(scores, g->d_top_scores, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (n && index) CK(cudaMemcpyAsync(index, g->d_top_index, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return ALZ_OK;
+}
+
+extern "C" int alz_gnn_top(alz_handle* h, uint32_t k, float min_score, alz_edge_out* rows, float* scores,
+                           uint32_t* index, size_t cap, size_t* n_out, alz_top_info* info) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const int rc = gnn_top_call(h, false, 0, k, min_score, n_out, info);
+  return rc != ALZ_OK ? rc : top_host_out(h, *n_out, rows, scores, index, cap);
+}
+
+extern "C" int alz_gnn_top_device(alz_handle* h, uint32_t k, float min_score, const alz_edge_out** dev_rows,
+                                  const float** dev_scores, const uint32_t** dev_index, size_t* n_out,
+                                  alz_top_info* info) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const int rc = gnn_top_call(h, false, 0, k, min_score, n_out, info);
+  if (rc == ALZ_OK) top_device_out(h, dev_rows, dev_scores, dev_index);
+  return rc;
+}
+
+extern "C" int alz_gnn_top_rollup(alz_handle* h, uint32_t kind, uint32_t k, float min_score, alz_edge_out* rows,
+                                  float* scores, uint32_t* index, size_t cap, size_t* n_out, alz_top_info* info) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const int rc = gnn_top_call(h, true, kind, k, min_score, n_out, info);
+  return rc != ALZ_OK ? rc : top_host_out(h, *n_out, rows, scores, index, cap);
+}
+
+extern "C" int alz_gnn_top_rollup_device(alz_handle* h, uint32_t kind, uint32_t k, float min_score,
+                                         const alz_edge_out** dev_rows, const float** dev_scores,
+                                         const uint32_t** dev_index, size_t* n_out, alz_top_info* info) {
+  if (!h || !n_out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  const int rc = gnn_top_call(h, true, kind, k, min_score, n_out, info);
+  if (rc == ALZ_OK) top_device_out(h, dev_rows, dev_scores, dev_index);
+  return rc;
+}
+
+// debug/test: the selection of alz_gnn_top over n scores in device memory, with the GNN state's scratch (grown to
+// top::scratch_rows(n, k) rows when smaller; a growth leaves no pass for alz_gnn_nodes to report). index: the
+// results' indices, or null.
+extern "C" int alz_debug_top_scores(alz_handle* h, const float* dev_scores, size_t n, uint32_t k, float min_score,
+                                    uint32_t* index, size_t cap, size_t* n_out, uint64_t* above) {
+  if (!h || !n_out || (!dev_scores && n)) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(h->mu);
+  *n_out = 0;
+  if (above) *above = 0;
+  if (k == 0 || std::isnan(min_score)) return ALZ_E_INVAL;
+  CK(cudaSetDevice(h->device));
+  int rc = gnn_init(h);
+  if (rc != ALZ_OK) return rc;
+  if (n > kMaxRows) return ALZ_E_CAPACITY;
+  const size_t need = top::scratch_rows(n, k);
+  const bool grows = need > h->gnn->cap_e;
+  rc = gnn_reserve(h, need);
+  if (rc != ALZ_OK) return rc;
+  if (grows) {                              // the buffers of the last pass are gone
+    h->gnn->n_e = h->gnn->n_v = 0;
+    h->gnn->n_v_known = true;
+    CK(cudaMemsetAsync(h->gnn->d_nv, 0, 4, h->stream));
+  }
+  uint64_t ab = 0;
+  rc = top_select(h, dev_scores, (uint32_t)n, k, min_score, nullptr, n_out, &ab);
+  if (rc != ALZ_OK) return rc;
+  if (above) *above = ab;
+  return top_host_out(h, *n_out, nullptr, nullptr, index, cap);
 }
 
 // debug/test: node keys ((kind << 32) | value, ascending) and the layer-2 embeddings of the last GNN pass, over a

@@ -280,6 +280,31 @@ std::vector<EdgeWindow> Aggregator::ToEdges(const alz_edge_out* rows, size_t n, 
   return edges;
 }
 
+int Aggregator::Anomalies(uint32_t source, uint32_t k, float min_score, std::vector<EdgeWindow>* out,
+                          alz_top_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  // into roll_ / scores_, grown once when the results do not fit (ALZ_E_CAPACITY with n = the results; nothing written)
+  auto call = [&](size_t* n) {
+    return source == kLastWindow
+               ? alz_gnn_top(h_, k, min_score, roll_.data(), scores_.data(), nullptr, roll_.size(), n, info)
+               : alz_gnn_top_rollup(h_, source, k, min_score, roll_.data(), scores_.data(), nullptr, roll_.size(), n,
+                                    info);
+  };
+  size_t n = 0;
+  scores_.resize(roll_.size());
+  int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {
+    roll_.resize(n);
+    scores_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToEdges(roll_.data(), n, scores_.data());
+  return ALZ_OK;
+}
+
 int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);

@@ -119,6 +119,13 @@ class Aggregator {
   // covered is info->r.windows), summed from every retained piece, go to ds->PersistEdgeWindow as a flush's rows do.
   // info may be null; with_scores as in Rollup. Returns 0 or an alz_status.
   int RollupSpan(uint64_t windows, uint32_t mode, alz_span_info* info = nullptr, bool with_scores = false);
+  // Anomalies' source for the last flushed window; the other sources are the rollup kinds ALZ_ROLLUP_*
+  static constexpr uint32_t kLastWindow = 0xFFFFFFFFu;
+  // the k rows of `source` with the highest GNN anomaly scores >= min_score (docs/SPEC.md §16: fewer when fewer
+  // qualify), best first, ties by row order, Score set, into *out (not to the data store). A rollup source is the
+  // last Rollup / RollupSpan of that kind. info may be null. Returns 0 or an alz_status.
+  int Anomalies(uint32_t source, uint32_t k, float min_score, std::vector<EdgeWindow>* out,
+                alz_top_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -169,7 +176,7 @@ class Aggregator {
   std::unordered_map<std::string, uint32_t> host_ids_;   // Host header text -> dense id (ALZ_NODE_OUTBOUND_HOST)
   std::vector<std::string> host_names_;
   std::vector<alz_edge_out> out_;
-  std::vector<alz_edge_out> roll_;   // rows of the last Rollup
+  std::vector<alz_edge_out> roll_;   // rows of the last Rollup or Anomalies
   std::vector<float> scores_;
   std::vector<alz_alive_conn> alive_;
 };

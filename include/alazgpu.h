@@ -408,6 +408,31 @@ int alz_gnn_score_rollup(alz_handle* h, uint32_t kind, float* scores, size_t cap
 /* same, scores left on the device (valid until the next GNN call on this handle) */
 int alz_gnn_score_rollup_device(alz_handle* h, uint32_t kind, const float** dev_scores, size_t* n_out);
 
+/* ---- top anomalous rows (docs/SPEC.md §16) ----------------------------------------
+ * The pass of §6 / §15, then only its best rows: the first min(k, above) rows in rank order, where each score maps to
+ * the key u ^ 0x80000000 (sign bit clear) or ~u (set) of its bits u (IEEE total order), rows rank by key descending,
+ * then by row index ascending, and a row is eligible when key(score) >= key(min_score). Result j: the row
+ * (byte for byte as in the window or rollup), its score (bit for bit what alz_gnn_score* returns for it) and its row
+ * index. rows, scores, index and info may each be NULL. *n_out is always set; cap too small: ALZ_E_CAPACITY, nothing
+ * written. k = 0, a NaN min_score or an unknown kind: ALZ_E_INVAL; no rollup rows to score: ALZ_E_STATE, as in §15; a
+ * 0-row source: *n_out = 0. More than 2^30 - 1 rows: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. Reads only, as §15;
+ * alz_gnn_nodes then refers to this pass. The pass always runs. The result is a function of the rows and their order
+ * alone: every rank gets the same result with no collective. Device results stay valid until the next GNN call. */
+typedef struct alz_top_info {
+  uint64_t scored;   /* rows the pass scored */
+  uint64_t above;    /* of those, rows whose score is >= min_score (before the cut at k) */
+} alz_top_info;
+/* over the last flushed window, the rows alz_gnn_score scores */
+int alz_gnn_top(alz_handle* h, uint32_t k, float min_score, alz_edge_out* rows, float* scores, uint32_t* index,
+                size_t cap, size_t* n_out, alz_top_info* info);
+int alz_gnn_top_device(alz_handle* h, uint32_t k, float min_score, const alz_edge_out** dev_rows,
+                       const float** dev_scores, const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
+/* over the rows the last rollup of `kind` (ALZ_ROLLUP_*) returned, the rows alz_gnn_score_rollup scores */
+int alz_gnn_top_rollup(alz_handle* h, uint32_t kind, uint32_t k, float min_score, alz_edge_out* rows, float* scores,
+                       uint32_t* index, size_t cap, size_t* n_out, alz_top_info* info);
+int alz_gnn_top_rollup_device(alz_handle* h, uint32_t kind, uint32_t k, float min_score, const alz_edge_out** dev_rows,
+                              const float** dev_scores, const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

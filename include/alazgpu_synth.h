@@ -28,6 +28,13 @@ int alz_fold(alz_handle* h);
 
 /* test/debug: node keys ((kind << 32) | value, ascending) and layer-2 embeddings [n x 64] of the last GNN pass */
 int alz_gnn_nodes(alz_handle* h, uint64_t* node_keys, float* h2, size_t cap, size_t* n_out);
+/* test/debug: the selection of alz_gnn_top (docs/SPEC.md §16) over n scores in device memory: *n_out results, their
+ * indices into index (or NULL; cap too small: ALZ_E_CAPACITY, nothing written), *above the eligible scores (or
+ * NULL). Uses the GNN state's scratch, grown when smaller to the rows the selection needs, about min(k, n) (then
+ * alz_gnn_nodes reports no nodes).
+ * n > 2^30 - 1: ALZ_E_CAPACITY; k = 0 or a NaN min_score: ALZ_E_INVAL. */
+int alz_debug_top_scores(alz_handle* h, const float* dev_scores, size_t n, uint32_t k, float min_score,
+                         uint32_t* index, size_t cap, size_t* n_out, uint64_t* above);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
