@@ -137,6 +137,21 @@ class TopInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+METRIC_COUNT, METRIC_ERR5XX, METRIC_ERR_RATE, METRIC_MEAN_NS, METRIC_QUANTILE = 0, 1, 2, 3, 4   # alz_metric kinds
+MAX_METRICS = 8
+
+
+class Metric(C.Structure):
+    """alz_metric: kind METRIC_*, q for METRIC_QUANTILE."""
+    _fields_ = [("kind", C.c_uint32), ("_pad", C.c_uint32), ("q", C.c_double)]
+
+
+def metrics(*specs):
+    """A ctypes array of alz_metric from kinds or (kind, q) pairs, e.g. metrics((METRIC_QUANTILE, 0.99), METRIC_COUNT)."""
+    ms = [Metric(s[0], 0, float(s[1])) if isinstance(s, tuple) else Metric(int(s), 0, 0.0) for s in specs]
+    return (Metric * max(len(ms), 1))(*ms)
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

@@ -27,7 +27,9 @@ EXPORTS = [
     "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device", "alz_window_tier_state",
     "alz_window_rollup_span", "alz_window_rollup_span_device", "alz_gnn_score",
     "alz_gnn_score_device", "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_gnn_top", "alz_gnn_top_device",
-    "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_edge_metrics", "alz_edge_metrics_device",
+    "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device", "alz_edge_top", "alz_edge_top_device",
+    "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -87,6 +89,18 @@ def load(rebuild=False):
         "alz_gnn_top_rollup_device": ([vp, u32, u32, C.c_float, pp, pp, pp, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
         "alz_gnn_nodes": ([vp, vp, vp, sz, C.POINTER(sz)], i),
         "alz_debug_top_scores": ([vp, vp, sz, u32, C.c_float, vp, sz, C.POINTER(sz), C.POINTER(u64)], i),
+        "alz_edge_metrics": ([vp, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_edge_metrics_device": ([vp, vp, u32, pp, C.POINTER(sz)], i),
+        "alz_edge_metrics_rollup": ([vp, u32, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_edge_metrics_rollup_device": ([vp, u32, vp, u32, pp, C.POINTER(sz)], i),
+        "alz_edge_top": ([vp, vp, u32, C.c_double, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_edge_top_device": ([vp, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_edge_top_rollup": ([vp, u32, vp, u32, C.c_double, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)],
+                                i),
+        "alz_edge_top_rollup_device": ([vp, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
+                                        C.POINTER(abi.TopInfo)], i),
+        "alz_debug_edge_metrics_rows": ([vp, vp, sz, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_debug_top_keys64": ([vp, vp, sz, u32, C.c_double, vp, sz, C.POINTER(sz), C.POINTER(u64)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -122,7 +136,10 @@ def load(rebuild=False):
                   "alz_window_history_tiers", "alz_window_rollup_tier", "alz_window_rollup_tier_device",
                   "alz_window_tier_state", "alz_window_rollup_span", "alz_window_rollup_span_device",
                   "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_gnn_top", "alz_gnn_top_device",
-                  "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_debug_top_scores"):
+                  "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_debug_top_scores", "alz_edge_metrics",
+                  "alz_edge_metrics_device", "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device",
+                  "alz_edge_top", "alz_edge_top_device", "alz_edge_top_rollup", "alz_edge_top_rollup_device",
+                  "alz_debug_edge_metrics_rows", "alz_debug_top_keys64"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -438,6 +455,81 @@ class Handle:
     def gnn_top_rollup_device(self, kind, k, min_score=0.0):
         """alz_gnn_top_rollup_device: (rows, scores, index device pointers, results, info dict)."""
         return self._top_device("alz_gnn_top_rollup_device", (int(kind),), k, min_score)
+
+    # ---- edge metrics and the top edges by a metric (alz_metrics.cu, docs/SPEC.md §17)
+    def _edge_metrics(self, fn, args, specs):
+        """fn(h, *args, m, nm, values, cap, &n): values [rows x nm] float64; the first call with cap 0 sizes it."""
+        m, nm = abi.metrics(*specs), len(specs)
+        f, n = getattr(self.L, fn), C.c_size_t(0)
+        if self._ck(f(self.h, *args, m, nm, None, 0, C.byref(n)), fn, allow=(abi.E_CAPACITY,)) == 0:
+            return np.zeros((0, nm))
+        out = np.zeros((n.value, nm))
+        self._ck(f(self.h, *args, m, nm, _ptr(out), n.value, C.byref(n)), fn)
+        return out
+
+    def _edge_metrics_device(self, fn, args, specs):
+        """fn(h, *args, m, nm, &values, &n): (device pointer, rows)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        self._ck(getattr(self.L, fn)(self.h, *args, abi.metrics(*specs), len(specs), C.byref(p), C.byref(n)), fn)
+        return p.value, n.value
+
+    def edge_metrics(self, *specs):
+        """alz_edge_metrics over the last flushed window: values [rows x len(specs)]; a spec is a METRIC_* kind or a
+        (kind, q) pair."""
+        return self._edge_metrics("alz_edge_metrics", (), specs)
+
+    def edge_metrics_device(self, *specs):
+        """alz_edge_metrics_device: (device pointer, rows)."""
+        return self._edge_metrics_device("alz_edge_metrics_device", (), specs)
+
+    def edge_metrics_rollup(self, kind, *specs):
+        """alz_edge_metrics_rollup over the rows the last rollup of `kind` (abi.ROLLUP_*) returned."""
+        return self._edge_metrics("alz_edge_metrics_rollup", (int(kind),), specs)
+
+    def edge_metrics_rollup_device(self, kind, *specs):
+        """alz_edge_metrics_rollup_device: (device pointer, rows)."""
+        return self._edge_metrics_device("alz_edge_metrics_rollup_device", (int(kind),), specs)
+
+    def _edge_top(self, fn, args, spec, k, min_value):
+        """fn(h, *args, m, k, min_value, rows, values, index, cap, &n, &info): (rows, values, index, info dict). The
+        first call offers room for min(k, 65536) results; when more came out, the call is repeated with room for all."""
+        f, n, info, m = getattr(self.L, fn), C.c_size_t(0), abi.TopInfo(), abi.metrics(spec)
+        cap = min(int(k), 1 << 16)
+        while True:
+            rows = np.zeros(cap, dtype=abi.EDGE_OUT)
+            values = np.zeros(cap, dtype=np.float64)
+            index = np.zeros(cap, dtype=np.uint32)
+            rc = self._ck(f(self.h, *args, m, int(k), float(min_value), _ptr(rows), _ptr(values), _ptr(index), cap,
+                            C.byref(n), C.byref(info)), fn, allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                r = n.value
+                return rows[:r].copy(), values[:r].copy(), index[:r].copy(), info.as_dict()
+            cap = n.value
+
+    def _edge_top_device(self, fn, args, spec, k, min_value):
+        """fn(h, *args, m, k, min_value, &rows, &values, &index, &n, &info): (rows, values, index device pointers,
+        results, info dict)."""
+        pr, pv, pi, n, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), abi.TopInfo()
+        self._ck(getattr(self.L, fn)(self.h, *args, abi.metrics(spec), int(k), float(min_value), C.byref(pr),
+                                     C.byref(pv), C.byref(pi), C.byref(n), C.byref(info)), fn)
+        return pr.value, pv.value, pi.value, n.value, info.as_dict()
+
+    def edge_top(self, spec, k, min_value=0.0):
+        """alz_edge_top over the last flushed window by one metric (a METRIC_* kind or a (kind, q) pair): (rows,
+        values, index, info dict), rank order."""
+        return self._edge_top("alz_edge_top", (), spec, k, min_value)
+
+    def edge_top_device(self, spec, k, min_value=0.0):
+        """alz_edge_top_device: (rows, values, index device pointers, results, info dict)."""
+        return self._edge_top_device("alz_edge_top_device", (), spec, k, min_value)
+
+    def edge_top_rollup(self, kind, spec, k, min_value=0.0):
+        """alz_edge_top_rollup over the rows the last rollup of `kind` (abi.ROLLUP_*) returned."""
+        return self._edge_top("alz_edge_top_rollup", (int(kind),), spec, k, min_value)
+
+    def edge_top_rollup_device(self, kind, spec, k, min_value=0.0):
+        """alz_edge_top_rollup_device: (rows, values, index device pointers, results, info dict)."""
+        return self._edge_top_device("alz_edge_top_rollup_device", (int(kind),), spec, k, min_value)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -235,6 +235,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   cudaDeviceSynchronize();
   alz_internal_free_comm(h);
   alz_internal_free_gnn(h);
+  alz_internal_free_metrics(h);
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);

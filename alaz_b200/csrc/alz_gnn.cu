@@ -25,6 +25,7 @@
 
 #include "alz_handle.h"
 #include "alz_mbar.cuh"
+#include "alz_top.cuh"
 
 using namespace alz;
 
@@ -681,197 +682,15 @@ static int gnn_run(alz_handle* h, const alz_edge_out* rows, size_t n_rows, size_
   return ALZ_OK;
 }
 
-// ---------------------------------------------------------------------------
-// Top anomalous rows (docs/SPEC.md §16): the min(k, above) best of n scores, ranked by the order key descending, then
-// by index ascending. Radix select on the inverted key ik = ~key (ascending ik = rank order), state on the device:
-//   hist<P>  digit P (11/11/10 bits from the top) of every item whose higher digits equal the prefix so far: a
-//            shared-memory histogram per CTA, added into one global histogram; pass 0 also counts the eligible items
-//            (ik <= ~key(min_score)) and takes the largest key
-//   pick<P>  one CTA: the digit the remaining rank falls into; prefix and remaining rank stay in device memory
-//   after pass 2 the threshold T is the m-th smallest ik and r of the items with ik == T are taken, lowest index first:
-//   ties     per tile of 4096 items, the items with ik == T; an exclusive scan gives each tile its first tie rank
-//   emit     every item with ik < T, and the ties of rank < r: m candidates (ik - ik_min) << ib | index, unordered
-// One wait reads m, T and ik_min; a radix sort of the m candidates over the bits that can differ orders them, and the
-// gather copies index, score and row of each. Scores are read five times; rows only for the m results. The scratch is
-// the pass's: histogram and control words in d_flags, tile counts in d_pos, candidates in d_nk / d_iota, sorted in
+// Top anomalous rows (docs/SPEC.md §16): the selection of alz_top.cu over the float32 score bits. Its scratch is the
+// pass's: histogram and control block in d_flags, tile counts in d_pos, candidates in d_nk / d_iota, sorted in
 // d_nk_sorted / d_vals, CUB in d_tmp. The node keys, h2, the node count and the scores are not touched.
-// ---------------------------------------------------------------------------
-namespace top {
-constexpr uint32_t kThreads = 256, kRounds = 16, kTile = kThreads * kRounds, kWarps = kThreads / 32;
-constexpr uint32_t kHistWords = 2048;                             // the widest digit: 11 bits
-enum Ctl : uint32_t { kAbove, kM, kPrefix, kRank, kKeyMax, kCand, kCtlWords = 16 };
-constexpr uint32_t kScratchRows = (kHistWords + kCtlWords + 1) / 2;   // d_flags holds 2 words per row
+constexpr uint32_t kTopScratchRows = (uint32_t)((top::kWordsBytes / 4 + 1) / 2);   // d_flags holds 2 words per row
 // The rows of GNN state the selection of at most k of n scores needs: at most min(k, n) candidates, 2 words of d_pos
-// per tile, the histogram and the control words. A pass over n rows already holds n.
-inline size_t scratch_rows(size_t n, uint32_t k) {
-  return std::max<size_t>({std::min<size_t>(n, k), n / kTile + 1, kScratchRows});
+// per tile, the histogram and the control block. A pass over n rows already holds n.
+static size_t top_scratch_rows(size_t n, uint32_t k) {
+  return std::max<size_t>({std::min<size_t>(n, k), n / top::kTile + 1, kTopScratchRows});
 }
-
-__host__ __device__ __forceinline__ uint32_t order_key(uint32_t u) { return (u & 0x80000000u) ? ~u : u ^ 0x80000000u; }
-
-template <int P> struct Digit;   // pass P: digit = (ik >> kShift) & (kBins - 1), prefix = ik >> (kShift + kBits)
-template <> struct Digit<0> { static constexpr uint32_t kShift = 21, kBits = 11; };
-template <> struct Digit<1> { static constexpr uint32_t kShift = 10, kBits = 11; };
-template <> struct Digit<2> { static constexpr uint32_t kShift = 0, kBits = 10; };
-
-template <int P>
-__global__ void __launch_bounds__(kThreads) top_hist_kernel(const float* __restrict__ s, uint32_t n, uint32_t ik_elig,
-                                                            uint32_t* __restrict__ hist, uint32_t* __restrict__ ctl) {
-  constexpr uint32_t kShift = Digit<P>::kShift, kBins = 1u << Digit<P>::kBits;
-  constexpr uint32_t kHi = P == 0 ? 0u : kShift + Digit<P>::kBits;   // the prefix's bits: ik >> kHi (pass 0: none)
-  __shared__ uint32_t sh[kBins];
-  if (P > 0 && ctl[kM] == 0) return;
-  const uint32_t prefix = P > 0 ? ctl[kPrefix] : 0u;
-  for (uint32_t b = threadIdx.x; b < kBins; b += kThreads) sh[b] = 0;
-  __syncthreads();
-  const uint32_t lane = threadIdx.x & 31u;
-  uint32_t above = 0, key_max = 0;
-  // i0 is the same in every lane of a warp: the whole warp reaches the __match_any_sync
-  for (uint32_t i0 = blockIdx.x * kThreads + (threadIdx.x & ~31u); i0 < n; i0 += gridDim.x * kThreads) {
-    const uint32_t i = i0 + lane;
-    uint32_t d = 0xFFFFFFFFu;
-    if (i < n) {
-      const uint32_t key = order_key(__float_as_uint(s[i])), ik = ~key;
-      if (P == 0) {
-        above += ik <= ik_elig;
-        key_max = max(key_max, key);
-      }
-      if (P == 0 || (ik >> kHi) == prefix) d = (ik >> kShift) & (kBins - 1);
-    }
-    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, d);   // one shared atomic per distinct digit of the warp
-    if (d != 0xFFFFFFFFu && lane == (uint32_t)__ffs(peers) - 1u) atomicAdd(&sh[d], (uint32_t)__popc(peers));
-  }
-  if (P == 0) {
-    above = __reduce_add_sync(0xFFFFFFFFu, above);
-    key_max = __reduce_max_sync(0xFFFFFFFFu, key_max);
-    if (lane == 0) {
-      if (above) atomicAdd(&ctl[kAbove], above);
-      atomicMax(&ctl[kKeyMax], key_max);
-    }
-  }
-  __syncthreads();
-  for (uint32_t b = threadIdx.x; b < kBins; b += kThreads)
-    if (sh[b]) atomicAdd(&hist[b], sh[b]);
-}
-
-// one CTA of 1024 threads, 2 bins each: the digit whose bucket holds the remaining rank; the histogram is cleared for
-// the next pass
-template <int P>
-__global__ void __launch_bounds__(1024) top_pick_kernel(uint32_t k, uint32_t* __restrict__ hist,
-                                                        uint32_t* __restrict__ ctl) {
-  using Scan = cub::BlockScan<uint32_t, 1024>;
-  __shared__ typename Scan::TempStorage tmp;
-  const uint32_t t = threadIdx.x;
-  const uint32_t m = P == 0 ? min(k, ctl[kAbove]) : ctl[kM];
-  const uint32_t rank = P == 0 ? m : ctl[kRank];
-  const uint32_t prefix = P == 0 ? 0u : ctl[kPrefix];
-  const uint32_t a = hist[2 * t], b = hist[2 * t + 1];
-  hist[2 * t] = hist[2 * t + 1] = 0;
-  if (P == 0 && t == 0) ctl[kM] = m;
-  if (m == 0) return;                                  // the same in every thread
-  uint32_t ex;
-  Scan(tmp).ExclusiveSum(a + b, ex);
-  const uint32_t bits = Digit<P>::kBits;
-  if (ex < rank && rank <= ex + a) {
-    ctl[kPrefix] = (prefix << bits) | (2 * t);
-    ctl[kRank] = rank - ex;
-  } else if (ex + a < rank && rank <= ex + a + b) {
-    ctl[kPrefix] = (prefix << bits) | (2 * t + 1);
-    ctl[kRank] = rank - ex - a;
-  }
-}
-
-// per tile: the items with ik == T
-__global__ void __launch_bounds__(kThreads) top_ties_kernel(const float* __restrict__ s, uint32_t n,
-                                                            const uint32_t* __restrict__ ctl, uint32_t* __restrict__ eq) {
-  if (ctl[kM] == 0) return;
-  const uint32_t T = ctl[kPrefix];
-  __shared__ uint32_t total;
-  if (threadIdx.x == 0) total = 0;
-  __syncthreads();
-  uint32_t c = 0;
-  for (uint32_t j = 0; j < kRounds; ++j) {
-    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
-    c += i < n && ~order_key(__float_as_uint(s[i])) == T;
-  }
-  c = __reduce_add_sync(0xFFFFFFFFu, c);
-  if ((threadIdx.x & 31u) == 0 && c) atomicAdd(&total, c);
-  __syncthreads();
-  if (threadIdx.x == 0) eq[blockIdx.x] = total;
-}
-
-// per tile, in index order (round j, warp w, lane l holds item tile + 256 j + 32 w + l): the candidates, appended
-__global__ void __launch_bounds__(kThreads) top_emit_kernel(const float* __restrict__ s, uint32_t n, uint32_t ib,
-                                                            uint32_t* __restrict__ ctl,
-                                                            const uint32_t* __restrict__ tie_base,
-                                                            uint64_t* __restrict__ cand_key,
-                                                            uint32_t* __restrict__ cand_idx) {
-  if (ctl[kM] == 0) return;
-  const uint32_t T = ctl[kPrefix], r = ctl[kRank], ik_min = ~ctl[kKeyMax];
-  __shared__ uint32_t ties[kRounds * kWarps];          // ties per (round, warp), then their exclusive scan
-  const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
-  uint32_t ik[kRounds], eq_mask[kRounds];
-#pragma unroll
-  for (uint32_t j = 0; j < kRounds; ++j) {
-    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
-    ik[j] = i < n ? ~order_key(__float_as_uint(s[i])) : 0xFFFFFFFFu;
-    eq_mask[j] = __ballot_sync(0xFFFFFFFFu, i < n && ik[j] == T);
-    if (lane == 0) ties[j * kWarps + warp] = __popc(eq_mask[j]);
-  }
-  __syncthreads();
-  if (warp == 0) {                                     // exclusive scan of the 128 counts, 4 per lane
-    uint32_t v[4], sum = 0;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { v[q] = ties[lane * 4 + q]; sum += v[q]; }
-    uint32_t incl = sum;
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-      if ((int)lane >= o) incl += x;
-    }
-    uint32_t run = incl - sum;
-#pragma unroll
-    for (int q = 0; q < 4; ++q) { ties[lane * 4 + q] = run; run += v[q]; }
-  }
-  __syncthreads();
-  const uint32_t base = tie_base[blockIdx.x];
-#pragma unroll
-  for (uint32_t j = 0; j < kRounds; ++j) {
-    const uint32_t i = blockIdx.x * kTile + j * kThreads + threadIdx.x;
-    const uint32_t tie_rank = base + ties[j * kWarps + warp] + __popc(eq_mask[j] & lt);
-    const bool keep = i < n && (ik[j] < T || (ik[j] == T && tie_rank < r));
-    const uint32_t keep_mask = __ballot_sync(0xFFFFFFFFu, keep);
-    if (!keep_mask) continue;
-    uint32_t pos = 0;
-    if (lane == 0) pos = atomicAdd(&ctl[kCand], (uint32_t)__popc(keep_mask));
-    pos = __shfl_sync(0xFFFFFFFFu, pos, 0) + __popc(keep_mask & lt);
-    if (keep) {
-      cand_key[pos] = ((uint64_t)(ik[j] - ik_min) << ib) | i;
-      cand_idx[pos] = i;
-    }
-  }
-}
-
-// result j: the index, score and (with rows) row of the j-th candidate in sorted order; a warp per result
-__global__ void __launch_bounds__(kThreads) top_gather_kernel(const uint32_t* __restrict__ sorted_idx, uint32_t m,
-                                                              const float* __restrict__ s,
-                                                              const alz_edge_out* __restrict__ rows,
-                                                              uint32_t* __restrict__ out_index, float* __restrict__ out_scores,
-                                                              alz_edge_out* __restrict__ out_rows) {
-  constexpr uint32_t kWords = sizeof(alz_edge_out) / 8;
-  const uint32_t lane = threadIdx.x & 31u;
-  const uint32_t warps_per_grid = (gridDim.x * blockDim.x) >> 5;
-  for (uint32_t j = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < m; j += warps_per_grid) {
-    const uint32_t i = sorted_idx[j];
-    if (lane == 0) { out_index[j] = i; out_scores[j] = s[i]; }
-    if (rows) {
-      const uint64_t* src = reinterpret_cast<const uint64_t*>(rows + i);
-      uint64_t* dst = reinterpret_cast<uint64_t*>(out_rows + j);
-      for (uint32_t w = lane; w < kWords; w += 32) dst[w] = src[w];
-    }
-  }
-}
-static_assert(sizeof(alz_edge_out) % 8 == 0, "rows are copied in 8-byte words");
-}  // namespace top
 
 // The result buffers hold at least m rows: grown on demand, never shrunk; freed with the GNN state
 static int top_reserve(alz_handle* h, size_t m) {
@@ -893,56 +712,28 @@ static int top_reserve(alz_handle* h, size_t m) {
 }
 
 // The selection over n scores on the device (rows: n rows to gather from, or null). The state holds at least
-// top::scratch_rows(n, k) rows. *m_out = results, *above = eligible scores. One wait, for m.
+// top_scratch_rows(n, k) rows. *m_out = results, *above = eligible scores. One wait, for m.
 static int top_select(alz_handle* h, const float* scores, uint32_t n, uint32_t k, float min_score,
                       const alz_edge_out* rows, size_t* m_out, uint64_t* above) {
-  using namespace top;
   alz_gnn_state* g = h->gnn;
-  cudaStream_t s = h->stream;
   *m_out = 0;
   *above = 0;
-  if (n == 0) return ALZ_OK;
-  uint32_t* hist = g->d_flags;
-  uint32_t* ctl = g->d_flags + kHistWords;
-  const uint32_t tiles = (n + kTile - 1) / kTile;
-  uint32_t* tie_eq = g->d_pos;
-  uint32_t* tie_base = g->d_pos + tiles;
-  uint32_t ik_elig;
-  {
-    uint32_t u;
-    memcpy(&u, &min_score, 4);
-    ik_elig = ~order_key(u);
-  }
-  const unsigned grid = std::min<unsigned>(tiles, (unsigned)h->sms * 2);
-  CK(cudaMemsetAsync(g->d_flags, 0, (kHistWords + kCtlWords) * 4, s));
-  top_hist_kernel<0><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
-  top_pick_kernel<0><<<1, 1024, 0, s>>>(k, hist, ctl);
-  top_hist_kernel<1><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
-  top_pick_kernel<1><<<1, 1024, 0, s>>>(k, hist, ctl);
-  top_hist_kernel<2><<<grid, kThreads, 0, s>>>(scores, n, ik_elig, hist, ctl);
-  top_pick_kernel<2><<<1, 1024, 0, s>>>(k, hist, ctl);
-  top_ties_kernel<<<tiles, kThreads, 0, s>>>(scores, n, ctl, tie_eq);
-  CK(exclusive_scan_u32(g->d_tmp, g->tmp_bytes, tie_eq, tie_base, tiles, s));
-  const uint32_t ib = (uint32_t)bits_for(n - 1);
-  top_emit_kernel<<<tiles, kThreads, 0, s>>>(scores, n, ib, ctl, tie_base, g->d_nk, g->d_iota);
-  h->launches += 8;
-  CK(cudaGetLastError());
-  uint32_t c[kCtlWords];
-  CK(cudaMemcpyAsync(c, ctl, sizeof c, cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  *above = c[kAbove];
-  const uint32_t m = c[kM];
-  if (m == 0) return ALZ_OK;
-  const int rc = top_reserve(h, m);
+  const top::Scratch sc{g->d_flags, reinterpret_cast<uint64_t*>(g->d_pos), g->d_nk, g->d_iota, g->d_nk_sorted,
+                        g->d_vals, g->d_tmp, g->tmp_bytes};
+  const uint32_t* bits = reinterpret_cast<const uint32_t*>(scores);
+  uint32_t min_bits;
+  memcpy(&min_bits, &min_score, 4);
+  top::Ctl<uint32_t> c;
+  int rc = top::select_candidates<uint32_t>(h, bits, n, k, min_bits, sc, &c);
   if (rc != ALZ_OK) return rc;
-  const uint32_t ik_min = ~c[kKeyMax], T = c[kPrefix];
-  CK(sort_pairs(g->d_tmp, g->tmp_bytes, g->d_nk, g->d_nk_sorted, g->d_iota, g->d_vals, m, s,
-                (int)ib + bits_for(T - ik_min)));
-  top_gather_kernel<<<std::min<unsigned>((m + kWarps - 1) / kWarps, (unsigned)h->sms * 4), kThreads, 0, s>>>(
-      g->d_vals, m, scores, rows, g->d_top_index, g->d_top_scores, g->d_top_rows);
-  h->launches += 1;
-  CK(cudaGetLastError());
-  *m_out = m;
+  *above = c.above;
+  if (c.m == 0) return ALZ_OK;
+  rc = top_reserve(h, c.m);
+  if (rc != ALZ_OK) return rc;
+  rc = top::select_results<uint32_t>(h, bits, n, c, rows, sc, g->d_top_index,
+                                     reinterpret_cast<uint32_t*>(g->d_top_scores), g->d_top_rows);
+  if (rc != ALZ_OK) return rc;
+  *m_out = c.m;
   return ALZ_OK;
 }
 
@@ -1010,7 +801,7 @@ extern "C" int alz_gnn_score_rollup(alz_handle* h, uint32_t kind, float* scores,
 static int gnn_top_locked(alz_handle* h, const alz_edge_out* rows, size_t n_rows, uint32_t k, float min_score,
                           size_t* n_out, alz_top_info* info) {
   CK(cudaSetDevice(h->device));
-  int rc = gnn_run(h, rows, n_rows, top::scratch_rows(n_rows, k));
+  int rc = gnn_run(h, rows, n_rows, top_scratch_rows(n_rows, k));
   if (rc != ALZ_OK) return rc;
   uint64_t above = 0;
   rc = top_select(h, h->gnn->d_scores, (uint32_t)n_rows, k, min_score, rows, n_out, &above);
@@ -1089,7 +880,7 @@ extern "C" int alz_gnn_top_rollup_device(alz_handle* h, uint32_t kind, uint32_t 
 }
 
 // debug/test: the selection of alz_gnn_top over n scores in device memory, with the GNN state's scratch (grown to
-// top::scratch_rows(n, k) rows when smaller; a growth leaves no pass for alz_gnn_nodes to report). index: the
+// top_scratch_rows(n, k) rows when smaller; a growth leaves no pass for alz_gnn_nodes to report). index: the
 // results' indices, or null.
 extern "C" int alz_debug_top_scores(alz_handle* h, const float* dev_scores, size_t n, uint32_t k, float min_score,
                                     uint32_t* index, size_t cap, size_t* n_out, uint64_t* above) {
@@ -1102,7 +893,7 @@ extern "C" int alz_debug_top_scores(alz_handle* h, const float* dev_scores, size
   int rc = gnn_init(h);
   if (rc != ALZ_OK) return rc;
   if (n > kMaxRows) return ALZ_E_CAPACITY;
-  const size_t need = top::scratch_rows(n, k);
+  const size_t need = top_scratch_rows(n, k);
   const bool grows = need > h->gnn->cap_e;
   rc = gnn_reserve(h, need);
   if (rc != ALZ_OK) return rc;

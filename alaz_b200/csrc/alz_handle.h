@@ -32,6 +32,7 @@ struct alz_comm_state;  // alz_comm.cu
 struct alz_rollup_state;  // alz_rollup.cu
 struct alz_tier_set;      // alz_rollup.cu
 struct alz_span_state;    // alz_rollup.cu
+struct alz_metrics_state; // alz_metrics.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -123,6 +124,7 @@ struct alz_handle {
   alz_rollup_state* roll = nullptr;       // rolling windows (alz_window_history); null = off
   alz_tier_set* tiers = nullptr;          // tiered history (alz_window_history_tiers); null = off
   alz_span_state* span = nullptr;         // span rollup scratch (alz_window_rollup_span); null until the first one
+  alz_metrics_state* metrics = nullptr;   // edge metric buffers (alz_edge_metrics*, alz_edge_top*); null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -150,4 +152,5 @@ void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_span(alz_handle* h);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
+void alz_internal_free_metrics(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -305,6 +305,52 @@ int Aggregator::Anomalies(uint32_t source, uint32_t k, float min_score, std::vec
   return ALZ_OK;
 }
 
+int Aggregator::EdgeMetrics(uint32_t source, const std::vector<alz_metric>& metrics, std::vector<double>* values) {
+  if (!h_) return ALZ_E_STATE;
+  if (!values) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t nm = (uint32_t)metrics.size();
+  auto call = [&](double* v, size_t cap, size_t* n) {
+    return source == kLastWindow ? alz_edge_metrics(h_, metrics.data(), nm, v, cap, n)
+                                 : alz_edge_metrics_rollup(h_, source, metrics.data(), nm, v, cap, n);
+  };
+  size_t n = 0;
+  int rc = call(nullptr, 0, &n);                 // the row count, then the values
+  if (rc == ALZ_E_CAPACITY) {
+    values->assign(n * nm, 0.0);
+    rc = call(values->data(), n, &n);
+  } else if (rc == ALZ_OK) {
+    values->clear();
+  }
+  return rc;
+}
+
+int Aggregator::TopEdges(uint32_t source, const alz_metric& metric, uint32_t k, double min_value,
+                         std::vector<EdgeWindow>* out, alz_top_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  // into roll_ / values_, grown once when the results do not fit (ALZ_E_CAPACITY with n = the results; nothing written)
+  auto call = [&](size_t* n) {
+    return source == kLastWindow
+               ? alz_edge_top(h_, &metric, k, min_value, roll_.data(), values_.data(), nullptr, roll_.size(), n, info)
+               : alz_edge_top_rollup(h_, source, &metric, k, min_value, roll_.data(), values_.data(), nullptr,
+                                     roll_.size(), n, info);
+  };
+  size_t n = 0;
+  values_.resize(roll_.size());
+  int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {
+    roll_.resize(n);
+    values_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToEdges(roll_.data(), n, nullptr);
+  for (size_t i = 0; i < n; ++i) (*out)[i].Value = values_[i];
+  return ALZ_OK;
+}
+
 int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);

@@ -57,6 +57,7 @@ struct EdgeWindow {
   uint64_t Count = 0, Err5xx = 0, LatSumNs = 0;
   uint32_t Hist[ALZ_NB] = {0};
   float Score = 0.f;                              // GNN anomaly score when requested
+  double Value = 0.0;                             // the ranking metric's value (TopEdges)
 };
 
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
@@ -126,6 +127,14 @@ class Aggregator {
   // last Rollup / RollupSpan of that kind. info may be null. Returns 0 or an alz_status.
   int Anomalies(uint32_t source, uint32_t k, float min_score, std::vector<EdgeWindow>* out,
                 alz_top_info* info = nullptr);
+  // Edge metrics (docs/SPEC.md §17) of `source` (kLastWindow or a rollup kind, as in Anomalies): (*values)[i * m.size()
+  // + j] is metric j of row i, in the source's row order. Returns 0 or an alz_status.
+  int EdgeMetrics(uint32_t source, const std::vector<alz_metric>& metrics, std::vector<double>* values);
+  // the k rows of `source` with the highest values of `metric` >= min_value (fewer when fewer qualify), highest
+  // first, ties by row order, Value set, into *out (not to the data store): "the slowest / most failing edges".
+  // info may be null. Returns 0 or an alz_status.
+  int TopEdges(uint32_t source, const alz_metric& metric, uint32_t k, double min_value, std::vector<EdgeWindow>* out,
+               alz_top_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -176,8 +185,9 @@ class Aggregator {
   std::unordered_map<std::string, uint32_t> host_ids_;   // Host header text -> dense id (ALZ_NODE_OUTBOUND_HOST)
   std::vector<std::string> host_names_;
   std::vector<alz_edge_out> out_;
-  std::vector<alz_edge_out> roll_;   // rows of the last Rollup or Anomalies
+  std::vector<alz_edge_out> roll_;   // rows of the last Rollup, Anomalies or TopEdges
   std::vector<float> scores_;
+  std::vector<double> values_;       // values of the last TopEdges
   std::vector<alz_alive_conn> alive_;
 };
 

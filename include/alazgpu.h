@@ -433,6 +433,54 @@ int alz_gnn_top_rollup(alz_handle* h, uint32_t kind, uint32_t k, float min_score
 int alz_gnn_top_rollup_device(alz_handle* h, uint32_t kind, uint32_t k, float min_score, const alz_edge_out** dev_rows,
                               const float** dev_scores, const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
 
+/* ---- edge metrics and the top edges by a metric (docs/SPEC.md §17) ------------------------------------------------
+ * A metric's value for one row is a float64: COUNT (double)count; ERR5XX (double)err5xx; ERR_RATE err5xx / count;
+ * MEAN_NS lat_sum_ns / count (the stored sum, mod 2^64); the last two are 0 for count = 0. QUANTILE: the SPEC §5
+ * q-quantile of the row's histogram, bit for bit what alz_edge_quantiles(row, &q, 1, &v) returns. q must be in [0, 1]
+ * for QUANTILE and is ignored otherwise. Every value is finite and >= +0.
+ * Sources: the last flushed window (the rows alz_gnn_score scores), or the rows the last rollup of `kind`
+ * (ALZ_ROLLUP_*) returned, with the availability rule of §15 (none: ALZ_E_STATE). *n_out is always set; a host call
+ * whose cap (in rows) is below it returns ALZ_E_CAPACITY and writes nothing. k = 0, nm of 0 or more than
+ * ALZ_MAX_METRICS, an unknown metric or rollup kind, a q outside [0, 1] or NaN, a NaN min_value or a null required
+ * pointer: ALZ_E_INVAL. A 0-row source: *n_out = 0. More than 2^30 - 1 rows: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM.
+ * Reads only: no GNN pass runs and the GNN's scores, top results and alz_gnn_nodes stay valid; the source rows stay
+ * scorable. Device results stay valid until the next metric call on the handle. Every rank holds the same rows, so
+ * every rank gets the same result with no collective. */
+#define ALZ_METRIC_COUNT    0u
+#define ALZ_METRIC_ERR5XX   1u
+#define ALZ_METRIC_ERR_RATE 2u
+#define ALZ_METRIC_MEAN_NS  3u
+#define ALZ_METRIC_QUANTILE 4u
+#define ALZ_MAX_METRICS     8u
+typedef struct alz_metric {
+  uint32_t kind;   /* ALZ_METRIC_* */
+  uint32_t _pad;
+  double q;        /* ALZ_METRIC_QUANTILE: the quantile, in [0, 1] */
+} alz_metric;
+/* values[i * nm + j]: metric j of row i of the last flushed window, in its row order; cap counts rows */
+int alz_edge_metrics(alz_handle* h, const alz_metric* m, uint32_t nm, double* values, size_t cap, size_t* n_out);
+int alz_edge_metrics_device(alz_handle* h, const alz_metric* m, uint32_t nm, const double** dev_values, size_t* n_out);
+/* same, over the rows the last rollup of `kind` (ALZ_ROLLUP_*) returned */
+int alz_edge_metrics_rollup(alz_handle* h, uint32_t kind, const alz_metric* m, uint32_t nm, double* values, size_t cap,
+                            size_t* n_out);
+int alz_edge_metrics_rollup_device(alz_handle* h, uint32_t kind, const alz_metric* m, uint32_t nm,
+                                   const double** dev_values, size_t* n_out);
+/* The first min(k, above) rows by one metric's value, ranked as alz_gnn_top ranks scores but on the 64-bit key of the
+ * float64 value (u ^ 2^63 with the sign bit clear, ~u with it set), key descending, then row index ascending; a row is
+ * eligible when key(value) >= key(min_value). Result j: the row (byte for byte), its value (bit for bit what
+ * alz_edge_metrics* gives) and its row index; rows, values, index and info may each be NULL. info->scored = the
+ * source's rows, info->above = the eligible ones. Counts above 2^53 rank by their float64 value. */
+int alz_edge_top(alz_handle* h, const alz_metric* m, uint32_t k, double min_value, alz_edge_out* rows, double* values,
+                 uint32_t* index, size_t cap, size_t* n_out, alz_top_info* info);
+int alz_edge_top_device(alz_handle* h, const alz_metric* m, uint32_t k, double min_value, const alz_edge_out** dev_rows,
+                        const double** dev_values, const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
+int alz_edge_top_rollup(alz_handle* h, uint32_t kind, const alz_metric* m, uint32_t k, double min_value,
+                        alz_edge_out* rows, double* values, uint32_t* index, size_t cap, size_t* n_out,
+                        alz_top_info* info);
+int alz_edge_top_rollup_device(alz_handle* h, uint32_t kind, const alz_metric* m, uint32_t k, double min_value,
+                               const alz_edge_out** dev_rows, const double** dev_values, const uint32_t** dev_index,
+                               size_t* n_out, alz_top_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

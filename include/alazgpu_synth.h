@@ -35,6 +35,16 @@ int alz_gnn_nodes(alz_handle* h, uint64_t* node_keys, float* h2, size_t cap, siz
  * n > 2^30 - 1: ALZ_E_CAPACITY; k = 0 or a NaN min_score: ALZ_E_INVAL. */
 int alz_debug_top_scores(alz_handle* h, const float* dev_scores, size_t n, uint32_t k, float min_score,
                          uint32_t* index, size_t cap, size_t* n_out, uint64_t* above);
+/* test/debug: the metric kernel of alz_edge_metrics (docs/SPEC.md §17) over n rows in device memory, which may hold
+ * histograms the ingest path cannot make (cells of 2^32 - 1, count = 0 with a non-empty histogram); the rules of
+ * alz_edge_metrics otherwise */
+int alz_debug_edge_metrics_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, const alz_metric* m,
+                                uint32_t nm, double* values, size_t cap, size_t* n_out);
+/* test/debug: the selection of alz_edge_top over n float64 values in device memory: *n_out results, their indices
+ * into index (or NULL; cap too small: ALZ_E_CAPACITY, nothing written), *above the eligible values (or NULL).
+ * n > 2^30 - 1: ALZ_E_CAPACITY; k = 0 or a NaN min_value: ALZ_E_INVAL. */
+int alz_debug_top_keys64(alz_handle* h, const double* dev_values, size_t n, uint32_t k, double min_value,
+                         uint32_t* index, size_t cap, size_t* n_out, uint64_t* above);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
