@@ -189,6 +189,7 @@ extern "C" int alz_create(const alz_config* cfg, alz_handle** out) {
   CKC(cudaMemsetAsync(h->d_ctr, 0, sizeof(Counters), h->stream));
   CKC(cudaMalloc(&h->d_hot, sizeof(HotState)));
   CKC(cudaMemsetAsync(h->d_hot, 0, sizeof(HotState), h->stream));
+  CKC(cudaMalloc(&h->d_cursor, ingest_cursor_bytes()));
   int rc;
   if (!(h->cfg.flags & ALZ_CFG_EAGER_JOIN)) {
     if ((rc = alloc_table(h, &h->pairs, h->cfg.max_pairs, &h->d_ctr->pair_rows)) != ALZ_OK) return fail(rc);
@@ -241,7 +242,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_tiers(h);
   alz_internal_free_span(h);
   free_table(&h->pairs); free_table(&h->edges);
-  cudaFree(h->d_ep); cudaFree(h->d_ctr); cudaFree(h->d_hot); cudaFree(h->d_patch);
+  cudaFree(h->d_ep); cudaFree(h->d_ctr); cudaFree(h->d_hot); cudaFree(h->d_cursor); cudaFree(h->d_patch);
   cudaFree(h->d_win); cudaFree(h->d_defer[0]); cudaFree(h->d_defer[1]); cudaFree(h->d_bloom);
   if (h->h_bloom) cudaFreeHost(h->h_bloom);
   if (h->h_patch) cudaFreeHost(h->h_patch);
@@ -566,18 +567,19 @@ static int ingest_device(alz_handle* h, const void* d, uint64_t n, bool rec16, c
     const void* p = (const char*)d + done * rec_bytes;
     if (rec16) {   // overflow indices are absolute: every piece takes the same side array
       launch_ingest_pairs_rec16((const alz_l7_rec16*)p, m, d_ovf, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
-                                h->d_bloom, h->sms, h->stream);
+                                h->d_bloom, h->d_cursor, h->sms, h->stream);
     } else if (eager) {
       launch_ingest_eager((const alz_l7_rec*)p, m, h->d_ep, h->ep_cap - 1, h->edges, h->d_ctr, h->sms, h->stream);
     } else if (h->cfg.flags & ALZ_CFG_NO_SMEM_CACHE) {
       launch_ingest_pairs_v1((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_ep, h->ep_cap - 1, h->sms, h->stream);
     } else if (h->win_on) {
       launch_ingest_pairs_windowed((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1,
-                                   h->d_bloom, h->d_win, h->d_defer[h->defer_cur], h->defer_cap, h->sms, h->stream);
+                                   h->d_bloom, h->d_win, h->d_defer[h->defer_cur], h->defer_cap, h->d_cursor, h->sms,
+                                   h->stream);
       h->launches += 1;
     } else {
       launch_ingest_pairs((const alz_l7_rec*)p, m, h->pairs, h->d_ctr, h->d_hot, h->d_ep, h->ep_cap - 1, h->d_bloom,
-                          h->sms, h->stream);
+                          h->d_cursor, h->sms, h->stream);
     }
     CK(cudaGetLastError());
     h->launches += m ? 1 : 0;

@@ -87,6 +87,7 @@ struct alz_handle {
   alz::Counters* d_ctr = nullptr;
   alz::Counters* h_ctr = nullptr;  // pinned
   alz::HotState* d_hot = nullptr;
+  uint32_t* d_cursor = nullptr;           // the ingest's claim cursors (zeroed before each launch)
 
   // flush scratch
   uint64_t* d_keys[2] = {nullptr, nullptr};

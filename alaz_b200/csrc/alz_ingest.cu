@@ -50,12 +50,48 @@ __device__ unsigned long long g_ingest_phase[4];   // per CTA, summed: prologue,
 #define PROF_NOW() clock64()
 #define PROF_ADD(i, v) pt[i] += (unsigned long long)(v)
 #define PROF_FLUSH() do { if ((threadIdx.x & 31u) == 0) for (int i_ = 0; i_ < 8; ++i_) atomicAdd(&g_ingest_prof[i_], pt[i_]); } while (0)
+// Per-CTA timeline of the last kTlLaunches launches (read with alz_debug_ingest_timeline): for every CTA, %globaltimer
+// at entry, at the end of the main loop (after its __syncthreads) and at the end of the drain, %smid, clock64 at entry
+// and at the end (their ratio to the timer is the SM clock), and the chunks its warps took. Launches are numbered in
+// stream order: the last CTA of a launch to finish moves the number on, before the next launch can start.
+constexpr uint32_t kTlLaunches = 64, kTlCtas = 256, kTlWords = 8;
+__device__ unsigned long long g_ingest_tl[kTlLaunches][kTlCtas][kTlWords];
+__device__ unsigned int g_ingest_tl_launch, g_ingest_tl_done;
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ unsigned int sm_id() {
+  unsigned int r;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(r));
+  return r;
+}
+#define TL_DECL unsigned long long tl_t0 = 0, tl_c0 = 0, tl_t1 = 0; unsigned int tl_launch = 0; (void)tl_t1; (void)tl_launch
+#define TL_ENTRY() do { if (threadIdx.x == 0) { tl_launch = *(volatile unsigned int*)&g_ingest_tl_launch; tl_c0 = clock64(); tl_t0 = global_ns(); } } while (0)
+#define TL_LOOP_END() do { if (threadIdx.x == 0) tl_t1 = global_ns(); } while (0)
+#define TL_CHUNKS(v) do { if ((threadIdx.x & 31u) == 0 && blockIdx.x < kTlCtas) \
+    atomicAdd(&g_ingest_tl[*(volatile unsigned int*)&g_ingest_tl_launch % kTlLaunches][blockIdx.x][6], (unsigned long long)(v)); } while (0)
+#define TL_EXIT() do { if (threadIdx.x == 0) {                                                              \
+    const unsigned long long t2_ = global_ns(), c2_ = clock64();                                            \
+    if (blockIdx.x < kTlCtas) {                                                                             \
+      unsigned long long* e_ = g_ingest_tl[tl_launch % kTlLaunches][blockIdx.x];                           \
+      e_[0] = tl_t0; e_[1] = tl_t1; e_[2] = t2_; e_[3] = sm_id(); e_[4] = tl_c0; e_[5] = c2_;             \
+    }                                                                                                       \
+    __threadfence();                                                                                        \
+    if (atomicAdd(&g_ingest_tl_done, 1u) == gridDim.x - 1u) { g_ingest_tl_done = 0u; atomicAdd(&g_ingest_tl_launch, 1u); } \
+  } } while (0)
 #else
 #define PROF_DECL long long pc0 = 0, pc1 = 0; (void)pc0; (void)pc1
 #define PROF_NOW() 0ll
 #define PROF_ADD(i, v)
 #define PROF_FLUSH()
 #define PROF_PHASE(i, v)
+#define TL_DECL
+#define TL_ENTRY()
+#define TL_LOOP_END()
+#define TL_CHUNKS(v)
+#define TL_EXIT()
 #endif
 
 namespace {
@@ -70,8 +106,13 @@ constexpr uint32_t kColdQ = 128;           // cold queue entries per warp (ring)
 constexpr uint32_t kSlowQ = 64;            // slow queue entries per warp (ring)
 constexpr uint32_t kQBytes = 16;           // queue entry {key u64, dur_lo u32, meta u32}
 constexpr uint32_t kSmemMax = 232448;      // 227 KB per CTA on sm_90
+constexpr int kDefaultWarps = 16;
+constexpr int kMaxWarps = kDefaultWarps;   // cursors per handle (ChunkSched)
 constexpr int kU = 2;                      // events per lane per iteration
 constexpr uint32_t kChunk = 32u * kU;      // events per warp per iteration = one TMA copy
+constexpr uint32_t kDynEighths = 3;        // the last 3/8 of a launch's rounds of chunks are claimed, not assigned
+constexpr uint32_t kClaim = 2;             // chunks per claim from a cursor
+constexpr uint32_t kCursorStride = 64;     // u32 words between two cursors: one 256-byte line each
 
 template <int kWarps, int kRecWords>
 struct Layout {
@@ -238,6 +279,59 @@ struct Queue {
 };
 using SlowQueue = Queue<kSlowQ>;
 using ColdQueue = Queue<kColdQ>;
+
+// Which chunks a warp takes, in order. The first rounds keep a static map: in round r, warp w of the grid takes
+// chunk r * stride + w. The chunks after them, the last kDynEighths / 8 of the rounds, are claimed, so a warp whose
+// SM runs fast takes more of them and every SM finishes the launch at about the same time (the static share alone
+// left the latest CTA ~0.45 ms after the median one at config 2, DESIGN.md §5.2). Claimed chunk dyn0 + j belongs to
+// warp slot j mod kWarps of whichever CTA claims it: slot p's chunks are handed out kClaim at a time from cursor p,
+// which is zero at the start of every launch. One cursor for all warps took ~0.3 G claims/s at config 2, enough to
+// queue the claims at that line's L2 slice for longer than two loop iterations; kWarps cursors on their own lines
+// see 1/kWarps of them each. Warps of one CTA run at about the same speed, so the split by slot costs no balance.
+// Lane 0 makes the claims; the result is broadcast only when its first chunk is needed, kClaim chunks later (two loop
+// iterations), so the issue of the copy does not wait on the atomic. The sequence is strictly increasing: static
+// chunks lie below `dyn0`, and one thread's claims on one address come back in increasing order. So once it reaches
+// n_chunks, the warp has taken every chunk it was handed, and every chunk below n_chunks is taken by exactly one warp
+// (tests/test_ingest_sched_model.py runs the protocol on the host). All lanes call next() together and hold the same
+// state, so any lane can be the one that issues the copy.
+template <int kWarps>
+struct ChunkSched {
+  uint32_t* cursor;                    // this warp slot's cursor
+  uint32_t st_next, st_left, stride;   // next static chunk, static chunks left, chunks per round
+  uint32_t dyn0;                       // first claimed chunk of this warp slot
+  uint32_t blk, blk_left;              // the claimed chunks being handed out: blk, blk + kWarps, ...
+  uint32_t claim;                      // lane 0: the cursor value of the claim made ahead
+  __device__ __forceinline__ void claim_ahead(uint32_t lane) { if (lane == 0u) claim = atomicAdd(cursor, kClaim); }
+  __device__ __forceinline__ void init(uint32_t* cursors, uint32_t n_chunks, uint32_t warp, uint32_t c_stride,
+                                       uint32_t lane) {
+    cursor = cursors + warp * kCursorStride;
+    stride = c_stride;
+    const uint32_t first = blockIdx.x * kWarps + warp;
+    const uint32_t rounds = (uint32_t)(((uint64_t)n_chunks + c_stride - 1u) / c_stride);
+    st_left = rounds - (uint32_t)((uint64_t)rounds * kDynEighths / 8u);
+    st_next = first;
+    dyn0 = st_left * c_stride + warp;
+    blk = 0u; blk_left = 0u; claim = 0u;
+    if (st_left <= kClaim) claim_ahead(lane);
+  }
+  __device__ __forceinline__ uint32_t next(uint32_t lane) {
+    if (st_left != 0u) {
+      const uint32_t c = st_next;
+      st_next += stride;
+      if (--st_left == kClaim) claim_ahead(lane);
+      return c;
+    }
+    if (blk_left == 0u) {
+      blk = dyn0 + __shfl_sync(0xFFFFFFFFu, claim, 0) * kWarps;
+      blk_left = kClaim;
+      claim_ahead(lane);
+    }
+    --blk_left;
+    const uint32_t c = blk;
+    blk += kWarps;
+    return c;
+  }
+};
 
 // the global path for one event whose pair row is known
 __device__ __forceinline__ uint64_t keep_policy() {
@@ -483,12 +577,15 @@ __global__ void __launch_bounds__(kWarps * 32, 1)
 ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable pairs, Counters* ctr,
                        const HotState* __restrict__ hot, const EpEntry* __restrict__ ep, uint32_t ep_mask,
                        const uint32_t* __restrict__ bloom_g, const uint64_t* __restrict__ dur_ovf,
-                       const WinClock* __restrict__ win, uint4* __restrict__ defer_buf, uint32_t defer_cap) {
+                       const WinClock* __restrict__ win, uint4* __restrict__ defer_buf, uint32_t defer_cap,
+                       uint32_t* __restrict__ cursor) {
   using L = Layout<kWarps, kRecWords>;
   constexpr uint32_t kRows = L::kRows;
   extern __shared__ __align__(128) uint8_t smem_raw[];
   const long long k_entry = PROF_NOW();
   (void)k_entry;
+  TL_DECL;
+  TL_ENTRY();
   const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t lane_lt = (1u << lane) - 1u;
   Shared s;
@@ -511,39 +608,35 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable 
   const uint32_t ring_a = smem_u32(ring);
   const uint32_t bar_a = smem_u32(smem_raw + L::kBars + warp * 16u);
 
-  // chunks of this warp: c, c + stride, ... (a chunk = 64 consecutive records); all but possibly the last chunk
-  // of the array are full. 32-bit chunk numbers: n < 2^37 events per launch (the ABI layer splits above).
+  // a chunk = 64 consecutive records; all but possibly the last chunk of the array are full. 32-bit chunk numbers:
+  // n < 2^37 events per launch (the ABI layer splits above).
   const uint32_t n_chunks = (uint32_t)((n + kChunk - 1u) / kChunk);
-  const uint32_t c_stride = gridDim.x * kWarps;
-  const uint32_t c_first = blockIdx.x * kWarps + warp;
   const uint32_t tail = (uint32_t)(n - (uint64_t)(n_chunks - 1u) * kChunk);   // events in the last chunk, 1..kChunk
   uint64_t policy;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(policy));
-  // producer state (used by the elected lane): the chunk two iterations ahead and its address
-  uint32_t c_next = c_first;
-  const uint32_t* src_next = recs + (uint64_t)c_first * (kChunk * kRecWords);
-  const uint64_t src_step = (uint64_t)c_stride * (kChunk * kRecWords);        // in words
+  ChunkSched<kWarps> sched;
+  sched.init(cursor, n_chunks, warp, gridDim.x * kWarps, lane);
   // `dep` is always 0 but computed from the words just loaded out of the stage (see the main loop): the copy cannot
   // be issued before those loads have returned
-  auto issue = [&](uint32_t stage, uint32_t dep) {   // one lane; requests chunk c_next if there is one
-    if (c_next < n_chunks) {
-      const uint32_t bytes = (c_next == n_chunks - 1u ? tail : kChunk) * (uint32_t)kRecWords * 4u + dep;
+  auto issue = [&](uint32_t stage, uint32_t c_req, uint32_t dep) {   // one lane; requests chunk c_req if there is one
+    if (c_req < n_chunks) {
+      const uint32_t bytes = (c_req == n_chunks - 1u ? tail : kChunk) * (uint32_t)kRecWords * 4u + dep;
       mbar_expect_tx(bar_a + stage * 8u, bytes);
-      tma_load(ring_a + stage * L::kChunkBytes, src_next, bytes, bar_a + stage * 8u, policy);
+      tma_load(ring_a + stage * L::kChunkBytes, recs + (uint64_t)c_req * (kChunk * kRecWords), bytes,
+               bar_a + stage * 8u, policy);
     }
   };
   // the first two chunks are requested before the table is even built
+  const uint32_t c_first = sched.next(lane);
+  uint32_t c_ahead = sched.next(lane);          // chunk of the next iteration (requested)
   if (lane == 0) {
     mbar_init(bar_a, 1u);
     mbar_init(bar_a + 8u, 1u);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    issue(0u, 0u);
-    c_next += c_stride; src_next += src_step;
-    issue(1u, 0u);
+    issue(0u, c_first, 0u);
+    issue(1u, c_ahead, 0u);
   }
-  c_next += 2u * c_stride - (lane == 0 ? c_stride : 0u);   // every lane tracks the producer state, so any lane can be elected
-  src_next += 2u * src_step - (lane == 0 ? src_step : 0u);
 
   for (uint32_t i = threadIdx.x; i < kTab; i += kWarps * 32) s.tab[i] = 0u;
   for (uint32_t i = threadIdx.x; i < ALZ_BLOOM_WORDS; i += kWarps * 32) s.bloom[i] = bloom_g ? bloom_g[i] : 0xFFFFFFFFu;
@@ -565,7 +658,8 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable 
   const long long p_begin = PROF_NOW();
   (void)p_begin;
   uint32_t it = 0;
-  for (uint32_t c = c_first; c < n_chunks; c += c_stride, ++it) {
+  uint32_t c_req = 0;                           // chunk two iterations ahead, requested in this iteration
+  for (uint32_t c = c_first; c < n_chunks; c = c_ahead, c_ahead = c_req, ++it) {
     const uint32_t stage = it & 1u;
     pc0 = PROF_NOW();
     mbar_wait(bar_a + stage * 8u, (it >> 1) & 1u);
@@ -594,8 +688,8 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable 
     // shared-memory loads, and under load the TMA write of the next chunk overtook the duration loads of this one
     // (right keys with the wrong latencies).
     __syncwarp();
-    if (elect_one()) issue(stage, seen & zero);
-    c_next += c_stride; src_next += src_step;
+    c_req = sched.next(lane);
+    if (elect_one()) issue(stage, c_req, seen & zero);
     uint32_t n_here = (c == n_chunks - 1u) ? tail : kChunk;
 
     bool live[kU];
@@ -739,15 +833,18 @@ ingest_pairs_v8_kernel(const uint32_t* __restrict__ recs, uint64_t n, PairTable 
   PROF_ADD(2, t_wait);
   PROF_ADD(4, t_slow);
   PROF_FLUSH();
+  TL_CHUNKS(it);
   __syncthreads();
   const long long k_loop_end = PROF_NOW();
   (void)k_loop_end;
+  TL_LOOP_END();
 
   drain_rows_and_count<kWarps, kRows, kWin>(s, pairs, ctr, ep, ep_mask, lost, unresolved, n_hit, n_live, n_cold, n_late);
   PROF_PHASE(0, p_begin - k_entry);
   PROF_PHASE(1, k_loop_end - p_begin);
   PROF_PHASE(2, PROF_NOW() - k_loop_end);
   PROF_PHASE(3, 1);
+  TL_EXIT();
 }
 
 // open the first window on the first record ever submitted: epoch = (write_time + off) / len, docs/SPEC.md §8
@@ -871,42 +968,45 @@ __global__ void __launch_bounds__(256) hot_emit_kernel(PairTable pairs, HotState
 template <int kWarps, int kRecWords, bool kWin = false>
 void launch_variant(const void* recs, uint64_t n, const PairTable& pairs, Counters* ctr, const HotState* hot,
                     const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, const uint64_t* dur_ovf, int sms,
-                    cudaStream_t s, const WinClock* win = nullptr, void* defer_buf = nullptr, uint32_t defer_cap = 0) {
+                    uint32_t* cursor, cudaStream_t s, const WinClock* win = nullptr, void* defer_buf = nullptr,
+                    uint32_t defer_cap = 0) {
   using L = Layout<kWarps, kRecWords>;
+  static_assert(kWarps <= kMaxWarps, "one cursor per warp slot");
+  cudaMemsetAsync(cursor, 0, kWarps * kCursorStride * sizeof(uint32_t), s);   // every launch's claims start over
   // per device (a process may drive several GPUs), so not cached in a static
   cudaFuncSetAttribute(ingest_pairs_v8_kernel<kWarps, kRecWords, kWin>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                        (int)L::kBytes);
   ingest_pairs_v8_kernel<kWarps, kRecWords, kWin><<<(unsigned)sms, kWarps * 32, L::kBytes, s>>>(
-      (const uint32_t*)recs, n, pairs, ctr, hot, ep, ep_mask, bloom, dur_ovf, win, (uint4*)defer_buf, defer_cap);
+      (const uint32_t*)recs, n, pairs, ctr, hot, ep, ep_mask, bloom, dur_ovf, win, (uint4*)defer_buf, defer_cap, cursor);
 }
-
-constexpr int kDefaultWarps = 16;
 
 }  // namespace
 
 uint32_t ingest_table_rows() { return Layout<kDefaultWarps, 8>::kRows; }
+size_t ingest_cursor_bytes() { return (size_t)kMaxWarps * kCursorStride * sizeof(uint32_t); }
 
 void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
-                         const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, int sms,
-                         cudaStream_t s) {
+                         const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
+                         uint32_t* cursor, int sms, cudaStream_t s) {
   if (n == 0) return;
-  launch_variant<kDefaultWarps, 8>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, s);
+  launch_variant<kDefaultWarps, 8>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, cursor, s);
 }
 
 void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const PairTable& pairs,
                                Counters* ctr, const HotState* hot, const EpEntry* ep, uint32_t ep_mask,
-                               const uint32_t* bloom, int sms, cudaStream_t s) {
+                               const uint32_t* bloom, uint32_t* cursor, int sms, cudaStream_t s) {
   if (n == 0) return;
-  launch_variant<kDefaultWarps, 4>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, dur_ovf, sms, s);
+  launch_variant<kDefaultWarps, 4>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, dur_ovf, sms, cursor, s);
 }
 
 // time-cut windows: `win` = device WinClock {lo, len, ready}; records beyond the open window land in defer_buf
 void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
-                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s) {
+                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, uint32_t* cursor, int sms,
+                                  cudaStream_t s) {
   if (n == 0) return;
   win_init_kernel<<<1, 32, 0, s>>>((const uint32_t*)recs, n, (WinClock*)win);
-  launch_variant<kDefaultWarps, 8, true>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, s,
+  launch_variant<kDefaultWarps, 8, true>(recs, n, pairs, ctr, hot, ep, ep_mask, bloom, nullptr, sms, cursor, s,
                                          (const WinClock*)win, defer_buf, defer_cap);
 }
 void launch_window_advance(uint64_t* win, cudaStream_t s) { win_advance_kernel<<<1, 32, 0, s>>>((WinClock*)win); }
@@ -929,6 +1029,27 @@ void launch_hot_select(const PairTable& pairs, HotState* hot, int sms, cudaStrea
 }  // namespace alz
 
 // profiling build only: cycles per section of the ingest main loop since the last call (see g_ingest_prof)
+// profiling build only: the per-CTA timeline (see g_ingest_tl) into out[kTlLaunches][kTlCtas][kTlWords], and the
+// number of launches recorded since the last call (only the last kTlLaunches are kept); then starts over
+extern "C" int alz_debug_ingest_timeline(unsigned long long* out, unsigned int* n_launches, unsigned int* dims) {
+#ifdef ALZ_INGEST_PROF
+  dims[0] = alz::kTlLaunches; dims[1] = alz::kTlCtas; dims[2] = alz::kTlWords;
+  if (out == nullptr) return ALZ_OK;   // sizes only
+  if (cudaDeviceSynchronize() != cudaSuccess) return ALZ_E_CUDA;
+  if (cudaMemcpyFromSymbol(out, alz::g_ingest_tl, sizeof(alz::g_ingest_tl)) != cudaSuccess) return ALZ_E_CUDA;
+  if (cudaMemcpyFromSymbol(n_launches, alz::g_ingest_tl_launch, sizeof(unsigned int)) != cudaSuccess) return ALZ_E_CUDA;
+  void* z = nullptr;
+  if (cudaGetSymbolAddress(&z, alz::g_ingest_tl) != cudaSuccess || cudaMemset(z, 0, sizeof(alz::g_ingest_tl)) != cudaSuccess)
+    return ALZ_E_CUDA;
+  const unsigned int zero = 0;
+  if (cudaMemcpyToSymbol(alz::g_ingest_tl_launch, &zero, sizeof(zero)) != cudaSuccess) return ALZ_E_CUDA;
+  return cudaDeviceSynchronize() == cudaSuccess ? ALZ_OK : ALZ_E_CUDA;
+#else
+  (void)out; (void)n_launches; (void)dims;
+  return ALZ_E_UNSUPPORTED;
+#endif
+}
+
 extern "C" int alz_debug_ingest_prof(unsigned long long* out12) {   // 8 section counters + 4 phase counters
 #ifdef ALZ_INGEST_PROF
   unsigned long long z[8] = {0, 0, 0, 0, 0, 0, 0, 0};

@@ -17,21 +17,24 @@ struct WinClock {
 };
 void launch_ingest_pairs_v1(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                             const EpEntry* ep, uint32_t ep_mask, int sms, cudaStream_t s);
+// cursor: the handle's claim cursors (ingest_cursor_bytes(), alz_ingest.cu ChunkSched), zeroed before every launch
 void launch_ingest_pairs(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
-                         const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom, int sms,
-                         cudaStream_t s);
+                         const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
+                         uint32_t* cursor, int sms, cudaStream_t s);
 void launch_ingest_pairs_rec16(const alz_l7_rec16* recs, uint64_t n, const uint64_t* dur_ovf, const PairTable& pairs,
                                Counters* ctr, const HotState* hot, const EpEntry* ep, uint32_t ep_mask,
-                               const uint32_t* bloom, int sms, cudaStream_t s);
+                               const uint32_t* bloom, uint32_t* cursor, int sms, cudaStream_t s);
 void launch_ingest_pairs_windowed(const alz_l7_rec* recs, uint64_t n, const PairTable& pairs, Counters* ctr,
                                   const HotState* hot, const EpEntry* ep, uint32_t ep_mask, const uint32_t* bloom,
-                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, int sms, cudaStream_t s);
+                                  uint64_t* win, alz_l7_rec* defer_buf, uint32_t defer_cap, uint32_t* cursor, int sms,
+                                  cudaStream_t s);
 void launch_window_advance(uint64_t* win, cudaStream_t s);
 void launch_defer_resolve(alz_l7_rec* buf, uint32_t lo, uint32_t hi, const EpEntry* ep, uint32_t ep_mask, Counters* ctr,
                           int sms, cudaStream_t s);
 void launch_defer_roll(const alz_l7_rec* src, uint32_t n, const uint64_t* win, alz_l7_rec* dst, uint32_t cap,
                        const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s);
 uint32_t ingest_table_rows();
+size_t ingest_cursor_bytes();   // the handle's claim cursors (alz_ingest.cu, ChunkSched)
 void launch_hot_select(const PairTable& pairs, HotState* hot, int sms, cudaStream_t s);
 void launch_ingest_eager(const alz_l7_rec* recs, uint64_t n, const EpEntry* ep, uint32_t ep_mask,
                          const EdgeTable& edges, Counters* ctr, int sms, cudaStream_t s);
