@@ -152,6 +152,29 @@ def metrics(*specs):
     return (Metric * max(len(ms), 1))(*ms)
 
 
+SOURCE_WINDOW = 0xFFFFFFFF                                    # alz_baseline_pin / alz_edge_changes* sources
+CHANGE_DELTA, CHANGE_DROP, CHANGE_RATIO = 0, 1, 2             # change modes
+PRESENT_BOTH, PRESENT_NEW, PRESENT_GONE = 0x1, 0x2, 0x4       # presence bits and filter masks
+PRESENT_ALL = PRESENT_BOTH | PRESENT_NEW | PRESENT_GONE
+ABSENT = 0xFFFFFFFF                                           # index / base_index of the side a row is absent from
+
+EDGE_CHANGE = np.dtype([
+    ("from_type", "u1"), ("to_type", "u1"), ("presence", "u1"), ("_pad", "u1", (5,)),
+    ("from", "<u4"), ("to", "<u4"), ("index", "<u4"), ("base_index", "<u4"),
+    ("value", "<f8"), ("base_value", "<f8"), ("change", "<f8"),
+])
+assert EDGE_CHANGE.itemsize == 48
+
+
+class ChangeInfo(C.Structure):
+    """alz_change_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("source_rows", "base_rows", "both", "added", "gone", "listed", "above")] + \
+        [("source_windows", C.c_uint32), ("base_windows", C.c_uint32)]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

@@ -29,7 +29,8 @@ EXPORTS = [
     "alz_gnn_score_device", "alz_gnn_score_rollup", "alz_gnn_score_rollup_device", "alz_gnn_top", "alz_gnn_top_device",
     "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_edge_metrics", "alz_edge_metrics_device",
     "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device", "alz_edge_top", "alz_edge_top_device",
-    "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_baseline_pin", "alz_baseline_clear", "alz_edge_changes",
+    "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -101,6 +102,16 @@ def load(rebuild=False):
                                         C.POINTER(abi.TopInfo)], i),
         "alz_debug_edge_metrics_rows": ([vp, vp, sz, vp, u32, vp, sz, C.POINTER(sz)], i),
         "alz_debug_top_keys64": ([vp, vp, sz, u32, C.c_double, vp, sz, C.POINTER(sz), C.POINTER(u64)], i),
+        "alz_baseline_pin": ([vp, u32, C.POINTER(abi.RollupInfo)], i),
+        "alz_baseline_clear": ([vp], i),
+        "alz_edge_changes": ([vp, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_edge_changes_device": ([vp, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_edge_changes_top": ([vp, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
+                                  C.POINTER(abi.ChangeInfo)], i),
+        "alz_edge_changes_top_device": ([vp, u32, vp, u32, u32, u32, C.c_double, pp, C.POINTER(sz),
+                                         C.POINTER(abi.ChangeInfo)], i),
+        "alz_debug_edge_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
+                                         C.POINTER(abi.ChangeInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -139,7 +150,9 @@ def load(rebuild=False):
                   "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_debug_top_scores", "alz_edge_metrics",
                   "alz_edge_metrics_device", "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device",
                   "alz_edge_top", "alz_edge_top_device", "alz_edge_top_rollup", "alz_edge_top_rollup_device",
-                  "alz_debug_edge_metrics_rows", "alz_debug_top_keys64"):
+                  "alz_debug_edge_metrics_rows", "alz_debug_top_keys64", "alz_baseline_pin", "alz_baseline_clear",
+                  "alz_edge_changes", "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device",
+                  "alz_debug_edge_changes_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -530,6 +543,79 @@ class Handle:
     def edge_top_rollup_device(self, kind, spec, k, min_value=0.0):
         """alz_edge_top_rollup_device: (rows, values, index device pointers, results, info dict)."""
         return self._edge_top_device("alz_edge_top_rollup_device", (int(kind),), spec, k, min_value)
+
+    # ---- edge changes against a pinned baseline (alz_changes.cu, docs/SPEC.md §18)
+    def baseline_pin(self, source=abi.SOURCE_WINDOW):
+        """alz_baseline_pin: the rows of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) become the baseline; its info
+        dict."""
+        info = abi.RollupInfo()
+        self._ck(self.L.alz_baseline_pin(self.h, int(source), C.byref(info)), "alz_baseline_pin")
+        return info.as_dict()
+
+    def baseline_clear(self):
+        self._ck(self.L.alz_baseline_clear(self.h), "alz_baseline_clear")
+
+    def _changes(self, fn, args):
+        """fn(h, *args, out, cap, &n, &info): (alz_edge_change records, info dict); a first call with cap 0 sizes the
+        buffer (ALZ_E_CAPACITY when there are records)."""
+        f, n, info = getattr(self.L, fn), C.c_size_t(0), abi.ChangeInfo()
+        cap = 0
+        while True:
+            out = np.zeros(cap, dtype=abi.EDGE_CHANGE)
+            rc = self._ck(f(self.h, *args, _ptr(out) if cap else None, cap, C.byref(n), C.byref(info)), fn,
+                          allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                return out[: n.value].copy(), info.as_dict()
+            if n.value <= cap:   # a capacity error that no buffer cures: the union is too large
+                raise AlzError(rc, fn)
+            cap = n.value
+
+    def edge_changes(self, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
+        """alz_edge_changes of `source` against the pinned baseline by one metric (a METRIC_* kind or a (kind, q)
+        pair): (records in ascending key order, info dict)."""
+        return self._changes("alz_edge_changes", (int(source), abi.metrics(spec), int(mode), int(presence)))
+
+    def edge_changes_device(self, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
+        """alz_edge_changes_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_edge_changes_device(self.h, int(source), abi.metrics(spec), int(mode), int(presence),
+                                                C.byref(p), C.byref(n), C.byref(info)), "alz_edge_changes_device")
+        return p.value, n.value, info.as_dict()
+
+    def edge_changes_top(self, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                         source=abi.SOURCE_WINDOW):
+        """alz_edge_changes_top: (the first min(k, above) records by change, rank order; info dict)."""
+        return self._changes("alz_edge_changes_top", (int(source), abi.metrics(spec), int(mode), int(presence),
+                                                      int(k), float(min_change)))
+
+    def edge_changes_top_device(self, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                source=abi.SOURCE_WINDOW):
+        """alz_edge_changes_top_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_edge_changes_top_device(self.h, int(source), abi.metrics(spec), int(mode), int(presence),
+                                                    int(k), float(min_change), C.byref(p), C.byref(n),
+                                                    C.byref(info)), "alz_edge_changes_top_device")
+        return p.value, n.value, info.as_dict()
+
+    def debug_edge_changes_rows(self, src, base, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                src_windows=1, base_windows=1):
+        """alz_debug_edge_changes_rows over two host row arrays (copied to the device, each in strictly ascending
+        key order): (records, info dict)."""
+        src = np.ascontiguousarray(src, dtype=abi.EDGE_OUT)
+        base = np.ascontiguousarray(base, dtype=abi.EDGE_OUT)
+        ps = self.dev_alloc(max(src.nbytes, 1))
+        pb = self.dev_alloc(max(base.nbytes, 1))
+        try:
+            if len(src):
+                self.h2d(ps, src)
+            if len(base):
+                self.h2d(pb, base)
+            return self._changes("alz_debug_edge_changes_rows",
+                                 (C.c_void_p(ps), len(src), int(src_windows), C.c_void_p(pb), len(base),
+                                  int(base_windows), abi.metrics(spec), int(mode), int(presence)))
+        finally:
+            self.dev_free(ps)
+            self.dev_free(pb)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

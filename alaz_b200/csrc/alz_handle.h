@@ -33,6 +33,7 @@ struct alz_rollup_state;  // alz_rollup.cu
 struct alz_tier_set;      // alz_rollup.cu
 struct alz_span_state;    // alz_rollup.cu
 struct alz_metrics_state; // alz_metrics.cu
+struct alz_changes_state; // alz_changes.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -126,6 +127,7 @@ struct alz_handle {
   alz_tier_set* tiers = nullptr;          // tiered history (alz_window_history_tiers); null = off
   alz_span_state* span = nullptr;         // span rollup scratch (alz_window_rollup_span); null until the first one
   alz_metrics_state* metrics = nullptr;   // edge metric buffers (alz_edge_metrics*, alz_edge_top*); null until the first
+  alz_changes_state* changes = nullptr;   // the pinned baseline and the change list's buffers; null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -145,13 +147,20 @@ const uint64_t* alz_internal_merged_clock(alz_handle* h);
 // the flush's roll advances it; null without a window clock. Nothing happens with the history off. Caller holds h->mu.
 // With tiers configured the window is also the next input of tier 1 (docs/SPEC.md §13).
 int alz_internal_history_append(alz_handle* h, const uint64_t* d_clk);
-// The rows the last rollup of `kind` (ALZ_ROLLUP_*) returned with ALZ_OK, on the device: *rows, *n (docs/SPEC.md
-// §15). ALZ_E_INVAL for an unknown kind; ALZ_E_STATE when there are none. Caller holds h->mu.
-int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n);
+// The rows the last rollup of `kind` (ALZ_ROLLUP_*) returned with ALZ_OK, on the device: *rows, *n, and what that
+// call reported into *info when not null (docs/SPEC.md §15). ALZ_E_INVAL for an unknown kind; ALZ_E_STATE when there
+// are none. Caller holds h->mu.
+int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n,
+                             alz_rollup_info* info = nullptr);
+// What a k = 1 window rollup reports for the last flushed window (docs/SPEC.md §18): windows 1, its rows, its
+// alz_stats.windows, and its clock when the window history holds it as its newest entry (one wait); not clocked
+// otherwise. Caller holds h->mu and has set the device.
+int alz_internal_window_info(alz_handle* h, alz_rollup_info* info);
 void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_span(alz_handle* h);
 void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_metrics(alz_handle* h);
+void alz_internal_free_changes(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -16,18 +16,13 @@
 #include <mutex>
 #include <string>
 
-#include "alz_handle.h"
+#include "alz_metrics.cuh"
 #include "alz_top.cuh"
 
 using namespace alz;
+using namespace alz::metrics;
 
 namespace {
-
-struct MetricSet {
-  uint32_t nm;
-  uint32_t kind[ALZ_MAX_METRICS];
-  double q[ALZ_MAX_METRICS];
-};
 
 // docs/SPEC.md §4/§5 bucket bounds, float64 (exact)
 __device__ __forceinline__ double bucket_lo(uint32_t b) {
@@ -106,37 +101,38 @@ __global__ void __launch_bounds__(256) edge_metrics_hist_kernel(const alz_edge_o
   }
 }
 
-// the CUB item counts are ints and the selection's tile counts pack two 32-bit counts: at most 2^30 - 1 rows
-constexpr uint32_t kMaxRows = (1u << 30) - 1u;
-
-struct DevBuf {
-  void* p = nullptr;
-  size_t bytes = 0;
-};
-
 }  // namespace
 
 // Buffers of the metric calls, each grown on demand and never shrunk; freed in alz_destroy
 struct alz_metrics_state {
   DevBuf values;                 // rows x nm float64 values
-  DevBuf words, tile_cnt, cand_key, cand_idx, sorted_key, sorted_idx, tmp;   // the selection's scratch
-  DevBuf top_rows, top_values, top_index;                                      // the top call's results
+  Selection sel;                 // the top call's selection and results
 };
 
 void alz_internal_free_metrics(alz_handle* h) {
   alz_metrics_state* s = h->metrics;
   if (!s) return;
-  for (DevBuf* b : {&s->values, &s->words, &s->tile_cnt, &s->cand_key, &s->cand_idx, &s->sorted_key, &s->sorted_idx,
-                    &s->tmp, &s->top_rows, &s->top_values, &s->top_index})
-    cudaFree(b->p);
+  free_bufs({&s->values});
+  s->sel.free();
   delete s;
   h->metrics = nullptr;
 }
 
-namespace {
+namespace alz {
+namespace metrics {
 
-// Every buffer in `need` holds at least its bytes. The last calls may still read them: one wait before the first
-// buffer is replaced. A failed allocation leaves that buffer empty and returns ALZ_E_NOMEM.
+void free_bufs(std::initializer_list<DevBuf*> bufs) {
+  for (DevBuf* b : bufs) {
+    cudaFree(b->p);
+    *b = DevBuf{};
+  }
+}
+
+void Selection::free() {
+  free_bufs({&words, &tile_cnt, &cand_key, &cand_idx, &sorted_key, &sorted_idx, &tmp, &top_rows, &top_values,
+             &top_index});
+}
+
 int reserve(alz_handle* h, std::initializer_list<std::pair<DevBuf*, size_t>> need) {
   bool waited = false;
   for (const auto& [b, bytes] : need) {
@@ -155,11 +151,6 @@ int reserve(alz_handle* h, std::initializer_list<std::pair<DevBuf*, size_t>> nee
   return ALZ_OK;
 }
 
-// allocated on first use; its buffers start empty
-void metrics_state(alz_handle* h) {
-  if (!h->metrics) h->metrics = new alz_metrics_state();
-}
-
 bool valid_metrics(const alz_metric* m, uint32_t nm, MetricSet* ms) {
   if (!m || nm == 0 || nm > ALZ_MAX_METRICS) return false;
   *ms = MetricSet{};
@@ -173,22 +164,10 @@ bool valid_metrics(const alz_metric* m, uint32_t nm, MetricSet* ms) {
   return true;
 }
 
-// the rows of the last flushed window (rollup false) or of the last rollup of `kind`; caller holds h->mu
-int source_rows(alz_handle* h, bool rollup, uint32_t kind, const alz_edge_out** rows, size_t* n) {
-  *rows = h->d_out;
-  *n = h->last_n_edges;
-  if (rollup) return alz_internal_rollup_rows(h, kind, rows, n);
-  return ALZ_OK;
-}
-
-// the metrics of n rows into the values buffer, on the stream; no wait
-int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms) {
-  alz_metrics_state* s = h->metrics;
-  int rc = reserve(h, {{&s->values, std::max<size_t>((size_t)n * ms.nm, 1) * 8}});
-  if (rc != ALZ_OK || n == 0) return rc;
+int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out) {
+  if (n == 0) return ALZ_OK;
   bool quant = false;
   for (uint32_t j = 0; j < ms.nm; ++j) quant |= ms.kind[j] == ALZ_METRIC_QUANTILE;
-  double* out = static_cast<double*>(s->values.p);
   if (quant) {
     const unsigned grid = std::min<unsigned>((n + 7) / 8, (unsigned)h->sms * 8);
     edge_metrics_hist_kernel<<<grid, 256, 0, h->stream>>>(rows, n, ms, out);
@@ -201,6 +180,67 @@ int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const Metri
   return ALZ_OK;
 }
 
+int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,
+               const alz_edge_out* rows, size_t* m_out, uint64_t* above) {
+  *m_out = 0;
+  *above = 0;
+  if (n == 0) return ALZ_OK;
+  const uint32_t m_max = std::min(n, k);
+  int rc = reserve(h, {{&s.words, top::kWordsBytes},
+                       {&s.tile_cnt, (size_t)top::tiles(n) * 8},
+                       {&s.cand_key, (size_t)m_max * 8},
+                       {&s.cand_idx, (size_t)m_max * 4},
+                       {&s.sorted_key, (size_t)m_max * 8},
+                       {&s.sorted_idx, (size_t)m_max * 4},
+                       {&s.tmp, top::tmp_bytes<uint64_t>(n, m_max)}});
+  if (rc != ALZ_OK) return rc;
+  const top::Scratch sc{static_cast<uint32_t*>(s.words.p), static_cast<uint64_t*>(s.tile_cnt.p), s.cand_key.p,
+                        static_cast<uint32_t*>(s.cand_idx.p), s.sorted_key.p, static_cast<uint32_t*>(s.sorted_idx.p),
+                        s.tmp.p, s.tmp.bytes};
+  uint64_t min_bits;
+  memcpy(&min_bits, &min_value, 8);
+  top::Ctl<uint64_t> c;
+  rc = top::select_candidates<uint64_t>(h, vals, n, k, min_bits, sc, &c);
+  if (rc != ALZ_OK) return rc;
+  *above = c.above;
+  if (c.m == 0) return ALZ_OK;
+  rc = reserve(h, {{&s.top_rows, rows ? (size_t)c.m * sizeof(alz_edge_out) : 0}, {&s.top_values, (size_t)c.m * 8},
+                   {&s.top_index, (size_t)c.m * 4}});
+  if (rc != ALZ_OK) return rc;
+  rc = top::select_results<uint64_t>(h, vals, n, c, rows, sc, static_cast<uint32_t*>(s.top_index.p),
+                                     static_cast<uint64_t*>(s.top_values.p),
+                                     rows ? static_cast<alz_edge_out*>(s.top_rows.p) : nullptr);
+  if (rc != ALZ_OK) return rc;
+  *m_out = c.m;
+  return ALZ_OK;
+}
+
+}  // namespace metrics
+}  // namespace alz
+
+namespace {
+
+// allocated on first use; its buffers start empty
+void metrics_state(alz_handle* h) {
+  if (!h->metrics) h->metrics = new alz_metrics_state();
+}
+
+// the rows of the last flushed window (rollup false) or of the last rollup of `kind`; caller holds h->mu
+int source_rows(alz_handle* h, bool rollup, uint32_t kind, const alz_edge_out** rows, size_t* n) {
+  *rows = h->d_out;
+  *n = h->last_n_edges;
+  if (rollup) return alz_internal_rollup_rows(h, kind, rows, n);
+  return ALZ_OK;
+}
+
+// the metrics of n rows into the values buffer, on the stream; no wait
+int run_metrics_values(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms) {
+  alz_metrics_state* s = h->metrics;
+  const int rc = reserve(h, {{&s->values, std::max<size_t>((size_t)n * ms.nm, 1) * 8}});
+  if (rc != ALZ_OK) return rc;
+  return run_metrics(h, rows, n, ms, static_cast<double*>(s->values.p));
+}
+
 // The metrics of a source or of caller rows (dev_rows, n). Device variant: values null, *dev set. Host variant:
 // cap rows in values, one wait. Caller holds h->mu.
 int metrics_call(alz_handle* h, const alz_edge_out* rows, size_t n, const MetricSet& ms, double* values, size_t cap,
@@ -209,7 +249,7 @@ int metrics_call(alz_handle* h, const alz_edge_out* rows, size_t n, const Metric
   *n_out = n;
   if (!dev && n > cap) return ALZ_E_CAPACITY;
   metrics_state(h);
-  const int rc = run_metrics(h, rows, (uint32_t)n, ms);
+  const int rc = run_metrics_values(h, rows, (uint32_t)n, ms);
   if (rc != ALZ_OK) { *n_out = 0; return rc; }
   if (dev) {
     *dev = static_cast<const double*>(h->metrics->values.p);
@@ -235,44 +275,6 @@ int metrics_entry(alz_handle* h, bool rollup, uint32_t kind, const alz_metric* m
   return metrics_call(h, rows, n, ms, values, cap, dev, n_out);
 }
 
-// The selection of the top k of n float64 values (their bits, in device memory) with the state's scratch; rows: the
-// rows to gather from, or null. *m_out results in top_index / top_values (/ top_rows), *above eligible values.
-int select_top(alz_handle* h, const uint64_t* vals, uint32_t n, uint32_t k, double min_value, const alz_edge_out* rows,
-               size_t* m_out, uint64_t* above) {
-  alz_metrics_state* s = h->metrics;
-  *m_out = 0;
-  *above = 0;
-  if (n == 0) return ALZ_OK;
-  const uint32_t m_max = std::min(n, k);
-  int rc = reserve(h, {{&s->words, top::kWordsBytes},
-                       {&s->tile_cnt, (size_t)top::tiles(n) * 8},
-                       {&s->cand_key, (size_t)m_max * 8},
-                       {&s->cand_idx, (size_t)m_max * 4},
-                       {&s->sorted_key, (size_t)m_max * 8},
-                       {&s->sorted_idx, (size_t)m_max * 4},
-                       {&s->tmp, top::tmp_bytes<uint64_t>(n, m_max)}});
-  if (rc != ALZ_OK) return rc;
-  const top::Scratch sc{static_cast<uint32_t*>(s->words.p), static_cast<uint64_t*>(s->tile_cnt.p), s->cand_key.p,
-                        static_cast<uint32_t*>(s->cand_idx.p), s->sorted_key.p, static_cast<uint32_t*>(s->sorted_idx.p),
-                        s->tmp.p, s->tmp.bytes};
-  uint64_t min_bits;
-  memcpy(&min_bits, &min_value, 8);
-  top::Ctl<uint64_t> c;
-  rc = top::select_candidates<uint64_t>(h, vals, n, k, min_bits, sc, &c);
-  if (rc != ALZ_OK) return rc;
-  *above = c.above;
-  if (c.m == 0) return ALZ_OK;
-  rc = reserve(h, {{&s->top_rows, rows ? (size_t)c.m * sizeof(alz_edge_out) : 0}, {&s->top_values, (size_t)c.m * 8},
-                   {&s->top_index, (size_t)c.m * 4}});
-  if (rc != ALZ_OK) return rc;
-  rc = top::select_results<uint64_t>(h, vals, n, c, rows, sc, static_cast<uint32_t*>(s->top_index.p),
-                                     static_cast<uint64_t*>(s->top_values.p),
-                                     rows ? static_cast<alz_edge_out*>(s->top_rows.p) : nullptr);
-  if (rc != ALZ_OK) return rc;
-  *m_out = c.m;
-  return ALZ_OK;
-}
-
 // The top call over a source: the one metric's values, then the selection. Caller holds h->mu; *n_out = results.
 int top_call(alz_handle* h, bool rollup, uint32_t kind, const alz_metric* m, uint32_t k, double min_value,
              size_t* n_out, alz_top_info* info) {
@@ -285,11 +287,11 @@ int top_call(alz_handle* h, bool rollup, uint32_t kind, const alz_metric* m, uin
   if (rc != ALZ_OK) return rc;
   if (n > kMaxRows) return ALZ_E_CAPACITY;
   metrics_state(h);
-  rc = run_metrics(h, rows, (uint32_t)n, ms);
+  rc = run_metrics_values(h, rows, (uint32_t)n, ms);
   if (rc != ALZ_OK) return rc;
   uint64_t above = 0;
-  rc = select_top(h, static_cast<const uint64_t*>(h->metrics->values.p), (uint32_t)n, k, min_value, rows, n_out,
-                  &above);
+  rc = select_top(h, h->metrics->sel, static_cast<const uint64_t*>(h->metrics->values.p), (uint32_t)n, k, min_value,
+                  rows, n_out, &above);
   if (rc != ALZ_OK) return rc;
   if (info) { info->scored = n; info->above = above; }
   return ALZ_OK;
@@ -304,19 +306,19 @@ int top_entry(alz_handle* h, bool rollup, uint32_t kind, const alz_metric* m, ui
   std::lock_guard<std::mutex> g(h->mu);
   const int rc = top_call(h, rollup, kind, m, k, min_value, n_out, info);
   if (rc != ALZ_OK) { *n_out = 0; return rc; }
-  alz_metrics_state* s = h->metrics;
+  const Selection& s = h->metrics->sel;
   if (device) {
-    if (dev_rows) *dev_rows = static_cast<const alz_edge_out*>(s->top_rows.p);
-    if (dev_values) *dev_values = static_cast<const double*>(s->top_values.p);
-    if (dev_index) *dev_index = static_cast<const uint32_t*>(s->top_index.p);
+    if (dev_rows) *dev_rows = static_cast<const alz_edge_out*>(s.top_rows.p);
+    if (dev_values) *dev_values = static_cast<const double*>(s.top_values.p);
+    if (dev_index) *dev_index = static_cast<const uint32_t*>(s.top_index.p);
     return ALZ_OK;
   }
   const size_t n = *n_out;
   if (n > cap) return ALZ_E_CAPACITY;
   cudaStream_t st = h->stream;
-  if (n && rows) CK(cudaMemcpyAsync(rows, s->top_rows.p, n * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, st));
-  if (n && values) CK(cudaMemcpyAsync(values, s->top_values.p, n * 8, cudaMemcpyDeviceToHost, st));
-  if (n && index) CK(cudaMemcpyAsync(index, s->top_index.p, n * 4, cudaMemcpyDeviceToHost, st));
+  if (n && rows) CK(cudaMemcpyAsync(rows, s.top_rows.p, n * sizeof(alz_edge_out), cudaMemcpyDeviceToHost, st));
+  if (n && values) CK(cudaMemcpyAsync(values, s.top_values.p, n * 8, cudaMemcpyDeviceToHost, st));
+  if (n && index) CK(cudaMemcpyAsync(index, s.top_index.p, n * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return ALZ_OK;
 }
@@ -394,12 +396,13 @@ extern "C" int alz_debug_top_keys64(alz_handle* h, const double* dev_values, siz
   CK(cudaSetDevice(h->device));
   metrics_state(h);
   uint64_t ab = 0;
-  const int rc = select_top(h, reinterpret_cast<const uint64_t*>(dev_values), (uint32_t)n, k, min_value, nullptr, n_out, &ab);
+  const int rc = select_top(h, h->metrics->sel, reinterpret_cast<const uint64_t*>(dev_values), (uint32_t)n, k, min_value,
+                            nullptr, n_out, &ab);
   if (rc != ALZ_OK) { *n_out = 0; return rc; }
   if (above) *above = ab;
   if (*n_out > cap) return ALZ_E_CAPACITY;
   if (*n_out && index)
-    CK(cudaMemcpyAsync(index, h->metrics->top_index.p, *n_out * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(index, h->metrics->sel.top_index.p, *n_out * 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }

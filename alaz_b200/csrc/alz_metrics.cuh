@@ -1,0 +1,49 @@
+// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu): the §17 metric values of a row
+// list, the grow-on-demand device buffers and the 64-bit top selection with its own scratch.
+#pragma once
+#include <cstdint>
+#include <initializer_list>
+#include <utility>
+
+#include "alz_handle.h"
+
+namespace alz {
+namespace metrics {
+
+// the CUB item counts are ints and the selection's tile counts pack two 32-bit counts: at most 2^30 - 1 rows
+constexpr uint32_t kMaxRows = (1u << 30) - 1u;
+
+struct MetricSet {
+  uint32_t nm;
+  uint32_t kind[ALZ_MAX_METRICS];
+  double q[ALZ_MAX_METRICS];
+};
+// m[0, nm) is a valid metric list (docs/SPEC.md §17); *ms its kernel form
+bool valid_metrics(const alz_metric* m, uint32_t nm, MetricSet* ms);
+
+struct DevBuf {
+  void* p = nullptr;
+  size_t bytes = 0;
+};
+void free_bufs(std::initializer_list<DevBuf*> bufs);
+
+// Every buffer in `need` holds at least its bytes. The last calls may still read them: one wait before the first
+// buffer is replaced. A failed allocation leaves that buffer empty and returns ALZ_E_NOMEM.
+int reserve(alz_handle* h, std::initializer_list<std::pair<DevBuf*, size_t>> need);
+
+// The metrics of n rows into out[n * ms.nm], on the stream; no wait
+int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out);
+
+// The scratch and the results of one top selection over 64-bit values, grown on demand
+struct Selection {
+  DevBuf words, tile_cnt, cand_key, cand_idx, sorted_key, sorted_idx, tmp;   // the selection's scratch
+  DevBuf top_rows, top_values, top_index;                                      // its results
+  void free();
+};
+// The selection of the top k of n float64 values (their bits, in device memory); rows: the rows to gather from, or
+// null. *m_out results in s.top_index / s.top_values (/ s.top_rows), *above eligible values.
+int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,
+               const alz_edge_out* rows, size_t* m_out, uint64_t* above);
+
+}  // namespace metrics
+}  // namespace alz

@@ -65,9 +65,11 @@ struct RollupScratch {
   size_t tmp_bytes = 0;
   alz_edge_out* d_sum = nullptr;              // the last rollup's rows
   size_t sum_rows = 0;
-  // the last call of this kind returned ALZ_OK with held_rows rows in d_sum: what alz_gnn_score_rollup scores
+  // the last call of this kind returned ALZ_OK with held_rows rows in d_sum: what alz_gnn_score_rollup scores;
+  // held_info is what that call reported (kept whether or not the caller asked for it)
   bool held = false;
   size_t held_rows = 0;
+  alz_rollup_info held_info{};
 };
 
 // the clock of a tier's open block and of each of its entries: the oldest and newest covered window's clocks
@@ -582,10 +584,10 @@ static int ring_rollup(alz_handle* h, Ring<Clk>& r, uint32_t level, uint32_t k, 
 }
 
 // The sum of the last k entries of the window history (level 0) or of tier `level` into the scratch of that kind of
-// rollup, so that each one's rows stay valid until the next of its kind; *rows, *n_out. Caller holds h->mu and has
-// set the device.
+// rollup, so that each one's rows stay valid until the next of its kind; *rows, *n_out, *info and, with ALZ_OK,
+// *caller_info (when not null) = *info. Caller holds h->mu and has set the device.
 static int rollup_locked(alz_handle* h, uint32_t level, uint32_t k, size_t* n_out, alz_rollup_info* info,
-                         const alz_edge_out** rows) {
+                         alz_rollup_info* caller_info, const alz_edge_out** rows) {
   RollupScratch* sc = nullptr;
   int rc;
   if (level == 0) {
@@ -601,6 +603,7 @@ static int rollup_locked(alz_handle* h, uint32_t level, uint32_t k, size_t* n_ou
     rc = ring_rollup(h, ts->tiers[level - 1].ring, level, k, *sc, n_out, info);
   }
   *rows = sc->d_sum;
+  if (rc == ALZ_OK && caller_info) *caller_info = *info;
   return rc;
 }
 
@@ -616,18 +619,43 @@ static RollupScratch* scratch_of(alz_handle* h, uint32_t kind) {
 
 static uint32_t kind_of_tier(uint32_t tier) { return tier == 0 ? ALZ_ROLLUP_WINDOWS : ALZ_ROLLUP_TIER; }
 
-int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n) {
+int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** rows, size_t* n,
+                             alz_rollup_info* info) {
   if (kind > ALZ_ROLLUP_SPAN) return ALZ_E_INVAL;
   const RollupScratch* sc = scratch_of(h, kind);
   if (!sc || !sc->held) return ALZ_E_STATE;
   *rows = sc->d_sum;
   *n = sc->held_rows;
+  if (info) *info = sc->held_info;
   return ALZ_OK;
 }
 
-// A rollup entry point of a kind (ALZ_ROLLUP_*): lock, set the device and run the rollup (run(&rows), which sets
-// *n_out). Into out (to_host): ALZ_E_CAPACITY when the rows do not fit, and nothing is written; else *dev_rows (when
-// not null) = the device rows. The kind's scratch holds rows to score only after a call that returns ALZ_OK.
+int alz_internal_window_info(alz_handle* h, alz_rollup_info* info) {
+  *info = alz_rollup_info{};
+  info->windows = 1;
+  info->window_first = info->window_last = h->windows;
+  info->rows_in = h->last_n_edges;
+  const alz_rollup_state* st = h->roll;
+  if (!st || st->ring.entries.empty() || st->ring.entries.back().window_last != h->windows) return ALZ_OK;
+  // the window history's newest entry is this window: its clock, as a k = 1 window rollup reads it
+  const Entry& e = st->ring.entries.back();
+  if (!e.clocked) return ALZ_OK;
+  WinClock c;
+  CK(cudaMemcpyAsync(&c, st->ring.d_clk + e.slot, sizeof(WinClock), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  uint64_t first, last;
+  if (clock_epochs(c, &first, &last)) {
+    info->clocked = 1u;
+    info->epoch_first = first;
+    info->epoch_last = last;
+  }
+  return ALZ_OK;
+}
+
+// A rollup entry point of a kind (ALZ_ROLLUP_*): lock, set the device and run the rollup (run(&rows, &info), which
+// sets *n_out and, with ALZ_OK, info). Into out (to_host): ALZ_E_CAPACITY when the rows do not fit, and nothing is
+// written; else *dev_rows (when not null) = the device rows. The kind's scratch holds rows to score, and their info,
+// only after a call that returns ALZ_OK.
 template <class Run>
 static int rollup_call(alz_handle* h, uint32_t kind, bool to_host, alz_edge_out* out, size_t cap,
                        const alz_edge_out** dev_rows, size_t* n_out, Run run) {
@@ -637,7 +665,8 @@ static int rollup_call(alz_handle* h, uint32_t kind, bool to_host, alz_edge_out*
   if (!n_out || (!out && cap)) return ALZ_E_INVAL;
   CK(cudaSetDevice(h->device));
   const alz_edge_out* rows = nullptr;
-  const int rc = run(&rows);
+  alz_rollup_info info{};
+  const int rc = run(&rows, &info);
   if (rc != ALZ_OK) return rc;
   if (to_host) {
     if (*n_out > cap) return ALZ_E_CAPACITY;
@@ -649,6 +678,7 @@ static int rollup_call(alz_handle* h, uint32_t kind, bool to_host, alz_edge_out*
   RollupScratch* sc = scratch_of(h, kind);
   sc->held = true;
   sc->held_rows = *n_out;
+  sc->held_info = info;
   return ALZ_OK;
 }
 
@@ -665,13 +695,17 @@ extern "C" int alz_window_rollup(alz_handle* h, uint32_t k, alz_edge_out* out, s
 extern "C" int alz_window_rollup_tier_device(alz_handle* h, uint32_t tier, uint32_t k, const alz_edge_out** dev_rows,
                                              size_t* n_out, alz_rollup_info* info) {
   return rollup_call(h, kind_of_tier(tier), false, nullptr, 0, dev_rows, n_out,
-                     [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
+                     [&](const alz_edge_out** rows, alz_rollup_info* ri) {
+                       return rollup_locked(h, tier, k, n_out, ri, info, rows);
+                     });
 }
 
 extern "C" int alz_window_rollup_tier(alz_handle* h, uint32_t tier, uint32_t k, alz_edge_out* out, size_t cap,
                                       size_t* n_out, alz_rollup_info* info) {
   return rollup_call(h, kind_of_tier(tier), true, out, cap, nullptr, n_out,
-                     [&](const alz_edge_out** rows) { return rollup_locked(h, tier, k, n_out, info, rows); });
+                     [&](const alz_edge_out** rows, alz_rollup_info* ri) {
+                       return rollup_locked(h, tier, k, n_out, ri, info, rows);
+                     });
 }
 
 // ---- tiered history (docs/SPEC.md §13) ------------------------------------------------------------------------------
@@ -996,11 +1030,21 @@ static int span_locked(alz_handle* h, uint64_t N, uint32_t mode, size_t* n_out, 
 extern "C" int alz_window_rollup_span_device(alz_handle* h, uint64_t windows, uint32_t mode,
                                              const alz_edge_out** dev_rows, size_t* n_out, alz_span_info* info) {
   return rollup_call(h, ALZ_ROLLUP_SPAN, false, nullptr, 0, dev_rows, n_out,
-                     [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
+                     [&](const alz_edge_out** rows, alz_rollup_info* ri) {
+                       alz_span_info si;
+                       const int rc = span_locked(h, windows, mode, n_out, &si, rows);
+                       if (rc == ALZ_OK) { *ri = si.r; if (info) *info = si; }
+                       return rc;
+                     });
 }
 
 extern "C" int alz_window_rollup_span(alz_handle* h, uint64_t windows, uint32_t mode, alz_edge_out* out, size_t cap,
                                       size_t* n_out, alz_span_info* info) {
   return rollup_call(h, ALZ_ROLLUP_SPAN, true, out, cap, nullptr, n_out,
-                     [&](const alz_edge_out** rows) { return span_locked(h, windows, mode, n_out, info, rows); });
+                     [&](const alz_edge_out** rows, alz_rollup_info* ri) {
+                       alz_span_info si;
+                       const int rc = span_locked(h, windows, mode, n_out, &si, rows);
+                       if (rc == ALZ_OK) { *ri = si.r; if (info) *info = si; }
+                       return rc;
+                     });
 }

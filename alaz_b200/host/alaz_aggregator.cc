@@ -111,8 +111,15 @@ uint32_t Aggregator::Interner::Acquire(const std::string& uid) {
   auto it = ids.find(uid);
   if (it != ids.end()) return it->second;
   uint32_t id;
-  if (!free_ids.empty()) { id = free_ids.back(); free_ids.pop_back(); names[id] = uid; }
-  else { id = (uint32_t)names.size(); names.push_back(uid); refs.push_back(0); unmapped_in.push_back(0); }
+  if (!free_ids.empty()) {
+    id = free_ids.back();
+    free_ids.pop_back();
+    names[id] = uid;
+    reused_after[id] = std::max(reused_after[id], unmapped_in[id]);
+  } else {
+    id = (uint32_t)names.size();
+    names.push_back(uid); refs.push_back(0); unmapped_in.push_back(0); reused_after.push_back(0);
+  }
   ids.emplace(uid, id);
   return id;
 }
@@ -132,16 +139,36 @@ void Aggregator::Interner::Unmap(uint32_t ip, uint64_t open_window) {
   // keeps its id, like the reference keeps the map entry: ADD/UPDATE never delete the old IP, persist.go:55-65)
   if (--refs[id] == 0) { unmapped_in[id] = open_window; pending_free.push_back(id); }
 }
-void Aggregator::Interner::EndWindow(uint64_t flushed, uint64_t hold) {
+void Aggregator::Interner::EndWindow(uint64_t flushed, uint64_t hold, uint64_t pinned_from) {
   size_t keep = 0;
   for (uint32_t id : pending_free) {
     auto it = ids.find(names[id]);
     if (refs[id] != 0 || it == ids.end() || it->second != id) continue;   // mapped again, or freed already
     if (unmapped_in[id] + hold > flushed) { pending_free[keep++] = id; continue; }   // inside the retained span
+    if (pinned_from && unmapped_in[id] >= pinned_from) { pending_free[keep++] = id; continue; }   // in the baseline
     ids.erase(it);
     free_ids.push_back(id);
   }
   pending_free.resize(keep);
+  keep = 0;
+  for (uint32_t id : held) {
+    if (pinned_from && unmapped_in[id] >= pinned_from) held[keep++] = id;
+    else free_ids.push_back(id);
+  }
+  held.resize(keep);
+}
+bool Aggregator::Interner::CanHold(uint64_t pinned_from) const {
+  for (uint64_t r : reused_after)
+    if (r >= pinned_from) return false;
+  return true;
+}
+void Aggregator::Interner::Hold(uint64_t pinned_from) {
+  size_t keep = 0;
+  for (uint32_t id : free_ids) {
+    if (unmapped_in[id] >= pinned_from) held.push_back(id);
+    else free_ids[keep++] = id;
+  }
+  free_ids.resize(keep);
 }
 
 // processPod / processSvc: ADD and UPDATE write map[ip] = uid, DELETE removes (persist.go:55-71, 114-130)
@@ -255,8 +282,8 @@ int Aggregator::Flush(bool with_scores) {
   }
   std::vector<EdgeWindow> edges = ToEdges(out_.data(), n, with_scores ? scores_.data() : nullptr);
   windows_ += 1;
-  pods_.EndWindow(windows_, hold_);
-  svcs_.EndWindow(windows_, hold_);
+  pods_.EndWindow(windows_, hold_, pinned_from_);
+  svcs_.EndWindow(windows_, hold_, pinned_from_);
   return ds_ ? ds_->PersistEdgeWindow(edges) : ALZ_OK;
 }
 
@@ -348,6 +375,77 @@ int Aggregator::TopEdges(uint32_t source, const alz_metric& metric, uint32_t k, 
   if (rc != ALZ_OK) return rc;
   *out = ToEdges(roll_.data(), n, nullptr);
   for (size_t i = 0; i < n; ++i) (*out)[i].Value = values_[i];
+  return ALZ_OK;
+}
+
+// An id unmapped while window u was open may be carried by windows u and later only (refs fell to 0 in u), so a
+// baseline whose oldest window is w may carry exactly the ids unmapped in w or later, whether they are still pending,
+// already free (taken back here) or already handed to another UID (the pin is refused).
+int Aggregator::PinBaseline(uint32_t source, alz_rollup_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  alz_rollup_info ri{};
+  int rc = alz_baseline_pin(h_, source, &ri);
+  if (rc != ALZ_OK) return rc;   // an earlier baseline, if any, is still pinned and its hold stays
+  // alz_stats.windows counts the handle's flushes, which are this adapter's (Flush); an empty window history pins
+  // window_first = 0, which holds every id freed from window 1 on
+  const uint64_t from = std::max<uint64_t>(ri.window_first, 1);
+  if (!pods_.CanHold(from) || !svcs_.CanHold(from)) {
+    err_ = "PinBaseline: an id the source may carry has gone to another UID";
+    rc = alz_baseline_clear(h_);
+    pinned_from_ = 0;
+    pods_.EndWindow(windows_, hold_, 0);
+    svcs_.EndWindow(windows_, hold_, 0);
+    return rc != ALZ_OK ? rc : ALZ_E_STATE;
+  }
+  if (info) *info = ri;
+  pinned_from_ = from;
+  pods_.EndWindow(windows_, hold_, pinned_from_);   // the previous baseline's hold goes now
+  svcs_.EndWindow(windows_, hold_, pinned_from_);
+  pods_.Hold(pinned_from_);                         // and ids already free that this one may carry come back
+  svcs_.Hold(pinned_from_);
+  return ALZ_OK;
+}
+
+int Aggregator::ClearBaseline() {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  const int rc = alz_baseline_clear(h_);
+  if (rc != ALZ_OK) return rc;
+  pinned_from_ = 0;
+  pods_.EndWindow(windows_, hold_, 0);
+  svcs_.EndWindow(windows_, hold_, 0);
+  return ALZ_OK;
+}
+
+int Aggregator::Changes(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
+                        double min_change, std::vector<EdgeChange>* out, alz_change_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  // into changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
+  auto call = [&](size_t* n) {
+    return k == 0 ? alz_edge_changes(h_, source, &metric, mode, presence, changes_.data(), changes_.size(), n, info)
+                  : alz_edge_changes_top(h_, source, &metric, mode, presence, k, min_change, changes_.data(),
+                                         changes_.size(), n, info);
+  };
+  size_t n = 0;
+  int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > changes_.size()) {
+    changes_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  out->assign(n, EdgeChange{});
+  for (size_t i = 0; i < n; ++i) {
+    const alz_edge_change& c = changes_[i];
+    alz_edge_out row{};
+    row.from_type = c.from_type; row.to_type = c.to_type; row.from = c.from; row.to = c.to;
+    const EdgeWindow w = ToEdges(&row, 1, nullptr)[0];
+    EdgeChange& e = (*out)[i];
+    e.FromType = w.FromType; e.FromUID = w.FromUID; e.ToType = w.ToType; e.ToUID = w.ToUID;
+    e.Presence = c.presence; e.Value = c.value; e.BaseValue = c.base_value; e.Change = c.change;
+  }
   return ALZ_OK;
 }
 

@@ -60,6 +60,14 @@ struct EdgeWindow {
   double Value = 0.0;                             // the ranking metric's value (TopEdges)
 };
 
+// one row of a change list (docs/SPEC.md §18): the edge by UID, where it is (ALZ_PRESENT_*) and the metric's value on
+// each side with their change
+struct EdgeChange {
+  std::string FromType, FromUID, ToType, ToUID;
+  uint32_t Presence = 0;
+  double Value = 0.0, BaseValue = 0.0, Change = 0.0;
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -135,6 +143,19 @@ class Aggregator {
   // info may be null. Returns 0 or an alz_status.
   int TopEdges(uint32_t source, const alz_metric& metric, uint32_t k, double min_value, std::vector<EdgeWindow>* out,
                alz_top_info* info = nullptr);
+  // Edge changes (docs/SPEC.md §18). PinBaseline copies the rows of `source` (kLastWindow or a rollup kind, as in
+  // Anomalies) into the library's baseline; info may be null. Rows are matched by id, so while a baseline is pinned
+  // no pod or service id unmapped in the oldest window it covers or later is handed to another UID, including ids
+  // that were already free when it was pinned; ClearBaseline or another pin releases that hold. A source in which
+  // such an id has already gone to another UID (a rollup result older than SetHistory's hold) cannot be compared by
+  // id: the pin is refused with ALZ_E_STATE and no baseline is left. Returns 0 or an alz_status.
+  int PinBaseline(uint32_t source, alz_rollup_info* info = nullptr);
+  int ClearBaseline();
+  // The rows of `source` and the baseline whose presence is in `presence` (ALZ_PRESENT_* mask) with one metric's
+  // change by `mode` (ALZ_CHANGE_*), into *out: k = 0 every such row in key order, else the k largest changes >=
+  // min_change, largest first, ties in key order. info may be null. Returns 0 or an alz_status.
+  int Changes(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
+              double min_change, std::vector<EdgeChange>* out, alz_change_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -164,10 +185,18 @@ class Aggregator {
     std::unordered_map<uint32_t, uint32_t> ip_to_id;  // mirror of the device table's value per IP
     std::vector<uint64_t> unmapped_in;                // the window that was open when refs last fell to 0
     std::vector<uint32_t> free_ids, pending_free;
+    std::vector<uint32_t> held;                       // freed ids taken back while a pinned baseline may carry them
+    std::vector<uint64_t> reused_after;               // unmapped_in of the id when another UID last took it (0: never)
     uint32_t Acquire(const std::string& uid);
     void Map(uint32_t ip, uint32_t id, uint64_t open_window);
     void Unmap(uint32_t ip, uint64_t open_window);
-    void EndWindow(uint64_t flushed, uint64_t hold);
+    // pinned_from: no id unmapped in that window or later is freed (0: no baseline pinned); held ids outside it are
+    // freed again
+    void EndWindow(uint64_t flushed, uint64_t hold, uint64_t pinned_from);
+    // whether no id unmapped in window pinned_from or later has gone to another UID since
+    bool CanHold(uint64_t pinned_from) const;
+    // the free ids unmapped in window pinned_from or later are held
+    void Hold(uint64_t pinned_from);
   };
 
   DataStore* ds_;
@@ -181,6 +210,7 @@ class Aggregator {
   uint64_t dropped_events_ = 0;
   uint64_t windows_ = 0;          // windows flushed through Flush
   uint64_t hold_ = 0;             // windows a retained entry or open block can reach back (SetHistory)
+  uint64_t pinned_from_ = 0;      // the oldest window the pinned baseline covers; 0: none pinned
   Interner pods_, svcs_;
   std::unordered_map<std::string, uint32_t> host_ids_;   // Host header text -> dense id (ALZ_NODE_OUTBOUND_HOST)
   std::vector<std::string> host_names_;
@@ -189,6 +219,7 @@ class Aggregator {
   std::vector<float> scores_;
   std::vector<double> values_;       // values of the last TopEdges
   std::vector<alz_alive_conn> alive_;
+  std::vector<alz_edge_change> changes_;   // records of the last Changes
 };
 
 }  // namespace alaz

@@ -481,6 +481,66 @@ int alz_edge_top_rollup_device(alz_handle* h, uint32_t kind, const alz_metric* m
                                const alz_edge_out** dev_rows, const double** dev_values, const uint32_t** dev_index,
                                size_t* n_out, alz_top_info* info);
 
+/* ---- edge changes against a pinned baseline (docs/SPEC.md §18) ----------------------------------------------------
+ * A source is the last flushed window (ALZ_SOURCE_WINDOW) or the rows the last rollup of a kind (ALZ_ROLLUP_*)
+ * returned, with the availability rule of §15 (none: ALZ_E_STATE). alz_baseline_pin copies the source's rows, their
+ * packed keys and its alz_rollup_info into a baseline the handle owns (a window: windows = 1 and what a k = 1
+ * alz_window_rollup reports for it; a rollup: what that rollup call reported). The baseline survives flushes,
+ * rollups, alz_window_history* and every GNN or metric call; it goes with the next pin, alz_baseline_clear or
+ * alz_destroy. An empty source pins an empty baseline. info may be NULL. A failed growth: ALZ_E_NOMEM, no baseline. */
+#define ALZ_SOURCE_WINDOW 0xFFFFFFFFu   /* the last flushed window; the other sources are ALZ_ROLLUP_* */
+int alz_baseline_pin(alz_handle* h, uint32_t source, alz_rollup_info* info);
+int alz_baseline_clear(alz_handle* h);
+/* The union of a source's rows and the baseline's, matched by packed key (§3), in ascending key order, keeping the
+ * rows whose presence bit is in `presence`. value / base_value: the §17 value of metric m on the source / baseline row,
+ * bit for bit what alz_edge_metrics* gives, divided by the side's windows for COUNT and ERR5XX (one rounding); 0 on a
+ * side where the row is absent. change: from value and base_value by mode, one rounding. Unknown metric, mode or
+ * source, presence 0 or above 7, or a null required pointer: ALZ_E_INVAL. No baseline, or no source rows: ALZ_E_STATE.
+ * *n_out is always set; a host call whose cap (in records) is below it returns ALZ_E_CAPACITY and writes nothing. A
+ * union of more than 2^30 - 1 rows: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. info may be NULL. Reads only: the source,
+ * the baseline, GNN state and metric results are unchanged. Device results stay valid until the next change call.
+ * Every rank holds the same rows and pins the same baseline, so every rank gets the same result with no collective. */
+#define ALZ_CHANGE_DELTA 0u   /* change = value - base_value */
+#define ALZ_CHANGE_DROP  1u   /* change = base_value - value */
+#define ALZ_CHANGE_RATIO 2u   /* base_value > 0: value / base_value; base_value = 0: +inf when value > 0, else 1.0 */
+#define ALZ_PRESENT_BOTH 0x1u /* presence bits, and the filter mask: in both */
+#define ALZ_PRESENT_NEW  0x2u /* in the source only */
+#define ALZ_PRESENT_GONE 0x4u /* in the baseline only */
+typedef struct alz_edge_change {   /* 48 B */
+  uint8_t from_type;     /* ALZ_NODE_* */
+  uint8_t to_type;
+  uint8_t presence;      /* ALZ_PRESENT_* */
+  uint8_t _pad[5];
+  uint32_t from;
+  uint32_t to;
+  uint32_t index;        /* row index in the source, 0xFFFFFFFF when absent */
+  uint32_t base_index;   /* row index in the baseline, 0xFFFFFFFF when absent */
+  double value;
+  double base_value;
+  double change;
+} alz_edge_change;
+typedef struct alz_change_info {
+  uint64_t source_rows, base_rows;    /* the two sides' rows */
+  uint64_t both, added, gone;         /* the union by presence, before the filter */
+  uint64_t listed;                    /* union rows that pass the presence filter */
+  uint64_t above;                     /* top calls: listed rows with key(change) >= key(min_change); 0 otherwise */
+  uint32_t source_windows, base_windows;
+} alz_change_info;
+/* every listed row, in ascending key order */
+int alz_edge_changes(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                     alz_edge_change* out, size_t cap, size_t* n_out, alz_change_info* info);
+int alz_edge_changes_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                            const alz_edge_change** dev_out, size_t* n_out, alz_change_info* info);
+/* The first min(k, above) listed rows by change, ranked as alz_edge_top ranks values (64-bit key of the float64,
+ * descending, then position in the list ascending); a row is eligible when key(change) >= key(min_change). k = 0 or a
+ * NaN min_change: ALZ_E_INVAL. */
+int alz_edge_changes_top(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                         uint32_t k, double min_change, alz_edge_change* out, size_t cap, size_t* n_out,
+                         alz_change_info* info);
+int alz_edge_changes_top_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                                uint32_t k, double min_change, const alz_edge_change** dev_out, size_t* n_out,
+                                alz_change_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

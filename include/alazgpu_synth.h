@@ -45,6 +45,13 @@ int alz_debug_edge_metrics_rows(alz_handle* h, const alz_edge_out* dev_rows, siz
  * n > 2^30 - 1: ALZ_E_CAPACITY; k = 0 or a NaN min_value: ALZ_E_INVAL. */
 int alz_debug_top_keys64(alz_handle* h, const double* dev_values, size_t n, uint32_t k, double min_value,
                          uint32_t* index, size_t cap, size_t* n_out, uint64_t* above);
+/* test/debug: the join of alz_edge_changes (docs/SPEC.md §18) over two caller row lists in device memory, each in
+ * strictly ascending packed-key order and covering src_windows / base_windows (>= 1) windows; the pinned baseline
+ * is not used or touched. The rules of alz_edge_changes otherwise. */
+int alz_debug_edge_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size_t n_src, uint32_t src_windows,
+                                const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows,
+                                const alz_metric* m, uint32_t mode, uint32_t presence, alz_edge_change* out,
+                                size_t cap, size_t* n_out, alz_change_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
