@@ -175,6 +175,24 @@ class ChangeInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+EDGE_ENDS = np.dtype([("from_type", "u1"), ("to_type", "u1"), ("_pad", "u1", (6,)), ("from", "<u4"), ("to", "<u4")])
+assert EDGE_ENDS.itemsize == 16
+
+
+class EdgeEnds(C.Structure):
+    """alz_edge_ends: the head of alz_edge_out, the key of an edge series row (_pad is ignored)."""
+    _fields_ = [("from_type", C.c_uint8), ("to_type", C.c_uint8), ("_pad", C.c_uint8 * 6), ("from_", C.c_uint32),
+                ("to", C.c_uint32)]
+
+
+class SeriesInfo(C.Structure):
+    """alz_series_info."""
+    _fields_ = [("edges", C.c_uint64), ("rows_in", C.c_uint64), ("points", C.c_uint32), ("tier", C.c_uint32)]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

@@ -30,7 +30,8 @@ EXPORTS = [
     "alz_gnn_top_rollup", "alz_gnn_top_rollup_device", "alz_edge_metrics", "alz_edge_metrics_device",
     "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device", "alz_edge_top", "alz_edge_top_device",
     "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_baseline_pin", "alz_baseline_clear", "alz_edge_changes",
-    "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device", "alz_edge_series",
+    "alz_edge_series_device", "alz_edge_series_keys", "alz_edge_series_keys_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -112,6 +113,14 @@ def load(rebuild=False):
                                          C.POINTER(abi.ChangeInfo)], i),
         "alz_debug_edge_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
                                          C.POINTER(abi.ChangeInfo)], i),
+        "alz_edge_series": ([vp, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                             C.POINTER(abi.SeriesInfo)], i),
+        "alz_edge_series_device": ([vp, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                    C.POINTER(abi.SeriesInfo)], i),
+        "alz_edge_series_keys": ([vp, vp, sz, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                                  C.POINTER(abi.SeriesInfo)], i),
+        "alz_edge_series_keys_device": ([vp, vp, sz, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                         C.POINTER(abi.SeriesInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -152,7 +161,8 @@ def load(rebuild=False):
                   "alz_edge_top", "alz_edge_top_device", "alz_edge_top_rollup", "alz_edge_top_rollup_device",
                   "alz_debug_edge_metrics_rows", "alz_debug_top_keys64", "alz_baseline_pin", "alz_baseline_clear",
                   "alz_edge_changes", "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device",
-                  "alz_debug_edge_changes_rows"):
+                  "alz_debug_edge_changes_rows", "alz_edge_series", "alz_edge_series_device", "alz_edge_series_keys",
+                  "alz_edge_series_keys_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -616,6 +626,68 @@ class Handle:
         finally:
             self.dev_free(ps)
             self.dev_free(pb)
+
+    # ---- edge series (alz_series.cu, docs/SPEC.md §19)
+    @staticmethod
+    def edge_ends(edges):
+        """An EDGE_ENDS array from an EDGE_ENDS or EDGE_OUT array (its key fields), or (from_type, from, to_type, to)
+        tuples."""
+        if isinstance(edges, np.ndarray) and edges.dtype.names:
+            out = np.zeros(len(edges), dtype=abi.EDGE_ENDS)
+            for f in ("from_type", "to_type", "from", "to"):
+                out[f] = edges[f]
+            return out
+        out = np.zeros(len(edges), dtype=abi.EDGE_ENDS)
+        for i, (ft, f, tt, t) in enumerate(edges):
+            out[i] = (ft, tt, (0,) * 6, f, t)
+        return out
+
+    def _series(self, fn, head, tail, specs):
+        """fn(h, *head, *tail, m, nm, values, present, cap, &n, &P, points, &info): (values [n, P, nm] float64,
+        present [n, P] uint8, points as a list of alz_rollup_info dicts, info dict). A first call with cap 0 and no
+        points gives n and P."""
+        m, nm = abi.metrics(*specs), len(specs)
+        f, n, p, info = getattr(self.L, fn), C.c_size_t(0), C.c_uint32(0), abi.SeriesInfo()
+        self._ck(f(self.h, *head, *tail, m, nm, None, None, 0, C.byref(n), C.byref(p), None, C.byref(info)), fn,
+                 allow=(abi.E_CAPACITY,))
+        rows, P = n.value, p.value
+        values = np.zeros((rows, P, nm))
+        present = np.zeros((rows, P), dtype=np.uint8)
+        points = (abi.RollupInfo * max(P, 1))()
+        self._ck(f(self.h, *head, *tail, m, nm, _ptr(values), _ptr(present), rows, C.byref(n), C.byref(p), points,
+                   C.byref(info)), fn)
+        return values, present, [points[j].as_dict() for j in range(P)], info.as_dict()
+
+    def _series_device(self, fn, head, tail, specs):
+        """fn(h, *head, *tail, m, nm, &values, &present, &n, &P, points, &info): (values and present device pointers,
+        n, P, points, info dict). points has room for k entries."""
+        pv, pp_, n, p, info = C.c_void_p(), C.c_void_p(), C.c_size_t(0), C.c_uint32(0), abi.SeriesInfo()
+        k = int(tail[-1])
+        points = (abi.RollupInfo * max(min(k, 1 << 16), 1))()
+        self._ck(getattr(self.L, fn)(self.h, *head, *tail, abi.metrics(*specs), len(specs), C.byref(pv), C.byref(pp_),
+                                     C.byref(n), C.byref(p), points if k <= (1 << 16) else None, C.byref(info)), fn)
+        pts = [points[j].as_dict() for j in range(p.value)] if k <= (1 << 16) else None
+        return pv.value, pp_.value, n.value, p.value, pts, info.as_dict()
+
+    def edge_series(self, source, tier, k, *specs):
+        """alz_edge_series: every row of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) over the last k entries of
+        `tier` (0: the window history): (values [rows, P, nm], present [rows, P], points, info dict)."""
+        return self._series("alz_edge_series", (int(source),), (int(tier), int(k)), specs)
+
+    def edge_series_device(self, source, tier, k, *specs):
+        """alz_edge_series_device: (values and present device pointers, rows, P, points, info dict)."""
+        return self._series_device("alz_edge_series_device", (int(source),), (int(tier), int(k)), specs)
+
+    def edge_series_keys(self, edges, tier, k, *specs):
+        """alz_edge_series_keys: the caller's edges (see edge_ends), in their order, over the last k entries of
+        `tier`: (values [n, P, nm], present [n, P], points, info dict)."""
+        keys = np.ascontiguousarray(self.edge_ends(edges))
+        return self._series("alz_edge_series_keys", (_ptr(keys), len(keys)), (int(tier), int(k)), specs)
+
+    def edge_series_keys_device(self, edges, tier, k, *specs):
+        """alz_edge_series_keys_device: (values and present device pointers, n, P, points, info dict)."""
+        keys = np.ascontiguousarray(self.edge_ends(edges))
+        return self._series_device("alz_edge_series_keys_device", (_ptr(keys), len(keys)), (int(tier), int(k)), specs)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

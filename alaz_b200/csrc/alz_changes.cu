@@ -201,11 +201,15 @@ int source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_
   return alz_internal_rollup_rows(h, source, rows, n, info);
 }
 
-void launch_keys(alz_handle* h, const alz_edge_out* rows, uint32_t n, uint64_t* keys) {
+}  // namespace
+
+void alz::metrics::launch_row_keys(alz_handle* h, const alz_edge_out* rows, uint32_t n, uint64_t* keys) {
   if (n == 0) return;
   change_keys_kernel<<<std::min<unsigned>((n + 255) / 256, (unsigned)h->sms * 8), 256, 0, h->stream>>>(rows, n, keys);
   h->launches += 1;
 }
+
+namespace {
 
 // The join of a and b (docs/SPEC.md §18) into s->list, *listed records, and with top their changes into s->chg.
 // One wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
@@ -227,8 +231,8 @@ int join(alz_handle* h, Side a, Side b, const MetricSet& ms, uint32_t mode, uint
                        {&s->both, 4},
                        {&s->tmp, scan_temp_bytes((uint32_t)std::max(na, nb) + 1)}});
   if (rc != ALZ_OK) return rc;
-  if (!a.keys) { launch_keys(h, a.rows, a.n, static_cast<uint64_t*>(s->keys_a.p)); a.keys = static_cast<uint64_t*>(s->keys_a.p); }
-  if (!b.keys) { launch_keys(h, b.rows, b.n, static_cast<uint64_t*>(s->keys_b.p)); b.keys = static_cast<uint64_t*>(s->keys_b.p); }
+  if (!a.keys) { launch_row_keys(h, a.rows, a.n, static_cast<uint64_t*>(s->keys_a.p)); a.keys = static_cast<uint64_t*>(s->keys_a.p); }
+  if (!b.keys) { launch_row_keys(h, b.rows, b.n, static_cast<uint64_t*>(s->keys_b.p)); b.keys = static_cast<uint64_t*>(s->keys_b.p); }
   uint32_t* lb_a = static_cast<uint32_t*>(s->lb_a.p);
   uint32_t* lb_b = static_cast<uint32_t*>(s->lb_b.p);
   uint32_t* keep_a = static_cast<uint32_t*>(s->keep_a.p);
@@ -382,7 +386,7 @@ extern "C" int alz_baseline_pin(alz_handle* h, uint32_t source, alz_rollup_info*
   if (rc != ALZ_OK) return rc;
   if (n) {
     CK(cudaMemcpyAsync(s->base_rows.p, rows, n * sizeof(alz_edge_out), cudaMemcpyDeviceToDevice, h->stream));
-    launch_keys(h, static_cast<const alz_edge_out*>(s->base_rows.p), (uint32_t)n, static_cast<uint64_t*>(s->base_keys.p));
+    launch_row_keys(h, static_cast<const alz_edge_out*>(s->base_rows.p), (uint32_t)n, static_cast<uint64_t*>(s->base_keys.p));
     CK(cudaGetLastError());
   }
   s->base_n = n;

@@ -95,6 +95,18 @@ __device__ __forceinline__ uint64_t row_key_of(const alz_edge_out* r) {
   if (ft == ALZ_NODE_POD) return ((uint64_t)tt << 61) | ((uint64_t)(ft_.x & 0x1FFFFFFFu) << 32) | ft_.y;
   return (1ull << 63) | ((uint64_t)ft << 61) | ((uint64_t)(ft_.y & 0x1FFFFFFFu) << 32) | ft_.x;
 }
+// packed edge key of a caller's edge (the inverse of unpack_edge_key, what row_key_of gives for the row a flush
+// emitted with these ends); false for ends no flush emits: a type above ALZ_NODE_OUTBOUND_HOST, no pod end, or a pod
+// or service id >= 2^29. A pod <-> pod edge is keyed with its from end as the pod.
+inline bool pack_edge_ends(const alz_edge_ends& e, uint64_t* key) {
+  const uint32_t ft = e.from_type, tt = e.to_type;
+  if (ft > ALZ_NODE_OUTBOUND_HOST || tt > ALZ_NODE_OUTBOUND_HOST) return false;
+  auto id_ok = [](uint32_t type, uint32_t v) { return (type != ALZ_NODE_POD && type != ALZ_NODE_SVC) || v < (1u << 29); };
+  if (!id_ok(ft, e.from) || !id_ok(tt, e.to)) return false;
+  if (ft == ALZ_NODE_POD) { *key = ((uint64_t)tt << 61) | ((uint64_t)e.from << 32) | e.to; return true; }
+  if (tt == ALZ_NODE_POD) { *key = (1ull << 63) | ((uint64_t)ft << 61) | ((uint64_t)e.to << 32) | e.from; return true; }
+  return false;
+}
 // the fixed part of an output row and the lane's 8 histogram cells (hist sits at byte 40 of a 296-byte row:
 // 8-byte aligned only)
 __device__ __forceinline__ void store_edge_out(alz_edge_out* o, uint32_t sl, uint64_t key, const uint32_t (&c)[8],

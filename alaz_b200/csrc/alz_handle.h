@@ -34,6 +34,7 @@ struct alz_tier_set;      // alz_rollup.cu
 struct alz_span_state;    // alz_rollup.cu
 struct alz_metrics_state; // alz_metrics.cu
 struct alz_changes_state; // alz_changes.cu
+struct alz_series_state;  // alz_series.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -128,6 +129,7 @@ struct alz_handle {
   alz_span_state* span = nullptr;         // span rollup scratch (alz_window_rollup_span); null until the first one
   alz_metrics_state* metrics = nullptr;   // edge metric buffers (alz_edge_metrics*, alz_edge_top*); null until the first
   alz_changes_state* changes = nullptr;   // the pinned baseline and the change list's buffers; null until the first
+  alz_series_state* series = nullptr;     // the edge series' buffers (alz_edge_series*); null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -156,6 +158,19 @@ int alz_internal_rollup_rows(alz_handle* h, uint32_t kind, const alz_edge_out** 
 // alz_stats.windows, and its clock when the window history holds it as its newest entry (one wait); not clocked
 // otherwise. Caller holds h->mu and has set the device.
 int alz_internal_window_info(alz_handle* h, alz_rollup_info* info);
+// The last min(k, retained) closed entries of one ring, oldest first, read only: the window history (tier 0) or tier
+// t >= 1. Each is a run of rows [first_row, first_row + n) of the ring's arena.
+struct alz_ring_view {
+  const alz_edge_out* arena = nullptr;
+  std::vector<uint64_t> first_row, n;
+};
+// *v for tier `tier` and k >= 1; enqueues the copy of the ring's clocks to the host, which alz_internal_ring_points
+// reads once the stream has passed it. ALZ_E_STATE: tier 0 without the window history, t >= 1 without tiers;
+// ALZ_E_INVAL: a tier above the configured ones. Caller holds h->mu and has set the device.
+int alz_internal_ring_view(alz_handle* h, uint32_t tier, uint32_t k, alz_ring_view* v);
+// points[j] = what a rollup of view entry j alone reports, for the view the last alz_internal_ring_view call gave
+// (same tier and k, no call on the handle in between), after a wait on the stream. Caller holds h->mu.
+void alz_internal_ring_points(alz_handle* h, uint32_t tier, uint32_t k, alz_rollup_info* points);
 void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_span(alz_handle* h);
@@ -163,4 +178,5 @@ void alz_internal_free_comm(alz_handle* h);
 void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_metrics(alz_handle* h);
 void alz_internal_free_changes(alz_handle* h);
+void alz_internal_free_series(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -41,12 +41,31 @@ __device__ __forceinline__ double scalar_metric(uint32_t kind, uint64_t count, u
   }
 }
 
+// Output row i reads the row rows(i). With RowOf::kMayBeAbsent, rows(i) may be null: every value of output row i is
+// +0.0, and rows.mark(i, present) records which it was.
+struct PlainRows {
+  static constexpr bool kMayBeAbsent = false;
+  const alz_edge_out* e;
+  __device__ __forceinline__ const alz_edge_out* operator()(uint32_t i) const { return e + i; }
+};
+
 // a thread per row: the three sums only
-__global__ void __launch_bounds__(256) edge_metrics_sums_kernel(const alz_edge_out* __restrict__ e, uint32_t n,
-                                                                MetricSet ms, double* __restrict__ out) {
+template <class RowOf>
+__global__ void __launch_bounds__(256) edge_metrics_sums_kernel(const RowOf rows, uint32_t n, MetricSet ms,
+                                                                double* __restrict__ out) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const uint64_t count = e[i].count, err = e[i].err5xx, lat = e[i].lat_sum_ns;
+    const alz_edge_out* __restrict__ r = rows(i);
+    if constexpr (RowOf::kMayBeAbsent) {
+      rows.mark(i, r != nullptr);
+      if (!r) {
+#pragma unroll
+        for (uint32_t j = 0; j < ALZ_MAX_METRICS; ++j)
+          if (j < ms.nm) out[(size_t)i * ms.nm + j] = 0.0;
+        continue;
+      }
+    }
+    const uint64_t count = r->count, err = r->err5xx, lat = r->lat_sum_ns;
 #pragma unroll
     for (uint32_t j = 0; j < ALZ_MAX_METRICS; ++j)   // unrolled: ms stays in the parameter space, no local copy
       if (j < ms.nm) out[(size_t)i * ms.nm + j] = scalar_metric(ms.kind[j], count, err, lat);
@@ -54,12 +73,21 @@ __global__ void __launch_bounds__(256) edge_metrics_sums_kernel(const alz_edge_o
 }
 
 // a warp per row: one read of the histogram for every metric of the row; lane j < nm writes metric j
-__global__ void __launch_bounds__(256) edge_metrics_hist_kernel(const alz_edge_out* __restrict__ e, uint32_t n,
-                                                                MetricSet ms, double* __restrict__ out) {
+template <class RowOf>
+__global__ void __launch_bounds__(256) edge_metrics_hist_kernel(const RowOf rows, uint32_t n, MetricSet ms,
+                                                                double* __restrict__ out) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t warps_per_grid = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps_per_grid) {
-    const uint2 cc = *reinterpret_cast<const uint2*>(&e[i].hist[2 * lane]);
+    const alz_edge_out* __restrict__ r = rows(i);
+    if constexpr (RowOf::kMayBeAbsent) {   // the same row in every lane: the warp stays converged
+      if (lane == 0) rows.mark(i, r != nullptr);
+      if (!r) {
+        if (lane < ms.nm) out[(size_t)i * ms.nm + lane] = 0.0;
+        continue;
+      }
+    }
+    const uint2 cc = *reinterpret_cast<const uint2*>(&r->hist[2 * lane]);
     const uint64_t c0 = cc.x, c1 = cc.y;
     uint64_t incl = c0 + c1;                      // integer sums: exact, as the host's float64 sums of the cells are
     for (int o = 1; o < 32; o <<= 1) {
@@ -68,7 +96,7 @@ __global__ void __launch_bounds__(256) edge_metrics_hist_kernel(const alz_edge_o
     }
     const uint64_t total = __shfl_sync(0xFFFFFFFFu, (unsigned long long)incl, 31);
     const uint64_t before = incl - (c0 + c1);
-    const uint64_t count = e[i].count, err = e[i].err5xx, lat = e[i].lat_sum_ns;
+    const uint64_t count = r->count, err = r->err5xx, lat = r->lat_sum_ns;
     double mine = 0.0;
 #pragma unroll
     for (uint32_t j = 0; j < ALZ_MAX_METRICS; ++j) {   // unrolled: ms stays in the parameter space, no local copy
@@ -164,7 +192,13 @@ bool valid_metrics(const alz_metric* m, uint32_t nm, MetricSet* ms) {
   return true;
 }
 
-int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out) {
+}  // namespace metrics
+}  // namespace alz
+
+namespace {
+
+template <class RowOf>
+int launch_metrics(alz_handle* h, const RowOf& rows, uint32_t n, const MetricSet& ms, double* out) {
   if (n == 0) return ALZ_OK;
   bool quant = false;
   for (uint32_t j = 0; j < ms.nm; ++j) quant |= ms.kind[j] == ALZ_METRIC_QUANTILE;
@@ -178,6 +212,19 @@ int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const Metri
   h->launches += 1;
   CK(cudaGetLastError());
   return ALZ_OK;
+}
+
+}  // namespace
+
+namespace alz {
+namespace metrics {
+
+int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out) {
+  return launch_metrics(h, PlainRows{rows}, n, ms, out);
+}
+
+int run_metrics_series(alz_handle* h, const SeriesRows& rows, uint32_t n, const MetricSet& ms, double* out) {
+  return launch_metrics(h, rows, n, ms, out);
 }
 
 int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,

@@ -1,5 +1,6 @@
-// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu): the §17 metric values of a row
-// list, the grow-on-demand device buffers and the 64-bit top selection with its own scratch.
+// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu) and the edge series
+// (alz_series.cu): the §17 metric values of a row list or of series slots, the rows' packed keys, the grow-on-demand
+// device buffers and the 64-bit top selection with its own scratch.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -33,6 +34,32 @@ int reserve(alz_handle* h, std::initializer_list<std::pair<DevBuf*, size_t>> nee
 
 // The metrics of n rows into out[n * ms.nm], on the stream; no wait
 int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out);
+
+// The packed keys of n rows into keys[n], on the stream (16 of a row's 296 bytes read)
+void launch_row_keys(alz_handle* h, const alz_edge_out* rows, uint32_t n, uint64_t* keys);
+
+// The rows of an edge series (alz_series.cu): output row i = (series row i / P, point i % P) reads the arena row in
+// slot[u * P + point], u = map[series row] (map null: u = the series row), or nothing when that slot is kSlotAbsent;
+// present[i] says which.
+constexpr uint32_t kSlotAbsent = 0xFFFFFFFFu;
+struct SeriesRows {
+  static constexpr bool kMayBeAbsent = true;
+  const alz_edge_out* arena;
+  const uint32_t* slot;
+  const uint32_t* map;
+  uint32_t points;
+  uint8_t* present;
+#ifdef __CUDACC__
+  __device__ __forceinline__ const alz_edge_out* operator()(uint32_t i) const {
+    const uint32_t e = i / points, j = i - e * points;
+    const uint32_t s = slot[(map ? map[e] : e) * points + j];
+    return s == kSlotAbsent ? nullptr : arena + s;
+  }
+  __device__ __forceinline__ void mark(uint32_t i, bool p) const { present[i] = p ? 1u : 0u; }
+#endif
+};
+// The metrics of the n = rows x P series slots into out[n * ms.nm] and present[n], on the stream; no wait
+int run_metrics_series(alz_handle* h, const SeriesRows& rows, uint32_t n, const MetricSet& ms, double* out);
 
 // The scratch and the results of one top selection over 64-bit values, grown on demand
 struct Selection {

@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <deque>
 #include <new>
+#include <type_traits>
 #include <unordered_map>
 #include <vector>
 
@@ -115,6 +116,7 @@ struct Piece {
 // entry's the TierClk of its block.
 template <class Clk>
 struct Ring {
+  using value_type = Clk;
   uint32_t depth = 0;
   uint64_t arena_rows = 0;
   alz_edge_out* d_arena = nullptr;    // [arena_rows]
@@ -650,6 +652,49 @@ int alz_internal_window_info(alz_handle* h, alz_rollup_info* info) {
     info->epoch_last = last;
   }
   return ALZ_OK;
+}
+
+// the ring of tier `tier` (0: the window history) as f(ring, level), or the status when there is none
+template <class F>
+static int with_ring(alz_handle* h, uint32_t tier, F f) {
+  if (tier == 0) {
+    if (!h->roll) return ALZ_E_STATE;
+    f(h->roll->ring);
+    return ALZ_OK;
+  }
+  if (!h->tiers) return ALZ_E_STATE;
+  if (tier > h->tiers->tiers.size()) return ALZ_E_INVAL;
+  f(h->tiers->tiers[tier - 1].ring);
+  return ALZ_OK;
+}
+
+int alz_internal_ring_view(alz_handle* h, uint32_t tier, uint32_t k, alz_ring_view* v) {
+  int rc = ALZ_OK;
+  const int st = with_ring(h, tier, [&](auto& r) {
+    using Clk = typename std::remove_reference_t<decltype(r)>::value_type;
+    const cudaError_t e = cudaMemcpyAsync(r.h_clk.data(), r.d_clk, (size_t)r.depth * sizeof(Clk),
+                                          cudaMemcpyDeviceToHost, h->stream);
+    if (e != cudaSuccess) { h->last_err = std::string("alz_internal_ring_view: ") + cudaGetErrorString(e); rc = ALZ_E_CUDA; }
+    v->arena = r.d_arena;
+    v->first_row.clear();
+    v->n.clear();
+    for (size_t i = r.entries.size() - std::min<size_t>(k, r.entries.size()); i < r.entries.size(); ++i) {
+      v->first_row.push_back(r.entries[i].first_row);
+      v->n.push_back(r.entries[i].n);
+    }
+  });
+  return st != ALZ_OK ? st : rc;
+}
+
+void alz_internal_ring_points(alz_handle* h, uint32_t tier, uint32_t k, alz_rollup_info* points) {
+  with_ring(h, tier, [&](auto& r) {
+    size_t j = 0;
+    for (size_t i = r.entries.size() - std::min<size_t>(k, r.entries.size()); i < r.entries.size(); ++i, ++j) {
+      std::vector<Piece> one{r.piece(r.entries[i], tier)};
+      one[0].clocked = r.clocked(r.entries[i], &one[0].epoch_first, &one[0].epoch_last);
+      fill_info(one, &points[j]);
+    }
+  });
 }
 
 // A rollup entry point of a kind (ALZ_ROLLUP_*): lock, set the device and run the rollup (run(&rows, &info), which

@@ -2,8 +2,10 @@
 #include "alaz_aggregator.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <cstdint>
 
 #include "../../include/alazgpu_synth.h"   // alz_pinned_alloc / alz_pinned_free
 
@@ -446,6 +448,121 @@ int Aggregator::Changes(uint32_t source, const alz_metric& metric, uint32_t mode
     e.FromType = w.FromType; e.FromUID = w.FromUID; e.ToType = w.ToType; e.ToUID = w.ToUID;
     e.Presence = c.presence; e.Value = c.value; e.BaseValue = c.base_value; e.Change = c.change;
   }
+  return ALZ_OK;
+}
+
+bool Aggregator::ToEnds(const EdgeRef& e, alz_edge_ends* out) const {
+  auto end = [&](const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) {
+    if (type == "pod" || type == "service") {
+      const Interner& in = type == "pod" ? pods_ : svcs_;
+      const auto it = in.ids.find(uid);
+      if (it == in.ids.end()) return false;
+      *t = type == "pod" ? ALZ_NODE_POD : ALZ_NODE_SVC;
+      *v = it->second;
+      return true;
+    }
+    if (type != "outbound") return false;
+    bool ok = false;
+    const uint32_t ip = ParseIPv4(uid, &ok);
+    if (ok) { *t = ALZ_NODE_OUTBOUND; *v = ip; return true; }
+    const auto it = host_ids_.find(uid);   // a destination keyed by its Host header (data.go:851-854)
+    if (it == host_ids_.end()) return false;
+    *t = ALZ_NODE_OUTBOUND_HOST;
+    *v = it->second;
+    return true;
+  };
+  *out = alz_edge_ends{};
+  return end(e.FromType, e.FromUID, &out->from_type, &out->from) && end(e.ToType, e.ToUID, &out->to_type, &out->to);
+}
+
+template <class Call>
+int Aggregator::RunSeries(size_t nm, std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points, Call call) {
+  size_t n = 0;
+  uint32_t P = 0;
+  int rc = call(nullptr, nullptr, 0, &n, &P, nullptr);   // the sizes, then the values
+  if (rc != ALZ_OK && rc != ALZ_E_CAPACITY) return rc;
+  series_values_.assign(n * P * nm, 0.0);
+  series_present_.assign(n * P, 0);
+  std::vector<alz_rollup_info> pts(P);
+  rc = call(series_values_.data(), series_present_.data(), n, &n, &P, pts.data());
+  if (rc != ALZ_OK) return rc;
+  out->assign(n, EdgeSeries{});
+  for (size_t i = 0; i < n; ++i) {
+    (*out)[i].Present.assign(series_present_.begin() + i * P, series_present_.begin() + (i + 1) * P);
+    (*out)[i].Values.assign(series_values_.begin() + i * P * nm, series_values_.begin() + (i + 1) * P * nm);
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::Series(uint32_t source, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                       std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t nm = (uint32_t)metrics.size();
+  int rc = RunSeries(nm, out, points, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                          alz_rollup_info* pts) {
+    return alz_edge_series(h_, source == kLastWindow ? ALZ_SOURCE_WINDOW : source, tier, k, metrics.data(), nm, v, p,
+                           cap, n, P, pts, nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  // the names: the source's rows in its row order, from its top list by count with every row eligible and each
+  // row's index (no other call returns a rollup's held rows)
+  const size_t n = out->size();
+  if (n == 0) return ALZ_OK;
+  std::vector<alz_edge_out> ranked(n), rows(n);
+  std::vector<uint32_t> index(n);
+  const alz_metric count{ALZ_METRIC_COUNT, 0, 0.0};
+  const double all = -HUGE_VAL;
+  size_t m = 0;
+  rc = source == kLastWindow
+           ? alz_edge_top(h_, &count, (uint32_t)n, all, ranked.data(), nullptr, index.data(), n, &m, nullptr)
+           : alz_edge_top_rollup(h_, source, &count, (uint32_t)n, all, ranked.data(), nullptr, index.data(), n, &m,
+                                 nullptr);
+  if (rc != ALZ_OK) return rc;
+  if (m != n) return ALZ_E_STATE;
+  for (size_t j = 0; j < n; ++j) rows[index[j]] = ranked[j];
+  const std::vector<EdgeWindow> names = ToEdges(rows.data(), n, nullptr);
+  for (size_t i = 0; i < n; ++i) {
+    EdgeSeries& e = (*out)[i];
+    e.FromType = names[i].FromType; e.FromUID = names[i].FromUID; e.ToType = names[i].ToType; e.ToUID = names[i].ToUID;
+  }
+  return ALZ_OK;
+}
+
+int Aggregator::SeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint32_t k,
+                          const std::vector<alz_metric>& metrics, std::vector<EdgeSeries>* out,
+                          std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  // the edges with ids go to the library; the others are absent at every point
+  std::vector<alz_edge_ends> keys;
+  std::vector<size_t> row_of;   // edge -> row of keys, or SIZE_MAX
+  for (const EdgeRef& e : edges) {
+    alz_edge_ends k_{};
+    if (ToEnds(e, &k_)) { row_of.push_back(keys.size()); keys.push_back(k_); }
+    else row_of.push_back(SIZE_MAX);
+  }
+  const uint32_t nm = (uint32_t)metrics.size();
+  std::vector<EdgeSeries> known;
+  std::vector<alz_rollup_info> pts;
+  const int rc = RunSeries(nm, &known, &pts, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                                 alz_rollup_info* pp) {
+    return alz_edge_series_keys(h_, keys.data(), keys.size(), tier, k, metrics.data(), nm, v, p, cap, n, P, pp,
+                                nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  const size_t P = pts.size();
+  out->assign(edges.size(), EdgeSeries{});
+  for (size_t i = 0; i < edges.size(); ++i) {
+    EdgeSeries& e = (*out)[i];
+    if (row_of[i] != SIZE_MAX) e = known[row_of[i]];
+    else { e.Present.assign(P, 0); e.Values.assign(P * nm, 0.0); }
+    e.FromType = edges[i].FromType; e.FromUID = edges[i].FromUID; e.ToType = edges[i].ToType; e.ToUID = edges[i].ToUID;
+  }
+  if (points) *points = pts;
   return ALZ_OK;
 }
 

@@ -68,6 +68,20 @@ struct EdgeChange {
   double Value = 0.0, BaseValue = 0.0, Change = 0.0;
 };
 
+// an edge named by UID, as EdgeWindow names it: FromType / ToType "pod" | "service" | "outbound"; an outbound end's UID
+// is its dotted quad or its Host header text
+struct EdgeRef {
+  std::string FromType, FromUID, ToType, ToUID;
+};
+
+// one edge's series (docs/SPEC.md §19): per point, oldest first, whether that entry holds the edge and the metrics'
+// values on its row there (every value 0 where it does not)
+struct EdgeSeries {
+  std::string FromType, FromUID, ToType, ToUID;
+  std::vector<uint8_t> Present;   // [points]
+  std::vector<double> Values;     // [points * metrics]: metric j at point p is Values[p * metrics + j]
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -156,6 +170,18 @@ class Aggregator {
   // min_change, largest first, ties in key order. info may be null. Returns 0 or an alz_status.
   int Changes(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
               double min_change, std::vector<EdgeChange>* out, alz_change_info* info = nullptr);
+  // Edge series (docs/SPEC.md §19) over the last k entries of `tier` (0: flushed windows, 1..n: the tiers), oldest
+  // first; *points (may be null) gets what a rollup of each entry alone reports. Series gives one series per row of
+  // `source` (kLastWindow or a rollup kind, as in Anomalies), in its row order. SeriesFor gives one per edge named by
+  // UID, in the caller's order; an edge whose UID has no id (never seen, or freed) is absent at every point. Both match
+  // rows by id. That is correct by UID because SetHistory's hold never hands an id to another UID while a retained
+  // entry may carry it: a deleted pod's id stays its own until no entry covers the window it was deleted in, so its
+  // edges show under its UID up to its deletion and under no other UID. Series names the source's rows through
+  // alz_edge_top*, so the library's metric results refer to that call afterwards. Returns 0 or an alz_status.
+  int Series(uint32_t source, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+             std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int SeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -175,6 +201,12 @@ class Aggregator {
   int PersistRollup(uint32_t kind, bool with_scores, Call call);
   // rows -> EdgeWindow with the UIDs the interners hold (scores: one per row, or null)
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
+  // ends -> the library's key of an edge named by UID; false when a UID has no id
+  bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
+  // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then *out (names from
+  // `names`, one per series row); requires mu_
+  template <class Call>
+  int RunSeries(size_t nm, std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points, Call call);
   // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by
   // window w, and by every retained entry and open block that covers w: it is recycled once `hold` more windows
   // have been flushed after w (hold 0: when w is flushed).
@@ -220,6 +252,8 @@ class Aggregator {
   std::vector<double> values_;       // values of the last TopEdges
   std::vector<alz_alive_conn> alive_;
   std::vector<alz_edge_change> changes_;   // records of the last Changes
+  std::vector<double> series_values_;      // values and presence of the last Series / SeriesFor
+  std::vector<uint8_t> series_present_;
 };
 
 }  // namespace alaz

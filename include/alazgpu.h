@@ -541,6 +541,51 @@ int alz_edge_changes_top_device(alz_handle* h, uint32_t source, const alz_metric
                                 uint32_t k, double min_change, const alz_edge_change** dev_out, size_t* n_out,
                                 alz_change_info* info);
 
+/* ---- edge series (docs/SPEC.md §19) --------------------------------------------------------------------------------
+ * The §17 metric values of a set of edges in each of the last P = min(k, retained) closed entries of one ring, oldest
+ * first: the window history (tier 0) or tier t >= 1. Series row i is row i of a source (ALZ_SOURCE_WINDOW or
+ * ALZ_ROLLUP_*, with the availability rule of §15) or the caller's edge keys[i]. values[(i * P + j) * nm + m] is metric
+ * m on the row entry j holds for edge i (matched by packed key, §3), bit for bit what alz_edge_metrics* gives for that
+ * row; present[i * P + j] = 1 when the entry holds the edge, else 0 and every value +0.0. points[j] is what a rollup of
+ * entry j alone reports; points needs room for P <= k entries. *n_out (series rows) and *n_points (P) are always set;
+ * a host call whose cap (in series rows) is below *n_out returns ALZ_E_CAPACITY and writes nothing else. k = 0, a tier
+ * above the configured ones, a bad metric list (§17), an unknown source, a malformed key or a null required pointer:
+ * ALZ_E_INVAL. Tier 0 without the window history, t >= 1 without tiers, or no rows of a rollup source: ALZ_E_STATE.
+ * More than 2^30 - 1 slots (rows x P): ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. No retained entry: P = 0, ALZ_OK.
+ * present, points and info may be NULL. Reads only: the window, the retained entries, the open blocks, every rollup's
+ * rows, the baseline, metric, top, change and GNN results are unchanged. Device results stay valid until the next
+ * series call. Every rank holds the same history, so every rank gets the same result with no collective. */
+typedef struct alz_edge_ends {   /* 16 B: the head of alz_edge_out; _pad is ignored */
+  uint8_t from_type;   /* ALZ_NODE_* */
+  uint8_t to_type;
+  uint8_t _pad[6];
+  uint32_t from;
+  uint32_t to;
+} alz_edge_ends;
+typedef struct alz_series_info {
+  uint64_t edges;      /* series rows: the source's rows or n_keys */
+  uint64_t rows_in;    /* entry rows read: the sum of the P entries' rows */
+  uint32_t points;     /* P */
+  uint32_t tier;
+} alz_series_info;
+/* every row of a source; cap counts series rows */
+int alz_edge_series(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m, uint32_t nm,
+                    double* values, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                    alz_rollup_info* points, alz_series_info* info);
+int alz_edge_series_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m, uint32_t nm,
+                           const double** dev_values, const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                           alz_rollup_info* points, alz_series_info* info);
+/* the caller's edges, keys in host memory, in the caller's order; duplicates get identical rows. A key no flush can
+ * produce (a node type above 3, neither end a pod, a pod or service id >= 2^29) is malformed. A pod <-> pod edge named
+ * (A, B) is the row a flush emitted with from = A, to = B. */
+int alz_edge_series_keys(alz_handle* h, const alz_edge_ends* keys, size_t n_keys, uint32_t tier, uint32_t k,
+                         const alz_metric* m, uint32_t nm, double* values, uint8_t* present, size_t cap, size_t* n_out,
+                         uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+int alz_edge_series_keys_device(alz_handle* h, const alz_edge_ends* keys, size_t n_keys, uint32_t tier, uint32_t k,
+                                const alz_metric* m, uint32_t nm, const double** dev_values,
+                                const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                alz_rollup_info* points, alz_series_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces
