@@ -193,6 +193,33 @@ class SeriesInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+TREND_SLOPE, TREND_SHIFT, TREND_RATIO, TREND_ZSCORE = 0, 1, 2, 3   # alz_trend stats
+TREND_RISING, TREND_FALLING = 0, 1                                  # directions
+TREND_ABSENT_SKIP, TREND_ABSENT_ZERO = 0, 1                         # absent modes
+
+EDGE_TREND = np.dtype([
+    ("from_type", "u1"), ("to_type", "u1"), ("valid", "u1"), ("_pad", "u1", (5,)),
+    ("from", "<u4"), ("to", "<u4"), ("index", "<u4"), ("used", "<u4"),
+    ("trend", "<f8"), ("recent", "<f8"), ("before", "<f8"),
+])
+assert EDGE_TREND.itemsize == 48
+
+
+class Trend(C.Structure):
+    """alz_trend: stat TREND_*, direction TREND_RISING / TREND_FALLING, absent TREND_ABSENT_*, the last `recent`
+    points are recent, a valid row uses at least min_points points."""
+    _fields_ = [(n, C.c_uint32) for n in ("stat", "direction", "absent", "recent", "min_points", "_pad")]
+
+
+class TrendInfo(C.Structure):
+    """alz_trend_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("edges", "rows_in", "valid", "above")] + \
+        [("points", C.c_uint32), ("tier", C.c_uint32)]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

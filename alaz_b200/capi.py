@@ -31,7 +31,8 @@ EXPORTS = [
     "alz_edge_metrics_rollup", "alz_edge_metrics_rollup_device", "alz_edge_top", "alz_edge_top_device",
     "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_baseline_pin", "alz_baseline_clear", "alz_edge_changes",
     "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device", "alz_edge_series",
-    "alz_edge_series_device", "alz_edge_series_keys", "alz_edge_series_keys_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_edge_series_device", "alz_edge_series_keys", "alz_edge_series_keys_device", "alz_edge_trends",
+    "alz_edge_trends_device", "alz_edge_trends_top", "alz_edge_trends_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -121,6 +122,14 @@ def load(rebuild=False):
                                   C.POINTER(abi.SeriesInfo)], i),
         "alz_edge_series_keys_device": ([vp, vp, sz, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
                                          C.POINTER(abi.SeriesInfo)], i),
+        "alz_edge_trends": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                             C.POINTER(abi.TrendInfo)], i),
+        "alz_edge_trends_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), pp, C.POINTER(sz), C.POINTER(u32),
+                                    vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_edge_trends_top": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, vp, vp, vp, vp, sz,
+                                 C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_edge_trends_top_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp, pp, pp, pp,
+                                        C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -162,7 +171,8 @@ def load(rebuild=False):
                   "alz_debug_edge_metrics_rows", "alz_debug_top_keys64", "alz_baseline_pin", "alz_baseline_clear",
                   "alz_edge_changes", "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device",
                   "alz_debug_edge_changes_rows", "alz_edge_series", "alz_edge_series_device", "alz_edge_series_keys",
-                  "alz_edge_series_keys_device"):
+                  "alz_edge_series_keys_device", "alz_edge_trends", "alz_edge_trends_device", "alz_edge_trends_top",
+                  "alz_edge_trends_top_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -688,6 +698,70 @@ class Handle:
         """alz_edge_series_keys_device: (values and present device pointers, n, P, points, info dict)."""
         keys = np.ascontiguousarray(self.edge_ends(edges))
         return self._series_device("alz_edge_series_keys_device", (_ptr(keys), len(keys)), (int(tier), int(k)), specs)
+
+    # ---- edge trends (alz_trends.cu, docs/SPEC.md §20)
+    @staticmethod
+    def trend(stat=abi.TREND_SLOPE, direction=abi.TREND_RISING, absent=abi.TREND_ABSENT_SKIP, recent=1, min_points=0):
+        """An alz_trend."""
+        return abi.Trend(int(stat), int(direction), int(absent), int(recent), int(min_points), 0)
+
+    def edge_trends(self, source, tier, k, spec, trend):
+        """alz_edge_trends: every row of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) over the last k entries of
+        `tier` by one metric (a METRIC_* kind or a (kind, q) pair) and an abi.Trend: (EDGE_TREND records in source
+        order, points as a list of alz_rollup_info dicts, info dict). A first call with cap 0 gives the rows."""
+        f, n, p, info, m = self.L.alz_edge_trends, C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
+        self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), None, 0, C.byref(n), C.byref(p), None,
+                   C.byref(info)), "alz_edge_trends", allow=(abi.E_CAPACITY,))
+        out = np.zeros(n.value, dtype=abi.EDGE_TREND)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), _ptr(out), len(out), C.byref(n),
+                   C.byref(p), points, C.byref(info)), "alz_edge_trends")
+        return out, [points[j].as_dict() for j in range(p.value)], info.as_dict()
+
+    def edge_trends_device(self, source, tier, k, spec, trend):
+        """alz_edge_trends_device: (device pointer to the records, rows, P, points, info dict)."""
+        d, n, p, info = C.c_void_p(), C.c_size_t(0), C.c_uint32(0), abi.TrendInfo()
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(self.L.alz_edge_trends_device(self.h, int(source), int(tier), int(k), abi.metrics(spec),
+                                               C.byref(trend), C.byref(d), C.byref(n), C.byref(p), points,
+                                               C.byref(info)), "alz_edge_trends_device")
+        return d.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)], info.as_dict()
+
+    def edge_trends_top(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_edge_trends_top: the first min(top, above) valid rows by trend, rank order: (records, source rows,
+        series [m, P] float64, present [m, P] uint8, points, info dict). The first call offers room for min(top, 4096) results; when more came out, it is repeated with room for all."""
+        f, n, p, info, m = self.L.alz_edge_trends_top, C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
+        cap = min(int(top), 1 << 12)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        while True:
+            out = np.zeros(cap, dtype=abi.EDGE_TREND)
+            rows = np.zeros(cap, dtype=abi.EDGE_OUT)
+            series = np.zeros(cap * int(k))
+            present = np.zeros(cap * int(k), dtype=np.uint8)
+            rc = self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), int(top), float(min_trend),
+                            _ptr(out), _ptr(rows), _ptr(series), _ptr(present), cap, C.byref(n), C.byref(p), points,
+                            C.byref(info)), "alz_edge_trends_top", allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                break
+            if n.value <= cap:   # a capacity error that no buffer cures: too many slots
+                raise AlzError(rc, "alz_edge_trends_top")
+            cap = n.value
+        r, P = n.value, p.value
+        return (out[:r].copy(), rows[:r].copy(), series[: r * P].reshape(r, P).copy(),
+                present[: r * P].reshape(r, P).copy(), [points[j].as_dict() for j in range(P)], info.as_dict())
+
+    def edge_trends_top_device(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_edge_trends_top_device: (records, rows, series and present device pointers, results, P, points, info
+        dict)."""
+        pr, pw, ps, pp_ = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        n, p, info = C.c_size_t(0), C.c_uint32(0), abi.TrendInfo()
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(self.L.alz_edge_trends_top_device(self.h, int(source), int(tier), int(k), abi.metrics(spec),
+                                                   C.byref(trend), int(top), float(min_trend), C.byref(pr),
+                                                   C.byref(pw), C.byref(ps), C.byref(pp_), C.byref(n), C.byref(p),
+                                                   points, C.byref(info)), "alz_edge_trends_top_device")
+        return (pr.value, pw.value, ps.value, pp_.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)],
+                info.as_dict())
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

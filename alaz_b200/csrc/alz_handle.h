@@ -35,6 +35,7 @@ struct alz_span_state;    // alz_rollup.cu
 struct alz_metrics_state; // alz_metrics.cu
 struct alz_changes_state; // alz_changes.cu
 struct alz_series_state;  // alz_series.cu
+struct alz_trend_state;   // alz_trends.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -130,6 +131,7 @@ struct alz_handle {
   alz_metrics_state* metrics = nullptr;   // edge metric buffers (alz_edge_metrics*, alz_edge_top*); null until the first
   alz_changes_state* changes = nullptr;   // the pinned baseline and the change list's buffers; null until the first
   alz_series_state* series = nullptr;     // the edge series' buffers (alz_edge_series*); null until the first
+  alz_trend_state* trends = nullptr;      // the edge trends' buffers (alz_edge_trends*); null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -179,4 +181,5 @@ void alz_internal_free_gnn(alz_handle* h);
 void alz_internal_free_metrics(alz_handle* h);
 void alz_internal_free_changes(alz_handle* h);
 void alz_internal_free_series(alz_handle* h);
+void alz_internal_free_trends(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -1,6 +1,7 @@
-// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu) and the edge series
-// (alz_series.cu): the §17 metric values of a row list or of series slots, the rows' packed keys, the grow-on-demand
-// device buffers and the 64-bit top selection with its own scratch.
+// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
+// (alz_series.cu) and the edge trends (alz_trends.cu): the §17 metric values of a row list or of series slots, the
+// rows' packed keys, the grow-on-demand device buffers, a source's series into given buffers and the 64-bit top
+// selection with its own scratch.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -60,6 +61,20 @@ struct SeriesRows {
 };
 // The metrics of the n = rows x P series slots into out[n * ms.nm] and present[n], on the stream; no wait
 int run_metrics_series(alz_handle* h, const SeriesRows& rows, uint32_t n, const MetricSet& ms, double* out);
+
+// The buffers one edge series fills (alz_series.cu), grown on demand: the series calls own one set, the trend calls
+// (alz_trends.cu) another, so neither clobbers the other's device results
+struct SeriesBufs {
+  DevBuf keys, map, runs, slot;   // the distinct query keys, caller row -> distinct key, the entries' runs, the slots
+  DevBuf values, present;         // the results
+  alz_ring_view view;
+  void free();
+};
+// The series of the n source rows `rows` over the last min(k, retained) entries of tier `tier` into b.values /
+// b.present, on the stream, with no wait of its own. *n_out = n, *n_points = P, *rows_in = the entries' rows.
+// ALZ_E_CAPACITY for more than 2^30 - 1 slots or n > cap. Caller holds h->mu and has set the device.
+int run_series_rows(alz_handle* h, SeriesBufs& b, const alz_edge_out* rows, size_t n, uint32_t tier, uint32_t k,
+                    const MetricSet& ms, size_t cap, size_t* n_out, uint32_t* n_points, uint64_t* rows_in);
 
 // The scratch and the results of one top selection over 64-bit values, grown on demand
 struct Selection {

@@ -48,15 +48,15 @@ __global__ void __launch_bounds__(256) series_match_kernel(const alz_edge_out* _
 
 // Buffers of the series calls, each grown on demand and never shrunk; freed in alz_destroy
 struct alz_series_state {
-  DevBuf keys, map, runs, slot;   // the distinct query keys, caller row -> distinct key, the entries' runs, the slots
-  DevBuf values, present;         // the results
-  alz_ring_view view;
+  SeriesBufs b;
 };
+
+void alz::metrics::SeriesBufs::free() { free_bufs({&keys, &map, &runs, &slot, &values, &present}); }
 
 void alz_internal_free_series(alz_handle* h) {
   alz_series_state* s = h->series;
   if (!s) return;
-  free_bufs({&s->keys, &s->map, &s->runs, &s->slot, &s->values, &s->present});
+  s->b.free();
   delete s;
   h->series = nullptr;
 }
@@ -87,25 +87,21 @@ bool caller_edges(Edges* e) {
   return true;
 }
 
-// The series of `edges` over the last min(k, retained) entries of tier `tier`. Device call: *dev_values /
-// *dev_present; host call: cap series rows into values / present (either may be null when nothing is copied).
-// Caller holds h->mu.
-int series_locked(alz_handle* h, Edges& edges, uint32_t tier, uint32_t k, const MetricSet& ms, bool device,
-                  double* values, uint8_t* present, size_t cap, const double** dev_values,
-                  const uint8_t** dev_present, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
-                  alz_series_info* info) {
-  CK(cudaSetDevice(h->device));
-  if (!h->series) h->series = new alz_series_state();
-  alz_series_state* s = h->series;
-  int rc = alz_internal_ring_view(h, tier, k, &s->view);
+// The series of `edges` over the last min(k, retained) entries of tier `tier` into b, on the stream: *n_out series
+// rows, *n_points = P, *rows_in entry rows read. n_out > cap: ALZ_E_CAPACITY before anything is enqueued. wait_first:
+// one wait once the buffers are in place, before the first launch (the series device call's wait for the ring's
+// clocks); otherwise no wait of its own. Caller holds h->mu and has set the device.
+int series_enqueue(alz_handle* h, SeriesBufs& b, Edges& edges, uint32_t tier, uint32_t k, const MetricSet& ms,
+                   size_t cap, bool wait_first, size_t* n_out, uint32_t* n_points, uint64_t* rows_in_out) {
+  int rc = alz_internal_ring_view(h, tier, k, &b.view);
   if (rc != ALZ_OK) return rc;
-  const alz_ring_view& v = s->view;
+  const alz_ring_view& v = b.view;
   const uint32_t P = (uint32_t)v.n.size();
   const size_t n = edges.n;
   *n_out = n;
   *n_points = P;
   if ((uint64_t)n * P > kMaxRows) return ALZ_E_CAPACITY;
-  if (!device && n > cap) return ALZ_E_CAPACITY;
+  if (n > cap) return ALZ_E_CAPACITY;
   const bool by_source = edges.by_source;
   if (!by_source && !caller_edges(&edges)) return ALZ_E_INVAL;   // packed once the sizes are known to fit
   const size_t n_keys = by_source ? n : edges.keys.size();
@@ -118,55 +114,69 @@ int series_locked(alz_handle* h, Edges& edges, uint32_t tier, uint32_t k, const 
     rows_in += v.n[j];
   }
   runs[2 * (size_t)P] = (uint32_t)rows_in;
-  rc = reserve(h, {{&s->keys, std::max<size_t>(n_keys, 1) * 8},
-                   {&s->map, by_source ? 0 : std::max<size_t>(n, 1) * 4},
-                   {&s->runs, runs.size() * 4},
-                   {&s->slot, std::max<size_t>(n_keys * P, 1) * 4},
-                   {&s->values, std::max<size_t>(slots * ms.nm, 1) * 8},
-                   {&s->present, std::max<size_t>(slots, 1)}});
+  *rows_in_out = rows_in;
+  rc = reserve(h, {{&b.keys, std::max<size_t>(n_keys, 1) * 8},
+                   {&b.map, by_source ? 0 : std::max<size_t>(n, 1) * 4},
+                   {&b.runs, runs.size() * 4},
+                   {&b.slot, std::max<size_t>(n_keys * P, 1) * 4},
+                   {&b.values, std::max<size_t>(slots * ms.nm, 1) * 8},
+                   {&b.present, std::max<size_t>(slots, 1)}});
   if (rc != ALZ_OK) return rc;
   cudaStream_t st = h->stream;
-  if (device) {
-    CK(cudaStreamSynchronize(st));   // the one wait: the ring's clocks
-    if (points) alz_internal_ring_points(h, tier, k, points);
+  if (wait_first) CK(cudaStreamSynchronize(st));   // the one wait: the ring's clocks
+  uint64_t* d_keys = static_cast<uint64_t*>(b.keys.p);
+  uint32_t* d_runs = static_cast<uint32_t*>(b.runs.p);
+  uint32_t* d_slot = static_cast<uint32_t*>(b.slot.p);
+  if (!slots) return ALZ_OK;
+  if (by_source) {
+    launch_row_keys(h, edges.rows, (uint32_t)n, d_keys);
+  } else {
+    CK(cudaMemcpyAsync(d_keys, edges.keys.data(), n_keys * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(b.map.p, edges.map.data(), n * 4, cudaMemcpyHostToDevice, st));
   }
-  uint64_t* d_keys = static_cast<uint64_t*>(s->keys.p);
-  uint32_t* d_runs = static_cast<uint32_t*>(s->runs.p);
-  uint32_t* d_slot = static_cast<uint32_t*>(s->slot.p);
-  if (slots) {
-    if (by_source) {
-      launch_row_keys(h, edges.rows, (uint32_t)n, d_keys);
-    } else {
-      CK(cudaMemcpyAsync(d_keys, edges.keys.data(), n_keys * 8, cudaMemcpyHostToDevice, st));
-      CK(cudaMemcpyAsync(s->map.p, edges.map.data(), n * 4, cudaMemcpyHostToDevice, st));
-    }
-    CK(cudaMemcpyAsync(d_runs, runs.data(), runs.size() * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemsetAsync(d_slot, 0xFF, n_keys * P * 4, st));
-    if (rows_in) {
-      const unsigned grid = (unsigned)std::min<uint64_t>((rows_in + 255) / 256, (uint64_t)h->sms * 8);
-      series_match_kernel<<<grid, 256, 0, st>>>(v.arena, d_runs, d_runs + P, P, (uint32_t)rows_in, d_keys,
-                                                (uint32_t)n_keys, d_slot);
-      h->launches += 1;
-    }
-    const SeriesRows sr{v.arena, d_slot, by_source ? nullptr : static_cast<const uint32_t*>(s->map.p), P,
-                        static_cast<uint8_t*>(s->present.p)};
-    rc = run_metrics_series(h, sr, (uint32_t)slots, ms, static_cast<double*>(s->values.p));
-    if (rc != ALZ_OK) return rc;
+  CK(cudaMemcpyAsync(d_runs, runs.data(), runs.size() * 4, cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(d_slot, 0xFF, n_keys * P * 4, st));
+  if (rows_in) {
+    const unsigned grid = (unsigned)std::min<uint64_t>((rows_in + 255) / 256, (uint64_t)h->sms * 8);
+    series_match_kernel<<<grid, 256, 0, st>>>(v.arena, d_runs, d_runs + P, P, (uint32_t)rows_in, d_keys,
+                                              (uint32_t)n_keys, d_slot);
+    h->launches += 1;
   }
+  const SeriesRows sr{v.arena, d_slot, by_source ? nullptr : static_cast<const uint32_t*>(b.map.p), P,
+                      static_cast<uint8_t*>(b.present.p)};
+  return run_metrics_series(h, sr, (uint32_t)slots, ms, static_cast<double*>(b.values.p));
+}
+
+// The series of `edges` over the last min(k, retained) entries of tier `tier`. Device call: *dev_values /
+// *dev_present; host call: cap series rows into values / present (either may be null when nothing is copied).
+// Caller holds h->mu.
+int series_locked(alz_handle* h, Edges& edges, uint32_t tier, uint32_t k, const MetricSet& ms, bool device,
+                  double* values, uint8_t* present, size_t cap, const double** dev_values,
+                  const uint8_t** dev_present, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                  alz_series_info* info) {
+  CK(cudaSetDevice(h->device));
+  if (!h->series) h->series = new alz_series_state();
+  SeriesBufs& b = h->series->b;
+  uint64_t rows_in = 0;
+  const int rc = series_enqueue(h, b, edges, tier, k, ms, device ? SIZE_MAX : cap, device, n_out, n_points, &rows_in);
+  if (rc != ALZ_OK) return rc;
+  const size_t slots = *n_out * *n_points;
   if (info) {
     *info = alz_series_info{};
-    info->edges = n;
+    info->edges = *n_out;
     info->rows_in = rows_in;
-    info->points = P;
+    info->points = *n_points;
     info->tier = tier;
   }
   if (device) {
-    *dev_values = static_cast<const double*>(s->values.p);
-    if (dev_present) *dev_present = static_cast<const uint8_t*>(s->present.p);
+    if (points) alz_internal_ring_points(h, tier, k, points);   // the clocks arrived before the first launch
+    *dev_values = static_cast<const double*>(b.values.p);
+    if (dev_present) *dev_present = static_cast<const uint8_t*>(b.present.p);
     return ALZ_OK;
   }
-  if (slots && values) CK(cudaMemcpyAsync(values, s->values.p, slots * ms.nm * 8, cudaMemcpyDeviceToHost, st));
-  if (slots && present) CK(cudaMemcpyAsync(present, s->present.p, slots, cudaMemcpyDeviceToHost, st));
+  cudaStream_t st = h->stream;
+  if (slots && values) CK(cudaMemcpyAsync(values, b.values.p, slots * ms.nm * 8, cudaMemcpyDeviceToHost, st));
+  if (slots && present) CK(cudaMemcpyAsync(present, b.present.p, slots, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));   // the one wait of a host call: the results and the ring's clocks
   if (points) alz_internal_ring_points(h, tier, k, points);
   return ALZ_OK;
@@ -212,6 +222,16 @@ int series_entry(alz_handle* h, bool by_source, uint32_t source, const alz_edge_
 }
 
 }  // namespace
+
+int alz::metrics::run_series_rows(alz_handle* h, SeriesBufs& b, const alz_edge_out* rows, size_t n, uint32_t tier,
+                                  uint32_t k, const MetricSet& ms, size_t cap, size_t* n_out, uint32_t* n_points,
+                                  uint64_t* rows_in) {
+  Edges edges;
+  edges.by_source = true;
+  edges.rows = rows;
+  edges.n = n;
+  return series_enqueue(h, b, edges, tier, k, ms, cap, false, n_out, n_points, rows_in);
+}
 
 extern "C" int alz_edge_series(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
                                uint32_t nm, double* values, uint8_t* present, size_t cap, size_t* n_out,

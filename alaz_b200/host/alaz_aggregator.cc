@@ -566,6 +566,44 @@ int Aggregator::SeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint
   return ALZ_OK;
 }
 
+int Aggregator::Trends(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_trend& trend,
+                       uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+                       std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // a first call sizes the results (ALZ_E_CAPACITY with n = the results, P = the points; nothing written)
+  size_t n = 0;
+  uint32_t P = 0;
+  int rc = alz_edge_trends_top(h_, src, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr, nullptr,
+                               0, &n, &P, nullptr, nullptr);
+  std::vector<alz_rollup_info> pts(P);
+  if (rc == ALZ_E_CAPACITY && n > 0) {
+    trends_.resize(n);
+    trend_rows_.resize(n);
+    trend_values_.resize(n * P);
+    trend_present_.resize(n * P);
+    rc = alz_edge_trends_top(h_, src, tier, k, &metric, &trend, top, min_trend, trends_.data(), trend_rows_.data(),
+                             trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
+  }
+  if (rc != ALZ_OK) return rc;
+  const std::vector<EdgeWindow> names = ToEdges(trend_rows_.data(), n, nullptr);
+  out->assign(n, EdgeTrend{});
+  for (size_t i = 0; i < n; ++i) {
+    const alz_edge_trend& r = trends_[i];
+    EdgeTrend& e = (*out)[i];
+    e.FromType = names[i].FromType; e.FromUID = names[i].FromUID; e.ToType = names[i].ToType; e.ToUID = names[i].ToUID;
+    e.Valid = r.valid != 0;
+    e.Used = r.used;
+    e.Trend = r.trend; e.Recent = r.recent; e.Before = r.before;
+    e.Present.assign(trend_present_.begin() + i * P, trend_present_.begin() + (i + 1) * P);
+    e.Values.assign(trend_values_.begin() + i * P, trend_values_.begin() + (i + 1) * P);
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
 int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers) {
   if (!h_) return ALZ_E_STATE;
   std::lock_guard<std::mutex> g(mu_);

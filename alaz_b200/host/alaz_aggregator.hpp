@@ -82,6 +82,17 @@ struct EdgeSeries {
   std::vector<double> Values;     // [points * metrics]: metric j at point p is Values[p * metrics + j]
 };
 
+// one edge's trend (docs/SPEC.md §20) with the series it was computed from: per point, oldest first, whether that
+// entry holds the edge and the metric's value there (0 where it does not)
+struct EdgeTrend {
+  std::string FromType, FromUID, ToType, ToUID;
+  bool Valid = false;
+  uint32_t Used = 0;                  // points used
+  double Trend = 0.0, Recent = 0.0, Before = 0.0;
+  std::vector<uint8_t> Present;       // [points]
+  std::vector<double> Values;         // [points]
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -182,6 +193,14 @@ class Aggregator {
              std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points = nullptr);
   int SeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
                 std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points = nullptr);
+  // Edge trends (docs/SPEC.md §20): the `top` rows of `source` (kLastWindow or a rollup kind, as in Anomalies) with the
+  // largest valid trends >= min_trend of one metric over the last k entries of `tier`, largest first, ties in row
+  // order, each with its series, into *out; *points (may be null) as in Series. Rows are named by UID as Series names
+  // them, which SetHistory's hold makes correct over the whole retained history. top = 0: ALZ_E_INVAL. Returns 0 or an
+  // alz_status.
+  int Trends(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_trend& trend,
+             uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+             std::vector<alz_rollup_info>* points = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -254,6 +273,10 @@ class Aggregator {
   std::vector<alz_edge_change> changes_;   // records of the last Changes
   std::vector<double> series_values_;      // values and presence of the last Series / SeriesFor
   std::vector<uint8_t> series_present_;
+  std::vector<alz_edge_trend> trends_;     // records, rows, series and presence of the last Trends
+  std::vector<alz_edge_out> trend_rows_;
+  std::vector<double> trend_values_;
+  std::vector<uint8_t> trend_present_;
 };
 
 }  // namespace alaz

@@ -586,6 +586,78 @@ int alz_edge_series_keys_device(alz_handle* h, const alz_edge_ends* keys, size_t
                                 const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
                                 alz_rollup_info* points, alz_series_info* info);
 
+/* ---- edge trends (docs/SPEC.md §20) --------------------------------------------------------------------------------
+ * One statistic per row of a source (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability rule of §15) over that
+ * row's §19 series of one metric in the last P = min(k, retained) closed entries of one ring (tier 0: the window
+ * history; t >= 1: a tier), oldest first: the least-squares slope, or the recent points' mean against the earlier
+ * points' mean as a shift, a ratio or a z-score (SPEC §20 gives every rounding). The top calls rank the valid rows as
+ * alz_edge_top ranks values (64-bit key of the float64 trend, descending, then source row ascending; eligible when
+ * key(trend) >= key(min_trend)) and return the first min(top, above) with their source rows and their series.
+ * *n_out and *n_points (P) are always set; a host call whose cap is below *n_out returns ALZ_E_CAPACITY and writes
+ * nothing else. k < 2, recent outside [1, k - 1], an unknown stat, direction or absent mode, a bad metric (§17), an
+ * unknown source, top = 0, a NaN min_trend or a null required pointer: ALZ_E_INVAL. Tier 0 without the window history,
+ * t >= 1 without tiers, or no rows of a rollup source: ALZ_E_STATE. More than 2^30 - 1 slots (rows x P):
+ * ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. No retained entry: P = 0, every row invalid, ALZ_OK. points (room for k
+ * entries) and info may be NULL. Reads only: the window, the retained entries, the open blocks, every rollup's rows,
+ * the baseline, and the series, metric, top, change and GNN results are unchanged. Device results stay valid until the
+ * next trend call. Every rank holds the same history, so every rank gets the same result with no collective. */
+#define ALZ_TREND_SLOPE  0u   /* least-squares slope of y against the point index, in metric units per point */
+#define ALZ_TREND_SHIFT  1u   /* recent - before */
+#define ALZ_TREND_RATIO  2u   /* recent / before; before = 0: +inf when recent > 0, else 1.0 */
+#define ALZ_TREND_ZSCORE 3u   /* (recent - before) / the population standard deviation of the earlier points */
+#define ALZ_TREND_RISING  0u  /* the largest rises rank first */
+#define ALZ_TREND_FALLING 1u  /* the largest falls rank first: -slope, before - recent, before / recent */
+#define ALZ_TREND_ABSENT_SKIP 0u   /* a point where the entry does not hold the edge is left out */
+#define ALZ_TREND_ABSENT_ZERO 1u   /* ... counts as +0.0 (no traffic) */
+typedef struct alz_trend {   /* 24 B */
+  uint32_t stat;         /* ALZ_TREND_SLOPE / SHIFT / RATIO / ZSCORE */
+  uint32_t direction;    /* ALZ_TREND_RISING / FALLING */
+  uint32_t absent;       /* ALZ_TREND_ABSENT_SKIP / ABSENT_ZERO */
+  uint32_t recent;       /* r: the last r points are "recent"; 1 <= r <= k - 1 */
+  uint32_t min_points;   /* a valid row uses at least this many points (0: no extra bound) */
+  uint32_t _pad;
+} alz_trend;
+typedef struct alz_edge_trend {   /* 48 B; the head is laid out as alz_edge_ends / alz_edge_change */
+  uint8_t from_type;     /* ALZ_NODE_* */
+  uint8_t to_type;
+  uint8_t valid;         /* 1: the statistic is defined for this row */
+  uint8_t _pad[5];
+  uint32_t from;
+  uint32_t to;
+  uint32_t index;        /* row index in the source */
+  uint32_t used;         /* points used */
+  double trend;          /* +0.0 when not valid */
+  double recent;         /* mean of the used recent points */
+  double before;         /* mean of the used earlier points */
+} alz_edge_trend;
+typedef struct alz_trend_info {
+  uint64_t edges;        /* the source's rows */
+  uint64_t rows_in;      /* entry rows read: the sum of the P entries' rows */
+  uint64_t valid;        /* rows with a defined trend */
+  uint64_t above;        /* top calls: eligible rows before the cut; 0 otherwise */
+  uint32_t points;       /* P */
+  uint32_t tier;
+} alz_trend_info;
+/* every source row, in source order; cap counts records */
+int alz_edge_trends(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m, const alz_trend* t,
+                    alz_edge_trend* out, size_t cap, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                    alz_trend_info* info);
+int alz_edge_trends_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                           const alz_trend* t, const alz_edge_trend** dev_out, size_t* n_out, uint32_t* n_points,
+                           alz_rollup_info* points, alz_trend_info* info);
+/* the first min(top, above) valid rows by trend, in rank order: their records, their source rows, and their series
+ * (series[j * P + p], present[j * P + p], as alz_edge_series gives for the row with nm = 1). cap counts result rows;
+ * series and present need room for cap x k elements. out, rows, series and present may each be NULL (dev_rows,
+ * dev_series and dev_present too). */
+int alz_edge_trends_top(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                        const alz_trend* t, uint32_t top, double min_trend, alz_edge_trend* out, alz_edge_out* rows,
+                        double* series, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                        alz_rollup_info* points, alz_trend_info* info);
+int alz_edge_trends_top_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                               const alz_trend* t, uint32_t top, double min_trend, const alz_edge_trend** dev_out,
+                               const alz_edge_out** dev_rows, const double** dev_series, const uint8_t** dev_present,
+                               size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces
