@@ -220,6 +220,17 @@ class TrendInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+SIDE_IN, SIDE_OUT = 0, 1                                            # alz_node_metrics* / alz_node_top* sides
+
+NODE_SUMS = np.dtype([("count", "<u8"), ("err5xx", "<u8"), ("lat_sum_ns", "<u8"), ("hist", "<u4", (NB,))])
+assert NODE_SUMS.itemsize == 280
+NODE_OUT = np.dtype([
+    ("type", "u1"), ("_pad", "u1", (3,)), ("value", "<u4"), ("in_edges", "<u4"), ("out_edges", "<u4"),
+    ("in", NODE_SUMS), ("out", NODE_SUMS),
+])
+assert NODE_OUT.itemsize == 576
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

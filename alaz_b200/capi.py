@@ -32,7 +32,9 @@ EXPORTS = [
     "alz_edge_top_rollup", "alz_edge_top_rollup_device", "alz_baseline_pin", "alz_baseline_clear", "alz_edge_changes",
     "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device", "alz_edge_series",
     "alz_edge_series_device", "alz_edge_series_keys", "alz_edge_series_keys_device", "alz_edge_trends",
-    "alz_edge_trends_device", "alz_edge_trends_top", "alz_edge_trends_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_edge_trends_device", "alz_edge_trends_top", "alz_edge_trends_top_device", "alz_node_rows",
+    "alz_node_rows_device", "alz_node_metrics", "alz_node_metrics_device", "alz_node_top", "alz_node_top_device",
+    "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -130,6 +132,14 @@ def load(rebuild=False):
                                  C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
         "alz_edge_trends_top_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp, pp, pp, pp,
                                         C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_node_rows": ([vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_node_rows_device": ([vp, u32, pp, C.POINTER(sz)], i),
+        "alz_node_metrics": ([vp, u32, u32, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_node_metrics_device": ([vp, u32, u32, vp, u32, pp, C.POINTER(sz)], i),
+        "alz_node_top": ([vp, u32, u32, vp, u32, C.c_double, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)], i),
+        "alz_node_top_device": ([vp, u32, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
+                                 C.POINTER(abi.TopInfo)], i),
+        "alz_debug_node_rows": ([vp, vp, sz, vp, sz, C.POINTER(sz)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -172,7 +182,8 @@ def load(rebuild=False):
                   "alz_edge_changes", "alz_edge_changes_device", "alz_edge_changes_top", "alz_edge_changes_top_device",
                   "alz_debug_edge_changes_rows", "alz_edge_series", "alz_edge_series_device", "alz_edge_series_keys",
                   "alz_edge_series_keys_device", "alz_edge_trends", "alz_edge_trends_device", "alz_edge_trends_top",
-                  "alz_edge_trends_top_device"):
+                  "alz_edge_trends_top_device", "alz_node_rows", "alz_node_rows_device", "alz_node_metrics",
+                  "alz_node_metrics_device", "alz_node_top", "alz_node_top_device", "alz_debug_node_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -762,6 +773,71 @@ class Handle:
                                                    points, C.byref(info)), "alz_edge_trends_top_device")
         return (pr.value, pw.value, ps.value, pp_.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)],
                 info.as_dict())
+
+    # ---- node metrics (alz_nodes.cu, docs/SPEC.md §21)
+    def _node_rows(self, fn, args):
+        """fn(h, *args, out, cap, &n): NODE_OUT rows in node order; a first call with cap 0 gives the nodes."""
+        f, n = getattr(self.L, fn), C.c_size_t(0)
+        if self._ck(f(self.h, *args, None, 0, C.byref(n)), fn, allow=(abi.E_CAPACITY,)) == 0:
+            return np.zeros(0, dtype=abi.NODE_OUT)
+        out = np.zeros(n.value, dtype=abi.NODE_OUT)
+        self._ck(f(self.h, *args, _ptr(out), n.value, C.byref(n)), fn)
+        return out
+
+    def node_rows(self, source=abi.SOURCE_WINDOW):
+        """alz_node_rows: every node of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) as NODE_OUT rows, node order."""
+        return self._node_rows("alz_node_rows", (int(source),))
+
+    def node_rows_device(self, source=abi.SOURCE_WINDOW):
+        """alz_node_rows_device: (device pointer, nodes)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        self._ck(self.L.alz_node_rows_device(self.h, int(source), C.byref(p), C.byref(n)), "alz_node_rows_device")
+        return p.value, n.value
+
+    def node_metrics(self, source, side, *specs):
+        """alz_node_metrics: values [nodes x len(specs)] of side abi.SIDE_IN / SIDE_OUT; a spec is a METRIC_* kind or
+        a (kind, q) pair."""
+        return self._edge_metrics("alz_node_metrics", (int(source), int(side)), specs)
+
+    def node_metrics_device(self, source, side, *specs):
+        """alz_node_metrics_device: (device pointer, nodes)."""
+        return self._edge_metrics_device("alz_node_metrics_device", (int(source), int(side)), specs)
+
+    def node_top(self, source, side, spec, k, min_value=0.0):
+        """alz_node_top: the first min(k, above) nodes by one metric of one side: (NODE_OUT rows, values, node
+        indices, info dict), rank order. The first call offers room for min(k, 65536) results; when more came out,
+        it is repeated with room for all."""
+        f, n, info, m = self.L.alz_node_top, C.c_size_t(0), abi.TopInfo(), abi.metrics(spec)
+        cap = min(int(k), 1 << 16)
+        while True:
+            nodes = np.zeros(cap, dtype=abi.NODE_OUT)
+            values = np.zeros(cap, dtype=np.float64)
+            index = np.zeros(cap, dtype=np.uint32)
+            rc = self._ck(f(self.h, int(source), int(side), m, int(k), float(min_value), _ptr(nodes), _ptr(values),
+                            _ptr(index), cap, C.byref(n), C.byref(info)), "alz_node_top", allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                r = n.value
+                return nodes[:r].copy(), values[:r].copy(), index[:r].copy(), info.as_dict()
+            cap = n.value
+
+    def node_top_device(self, source, side, spec, k, min_value=0.0):
+        """alz_node_top_device: (nodes, values, index device pointers, results, info dict)."""
+        pn, pv, pi, n, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), abi.TopInfo()
+        self._ck(self.L.alz_node_top_device(self.h, int(source), int(side), abi.metrics(spec), int(k),
+                                            float(min_value), C.byref(pn), C.byref(pv), C.byref(pi), C.byref(n),
+                                            C.byref(info)), "alz_node_top_device")
+        return pn.value, pv.value, pi.value, n.value, info.as_dict()
+
+    def debug_node_rows(self, rows):
+        """alz_debug_node_rows over a host EDGE_OUT array (copied to the device): NODE_OUT rows in node order."""
+        rows = np.ascontiguousarray(rows, dtype=abi.EDGE_OUT)
+        p = self.dev_alloc(max(rows.nbytes, 1))
+        try:
+            if len(rows):
+                self.h2d(p, rows)
+            return self._node_rows("alz_debug_node_rows", (C.c_void_p(p), len(rows)))
+        finally:
+            self.dev_free(p)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

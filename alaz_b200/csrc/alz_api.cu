@@ -240,6 +240,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_changes(h);
   alz_internal_free_series(h);
   alz_internal_free_trends(h);
+  alz_internal_free_nodes(h);
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);

@@ -188,9 +188,10 @@ alz_changes_state* changes_state(alz_handle* h) {
   return h->changes;
 }
 
-// The rows of a source and its windows (ALZ_SOURCE_WINDOW: the last flushed window, 1), or of the last rollup of a
-// kind with what it reported. Caller holds h->mu.
-int source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n, alz_rollup_info* info) {
+}  // namespace
+
+int alz::metrics::source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n,
+                              alz_rollup_info* info) {
   if (source == ALZ_SOURCE_WINDOW) {
     *rows = h->d_out;
     *n = h->last_n_edges;
@@ -200,8 +201,6 @@ int source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_
   }
   return alz_internal_rollup_rows(h, source, rows, n, info);
 }
-
-}  // namespace
 
 void alz::metrics::launch_row_keys(alz_handle* h, const alz_edge_out* rows, uint32_t n, uint64_t* keys) {
   if (n == 0) return;

@@ -86,6 +86,10 @@ __host__ __device__ __forceinline__ void unpack_edge_key(uint64_t k, uint8_t* fr
   else      { *from_type = ot; *from = other; *to_type = ALZ_NODE_POD; *to = pod; }
 }
 
+// node key of an edge end (type, value), docs/SPEC.md §21: the GNN pass's node set (alz_gnn.cu) and the node calls'
+// group-by (alz_nodes.cu) both order nodes by it
+__device__ __forceinline__ uint64_t node_key(uint32_t kind, uint32_t value) { return ((uint64_t)kind << 32) | value; }
+
 // packed edge key of an output row (inverse of unpack_edge_key)
 __device__ __forceinline__ uint64_t row_key_of(const alz_edge_out* r) {
   // rows are 296 bytes apart: 8-byte aligned only

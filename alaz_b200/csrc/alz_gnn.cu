@@ -71,8 +71,6 @@ inline float tf32_round(float x) {
   return r;
 }
 
-__device__ __forceinline__ uint64_t node_key(uint32_t kind, uint32_t value) { return ((uint64_t)kind << 32) | value; }
-
 __global__ void edge_node_keys_kernel(const alz_edge_out* __restrict__ e, uint32_t n_e, uint64_t* __restrict__ out) {
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n_e; i += stride) {

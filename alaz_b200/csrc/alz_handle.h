@@ -36,6 +36,7 @@ struct alz_metrics_state; // alz_metrics.cu
 struct alz_changes_state; // alz_changes.cu
 struct alz_series_state;  // alz_series.cu
 struct alz_trend_state;   // alz_trends.cu
+struct alz_node_state;    // alz_nodes.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -132,6 +133,7 @@ struct alz_handle {
   alz_changes_state* changes = nullptr;   // the pinned baseline and the change list's buffers; null until the first
   alz_series_state* series = nullptr;     // the edge series' buffers (alz_edge_series*); null until the first
   alz_trend_state* trends = nullptr;      // the edge trends' buffers (alz_edge_trends*); null until the first
+  alz_node_state* nodes = nullptr;        // the node calls' buffers (alz_node_*); null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -182,4 +184,5 @@ void alz_internal_free_metrics(alz_handle* h);
 void alz_internal_free_changes(alz_handle* h);
 void alz_internal_free_series(alz_handle* h);
 void alz_internal_free_trends(alz_handle* h);
+void alz_internal_free_nodes(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

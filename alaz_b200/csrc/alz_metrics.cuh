@@ -62,6 +62,27 @@ struct SeriesRows {
 // The metrics of the n = rows x P series slots into out[n * ms.nm] and present[n], on the stream; no wait
 int run_metrics_series(alz_handle* h, const SeriesRows& rows, uint32_t n, const MetricSet& ms, double* out);
 
+// The rows of a node metric (alz_nodes.cu): output row i reads side `side` of node row i in place. A side's sums are
+// laid out as alz_edge_out from count on, so the row it reads starts sizeof(alz_node_sums) x side bytes into the node
+// row (alz_nodes.cu asserts the offsets this relies on).
+struct NodeRows {
+  static constexpr bool kMayBeAbsent = false;
+  const alz_node_out* nodes;
+  uint32_t side;
+#ifdef __CUDACC__
+  __device__ __forceinline__ const alz_edge_out* operator()(uint32_t i) const {
+    return reinterpret_cast<const alz_edge_out*>(reinterpret_cast<const char*>(nodes + i) +
+                                                 (size_t)side * sizeof(alz_node_sums));
+  }
+#endif
+};
+// The metrics of n node rows' one side into out[n * ms.nm], on the stream; no wait
+int run_metrics_nodes(alz_handle* h, const NodeRows& rows, uint32_t n, const MetricSet& ms, double* out);
+
+// The rows of a source and its windows (ALZ_SOURCE_WINDOW: the last flushed window, 1), or of the last rollup of a
+// kind with what it reported (alz_changes.cu). Caller holds h->mu.
+int source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n, alz_rollup_info* info);
+
 // The buffers one edge series fills (alz_series.cu), grown on demand: the series calls own one set, the trend calls
 // (alz_trends.cu) another, so neither clobbers the other's device results
 struct SeriesBufs {

@@ -289,19 +289,20 @@ int Aggregator::Flush(bool with_scores) {
   return ds_ ? ds_->PersistEdgeWindow(edges) : ALZ_OK;
 }
 
+std::string Aggregator::UidOf(uint8_t t, uint32_t v) const {
+  if (t == ALZ_NODE_POD) return v < pods_.names.size() ? pods_.names[v] : std::string("?");
+  if (t == ALZ_NODE_SVC) return v < svcs_.names.size() ? svcs_.names[v] : std::string("?");
+  if (t == ALZ_NODE_OUTBOUND_HOST) return v < host_names_.size() ? host_names_[v] : std::string("?");   // data.go:852
+  return FormatIPv4(v);   // outbound: the raw daddr string (data.go:862)
+}
+
 std::vector<EdgeWindow> Aggregator::ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const {
   std::vector<EdgeWindow> edges(n);
   for (size_t i = 0; i < n; ++i) {
     const alz_edge_out& o = rows[i];
     EdgeWindow& w = edges[i];
-    auto uid = [&](uint8_t t, uint32_t v) -> std::string {
-      if (t == ALZ_NODE_POD) return v < pods_.names.size() ? pods_.names[v] : std::string("?");
-      if (t == ALZ_NODE_SVC) return v < svcs_.names.size() ? svcs_.names[v] : std::string("?");
-      if (t == ALZ_NODE_OUTBOUND_HOST) return v < host_names_.size() ? host_names_[v] : std::string("?");   // data.go:852
-      return FormatIPv4(v);   // outbound: the raw daddr string (data.go:862)
-    };
-    w.FromType = NodeTypeName(o.from_type); w.FromUID = uid(o.from_type, o.from);
-    w.ToType = NodeTypeName(o.to_type);     w.ToUID = uid(o.to_type, o.to);
+    w.FromType = NodeTypeName(o.from_type); w.FromUID = UidOf(o.from_type, o.from);
+    w.ToType = NodeTypeName(o.to_type);     w.ToUID = UidOf(o.to_type, o.to);
     w.Count = o.count; w.Err5xx = o.err5xx; w.LatSumNs = o.lat_sum_ns;
     memcpy(w.Hist, o.hist, sizeof w.Hist);
     if (scores) w.Score = scores[i];
@@ -601,6 +602,71 @@ int Aggregator::Trends(uint32_t source, uint32_t tier, uint32_t k, const alz_met
     e.Values.assign(trend_values_.begin() + i * P, trend_values_.begin() + (i + 1) * P);
   }
   if (points) *points = pts;
+  return ALZ_OK;
+}
+
+std::vector<NodeWindow> Aggregator::ToNodes(const alz_node_out* rows, size_t n, const double* values,
+                                            size_t nm) const {
+  std::vector<NodeWindow> nodes(n);
+  for (size_t i = 0; i < n; ++i) {
+    const alz_node_out& o = rows[i];
+    NodeWindow& w = nodes[i];
+    w.Type = NodeTypeName(o.type);
+    w.UID = UidOf(o.type, o.value);
+    w.InEdges = o.in_edges;
+    w.OutEdges = o.out_edges;
+    w.In = o.in;
+    w.Out = o.out;
+    if (values) w.Values.assign(values + i * nm, values + (i + 1) * nm);
+  }
+  return nodes;
+}
+
+int Aggregator::Nodes(uint32_t source, uint32_t side, const std::vector<alz_metric>& metrics,
+                      std::vector<NodeWindow>* out) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const uint32_t nm = (uint32_t)metrics.size();
+  // the node count (ALZ_E_CAPACITY with n = the nodes; nothing written), then the rows and the values
+  size_t n = 0;
+  int rc = alz_node_rows(h_, src, nullptr, 0, &n);
+  if (rc == ALZ_E_CAPACITY) {
+    nodes_.resize(n);
+    rc = alz_node_rows(h_, src, nodes_.data(), n, &n);
+  }
+  if (rc != ALZ_OK) return rc;
+  node_values_.assign(n * nm, 0.0);
+  size_t nv = 0;
+  rc = alz_node_metrics(h_, src, side, metrics.data(), nm, node_values_.data(), n, &nv);
+  if (rc != ALZ_OK) return rc;
+  if (nv != n) return ALZ_E_STATE;
+  *out = ToNodes(nodes_.data(), n, node_values_.data(), nm);
+  return ALZ_OK;
+}
+
+int Aggregator::TopNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
+                         std::vector<NodeWindow>* out, alz_top_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into nodes_ / node_values_, grown once when the results do not fit (ALZ_E_CAPACITY with n = the results)
+  auto call = [&](size_t* n) {
+    return alz_node_top(h_, src, side, &metric, k, min_value, nodes_.data(), node_values_.data(), nullptr,
+                        nodes_.size(), n, info);
+  };
+  size_t n = 0;
+  node_values_.resize(nodes_.size());
+  int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > nodes_.size()) {
+    nodes_.resize(n);
+    node_values_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToNodes(nodes_.data(), n, node_values_.data(), 1);
   return ALZ_OK;
 }
 

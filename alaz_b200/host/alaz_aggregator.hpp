@@ -93,6 +93,16 @@ struct EdgeTrend {
   std::vector<double> Values;         // [points]
 };
 
+// one node of a source (docs/SPEC.md §21) by UID: Type "pod" | "service" | "outbound" as EdgeWindow names an end (an
+// outbound node's UID is its dotted quad or its Host header text), the rows into it (In) and out of it (Out) with their
+// sums, and metric values of one side
+struct NodeWindow {
+  std::string Type, UID;
+  uint32_t InEdges = 0, OutEdges = 0;
+  alz_node_sums In{}, Out{};
+  std::vector<double> Values;   // Nodes: the metrics in the caller's order; TopNodes: the ranking metric's value
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -201,6 +211,17 @@ class Aggregator {
   int Trends(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_trend& trend,
              uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
              std::vector<alz_rollup_info>* points = nullptr);
+  // Node metrics (docs/SPEC.md §21) of `source` (kLastWindow or a rollup kind, as in Anomalies): every node of its rows
+  // with both sides' sums and `metrics` of side `side` (ALZ_SIDE_IN: the requests a node served; ALZ_SIDE_OUT: the ones
+  // it made), in node order. Nodes are grouped and named by id; that is correct by UID over a rollup because
+  // SetHistory's hold never hands an id to another UID while a retained entry or an open block can carry it, so a pod
+  // deleted inside the rollup's span still shows under its own UID. Returns 0 or an alz_status.
+  int Nodes(uint32_t source, uint32_t side, const std::vector<alz_metric>& metrics, std::vector<NodeWindow>* out);
+  // the k nodes of `source` with the highest values of `metric` on side `side` >= min_value (fewer when fewer qualify),
+  // highest first, ties in node order, Values = {the value}: "the slowest / most failing services". Named as Nodes
+  // names them. info may be null. Returns 0 or an alz_status.
+  int TopNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
+               std::vector<NodeWindow>* out, alz_top_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -220,6 +241,10 @@ class Aggregator {
   int PersistRollup(uint32_t kind, bool with_scores, Call call);
   // rows -> EdgeWindow with the UIDs the interners hold (scores: one per row, or null)
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
+  // the UID of an edge end or node (type, id) as the interners and the Host table hold it
+  std::string UidOf(uint8_t type, uint32_t id) const;
+  // node rows -> NodeWindow (values: nm per row, or null)
+  std::vector<NodeWindow> ToNodes(const alz_node_out* rows, size_t n, const double* values, size_t nm) const;
   // ends -> the library's key of an edge named by UID; false when a UID has no id
   bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
   // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then *out (names from
@@ -277,6 +302,8 @@ class Aggregator {
   std::vector<alz_edge_out> trend_rows_;
   std::vector<double> trend_values_;
   std::vector<uint8_t> trend_present_;
+  std::vector<alz_node_out> nodes_;       // node rows, values and indices of the last Nodes / TopNodes
+  std::vector<double> node_values_;
 };
 
 }  // namespace alaz

@@ -658,6 +658,58 @@ int alz_edge_trends_top_device(alz_handle* h, uint32_t source, uint32_t tier, ui
                                const alz_edge_out** dev_rows, const double** dev_series, const uint8_t** dev_present,
                                size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
 
+/* ---- node metrics (docs/SPEC.md §21) -------------------------------------------------------------------------------
+ * A node is an edge end (type, value) as in §2: pod 7 and service 7 are different nodes, and so are outbound v and
+ * Host-keyed v. The nodes of a source (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability rule of §15) are every
+ * from end and every to end of its rows, in ascending node key (type << 32) | value, the key alz_gnn_nodes reports; a
+ * node's index is its position in that list. Side IN of a node sums the rows whose to end is the node, side OUT the
+ * rows whose from end is; a row whose two ends are one node counts on both. count, err5xx and lat_sum_ns are u64 sums
+ * mod 2^64, hist[b] the u32 sum of the rows' cells mod 2^32 (§3); in_edges / out_edges count each side's rows. A node
+ * metric is the §17 value of one side's sums, bit for bit what alz_edge_metrics* gives for an alz_edge_out that
+ * carries them. Top nodes rank as alz_edge_top ranks rows: 64-bit key of the float64 value, descending, then node
+ * index ascending; eligible when key(value) >= key(min_value); the first min(k, above) nodes.
+ * *n_out is always set; a host call whose cap (in nodes) is below it returns ALZ_E_CAPACITY and writes nothing. An
+ * unknown source, side or metric, nm of 0 or more than ALZ_MAX_METRICS, a q outside [0, 1] or NaN, k = 0, a NaN
+ * min_value or a null required pointer: ALZ_E_INVAL. No rows of a rollup source: ALZ_E_STATE. A 0-row source: 0 nodes,
+ * ALZ_OK. More than 2^29 - 1 source rows: ALZ_E_CAPACITY, before anything runs; no memory: ALZ_E_NOMEM.
+ * Reads only: the window, the retained entries, the open blocks, every rollup's rows and the baseline are unchanged, and
+ * so are the GNN, metric, top, change, series and trend results, device pointers included. Device results stay valid
+ * until the next node call on the handle. Every rank holds the same rows, so every rank gets the same result with no
+ * collective. */
+#define ALZ_SIDE_IN  0u   /* the rows into the node: requests it served, messages delivered to it */
+#define ALZ_SIDE_OUT 1u   /* the rows out of the node */
+typedef struct alz_node_sums {   /* 280 B: laid out as the tail of alz_edge_out from count on */
+  uint64_t count;
+  uint64_t err5xx;
+  uint64_t lat_sum_ns;
+  uint32_t hist[ALZ_NB];
+} alz_node_sums;
+typedef struct alz_node_out {    /* 576 B */
+  uint8_t type;          /* ALZ_NODE_* */
+  uint8_t _pad[3];
+  uint32_t value;
+  uint32_t in_edges;     /* rows on the IN side */
+  uint32_t out_edges;    /* rows on the OUT side */
+  alz_node_sums in;      /* in.count sits at offset 16, as alz_edge_out.count does */
+  alz_node_sums out;
+} alz_node_out;
+/* every node of a source, in node order; cap counts nodes */
+int alz_node_rows(alz_handle* h, uint32_t source, alz_node_out* out, size_t cap, size_t* n_out);
+int alz_node_rows_device(alz_handle* h, uint32_t source, const alz_node_out** dev_out, size_t* n_out);
+/* values[i * nm + j]: metric j of node i's side `side` (ALZ_SIDE_*), in node order; cap counts nodes */
+int alz_node_metrics(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t nm, double* values,
+                     size_t cap, size_t* n_out);
+int alz_node_metrics_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t nm,
+                            const double** dev_values, size_t* n_out);
+/* The first min(k, above) nodes by one metric of one side. Result j: the node's row, its value (bit for bit what
+ * alz_node_metrics* gives) and its node index; nodes, values, index and info may each be NULL (dev_nodes, dev_values and
+ * dev_index too). info->scored = the source's nodes, info->above = the eligible ones. */
+int alz_node_top(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t k, double min_value,
+                 alz_node_out* nodes, double* values, uint32_t* index, size_t cap, size_t* n_out, alz_top_info* info);
+int alz_node_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t k,
+                        double min_value, const alz_node_out** dev_nodes, const double** dev_values,
+                        const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

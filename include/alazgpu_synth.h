@@ -52,6 +52,11 @@ int alz_debug_edge_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size
                                 const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows,
                                 const alz_metric* m, uint32_t mode, uint32_t presence, alz_edge_change* out,
                                 size_t cap, size_t* n_out, alz_change_info* info);
+/* test/debug: the group-by of alz_node_rows (docs/SPEC.md §21) over n caller rows in device memory, which may hold
+ * layouts ingest cannot make (one node on 2^20 rows, cells of 2^32 - 1, any row order, repeated edges); the rules of
+ * alz_node_rows otherwise. Uses the node calls' buffers. */
+int alz_debug_node_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, alz_node_out* out, size_t cap,
+                        size_t* n_out);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
