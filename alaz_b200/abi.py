@@ -230,6 +230,17 @@ NODE_OUT = np.dtype([
 ])
 assert NODE_OUT.itemsize == 576
 
+NODE_ENDS = np.dtype([("type", "u1"), ("_pad", "u1", (3,)), ("value", "<u4")])   # the head of NODE_OUT
+assert NODE_ENDS.itemsize == 8 and NODE_ENDS.fields["value"][1] == NODE_OUT.fields["value"][1]
+NODE_TREND = np.dtype([
+    ("type", "u1"), ("_pad0", "u1"), ("valid", "u1"), ("_pad1", "u1", (5,)),
+    ("value", "<u4"), ("_pad2", "<u4"), ("index", "<u4"), ("used", "<u4"),
+    ("trend", "<f8"), ("recent", "<f8"), ("before", "<f8"),
+])
+assert NODE_TREND.itemsize == 48
+assert all(NODE_TREND.fields[f][1] == EDGE_TREND.fields[f][1]
+           for f in ("valid", "index", "used", "trend", "recent", "before"))   # laid out as EDGE_TREND from valid on
+
 
 class SpanInfo(C.Structure):
     """alz_span_info."""

@@ -34,6 +34,8 @@ EXPORTS = [
     "alz_edge_series_device", "alz_edge_series_keys", "alz_edge_series_keys_device", "alz_edge_trends",
     "alz_edge_trends_device", "alz_edge_trends_top", "alz_edge_trends_top_device", "alz_node_rows",
     "alz_node_rows_device", "alz_node_metrics", "alz_node_metrics_device", "alz_node_top", "alz_node_top_device",
+    "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
+    "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -140,6 +142,22 @@ def load(rebuild=False):
         "alz_node_top_device": ([vp, u32, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
                                  C.POINTER(abi.TopInfo)], i),
         "alz_debug_node_rows": ([vp, vp, sz, vp, sz, C.POINTER(sz)], i),
+        "alz_node_series": ([vp, u32, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                             C.POINTER(abi.SeriesInfo)], i),
+        "alz_node_series_device": ([vp, u32, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                    C.POINTER(abi.SeriesInfo)], i),
+        "alz_node_series_keys": ([vp, vp, sz, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                                  C.POINTER(abi.SeriesInfo)], i),
+        "alz_node_series_keys_device": ([vp, vp, sz, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32),
+                                         vp, C.POINTER(abi.SeriesInfo)], i),
+        "alz_node_trends": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), vp, sz, C.POINTER(sz), C.POINTER(u32),
+                             vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_node_trends_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), pp, C.POINTER(sz),
+                                    C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_node_trends_top": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, vp, vp, vp, vp,
+                                 sz, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_node_trends_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp, pp,
+                                        pp, pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -183,7 +201,9 @@ def load(rebuild=False):
                   "alz_debug_edge_changes_rows", "alz_edge_series", "alz_edge_series_device", "alz_edge_series_keys",
                   "alz_edge_series_keys_device", "alz_edge_trends", "alz_edge_trends_device", "alz_edge_trends_top",
                   "alz_edge_trends_top_device", "alz_node_rows", "alz_node_rows_device", "alz_node_metrics",
-                  "alz_node_metrics_device", "alz_node_top", "alz_node_top_device", "alz_debug_node_rows"):
+                  "alz_node_metrics_device", "alz_node_top", "alz_node_top_device", "alz_debug_node_rows",
+                  "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
+                  "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -716,63 +736,79 @@ class Handle:
         """An alz_trend."""
         return abi.Trend(int(stat), int(direction), int(absent), int(recent), int(min_points), 0)
 
-    def edge_trends(self, source, tier, k, spec, trend):
-        """alz_edge_trends: every row of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) over the last k entries of
-        `tier` by one metric (a METRIC_* kind or a (kind, q) pair) and an abi.Trend: (EDGE_TREND records in source
-        order, points as a list of alz_rollup_info dicts, info dict). A first call with cap 0 gives the rows."""
-        f, n, p, info, m = self.L.alz_edge_trends, C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
-        self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), None, 0, C.byref(n), C.byref(p), None,
-                   C.byref(info)), "alz_edge_trends", allow=(abi.E_CAPACITY,))
-        out = np.zeros(n.value, dtype=abi.EDGE_TREND)
+    def _trends(self, fn, head, k, spec, trend, dtype):
+        """fn(h, *head, k, m, &trend, out, cap, &n, &P, points, &info): (records in source order, points, info dict).
+        A first call with cap 0 gives the records."""
+        f, n, p, info, m = getattr(self.L, fn), C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
+        self._ck(f(self.h, *head, int(k), m, C.byref(trend), None, 0, C.byref(n), C.byref(p), None, C.byref(info)), fn,
+                 allow=(abi.E_CAPACITY,))
+        out = np.zeros(n.value, dtype=dtype)
         points = (abi.RollupInfo * max(int(k), 1))()
-        self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), _ptr(out), len(out), C.byref(n),
-                   C.byref(p), points, C.byref(info)), "alz_edge_trends")
+        self._ck(f(self.h, *head, int(k), m, C.byref(trend), _ptr(out), len(out), C.byref(n), C.byref(p), points,
+                   C.byref(info)), fn)
         return out, [points[j].as_dict() for j in range(p.value)], info.as_dict()
 
-    def edge_trends_device(self, source, tier, k, spec, trend):
-        """alz_edge_trends_device: (device pointer to the records, rows, P, points, info dict)."""
+    def _trends_device(self, fn, head, k, spec, trend):
         d, n, p, info = C.c_void_p(), C.c_size_t(0), C.c_uint32(0), abi.TrendInfo()
         points = (abi.RollupInfo * max(int(k), 1))()
-        self._ck(self.L.alz_edge_trends_device(self.h, int(source), int(tier), int(k), abi.metrics(spec),
-                                               C.byref(trend), C.byref(d), C.byref(n), C.byref(p), points,
-                                               C.byref(info)), "alz_edge_trends_device")
+        self._ck(getattr(self.L, fn)(self.h, *head, int(k), abi.metrics(spec), C.byref(trend), C.byref(d), C.byref(n),
+                                     C.byref(p), points, C.byref(info)), fn)
         return d.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)], info.as_dict()
 
-    def edge_trends_top(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
-        """alz_edge_trends_top: the first min(top, above) valid rows by trend, rank order: (records, source rows,
-        series [m, P] float64, present [m, P] uint8, points, info dict). The first call offers room for min(top, 4096) results; when more came out, it is repeated with room for all."""
-        f, n, p, info, m = self.L.alz_edge_trends_top, C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
+    def _trends_top(self, fn, head, k, spec, trend, top, min_trend, rec_dtype, row_dtype):
+        """fn(h, *head, k, m, &trend, top, min_trend, out, rows, series, present, cap, &n, &P, points, &info). The
+        first call offers room for min(top, 4096) results; when more came out, it is repeated with room for all."""
+        f, n, p, info, m = getattr(self.L, fn), C.c_size_t(0), C.c_uint32(0), abi.TrendInfo(), abi.metrics(spec)
         cap = min(int(top), 1 << 12)
         points = (abi.RollupInfo * max(int(k), 1))()
         while True:
-            out = np.zeros(cap, dtype=abi.EDGE_TREND)
-            rows = np.zeros(cap, dtype=abi.EDGE_OUT)
+            out = np.zeros(cap, dtype=rec_dtype)
+            rows = np.zeros(cap, dtype=row_dtype)
             series = np.zeros(cap * int(k))
             present = np.zeros(cap * int(k), dtype=np.uint8)
-            rc = self._ck(f(self.h, int(source), int(tier), int(k), m, C.byref(trend), int(top), float(min_trend),
-                            _ptr(out), _ptr(rows), _ptr(series), _ptr(present), cap, C.byref(n), C.byref(p), points,
-                            C.byref(info)), "alz_edge_trends_top", allow=(abi.E_CAPACITY,))
+            rc = self._ck(f(self.h, *head, int(k), m, C.byref(trend), int(top), float(min_trend), _ptr(out),
+                            _ptr(rows), _ptr(series), _ptr(present), cap, C.byref(n), C.byref(p), points,
+                            C.byref(info)), fn, allow=(abi.E_CAPACITY,))
             if rc == 0:
                 break
             if n.value <= cap:   # a capacity error that no buffer cures: too many slots
-                raise AlzError(rc, "alz_edge_trends_top")
+                raise AlzError(rc, fn)
             cap = n.value
         r, P = n.value, p.value
         return (out[:r].copy(), rows[:r].copy(), series[: r * P].reshape(r, P).copy(),
                 present[: r * P].reshape(r, P).copy(), [points[j].as_dict() for j in range(P)], info.as_dict())
 
-    def edge_trends_top_device(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
-        """alz_edge_trends_top_device: (records, rows, series and present device pointers, results, P, points, info
-        dict)."""
+    def _trends_top_device(self, fn, head, k, spec, trend, top, min_trend):
         pr, pw, ps, pp_ = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
         n, p, info = C.c_size_t(0), C.c_uint32(0), abi.TrendInfo()
         points = (abi.RollupInfo * max(int(k), 1))()
-        self._ck(self.L.alz_edge_trends_top_device(self.h, int(source), int(tier), int(k), abi.metrics(spec),
-                                                   C.byref(trend), int(top), float(min_trend), C.byref(pr),
-                                                   C.byref(pw), C.byref(ps), C.byref(pp_), C.byref(n), C.byref(p),
-                                                   points, C.byref(info)), "alz_edge_trends_top_device")
+        self._ck(getattr(self.L, fn)(self.h, *head, int(k), abi.metrics(spec), C.byref(trend), int(top),
+                                     float(min_trend), C.byref(pr), C.byref(pw), C.byref(ps), C.byref(pp_), C.byref(n),
+                                     C.byref(p), points, C.byref(info)), fn)
         return (pr.value, pw.value, ps.value, pp_.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)],
                 info.as_dict())
+
+    def edge_trends(self, source, tier, k, spec, trend):
+        """alz_edge_trends: every row of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) over the last k entries of
+        `tier` by one metric (a METRIC_* kind or a (kind, q) pair) and an abi.Trend: (EDGE_TREND records in source
+        order, points as a list of alz_rollup_info dicts, info dict). A first call with cap 0 gives the rows."""
+        return self._trends("alz_edge_trends", (int(source), int(tier)), k, spec, trend, abi.EDGE_TREND)
+
+    def edge_trends_device(self, source, tier, k, spec, trend):
+        """alz_edge_trends_device: (device pointer to the records, rows, P, points, info dict)."""
+        return self._trends_device("alz_edge_trends_device", (int(source), int(tier)), k, spec, trend)
+
+    def edge_trends_top(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_edge_trends_top: the first min(top, above) valid rows by trend, rank order: (records, source rows,
+        series [m, P] float64, present [m, P] uint8, points, info dict). The first call offers room for min(top, 4096) results; when more came out, it is repeated with room for all."""
+        return self._trends_top("alz_edge_trends_top", (int(source), int(tier)), k, spec, trend, top, min_trend,
+                                abi.EDGE_TREND, abi.EDGE_OUT)
+
+    def edge_trends_top_device(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_edge_trends_top_device: (records, rows, series and present device pointers, results, P, points, info
+        dict)."""
+        return self._trends_top_device("alz_edge_trends_top_device", (int(source), int(tier)), k, spec, trend, top,
+                                       min_trend)
 
     # ---- node metrics (alz_nodes.cu, docs/SPEC.md §21)
     def _node_rows(self, fn, args):
@@ -838,6 +874,61 @@ class Handle:
             return self._node_rows("alz_debug_node_rows", (C.c_void_p(p), len(rows)))
         finally:
             self.dev_free(p)
+
+    # ---- node series and trends (alz_node_series.cu, alz_trends.cu, docs/SPEC.md §22)
+    @staticmethod
+    def node_ends(nodes):
+        """A NODE_ENDS array from a NODE_ENDS or NODE_OUT array (its type and value), or (type, value) tuples."""
+        out = np.zeros(len(nodes), dtype=abi.NODE_ENDS)
+        if isinstance(nodes, np.ndarray) and nodes.dtype.names:
+            out["type"], out["value"] = nodes["type"], nodes["value"]
+            return out
+        for i, (t, v) in enumerate(nodes):
+            out[i] = (t, (0,) * 3, v)
+        return out
+
+    def node_series(self, source, side, tier, k, *specs):
+        """alz_node_series: every node of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*), side abi.SIDE_IN / SIDE_OUT,
+        over the last k entries of `tier` (0: the window history): (values [nodes, P, nm], present [nodes, P], points,
+        info dict)."""
+        return self._series("alz_node_series", (int(source), int(side)), (int(tier), int(k)), specs)
+
+    def node_series_device(self, source, side, tier, k, *specs):
+        """alz_node_series_device: (values and present device pointers, nodes, P, points, info dict)."""
+        return self._series_device("alz_node_series_device", (int(source), int(side)), (int(tier), int(k)), specs)
+
+    def node_series_keys(self, nodes, side, tier, k, *specs):
+        """alz_node_series_keys: the caller's nodes (see node_ends), in their order: (values [n, P, nm], present
+        [n, P], points, info dict)."""
+        keys = np.ascontiguousarray(self.node_ends(nodes))
+        return self._series("alz_node_series_keys", (_ptr(keys), len(keys), int(side)), (int(tier), int(k)), specs)
+
+    def node_series_keys_device(self, nodes, side, tier, k, *specs):
+        """alz_node_series_keys_device: (values and present device pointers, n, P, points, info dict)."""
+        keys = np.ascontiguousarray(self.node_ends(nodes))
+        return self._series_device("alz_node_series_keys_device", (_ptr(keys), len(keys), int(side)),
+                                   (int(tier), int(k)), specs)
+
+    def node_trends(self, source, side, tier, k, spec, trend):
+        """alz_node_trends: every node of `source`, side `side`, over the last k entries of `tier` by one metric and an
+        abi.Trend: (NODE_TREND records in node order, points, info dict)."""
+        return self._trends("alz_node_trends", (int(source), int(side), int(tier)), k, spec, trend, abi.NODE_TREND)
+
+    def node_trends_device(self, source, side, tier, k, spec, trend):
+        """alz_node_trends_device: (device pointer to the records, nodes, P, points, info dict)."""
+        return self._trends_device("alz_node_trends_device", (int(source), int(side), int(tier)), k, spec, trend)
+
+    def node_trends_top(self, source, side, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_node_trends_top: the first min(top, above) valid nodes by trend, rank order: (records, NODE_OUT rows,
+        series [m, P] float64, present [m, P] uint8, points, info dict)."""
+        return self._trends_top("alz_node_trends_top", (int(source), int(side), int(tier)), k, spec, trend, top,
+                                min_trend, abi.NODE_TREND, abi.NODE_OUT)
+
+    def node_trends_top_device(self, source, side, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_node_trends_top_device: (records, node rows, series and present device pointers, results, P, points,
+        info dict)."""
+        return self._trends_top_device("alz_node_trends_top_device", (int(source), int(side), int(tier)), k, spec,
+                                       trend, top, min_trend)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

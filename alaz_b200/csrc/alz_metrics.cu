@@ -231,6 +231,10 @@ int run_metrics_nodes(alz_handle* h, const NodeRows& rows, uint32_t n, const Met
   return launch_metrics(h, rows, n, ms, out);
 }
 
+int run_metrics_node_series(alz_handle* h, const NodeSeriesRows& rows, uint32_t n, const MetricSet& ms, double* out) {
+  return launch_metrics(h, rows, n, ms, out);
+}
+
 int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,
                const alz_edge_out* rows, size_t* m_out, uint64_t* above) {
   *m_out = 0;

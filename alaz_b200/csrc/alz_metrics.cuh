@@ -1,7 +1,8 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
-// (alz_series.cu) and the edge trends (alz_trends.cu): the §17 metric values of a row list or of series slots, the
-// rows' packed keys, the grow-on-demand device buffers, a source's series into given buffers and the 64-bit top
-// selection with its own scratch.
+// (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu) and the node series
+// (alz_node_series.cu): the §17 metric values of a row list, of node rows or of series slots, the rows' packed keys,
+// the grow-on-demand device buffers, the node group-by, a source's edge or node series into given buffers and the
+// 64-bit top selection with its own scratch.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -79,6 +80,54 @@ struct NodeRows {
 // The metrics of n node rows' one side into out[n * ms.nm], on the stream; no wait
 int run_metrics_nodes(alz_handle* h, const NodeRows& rows, uint32_t n, const MetricSet& ms, double* out);
 
+// The rows of a node series (alz_node_series.cu): output row i = (series row i / P, point i % P) reads side `side` of
+// the node row slot[u * P + point], u = map[series row] (map null: u = the series row), or nothing when that slot is
+// kSlotAbsent; present[i] says which.
+struct NodeSeriesRows {
+  static constexpr bool kMayBeAbsent = true;
+  const alz_node_out* nodes;
+  const uint32_t* slot;
+  const uint32_t* map;
+  uint32_t points, side;
+  uint8_t* present;
+#ifdef __CUDACC__
+  __device__ __forceinline__ const alz_edge_out* operator()(uint32_t i) const {
+    const uint32_t e = i / points, j = i - e * points;
+    const uint32_t s = slot[(map ? map[e] : e) * points + j];
+    return s == kSlotAbsent ? nullptr : NodeRows{nodes, side}(s);
+  }
+  __device__ __forceinline__ void mark(uint32_t i, bool p) const { present[i] = p ? 1u : 0u; }
+#endif
+};
+// The metrics of the n = rows x P node series slots into out[n * ms.nm] and present[n], on the stream; no wait
+int run_metrics_node_series(alz_handle* h, const NodeSeriesRows& rows, uint32_t n, const MetricSet& ms, double* out);
+
+// The node group-by of alz_nodes.cu over (key, 2 x row + side) pairs, in buffers its caller owns, so the node calls
+// and the node series each keep their own
+struct NodeGroup {
+  DevBuf keys_in, keys_out, vals_in, vals_out, heads, idx, tmp;
+  uint32_t* h_words = nullptr;   // pinned: [0] the runs of the last node_group_runs, [1] free for the caller
+  void free();
+};
+// node calls read sources of at most this many rows: their 2n pairs stay within the selection's 2^30 - 1
+constexpr uint32_t kMaxNodeSourceRows = (1u << 29) - 1u;
+// the node key's bits: a uint8 type above a 32-bit value
+constexpr int kNodeKeyBits = 40;
+// Room for n2 pairs in g.keys_in / g.vals_in and the scratch of node_group_runs. ALZ_E_NOMEM when one cannot grow.
+int node_group_reserve(alz_handle* h, NodeGroup& g, uint32_t n2);
+// The 2n pairs of n rows into g.keys_in / g.vals_in, on the stream: pair 2i + side is row i's end on `side` (§21)
+void node_group_keys(alz_handle* h, NodeGroup& g, const alz_edge_out* rows, uint32_t n);
+// g's n2 pairs sorted on the keys' low key_bits bits (g.keys_out / g.vals_out), the run heads (g.heads) and run
+// numbers (g.idx, an exclusive scan of the heads), then one wait; g.h_words[0] = the runs after it
+int node_group_runs(alz_handle* h, NodeGroup& g, uint32_t n2, int key_bits);
+// One node row per run of the first n2 sorted pairs into out[g.idx[run head]], on the stream; a pair's row is
+// rows + (val >> 1) and its side val & 1. A row's head word is its run's key as (key >> 32, key).
+int node_group_reduce(alz_handle* h, const NodeGroup& g, const alz_edge_out* rows, uint32_t n2, alz_node_out* out);
+// out[j] = nodes[idx[j]] for j < m, on the stream
+int node_gather(alz_handle* h, const uint32_t* idx, uint32_t m, const alz_node_out* nodes, alz_node_out* out);
+// The rows of `source`, checked against kMaxNodeSourceRows (ALZ_E_CAPACITY). Caller holds h->mu.
+int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n);
+
 // The rows of a source and its windows (ALZ_SOURCE_WINDOW: the last flushed window, 1), or of the last rollup of a
 // kind with what it reported (alz_changes.cu). Caller holds h->mu.
 int source_rows(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n, alz_rollup_info* info);
@@ -96,6 +145,27 @@ struct SeriesBufs {
 // ALZ_E_CAPACITY for more than 2^30 - 1 slots or n > cap. Caller holds h->mu and has set the device.
 int run_series_rows(alz_handle* h, SeriesBufs& b, const alz_edge_out* rows, size_t n, uint32_t tier, uint32_t k,
                     const MetricSet& ms, size_t cap, size_t* n_out, uint32_t* n_points, uint64_t* rows_in);
+
+// The buffers one node series fills (alz_node_series.cu), grown on demand: the node series calls own one set, the
+// node trend calls (alz_trends.cu) another
+struct NodeSeriesBufs {
+  NodeGroup g;                           // the group-by of the source's nodes, then of the entries' (node, point) slots
+  DevBuf keys, map, runs, slot, miss;    // the distinct node keys, caller row -> distinct key, the entries' runs,
+                                         // the slots' node rows, the entry rows that name no queried node
+  DevBuf slot_rows, src_rows;            // one node row per present slot; the source's node rows (with_rows)
+  DevBuf values, present;                // the results
+  alz_ring_view view;
+  void free();
+};
+// The node series of side `side` of the nodes of the n source rows `rows` over the last min(k, retained) entries of
+// tier `tier` into b.values / b.present, on the stream: *n_out = the source's nodes (their keys in b.keys), *n_points =
+// P, *rows_in = the entries' rows. with_rows: the source's node rows too, in b.src_rows. Waits once for the node count
+// and the ring's clocks (when the source has rows) and once for the present slots (when the entries have rows).
+// ALZ_E_CAPACITY for more than 2^30 - 1 slots or nodes > cap. Caller holds h->mu and has set the device;
+// n <= kMaxNodeSourceRows.
+int run_node_series_rows(alz_handle* h, NodeSeriesBufs& b, const alz_edge_out* rows, size_t n, uint32_t side,
+                         uint32_t tier, uint32_t k, const MetricSet& ms, bool with_rows, size_t cap, size_t* n_out,
+                         uint32_t* n_points, uint64_t* rows_in);
 
 // The scratch and the results of one top selection over 64-bit values, grown on demand
 struct Selection {

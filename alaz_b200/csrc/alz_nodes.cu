@@ -11,6 +11,8 @@
 //           tile is stored plainly, with the node's type, value and edge counts. A run that crosses a tile boundary
 //           (a hub) was zeroed and headed by the split kernel, and each of its tiles adds its part with red.add. The
 //           arithmetic is integer, mod 2^64 and mod 2^32, so every order of the adds gives the same bytes.
+//   The sort, heads and scan (node_group_runs) and the split and reduce (node_group_reduce) work on a NodeGroup their
+//   caller owns: the node series (alz_node_series.cu) run them a second time over (node, point) pairs.
 //   metrics the §17 kernels through NodeRows, which reads one side of a node row in place as an alz_edge_out
 //   top     the §17 selection over those values, then one gather of the selected node rows
 #include <algorithm>
@@ -40,10 +42,8 @@ static_assert(offsetof(alz_node_sums, err5xx) - offsetof(alz_node_sums, count) =
 
 namespace {
 
-constexpr uint32_t kMaxSourceRows = (1u << 29) - 1u;   // 2n contributions stay within the selection's 2^30 - 1
 constexpr uint32_t kTile = 32;                         // pairs per lane group; a longer run is split across groups
 constexpr uint32_t kGroups = 256 / 8;                  // lane groups per block
-constexpr int kKeyBits = 40;
 constexpr uint32_t kRowWords = sizeof(alz_node_out) / 8;
 
 // the row's fields at byte offset 8 x w (8-byte aligned: rows are 296 bytes apart)
@@ -205,19 +205,23 @@ __global__ void __launch_bounds__(256) node_gather_kernel(const uint32_t* __rest
 
 // Buffers of the node calls, each grown on demand and never shrunk; freed in alz_destroy
 struct alz_node_state {
-  DevBuf keys_in, keys_out, vals_in, vals_out, heads, idx, tmp;   // the group-by's scratch
-  DevBuf rows, values, top_rows;                                  // the results: node rows, metric values, top rows
-  Selection sel;                                                  // the top call's selection
-  uint32_t* h_count = nullptr;                                    // pinned: the node count
+  NodeGroup g;                      // the group-by's scratch
+  DevBuf rows, values, top_rows;    // the results: node rows, metric values, top rows
+  Selection sel;                    // the top call's selection
 };
+
+void alz::metrics::NodeGroup::free() {
+  free_bufs({&keys_in, &keys_out, &vals_in, &vals_out, &heads, &idx, &tmp});
+  if (h_words) cudaFreeHost(h_words);
+  h_words = nullptr;
+}
 
 void alz_internal_free_nodes(alz_handle* h) {
   alz_node_state* s = h->nodes;
   if (!s) return;
-  free_bufs({&s->keys_in, &s->keys_out, &s->vals_in, &s->vals_out, &s->heads, &s->idx, &s->tmp, &s->rows, &s->values,
-             &s->top_rows});
+  s->g.free();
+  free_bufs({&s->rows, &s->values, &s->top_rows});
   s->sel.free();
-  if (s->h_count) cudaFreeHost(s->h_count);
   delete s;
   h->nodes = nullptr;
 }
@@ -228,70 +232,110 @@ unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
   return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
 }
 
-// The node rows of n rows into s->rows, on the stream after one wait for the node count; *n_nodes = that count. More
-// nodes than cap: ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device;
-// n <= kMaxSourceRows.
-int group_nodes(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_nodes) {
-  *n_nodes = 0;
-  if (!h->nodes) h->nodes = new alz_node_state();
-  alz_node_state* s = h->nodes;
-  if (!s->h_count) {
+}  // namespace
+
+namespace alz {
+namespace metrics {
+
+int node_group_reserve(alz_handle* h, NodeGroup& g, uint32_t n2) {
+  if (!g.h_words) {
     void* p = nullptr;
-    if (cudaMallocHost(&p, sizeof(uint32_t)) != cudaSuccess) {
+    if (cudaMallocHost(&p, 2 * sizeof(uint32_t)) != cudaSuccess) {
       h->last_err = std::string("node metrics: ") + cudaGetErrorString(cudaGetLastError());
       return ALZ_E_NOMEM;
     }
-    s->h_count = static_cast<uint32_t*>(p);
+    g.h_words = static_cast<uint32_t*>(p);
   }
-  const uint32_t n2 = 2u * (uint32_t)n;
-  if (n == 0) return reserve(h, {{&s->rows, sizeof(alz_node_out)}});
-  int rc = reserve(h, {{&s->keys_in, (size_t)n2 * 8},
-                       {&s->keys_out, (size_t)n2 * 8},
-                       {&s->vals_in, (size_t)n2 * 4},
-                       {&s->vals_out, (size_t)n2 * 4},
-                       {&s->heads, ((size_t)n2 + 1) * 4},
-                       {&s->idx, ((size_t)n2 + 1) * 4},
-                       {&s->tmp, std::max(sort_pairs_temp_bytes(n2), scan_temp_bytes(n2 + 1))}});
-  if (rc != ALZ_OK) return rc;
+  return reserve(h, {{&g.keys_in, (size_t)n2 * 8},
+                     {&g.keys_out, (size_t)n2 * 8},
+                     {&g.vals_in, (size_t)n2 * 4},
+                     {&g.vals_out, (size_t)n2 * 4},
+                     {&g.heads, ((size_t)n2 + 1) * 4},
+                     {&g.idx, ((size_t)n2 + 1) * 4},
+                     {&g.tmp, std::max(sort_pairs_temp_bytes(n2), scan_temp_bytes(n2 + 1))}});
+}
+
+void node_group_keys(alz_handle* h, NodeGroup& g, const alz_edge_out* rows, uint32_t n) {
+  node_keys_kernel<<<grid_for(h, n, 8), 256, 0, h->stream>>>(rows, n, static_cast<uint64_t*>(g.keys_in.p),
+                                                             static_cast<uint32_t*>(g.vals_in.p));
+  h->launches += 1;
+}
+
+int node_group_runs(alz_handle* h, NodeGroup& g, uint32_t n2, int key_bits) {
   cudaStream_t st = h->stream;
-  uint64_t* keys = static_cast<uint64_t*>(s->keys_out.p);
-  uint32_t* vals = static_cast<uint32_t*>(s->vals_out.p);
-  uint32_t* heads = static_cast<uint32_t*>(s->heads.p);
-  uint32_t* idx = static_cast<uint32_t*>(s->idx.p);
-  node_keys_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(rows, (uint32_t)n, static_cast<uint64_t*>(s->keys_in.p),
-                                                      static_cast<uint32_t*>(s->vals_in.p));
+  uint64_t* keys = static_cast<uint64_t*>(g.keys_out.p);
+  uint32_t* heads = static_cast<uint32_t*>(g.heads.p);
+  uint32_t* idx = static_cast<uint32_t*>(g.idx.p);
   CK(cudaGetLastError());
-  CK(sort_pairs(s->tmp.p, s->tmp.bytes, static_cast<const uint64_t*>(s->keys_in.p), keys,
-                static_cast<const uint32_t*>(s->vals_in.p), vals, n2, st, kKeyBits));
+  CK(sort_pairs(g.tmp.p, g.tmp.bytes, static_cast<const uint64_t*>(g.keys_in.p), keys,
+                static_cast<const uint32_t*>(g.vals_in.p), static_cast<uint32_t*>(g.vals_out.p), n2, st, key_bits));
   node_heads_kernel<<<grid_for(h, n2, 8), 256, 0, st>>>(keys, n2, heads);
   CK(cudaGetLastError());
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, heads, idx, n2 + 1, st));
-  CK(cudaMemcpyAsync(s->h_count, idx + n2, 4, cudaMemcpyDeviceToHost, st));
-  h->launches += 4;
-  CK(cudaStreamSynchronize(st));   // the one wait: the node count
-  const size_t nodes = *s->h_count;
-  *n_nodes = nodes;
-  if (nodes > cap) return ALZ_E_CAPACITY;
-  rc = reserve(h, {{&s->rows, nodes * sizeof(alz_node_out)}});
-  if (rc != ALZ_OK) return rc;
-  alz_node_out* out = static_cast<alz_node_out*>(s->rows.p);
+  CK(exclusive_scan_u32(g.tmp.p, g.tmp.bytes, heads, idx, n2 + 1, st));
+  CK(cudaMemcpyAsync(g.h_words, idx + n2, 4, cudaMemcpyDeviceToHost, st));
+  h->launches += 3;
+  CK(cudaStreamSynchronize(st));   // the one wait: the run count
+  return ALZ_OK;
+}
+
+int node_group_reduce(alz_handle* h, const NodeGroup& g, const alz_edge_out* rows, uint32_t n2, alz_node_out* out) {
+  if (n2 == 0) return ALZ_OK;
+  cudaStream_t st = h->stream;
+  const uint64_t* keys = static_cast<const uint64_t*>(g.keys_out.p);
+  const uint32_t* idx = static_cast<const uint32_t*>(g.idx.p);
   if (n2 > kTile) {
     node_split_kernel<<<grid_for(h, (uint64_t)((n2 - 1) / kTile) * 32, 8), 256, 0, st>>>(keys, idx, n2, out);
     h->launches += 1;
   }
   const uint64_t tiles = (n2 + kTile - 1) / kTile;
-  node_reduce_kernel<<<grid_for(h, tiles * 8, 8), 256, 0, st>>>(rows, keys, vals, idx, n2, out);
+  node_reduce_kernel<<<grid_for(h, tiles * 8, 8), 256, 0, st>>>(rows, keys, static_cast<const uint32_t*>(g.vals_out.p),
+                                                                idx, n2, out);
   h->launches += 1;
   CK(cudaGetLastError());
   return ALZ_OK;
 }
 
-// The rows of `source`, checked against the node calls' row limit. Caller holds h->mu.
+int node_gather(alz_handle* h, const uint32_t* idx, uint32_t m, const alz_node_out* nodes, alz_node_out* out) {
+  if (m == 0) return ALZ_OK;
+  node_gather_kernel<<<grid_for(h, (uint64_t)m * (sizeof(alz_node_out) / 16), 4), 256, 0, h->stream>>>(idx, m, nodes,
+                                                                                                      out);
+  h->launches += 1;
+  CK(cudaGetLastError());
+  return ALZ_OK;
+}
+
 int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n) {
   alz_rollup_info ri;
   const int rc = source_rows(h, source, rows, n, &ri);
   if (rc != ALZ_OK) return rc;
-  return *n > kMaxSourceRows ? ALZ_E_CAPACITY : ALZ_OK;
+  return *n > kMaxNodeSourceRows ? ALZ_E_CAPACITY : ALZ_OK;
+}
+
+}  // namespace metrics
+}  // namespace alz
+
+namespace {
+
+// The node rows of n rows into s->rows, on the stream after one wait for the node count; *n_nodes = that count. More
+// nodes than cap: ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device;
+// n <= kMaxNodeSourceRows.
+int group_nodes(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_nodes) {
+  *n_nodes = 0;
+  if (!h->nodes) h->nodes = new alz_node_state();
+  alz_node_state* s = h->nodes;
+  const uint32_t n2 = 2u * (uint32_t)n;
+  if (n == 0) return reserve(h, {{&s->rows, sizeof(alz_node_out)}});
+  int rc = node_group_reserve(h, s->g, n2);
+  if (rc != ALZ_OK) return rc;
+  node_group_keys(h, s->g, rows, (uint32_t)n);
+  rc = node_group_runs(h, s->g, n2, kNodeKeyBits);
+  if (rc != ALZ_OK) return rc;
+  const size_t nodes = s->g.h_words[0];
+  *n_nodes = nodes;
+  if (nodes > cap) return ALZ_E_CAPACITY;
+  rc = reserve(h, {{&s->rows, nodes * sizeof(alz_node_out)}});
+  if (rc != ALZ_OK) return rc;
+  return node_group_reduce(h, s->g, rows, n2, static_cast<alz_node_out*>(s->rows.p));
 }
 
 bool valid_source(uint32_t source) { return source == ALZ_SOURCE_WINDOW || source <= ALZ_ROLLUP_SPAN; }
@@ -307,7 +351,7 @@ int rows_entry(alz_handle* h, bool hook, uint32_t source, const alz_edge_out* de
   CK(cudaSetDevice(h->device));
   const alz_edge_out* rows = dev_rows;
   size_t n = n_rows;
-  int rc = hook ? (n > kMaxSourceRows ? ALZ_E_CAPACITY : ALZ_OK) : node_source(h, source, &rows, &n);
+  int rc = hook ? (n > kMaxNodeSourceRows ? ALZ_E_CAPACITY : ALZ_OK) : node_source(h, source, &rows, &n);
   if (rc != ALZ_OK) return rc;
   rc = group_nodes(h, rows, n, dev ? SIZE_MAX : cap, n_out);
   if (rc != ALZ_OK) return rc;
@@ -387,13 +431,9 @@ int top_entry(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m
   rc = reserve(h, {{&s->top_rows, std::max<size_t>(mm, 1) * sizeof(alz_node_out)}});
   if (rc != ALZ_OK) return rc;
   cudaStream_t st = h->stream;
-  if (mm) {
-    node_gather_kernel<<<grid_for(h, mm * (sizeof(alz_node_out) / 16), 4), 256, 0, st>>>(
-        static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)mm, node_rows,
-        static_cast<alz_node_out*>(s->top_rows.p));
-    h->launches += 1;
-    CK(cudaGetLastError());
-  }
+  rc = node_gather(h, static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)mm, node_rows,
+                   static_cast<alz_node_out*>(s->top_rows.p));
+  if (rc != ALZ_OK) return rc;
   *n_out = mm;
   if (info) { info->scored = nodes; info->above = above; }
   const alz_node_out* top_rows = static_cast<const alz_node_out*>(s->top_rows.p);

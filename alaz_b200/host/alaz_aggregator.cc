@@ -452,32 +452,33 @@ int Aggregator::Changes(uint32_t source, const alz_metric& metric, uint32_t mode
   return ALZ_OK;
 }
 
-bool Aggregator::ToEnds(const EdgeRef& e, alz_edge_ends* out) const {
-  auto end = [&](const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) {
-    if (type == "pod" || type == "service") {
-      const Interner& in = type == "pod" ? pods_ : svcs_;
-      const auto it = in.ids.find(uid);
-      if (it == in.ids.end()) return false;
-      *t = type == "pod" ? ALZ_NODE_POD : ALZ_NODE_SVC;
-      *v = it->second;
-      return true;
-    }
-    if (type != "outbound") return false;
-    bool ok = false;
-    const uint32_t ip = ParseIPv4(uid, &ok);
-    if (ok) { *t = ALZ_NODE_OUTBOUND; *v = ip; return true; }
-    const auto it = host_ids_.find(uid);   // a destination keyed by its Host header (data.go:851-854)
-    if (it == host_ids_.end()) return false;
-    *t = ALZ_NODE_OUTBOUND_HOST;
+bool Aggregator::EndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const {
+  if (type == "pod" || type == "service") {
+    const Interner& in = type == "pod" ? pods_ : svcs_;
+    const auto it = in.ids.find(uid);
+    if (it == in.ids.end()) return false;
+    *t = type == "pod" ? ALZ_NODE_POD : ALZ_NODE_SVC;
     *v = it->second;
     return true;
-  };
-  *out = alz_edge_ends{};
-  return end(e.FromType, e.FromUID, &out->from_type, &out->from) && end(e.ToType, e.ToUID, &out->to_type, &out->to);
+  }
+  if (type != "outbound") return false;
+  bool ok = false;
+  const uint32_t ip = ParseIPv4(uid, &ok);
+  if (ok) { *t = ALZ_NODE_OUTBOUND; *v = ip; return true; }
+  const auto it = host_ids_.find(uid);   // a destination keyed by its Host header (data.go:851-854)
+  if (it == host_ids_.end()) return false;
+  *t = ALZ_NODE_OUTBOUND_HOST;
+  *v = it->second;
+  return true;
 }
 
-template <class Call>
-int Aggregator::RunSeries(size_t nm, std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points, Call call) {
+bool Aggregator::ToEnds(const EdgeRef& e, alz_edge_ends* out) const {
+  *out = alz_edge_ends{};
+  return EndOf(e.FromType, e.FromUID, &out->from_type, &out->from) && EndOf(e.ToType, e.ToUID, &out->to_type, &out->to);
+}
+
+template <class Row, class Call>
+int Aggregator::RunSeries(size_t nm, std::vector<Row>* out, std::vector<alz_rollup_info>* points, Call call) {
   size_t n = 0;
   uint32_t P = 0;
   int rc = call(nullptr, nullptr, 0, &n, &P, nullptr);   // the sizes, then the values
@@ -487,7 +488,7 @@ int Aggregator::RunSeries(size_t nm, std::vector<EdgeSeries>* out, std::vector<a
   std::vector<alz_rollup_info> pts(P);
   rc = call(series_values_.data(), series_present_.data(), n, &n, &P, pts.data());
   if (rc != ALZ_OK) return rc;
-  out->assign(n, EdgeSeries{});
+  out->assign(n, Row{});
   for (size_t i = 0; i < n; ++i) {
     (*out)[i].Present.assign(series_present_.begin() + i * P, series_present_.begin() + (i + 1) * P);
     (*out)[i].Values.assign(series_values_.begin() + i * P * nm, series_values_.begin() + (i + 1) * P * nm);
@@ -667,6 +668,109 @@ int Aggregator::TopNodes(uint32_t source, uint32_t side, const alz_metric& metri
   }
   if (rc != ALZ_OK) return rc;
   *out = ToNodes(nodes_.data(), n, node_values_.data(), 1);
+  return ALZ_OK;
+}
+
+int Aggregator::NodeSeries(uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                           const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                           std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const uint32_t nm = (uint32_t)metrics.size();
+  int rc = RunSeries(nm, out, points, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                          alz_rollup_info* pts) {
+    return alz_node_series(h_, src, side, tier, k, metrics.data(), nm, v, p, cap, n, P, pts, nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  // the names: the source's node rows, in the same node order
+  const size_t n = out->size();
+  if (n == 0) return ALZ_OK;
+  nodes_.resize(n);
+  size_t m = 0;
+  rc = alz_node_rows(h_, src, nodes_.data(), n, &m);
+  if (rc != ALZ_OK) return rc;
+  if (m != n) return ALZ_E_STATE;
+  for (size_t i = 0; i < n; ++i) {
+    (*out)[i].Type = NodeTypeName(nodes_[i].type);
+    (*out)[i].UID = UidOf(nodes_[i].type, nodes_[i].value);
+  }
+  return ALZ_OK;
+}
+
+int Aggregator::NodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
+                              const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                              std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  // the nodes with ids go to the library; the others are absent at every point
+  std::vector<alz_node_ends> keys;
+  std::vector<size_t> row_of;   // node -> row of keys, or SIZE_MAX
+  for (const NodeRef& r : nodes) {
+    alz_node_ends k_{};
+    if (EndOf(r.Type, r.UID, &k_.type, &k_.value)) { row_of.push_back(keys.size()); keys.push_back(k_); }
+    else row_of.push_back(SIZE_MAX);
+  }
+  const uint32_t nm = (uint32_t)metrics.size();
+  std::vector<NodeSeriesRow> known;
+  std::vector<alz_rollup_info> pts;
+  const int rc = RunSeries(nm, &known, &pts, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                                 alz_rollup_info* pp) {
+    return alz_node_series_keys(h_, keys.data(), keys.size(), side, tier, k, metrics.data(), nm, v, p, cap, n, P, pp,
+                                nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  const size_t P = pts.size();
+  out->assign(nodes.size(), NodeSeriesRow{});
+  for (size_t i = 0; i < nodes.size(); ++i) {
+    NodeSeriesRow& e = (*out)[i];
+    if (row_of[i] != SIZE_MAX) e = known[row_of[i]];
+    else { e.Present.assign(P, 0); e.Values.assign(P * nm, 0.0); }
+    e.Type = nodes[i].Type;
+    e.UID = nodes[i].UID;
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::NodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                           const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
+                           std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // a first call sizes the results (ALZ_E_CAPACITY with n = the results, P = the points; nothing written)
+  size_t n = 0;
+  uint32_t P = 0;
+  int rc = alz_node_trends_top(h_, src, side, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr,
+                               nullptr, 0, &n, &P, nullptr, nullptr);
+  std::vector<alz_rollup_info> pts(P);
+  if (rc == ALZ_E_CAPACITY && n > 0) {
+    node_trends_.resize(n);
+    node_trend_rows_.resize(n);
+    trend_values_.resize(n * P);
+    trend_present_.resize(n * P);
+    rc = alz_node_trends_top(h_, src, side, tier, k, &metric, &trend, top, min_trend, node_trends_.data(),
+                             node_trend_rows_.data(), trend_values_.data(), trend_present_.data(), n, &n, &P,
+                             pts.data(), nullptr);
+  }
+  if (rc != ALZ_OK) return rc;
+  const std::vector<NodeWindow> names = ToNodes(node_trend_rows_.data(), n, nullptr, 0);
+  out->assign(n, NodeTrend{});
+  for (size_t i = 0; i < n; ++i) {
+    const alz_node_trend& r = node_trends_[i];
+    NodeTrend& e = (*out)[i];
+    e.Node = names[i];
+    e.Valid = r.valid != 0;
+    e.Used = r.used;
+    e.Trend = r.trend; e.Recent = r.recent; e.Before = r.before;
+    e.Present.assign(trend_present_.begin() + i * P, trend_present_.begin() + (i + 1) * P);
+    e.Values.assign(trend_values_.begin() + i * P, trend_values_.begin() + (i + 1) * P);
+  }
+  if (points) *points = pts;
   return ALZ_OK;
 }
 

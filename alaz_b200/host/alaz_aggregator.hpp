@@ -103,6 +103,30 @@ struct NodeWindow {
   std::vector<double> Values;   // Nodes: the metrics in the caller's order; TopNodes: the ranking metric's value
 };
 
+// a node named by UID, as NodeWindow names it: Type "pod" | "service" | "outbound"; an outbound node's UID is its
+// dotted quad or its Host header text
+struct NodeRef {
+  std::string Type, UID;
+};
+
+// one node's series (docs/SPEC.md §22): per point, oldest first, whether that entry holds a row on the side of the
+// node and the metrics' values of the side's sums there (every value 0 where it does not)
+struct NodeSeriesRow {
+  std::string Type, UID;
+  std::vector<uint8_t> Present;   // [points]
+  std::vector<double> Values;     // [points * metrics]: metric j at point p is Values[p * metrics + j]
+};
+
+// one node's trend (docs/SPEC.md §22) with the series it was computed from, and the node's row in the source
+struct NodeTrend {
+  NodeWindow Node;                    // Type, UID, edge counts and both sides' sums in the source (Values empty)
+  bool Valid = false;
+  uint32_t Used = 0;                  // points used
+  double Trend = 0.0, Recent = 0.0, Before = 0.0;
+  std::vector<uint8_t> Present;       // [points]
+  std::vector<double> Values;         // [points]
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -222,6 +246,23 @@ class Aggregator {
   // names them. info may be null. Returns 0 or an alz_status.
   int TopNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
                std::vector<NodeWindow>* out, alz_top_info* info = nullptr);
+  // Node series (docs/SPEC.md §22) of side `side` over the last k entries of `tier` (0: flushed windows, 1..n: the
+  // tiers), oldest first; *points (may be null) as in Series. NodeSeries gives one series per node of `source`
+  // (kLastWindow or a rollup kind, as in Anomalies), in node order, named as Nodes names them. NodeSeriesFor gives one
+  // per node named by UID, in the caller's order; a node whose UID has no id (never seen, or freed) is absent at every
+  // point. Both group rows by id, which SetHistory's hold makes correct by UID over the whole retained history: a
+  // deleted pod's points show under its UID up to its deletion and under no other UID. Returns 0 or an alz_status.
+  int NodeSeries(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                 std::vector<NodeSeriesRow>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int NodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
+                    const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                    std::vector<alz_rollup_info>* points = nullptr);
+  // Node trends (docs/SPEC.md §22): the `top` nodes of `source` with the largest valid trends >= min_trend of one
+  // metric of side `side` over the last k entries of `tier`, largest first, ties in node order, each with its node row
+  // and its series, into *out; named as Nodes names them. top = 0: ALZ_E_INVAL. Returns 0 or an alz_status.
+  int NodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                 const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
+                 std::vector<alz_rollup_info>* points = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -245,12 +286,14 @@ class Aggregator {
   std::string UidOf(uint8_t type, uint32_t id) const;
   // node rows -> NodeWindow (values: nm per row, or null)
   std::vector<NodeWindow> ToNodes(const alz_node_out* rows, size_t n, const double* values, size_t nm) const;
+  // the library's (type, id) of an edge end or node named by UID; false when the UID has no id
+  bool EndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const;
   // ends -> the library's key of an edge named by UID; false when a UID has no id
   bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
-  // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then *out (names from
-  // `names`, one per series row); requires mu_
-  template <class Call>
-  int RunSeries(size_t nm, std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points, Call call);
+  // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then each series
+  // row's Present and Values in *out (EdgeSeries or NodeSeriesRow; the names are the caller's); requires mu_
+  template <class Row, class Call>
+  int RunSeries(size_t nm, std::vector<Row>* out, std::vector<alz_rollup_info>* points, Call call);
   // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by
   // window w, and by every retained entry and open block that covers w: it is recycled once `hold` more windows
   // have been flushed after w (hold 0: when w is flushed).
@@ -296,7 +339,7 @@ class Aggregator {
   std::vector<double> values_;       // values of the last TopEdges
   std::vector<alz_alive_conn> alive_;
   std::vector<alz_edge_change> changes_;   // records of the last Changes
-  std::vector<double> series_values_;      // values and presence of the last Series / SeriesFor
+  std::vector<double> series_values_;      // values and presence of the last Series / SeriesFor / NodeSeries*
   std::vector<uint8_t> series_present_;
   std::vector<alz_edge_trend> trends_;     // records, rows, series and presence of the last Trends
   std::vector<alz_edge_out> trend_rows_;
@@ -304,6 +347,8 @@ class Aggregator {
   std::vector<uint8_t> trend_present_;
   std::vector<alz_node_out> nodes_;       // node rows, values and indices of the last Nodes / TopNodes
   std::vector<double> node_values_;
+  std::vector<alz_node_trend> node_trends_;   // records, node rows, series and presence of the last NodeTrends
+  std::vector<alz_node_out> node_trend_rows_;
 };
 
 }  // namespace alaz

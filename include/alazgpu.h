@@ -710,6 +710,81 @@ int alz_node_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz
                         double min_value, const alz_node_out** dev_nodes, const double** dev_values,
                         const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
 
+/* ---- node series and trends (docs/SPEC.md §22) ---------------------------------------------------------------------
+ * The §17 metric values of one side (ALZ_SIDE_*) of a set of nodes in each of the last P = min(k, retained) closed
+ * entries of one ring, oldest first: the window history (tier 0) or tier t >= 1. Series row i is node i of a source
+ * (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability rule of §15, in §21 node order) or the caller's keys[i].
+ * Point j of node i is present when entry j holds a row on the side (IN: a row whose to end is the node, OUT: whose
+ * from end is); values[(i * P + j) * nm + m] is then metric m of the side's §21 sums over entry j's rows, bit for bit
+ * what alz_node_metrics* gives for the node over a source that held entry j alone. An absent point has present 0 and
+ * every value +0.0. points[j] is what a rollup of entry j alone reports (room for P <= k entries). *n_out (series rows)
+ * and *n_points (P) are always set; a host call whose cap (in series rows) is below *n_out returns ALZ_E_CAPACITY and
+ * writes nothing else. k = 0, an unknown side or source, a tier above the configured ones, a bad metric list (§17), a
+ * malformed key or a null required pointer: ALZ_E_INVAL. Tier 0 without the window history, t >= 1 without tiers, or
+ * no rows of a rollup source: ALZ_E_STATE. A source of more than 2^29 - 1 rows (before anything runs) or more than
+ * 2^30 - 1 slots (series rows x P, before the entries are read): ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. No retained
+ * entry: P = 0, ALZ_OK. present, points and info (info->edges counts series rows, here nodes) may be NULL.
+ * Reads only: the window, the retained entries, the open blocks, every rollup's rows, the baseline, and the node, edge
+ * series, edge trend, metric, top, change and GNN results are unchanged. Device results stay valid until the next call
+ * of the same family (node series, node trends). Every rank holds the same history, so every rank gets the same result
+ * with no collective. */
+typedef struct alz_node_ends {   /* 8 B: the head of alz_node_out; _pad is ignored */
+  uint8_t type;                  /* ALZ_NODE_* */
+  uint8_t _pad[3];
+  uint32_t value;
+} alz_node_ends;
+/* every node of a source; cap counts series rows */
+int alz_node_series(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric* m,
+                    uint32_t nm, double* values, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                    alz_rollup_info* points, alz_series_info* info);
+int alz_node_series_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                           const alz_metric* m, uint32_t nm, const double** dev_values, const uint8_t** dev_present,
+                           size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+/* the caller's nodes, keys in host memory, in the caller's order; duplicates get identical rows. A type above
+ * ALZ_NODE_OUTBOUND_HOST or a pod or service value >= 2^29 is malformed; a node no entry holds is absent everywhere. */
+int alz_node_series_keys(alz_handle* h, const alz_node_ends* keys, size_t n_keys, uint32_t side, uint32_t tier,
+                         uint32_t k, const alz_metric* m, uint32_t nm, double* values, uint8_t* present, size_t cap,
+                         size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+int alz_node_series_keys_device(alz_handle* h, const alz_node_ends* keys, size_t n_keys, uint32_t side, uint32_t tier,
+                                uint32_t k, const alz_metric* m, uint32_t nm, const double** dev_values,
+                                const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                alz_rollup_info* points, alz_series_info* info);
+/* Node trends: the §20 statistic of each source node's series of one metric of one side, with §20's directions,
+ * absent modes, validity rules and roundings; k < 2 and everything alz_edge_trends* refuses is refused the same way.
+ * The records are one per source node, in node order; the top calls rank the valid nodes in the §17 order of the trend
+ * (then node index ascending) and return the first min(top, above) with the source's alz_node_out rows (as
+ * alz_node_rows gives them) and their P-point series (series[j * P + p], present[j * P + p]; room for cap x k each).
+ * info->edges counts the source's nodes. */
+typedef struct alz_node_trend {  /* 48 B; from `valid` on, laid out as alz_edge_trend */
+  uint8_t type;                  /* ALZ_NODE_* */
+  uint8_t _pad0;
+  uint8_t valid;                 /* 1: the statistic is defined for this node */
+  uint8_t _pad1[5];
+  uint32_t value;
+  uint32_t _pad2;
+  uint32_t index;                /* node index in the source (§21 node order) */
+  uint32_t used;                 /* points used */
+  double trend;                  /* +0.0 when not valid */
+  double recent;                 /* mean of the used recent points */
+  double before;                 /* mean of the used earlier points */
+} alz_node_trend;
+int alz_node_trends(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric* m,
+                    const alz_trend* t, alz_node_trend* out, size_t cap, size_t* n_out, uint32_t* n_points,
+                    alz_rollup_info* points, alz_trend_info* info);
+int alz_node_trends_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                           const alz_metric* m, const alz_trend* t, const alz_node_trend** dev_out, size_t* n_out,
+                           uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+/* out, nodes, series and present may each be NULL (dev_nodes, dev_series and dev_present too) */
+int alz_node_trends_top(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric* m,
+                        const alz_trend* t, uint32_t top, double min_trend, alz_node_trend* out, alz_node_out* nodes,
+                        double* series, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                        alz_rollup_info* points, alz_trend_info* info);
+int alz_node_trends_top_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                               const alz_metric* m, const alz_trend* t, uint32_t top, double min_trend,
+                               const alz_node_trend** dev_out, const alz_node_out** dev_nodes,
+                               const double** dev_series, const uint8_t** dev_present, size_t* n_out,
+                               uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces
