@@ -240,6 +240,14 @@ NODE_TREND = np.dtype([
 assert NODE_TREND.itemsize == 48
 assert all(NODE_TREND.fields[f][1] == EDGE_TREND.fields[f][1]
            for f in ("valid", "index", "used", "trend", "recent", "before"))   # laid out as EDGE_TREND from valid on
+NODE_CHANGE = np.dtype([
+    ("type", "u1"), ("_pad0", "u1"), ("presence", "u1"), ("_pad1", "u1", (5,)),
+    ("node", "<u4"), ("_pad2", "<u4"), ("index", "<u4"), ("base_index", "<u4"),
+    ("value", "<f8"), ("base_value", "<f8"), ("change", "<f8"),
+])
+assert NODE_CHANGE.itemsize == 48
+assert all(NODE_CHANGE.fields[f][1] == EDGE_CHANGE.fields[f][1]
+           for f in ("presence", "index", "base_index", "value", "base_value", "change"))   # EDGE_CHANGE's offsets
 
 
 class SpanInfo(C.Structure):

@@ -36,6 +36,7 @@ EXPORTS = [
     "alz_node_rows_device", "alz_node_metrics", "alz_node_metrics_device", "alz_node_top", "alz_node_top_device",
     "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
     "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device",
+    "alz_node_changes", "alz_node_changes_device", "alz_node_changes_top", "alz_node_changes_top_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -158,6 +159,14 @@ def load(rebuild=False):
                                  sz, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
         "alz_node_trends_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp, pp,
                                         pp, pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_node_changes": ([vp, u32, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_node_changes_device": ([vp, u32, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_node_changes_top": ([vp, u32, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
+                                  C.POINTER(abi.ChangeInfo)], i),
+        "alz_node_changes_top_device": ([vp, u32, u32, vp, u32, u32, u32, C.c_double, pp, C.POINTER(sz),
+                                         C.POINTER(abi.ChangeInfo)], i),
+        "alz_debug_node_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
+                                         C.POINTER(abi.ChangeInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -203,7 +212,9 @@ def load(rebuild=False):
                   "alz_edge_trends_top_device", "alz_node_rows", "alz_node_rows_device", "alz_node_metrics",
                   "alz_node_metrics_device", "alz_node_top", "alz_node_top_device", "alz_debug_node_rows",
                   "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
-                  "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device"):
+                  "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device",
+                  "alz_node_changes", "alz_node_changes_device", "alz_node_changes_top",
+                  "alz_node_changes_top_device", "alz_debug_node_changes_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -606,13 +617,13 @@ class Handle:
     def baseline_clear(self):
         self._ck(self.L.alz_baseline_clear(self.h), "alz_baseline_clear")
 
-    def _changes(self, fn, args):
-        """fn(h, *args, out, cap, &n, &info): (alz_edge_change records, info dict); a first call with cap 0 sizes the
-        buffer (ALZ_E_CAPACITY when there are records)."""
+    def _changes(self, fn, args, dtype=abi.EDGE_CHANGE):
+        """fn(h, *args, out, cap, &n, &info): (alz_edge_change or alz_node_change records, info dict); a first call with
+        cap 0 sizes the buffer (ALZ_E_CAPACITY when there are records)."""
         f, n, info = getattr(self.L, fn), C.c_size_t(0), abi.ChangeInfo()
         cap = 0
         while True:
-            out = np.zeros(cap, dtype=abi.EDGE_CHANGE)
+            out = np.zeros(cap, dtype=dtype)
             rc = self._ck(f(self.h, *args, _ptr(out) if cap else None, cap, C.byref(n), C.byref(info)), fn,
                           allow=(abi.E_CAPACITY,))
             if rc == 0:
@@ -929,6 +940,58 @@ class Handle:
         info dict)."""
         return self._trends_top_device("alz_node_trends_top_device", (int(source), int(side), int(tier)), k, spec,
                                        trend, top, min_trend)
+
+    # ---- node changes against the pinned baseline (alz_node_changes.cu, docs/SPEC.md §23)
+    def node_changes(self, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
+        """alz_node_changes of side `side` (abi.SIDE_*) of the nodes of `source` against the pinned baseline by one
+        metric: (NODE_CHANGE records in ascending node key order, info dict)."""
+        return self._changes("alz_node_changes", (int(source), int(side), abi.metrics(spec), int(mode), int(presence)),
+                             abi.NODE_CHANGE)
+
+    def node_changes_device(self, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                            source=abi.SOURCE_WINDOW):
+        """alz_node_changes_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_node_changes_device(self.h, int(source), int(side), abi.metrics(spec), int(mode),
+                                                int(presence), C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_node_changes_device")
+        return p.value, n.value, info.as_dict()
+
+    def node_changes_top(self, side, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                         source=abi.SOURCE_WINDOW):
+        """alz_node_changes_top: (the first min(k, above) NODE_CHANGE records by change, rank order; info dict)."""
+        return self._changes("alz_node_changes_top", (int(source), int(side), abi.metrics(spec), int(mode),
+                                                      int(presence), int(k), float(min_change)), abi.NODE_CHANGE)
+
+    def node_changes_top_device(self, side, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                source=abi.SOURCE_WINDOW):
+        """alz_node_changes_top_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_node_changes_top_device(self.h, int(source), int(side), abi.metrics(spec), int(mode),
+                                                    int(presence), int(k), float(min_change), C.byref(p), C.byref(n),
+                                                    C.byref(info)), "alz_node_changes_top_device")
+        return p.value, n.value, info.as_dict()
+
+    def debug_node_changes_rows(self, src, base, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                src_windows=1, base_windows=1):
+        """alz_debug_node_changes_rows over two host row arrays (copied to the device, any order, repeats allowed):
+        (NODE_CHANGE records, info dict)."""
+        src = np.ascontiguousarray(src, dtype=abi.EDGE_OUT)
+        base = np.ascontiguousarray(base, dtype=abi.EDGE_OUT)
+        ps = self.dev_alloc(max(src.nbytes, 1))
+        pb = self.dev_alloc(max(base.nbytes, 1))
+        try:
+            if len(src):
+                self.h2d(ps, src)
+            if len(base):
+                self.h2d(pb, base)
+            return self._changes("alz_debug_node_changes_rows",
+                                 (C.c_void_p(ps), len(src), int(src_windows), C.c_void_p(pb), len(base),
+                                  int(base_windows), int(side), abi.metrics(spec), int(mode), int(presence)),
+                                 abi.NODE_CHANGE)
+        finally:
+            self.dev_free(ps)
+            self.dev_free(pb)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -12,7 +12,8 @@
 //   values  the §17 metric kernel over each side's rows
 //   emit    one 48-byte record per listed row, and for the top call its change into an 8-byte array, which the §17
 //           selection ranks; the selected records are gathered by position
-// One host wait per call reads the union's counts; the top call's selection adds its own (alz_top.cu).
+// One host wait per call reads the union's counts; the top call's selection adds its own (alz_top.cu). The node
+// changes (alz_node_changes.cu) read the baseline through pinned_baseline and share change_of and the gather.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -71,18 +72,6 @@ __global__ void __launch_bounds__(256) change_match_kernel(const uint64_t* __res
   if (t0 == 0) { keep_a[n_a] = 0u; keep_b[n_b] = 0u; }
 }
 
-// the side's value: COUNT and ERR5XX per window (one rounding), the others as they are
-__device__ __forceinline__ double per_window(double v, bool divide, double windows) {
-  return divide ? __ddiv_rn(v, windows) : v;
-}
-
-__device__ __forceinline__ double change_of(uint32_t mode, double cur, double base) {
-  if (mode == ALZ_CHANGE_DELTA) return __dsub_rn(cur, base);
-  if (mode == ALZ_CHANGE_DROP) return __dsub_rn(base, cur);
-  if (base > 0.0) return __ddiv_rn(cur, base);   // ALZ_CHANGE_RATIO
-  return cur > 0.0 ? __longlong_as_double(0x7FF0000000000000ll) : 1.0;
-}
-
 struct EmitArgs {
   const alz_edge_out* rows_a;
   const alz_edge_out* rows_b;
@@ -136,10 +125,13 @@ __global__ void __launch_bounds__(256) change_emit_kernel(const __grid_constant_
   }
 }
 
-// result j = the record at the j-th selected position
+// result j = the record at the j-th selected position (Record: alz_edge_change, or alz_node_change of
+// alz_node_changes.cu)
+template <class Record>
 __global__ void __launch_bounds__(256) change_gather_kernel(const uint32_t* __restrict__ idx, uint32_t m,
-                                                            const alz_edge_change* __restrict__ list,
-                                                            alz_edge_change* __restrict__ out) {
+                                                            const Record* __restrict__ list,
+                                                            Record* __restrict__ out) {
+  static_assert(sizeof(Record) == 48, "three 16-byte words");
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < 3u * m; t += stride) {   // three 16-byte words each
     const uint32_t j = t / 3u, w = t % 3u;
@@ -163,6 +155,7 @@ struct alz_changes_state {
   DevBuf base_rows, base_keys;   // the baseline: its rows and their packed keys
   size_t base_n = 0;
   bool pinned = false;
+  uint64_t generation = 0;       // pins so far: tells the node changes' cached baseline nodes from a later pin's
   alz_rollup_info base_info{};
   DevBuf keys_a, keys_b;         // the sides' keys when derived
   DevBuf lb_a, lb_b, keep_a, keep_b, scan_a, scan_b, val_a, val_b, both, tmp;   // the join's scratch
@@ -207,6 +200,31 @@ void alz::metrics::launch_row_keys(alz_handle* h, const alz_edge_out* rows, uint
   change_keys_kernel<<<std::min<unsigned>((n + 255) / 256, (unsigned)h->sms * 8), 256, 0, h->stream>>>(rows, n, keys);
   h->launches += 1;
 }
+
+int alz::metrics::pinned_baseline(alz_handle* h, const alz_edge_out** rows, size_t* n, alz_rollup_info* info,
+                                  uint64_t* generation) {
+  const alz_changes_state* s = h->changes;
+  if (!s || !s->pinned) return ALZ_E_STATE;
+  *rows = static_cast<const alz_edge_out*>(s->base_rows.p);
+  *n = s->base_n;
+  *info = s->base_info;
+  *generation = s->generation;
+  return ALZ_OK;
+}
+
+template <class Record>
+int alz::metrics::gather_changes(alz_handle* h, const uint32_t* idx, uint32_t m, const Record* list, Record* out) {
+  if (m == 0) return ALZ_OK;
+  change_gather_kernel<<<std::min<unsigned>((3u * m + 255) / 256, (unsigned)h->sms * 4), 256, 0, h->stream>>>(
+      idx, m, list, out);
+  h->launches += 1;
+  CK(cudaGetLastError());
+  return ALZ_OK;
+}
+template int alz::metrics::gather_changes(alz_handle*, const uint32_t*, uint32_t, const alz_edge_change*,
+                                          alz_edge_change*);
+template int alz::metrics::gather_changes(alz_handle*, const uint32_t*, uint32_t, const alz_node_change*,
+                                          alz_node_change*);
 
 namespace {
 
@@ -316,14 +334,9 @@ int changes_locked(alz_handle* h, uint32_t source, const MetricSet& ms, uint32_t
   ci->above = above;
   rc = reserve(h, {{&s->top_list, std::max<size_t>(m, 1) * sizeof(alz_edge_change)}});
   if (rc != ALZ_OK) return rc;
-  if (m) {
-    change_gather_kernel<<<std::min<unsigned>((unsigned)((3 * m + 255) / 256), (unsigned)h->sms * 4), 256, 0,
-                           h->stream>>>(static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)m,
-                                        static_cast<const alz_edge_change*>(s->list.p),
-                                        static_cast<alz_edge_change*>(s->top_list.p));
-    h->launches += 1;
-    CK(cudaGetLastError());
-  }
+  rc = gather_changes(h, static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)m,
+                      static_cast<const alz_edge_change*>(s->list.p), static_cast<alz_edge_change*>(s->top_list.p));
+  if (rc != ALZ_OK) return rc;
   *res = static_cast<const alz_edge_change*>(s->top_list.p);
   *n = m;
   return ALZ_OK;
@@ -379,6 +392,7 @@ extern "C" int alz_baseline_pin(alz_handle* h, uint32_t source, alz_rollup_info*
   alz_changes_state* s = changes_state(h);
   s->pinned = false;   // a failure below leaves no baseline
   s->base_n = 0;
+  s->generation += 1;
   if (n > kMaxRows) return ALZ_E_CAPACITY;
   rc = reserve(h, {{&s->base_rows, std::max<size_t>(n, 1) * sizeof(alz_edge_out)},
                    {&s->base_keys, std::max<size_t>(n, 1) * 8}});

@@ -1,8 +1,9 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
-// (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu) and the node series
-// (alz_node_series.cu): the §17 metric values of a row list, of node rows or of series slots, the rows' packed keys,
-// the grow-on-demand device buffers, the node group-by, a source's edge or node series into given buffers and the
-// 64-bit top selection with its own scratch.
+// (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
+// (alz_node_series.cu) and the node changes (alz_node_changes.cu): the §17 metric values of a row list, of node rows
+// or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node group-by, a source's edge or
+// node series into given buffers, the 64-bit top selection with its own scratch, and the pinned baseline with the
+// §18 change arithmetic.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -127,6 +128,27 @@ int node_group_reduce(alz_handle* h, const NodeGroup& g, const alz_edge_out* row
 int node_gather(alz_handle* h, const uint32_t* idx, uint32_t m, const alz_node_out* nodes, alz_node_out* out);
 // The rows of `source`, checked against kMaxNodeSourceRows (ALZ_E_CAPACITY). Caller holds h->mu.
 int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n);
+
+// The pinned baseline of the change calls (alz_changes.cu): its rows, their count, what its source reported, and the
+// generation of its pin, which every alz_baseline_pin moves on. ALZ_E_STATE when none is pinned. Caller holds h->mu.
+int pinned_baseline(alz_handle* h, const alz_edge_out** rows, size_t* n, alz_rollup_info* info, uint64_t* generation);
+// out[j] = list[idx[j]] for j < m, on the stream: 48-byte change records (alz_edge_change, alz_node_change)
+template <class Record>
+int gather_changes(alz_handle* h, const uint32_t* idx, uint32_t m, const Record* list, Record* out);
+
+#ifdef __CUDACC__
+// A §18 side's value: COUNT and ERR5XX per window (one rounding), the others as they are
+__device__ __forceinline__ double per_window(double v, bool divide, double windows) {
+  return divide ? __ddiv_rn(v, windows) : v;
+}
+// The §18 change of mode from a source value and a baseline value, one rounding
+__device__ __forceinline__ double change_of(uint32_t mode, double cur, double base) {
+  if (mode == ALZ_CHANGE_DELTA) return __dsub_rn(cur, base);
+  if (mode == ALZ_CHANGE_DROP) return __dsub_rn(base, cur);
+  if (base > 0.0) return __ddiv_rn(cur, base);   // ALZ_CHANGE_RATIO
+  return cur > 0.0 ? __longlong_as_double(0x7FF0000000000000ll) : 1.0;
+}
+#endif
 
 // The rows of a source and its windows (ALZ_SOURCE_WINDOW: the last flushed window, 1), or of the last rollup of a
 // kind with what it reported (alz_changes.cu). Caller holds h->mu.

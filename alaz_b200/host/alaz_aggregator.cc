@@ -647,6 +647,38 @@ int Aggregator::Nodes(uint32_t source, uint32_t side, const std::vector<alz_metr
   return ALZ_OK;
 }
 
+int Aggregator::NodeChanges(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t mode,
+                            uint32_t presence, uint32_t k, double min_change, std::vector<NodeChange>* out,
+                            alz_change_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into node_changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
+  auto call = [&](size_t* n) {
+    return k == 0 ? alz_node_changes(h_, src, side, &metric, mode, presence, node_changes_.data(),
+                                     node_changes_.size(), n, info)
+                  : alz_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change, node_changes_.data(),
+                                         node_changes_.size(), n, info);
+  };
+  size_t n = 0;
+  int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > node_changes_.size()) {
+    node_changes_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  out->assign(n, NodeChange{});
+  for (size_t i = 0; i < n; ++i) {
+    const alz_node_change& c = node_changes_[i];
+    NodeChange& e = (*out)[i];
+    e.Type = NodeTypeName(c.type);
+    e.UID = UidOf(c.type, c.node);
+    e.Presence = c.presence; e.Value = c.value; e.BaseValue = c.base_value; e.Change = c.change;
+  }
+  return ALZ_OK;
+}
+
 int Aggregator::TopNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
                          std::vector<NodeWindow>* out, alz_top_info* info) {
   if (!h_) return ALZ_E_STATE;

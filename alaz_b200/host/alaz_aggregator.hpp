@@ -68,6 +68,14 @@ struct EdgeChange {
   double Value = 0.0, BaseValue = 0.0, Change = 0.0;
 };
 
+// one node of a node change list (docs/SPEC.md §23): the node by UID as NodeWindow names it, where it is
+// (ALZ_PRESENT_*) and the metric's value of one side on each side of the comparison with their change
+struct NodeChange {
+  std::string Type, UID;
+  uint32_t Presence = 0;
+  double Value = 0.0, BaseValue = 0.0, Change = 0.0;
+};
+
 // an edge named by UID, as EdgeWindow names it: FromType / ToType "pod" | "service" | "outbound"; an outbound end's UID
 // is its dotted quad or its Host header text
 struct EdgeRef {
@@ -215,6 +223,14 @@ class Aggregator {
   // min_change, largest first, ties in key order. info may be null. Returns 0 or an alz_status.
   int Changes(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
               double min_change, std::vector<EdgeChange>* out, alz_change_info* info = nullptr);
+  // Node changes (docs/SPEC.md §23): the nodes with rows on side `side` (ALZ_SIDE_*) of `source` (kLastWindow or a
+  // rollup kind, as in Anomalies) and of the baseline whose presence is in `presence`, with one metric's change of that
+  // side by `mode`, into *out: k = 0 every such node in node order, else the k largest changes >= min_change, largest
+  // first, ties in node order: "what changed since the deploy, per service". Nodes are matched by id and named as
+  // Nodes names them; PinBaseline's hold makes that correct by UID, so a pod deleted after the pin is GONE under its
+  // own UID and a pod added since is NEW under its own. info may be null. Returns 0 or an alz_status.
+  int NodeChanges(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t mode, uint32_t presence,
+                  uint32_t k, double min_change, std::vector<NodeChange>* out, alz_change_info* info = nullptr);
   // Edge series (docs/SPEC.md §19) over the last k entries of `tier` (0: flushed windows, 1..n: the tiers), oldest
   // first; *points (may be null) gets what a rollup of each entry alone reports. Series gives one series per row of
   // `source` (kLastWindow or a rollup kind, as in Anomalies), in its row order. SeriesFor gives one per edge named by
@@ -347,6 +363,7 @@ class Aggregator {
   std::vector<uint8_t> trend_present_;
   std::vector<alz_node_out> nodes_;       // node rows, values and indices of the last Nodes / TopNodes
   std::vector<double> node_values_;
+  std::vector<alz_node_change> node_changes_;   // records of the last NodeChanges
   std::vector<alz_node_trend> node_trends_;   // records, node rows, series and presence of the last NodeTrends
   std::vector<alz_node_out> node_trend_rows_;
 };

@@ -785,6 +785,53 @@ int alz_node_trends_top_device(alz_handle* h, uint32_t source, uint32_t side, ui
                                const double** dev_series, const uint8_t** dev_present, size_t* n_out,
                                uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
 
+/* ---- node changes against a pinned baseline (docs/SPEC.md §23) ---------------------------------------------------
+ * The §18 comparison for nodes. The source is ALZ_SOURCE_WINDOW or ALZ_ROLLUP_* (availability rule of §15), the
+ * baseline the one alz_baseline_pin holds; each side's node list is the §21 node list of its rows. A node is a member
+ * of a list on side `side` when it has a row there (IN: in_edges > 0, OUT: out_edges > 0). The list is the union of
+ * the two lists' members, matched by node key (type << 32) | value, in ascending key order, keeping the nodes whose
+ * presence bit is in `presence`: a node that served requests before and now only makes them is GONE on IN. index /
+ * base_index: the node's position in the source's / baseline's full §21 node list (alz_node_rows order), 0xFFFFFFFF
+ * where it is not a member. value / base_value: the §17 value of m on that node's side sums, bit for bit what
+ * alz_node_metrics* gives, divided by the side's windows for COUNT and ERR5XX (one rounding); +0.0 where absent.
+ * change and the top calls' ranking and eligibility: as alz_edge_changes* (§18). info->source_rows / base_rows count
+ * each side's member nodes; both, added and gone are counted before the filter, listed after it. Unknown metric,
+ * mode, side or source, presence 0 or above 7, k = 0, a NaN min_change or a null required pointer: ALZ_E_INVAL. No
+ * baseline, or no rows of a rollup source: ALZ_E_STATE. A side of more than 2^29 - 1 rows (before anything runs) or a
+ * union of more than 2^30 - 1 nodes: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. *n_out is always set; a host call whose
+ * cap (in records) is below it returns ALZ_E_CAPACITY and writes nothing. info may be NULL. Reads only: the window,
+ * every ring, the open blocks, every rollup's rows and the baseline are unchanged, and so are the node, node series,
+ * node trend, change, metric, top, series, trend and GNN results, device pointers included. The baseline's node rows
+ * are grouped on the first node change call after a pin and kept for later calls. Device results stay valid until the
+ * next node change call. Every rank holds the same rows and pins the same baseline, so every rank gets the same
+ * result with no collective. */
+typedef struct alz_node_change {   /* 48 B; presence, index, base_index, value, base_value and change at the offsets
+                                      of alz_edge_change's */
+  uint8_t type;          /* ALZ_NODE_* */
+  uint8_t _pad0;         /* zero */
+  uint8_t presence;      /* ALZ_PRESENT_* */
+  uint8_t _pad1[5];      /* zero */
+  uint32_t node;         /* the node's value: pod or service id, IPv4, Host id (offset 8, as alz_node_trend.value) */
+  uint32_t _pad2;        /* zero */
+  uint32_t index;        /* §21 node index in the source, 0xFFFFFFFF when absent there */
+  uint32_t base_index;   /* §21 node index in the baseline's node list, 0xFFFFFFFF when absent there */
+  double value;
+  double base_value;
+  double change;
+} alz_node_change;
+/* every listed node, in ascending node key order */
+int alz_node_changes(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                     uint32_t presence, alz_node_change* out, size_t cap, size_t* n_out, alz_change_info* info);
+int alz_node_changes_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                            uint32_t presence, const alz_node_change** dev_out, size_t* n_out, alz_change_info* info);
+/* the first min(k, above) listed nodes by change, in rank order; info->above = the eligible ones */
+int alz_node_changes_top(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                         uint32_t presence, uint32_t k, double min_change, alz_node_change* out, size_t cap,
+                         size_t* n_out, alz_change_info* info);
+int alz_node_changes_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                                uint32_t presence, uint32_t k, double min_change,
+                                const alz_node_change** dev_out, size_t* n_out, alz_change_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

@@ -57,6 +57,14 @@ int alz_debug_edge_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size
  * alz_node_rows otherwise. Uses the node calls' buffers. */
 int alz_debug_node_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, alz_node_out* out, size_t cap,
                         size_t* n_out);
+/* test/debug: alz_node_changes (docs/SPEC.md §23) between the §21 node lists of two caller row lists in device memory,
+ * each in any order with repeats allowed and covering src_windows / base_windows (>= 1) windows; the pinned baseline
+ * and its cached node rows are not used. More than 2^29 - 1 rows in a list: ALZ_E_CAPACITY. The rules of
+ * alz_node_changes otherwise. Uses the node change calls' buffers. */
+int alz_debug_node_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size_t n_src, uint32_t src_windows,
+                                const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows, uint32_t side,
+                                const alz_metric* m, uint32_t mode, uint32_t presence, alz_node_change* out,
+                                size_t cap, size_t* n_out, alz_change_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);

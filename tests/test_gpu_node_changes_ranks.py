@@ -1,0 +1,74 @@
+"""GPU: node changes against a pinned baseline on several ranks, on one GPU through the loopback collective
+(tests/loopback_node_changes_ranks.py). After a merge every rank holds the merged rows, so every rank pins the same
+baseline, groups the same nodes and compares the same sources: every rank returns the same node lists and top
+changes, with no collective of their own, and they equal tests/node_change_ref.py over the merged rows."""
+import json
+import os
+import subprocess
+import sys
+
+import numpy as np
+import pytest
+
+import node_change_ref as ncr
+from alaz_b200 import abi
+from loopback_node_changes_ranks import CASES, INFO
+from test_gpu_loopback_ranks import HERE, ROOT, SMALL, shim, spread_groups  # noqa: F401  (shim is a fixture)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("pin", [["window"], ["span", 3, abi.SPAN_AT_MOST]])
+def test_three_ranks_return_identical_node_changes(shim, tmp_path, pin):  # noqa: F811
+    R, J, P, rng = 3, 7, 3, np.random.default_rng(57)
+    tabs, groups, _ = spread_groups(rng, 600)
+    own = np.arange(len(groups)) % R
+    per_rank = []
+    for j in range(J):
+        part = [g for i, g in enumerate(groups) if i % 5 != j % 5]
+        w = [np.concatenate([g for i, g in enumerate(groups) if i % 5 != j % 5 and own[i] == r]) for r in range(R)]
+        if j % 3 == 1:                                                            # keys on every rank
+            w = [np.concatenate([x, np.concatenate(part[:50])]) for x in w]
+        per_rank.append(w)
+    rollups = [["window", 2], ["tier", 1, 1], ["span", 4, abi.SPAN_AT_LEAST]]
+    k, mc = 25, 0.0
+    spec = {"nranks": R, "cfg": SMALL, "history": [4, 1 << 14], "tiers": [[2, 3, 1 << 14, 1 << 12]], "windows": J,
+            "pin_after": P, "pin": pin, "rollups": rollups, "k": k, "min_change": mc}
+    arrays = {"tab0": np.asarray(tabs, np.int64).reshape(-1, 3)}
+    for j, w in enumerate(per_rank):
+        for r in range(R):
+            arrays[f"w{j}_r{r}"] = np.ascontiguousarray(w[r], dtype=abi.L7_REC)
+    sp, ip, op = (str(tmp_path / x) for x in ("spec.json", "in.npz", "out.npz"))
+    with open(sp, "w") as f:
+        json.dump(spec, f)
+    np.savez(ip, **arrays)
+    env = dict(os.environ)
+    env["LD_LIBRARY_PATH"] = os.path.dirname(shim) + os.pathsep + env.get("LD_LIBRARY_PATH", "")
+    env["LOOPBACK_NCCL_TIMEOUT_S"] = "60"
+    p = subprocess.run([sys.executable, os.path.join(HERE, "loopback_node_changes_ranks.py"), sp, ip, op], cwd=ROOT,
+                       env=env, capture_output=True, text=True, timeout=600)
+    assert p.returncode == 0, p.stdout[-3000:] + p.stderr[-3000:]
+    z = np.load(op)
+    meta = json.loads(str(z["meta"]))
+    assert not meta["errors"], meta["errors"]
+    assert meta["maps"] == [shim], meta["maps"]
+    for r in range(1, R):
+        assert z[f"base_{r}"].tobytes() == z["base_0"].tobytes()
+    base, bw = z["base_0"], int(z["basew_0"][0])
+    assert len(base) > 0
+    listed = 0
+    for j in range(P + 1, J):
+        for s in range(1 + len(rollups)):
+            names = [f"{x}{c}_{{}}_{{}}_{s}" for c in range(len(CASES)) for x in ("list", "top", "info", "tinfo")]
+            for r in range(1, R):
+                for x in names + [f"rows_{{}}_{{}}_{s}"]:
+                    assert z[x.format(j, r)].tobytes() == z[x.format(j, 0)].tobytes(), (x, j, r, s)
+            rows, w = z[f"rows_{j}_0_{s}"], int(z[f"win_{j}_0_{s}"][0])
+            for c, (side, metric, mode, presence) in enumerate(CASES):
+                lst, info = ncr.changes(rows, base, side, metric, mode, presence, w, bw)
+                assert z[f"list{c}_{j}_0_{s}"].tobytes() == lst.tobytes(), (j, s, c)
+                assert z[f"info{c}_{j}_0_{s}"].tolist() == [info[x] for x in INFO], (j, s, c)
+                top, tinfo = ncr.top(rows, base, side, metric, mode, presence, k, mc, w, bw)
+                assert z[f"top{c}_{j}_0_{s}"].tobytes() == top.tobytes(), (j, s, c)
+                assert z[f"tinfo{c}_{j}_0_{s}"].tolist() == [tinfo[x] for x in INFO], (j, s, c)
+                listed += len(lst)
+    assert listed > 0
