@@ -50,6 +50,14 @@ static int alloc_dict(alz_handle* h, DictEnt** dict, uint32_t cap) {
   CK(cudaMemsetAsync(*dict, 0xFF, (size_t)cap * sizeof(DictEnt), h->stream));
   return ALZ_OK;
 }
+// a claimed-slot log of `cap` entries, empty
+static int alloc_log(alz_handle* h, SlotLog* l, uint32_t cap) {
+  l->cap = cap;
+  CK(cudaMalloc(&l->slot, (size_t)cap * 4));
+  CK(cudaMalloc(&l->n, 8));
+  CK(cudaMemsetAsync(l->n, 0, 8, h->stream));
+  return ALZ_OK;
+}
 static int alloc_table(alz_handle* h, PairTable* t, uint32_t max_rows, uint32_t* n_rows_dev) {
   memset(t, 0, sizeof(*t));
   t->max_rows = max_rows;
@@ -61,6 +69,7 @@ static int alloc_table(alz_handle* h, PairTable* t, uint32_t max_rows, uint32_t*
   t->dict_host_mask = host_cap - 1;
   int rc;
   if ((rc = alloc_dict(h, &t->dict, dict_cap)) != ALZ_OK || (rc = alloc_dict(h, &t->dict_host, host_cap)) != ALZ_OK) return rc;
+  if ((rc = alloc_log(h, &t->log, max_rows)) != ALZ_OK) return rc;
   const size_t rows = (size_t)max_rows + kPairKinds;
   CK(cudaMalloc(&t->row_key, rows * 8));
   CK(cudaMalloc(&t->sect, rows * kSectPerRow * 32));
@@ -80,8 +89,8 @@ static int alloc_table(alz_handle* h, EdgeTable* t, uint32_t max_rows, uint32_t*
   t->n_rows = n_rows_dev;
   const uint32_t dict_cap = next_pow2(2ull * max_rows);
   t->dict_mask = dict_cap - 1;
-  const int rc = alloc_dict(h, &t->dict, dict_cap);
-  if (rc != ALZ_OK) return rc;
+  int rc = alloc_dict(h, &t->dict, dict_cap);
+  if (rc != ALZ_OK || (rc = alloc_log(h, &t->log, max_rows)) != ALZ_OK) return rc;
   const size_t rows = (size_t)max_rows + 1;   // row max_rows: the free-marker key's
   CK(cudaMalloc(&t->row_key, rows * 8));
   CK(cudaMalloc(&t->count, rows * 8));
@@ -96,24 +105,26 @@ static int alloc_table(alz_handle* h, EdgeTable* t, uint32_t max_rows, uint32_t*
 }
 static void free_table(PairTable* t) {
   cudaFree(t->dict); cudaFree(t->dict_host); cudaFree(t->row_key); cudaFree(t->row_kind); cudaFree(t->row_cnt);
-  cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->sect);
+  cudaFree(t->row_base); cudaFree(t->row_aux); cudaFree(t->sect); cudaFree(t->log.slot); cudaFree(t->log.n);
   memset(t, 0, sizeof(*t));
 }
 static void free_table(EdgeTable* t) {
   cudaFree(t->dict); cudaFree(t->row_key); cudaFree(t->count); cudaFree(t->lat_sum); cudaFree(t->err5xx); cudaFree(t->hist);
+  cudaFree(t->log.slot); cudaFree(t->log.n);
   memset(t, 0, sizeof(*t));
 }
 // all keys out of the pair dictionaries; the rows keep their indices until clear_dict resets the allocator
 static int clear_keys(alz_handle* h, const PairTable& t) {
-  CK(cudaMemsetAsync(t.dict, 0xFF, ((size_t)t.dict_mask + 1) * sizeof(DictEnt), h->stream));
-  CK(cudaMemsetAsync(t.dict_host, 0xFF, ((size_t)t.dict_host_mask + 1) * sizeof(DictEnt), h->stream));
+  launch_pair_dict_clear(t, false, h->sms, h->stream);
+  h->launches += 1;
+  CK(cudaGetLastError());
   return ALZ_OK;
 }
 // all keys out of the pair dictionaries, row allocator back to zero (rows were zeroed by fold / emit)
 static int clear_dict(alz_handle* h, const PairTable& t) {
-  int rc = clear_keys(h, t);
-  if (rc != ALZ_OK) return rc;
-  CK(cudaMemsetAsync(t.n_rows, 0, 4, h->stream));
+  launch_pair_dict_clear(t, true, h->sms, h->stream);
+  h->launches += 1;
+  CK(cudaGetLastError());
   return ALZ_OK;
 }
 
@@ -202,8 +213,20 @@ extern "C" int alz_create(const alz_config* cfg, alz_handle** out) {
     CKC(cudaMalloc(&h->d_rows[b], (size_t)h->cfg.max_edges * 4));
   }
   // shared by the key sort and the scan of the bucket counts, which run one after the other in stream order
-  h->sort_tmp_bytes = std::max(sort_pairs_temp_bytes(h->cfg.max_edges), scan_temp_bytes(h->cfg.max_edges + 1));
+  // pod ids below max_endpoints (up to 2^20) get a segment of their own in the edge-key sort
+  h->es.pods = std::min<uint32_t>(h->cfg.max_endpoints, 1u << 20);
+  const uint32_t n_seg = 8u * h->es.pods + 1u;
+  h->sort_tmp_bytes = std::max(scan_temp_bytes(h->cfg.max_edges + 1), edge_sort_temp_bytes(h->es.pods));
   CKC(cudaMalloc(&h->d_sort_tmp, h->sort_tmp_bytes));
+  CKC(cudaMalloc(&h->es.cnt, (size_t)n_seg * 4));
+  CKC(cudaMemsetAsync(h->es.cnt, 0, (size_t)n_seg * 4, h->stream));
+  CKC(cudaMalloc(&h->es.off, (size_t)n_seg * 4));
+  CKC(cudaMalloc(&h->es.large, ((size_t)h->cfg.max_edges / 257 + 1) * 4));
+  CKC(cudaMalloc(&h->es.n_large, 8));
+  h->es.keys = h->d_keys[0];
+  h->es.rows = h->d_rows[0];
+  h->es.temp = h->d_sort_tmp;
+  h->es.temp_bytes = h->sort_tmp_bytes;
   if (!(h->cfg.flags & ALZ_CFG_EAGER_JOIN)) {
     const size_t n_cnt = (size_t)h->cfg.max_edges + 1;
     h->bk.cap = h->cfg.max_pairs + kPairKinds;
@@ -262,6 +285,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   if (h->ev_patch) cudaEventDestroy(h->ev_patch);
   for (int i = 0; i < 3; ++i) if (h->ev_t[i]) cudaEventDestroy(h->ev_t[i]);
   cudaFree(h->d_sort_tmp); cudaFree(h->d_out);
+  cudaFree(h->es.cnt); cudaFree(h->es.off); cudaFree(h->es.large); cudaFree(h->es.n_large);
   cudaFree(h->bk.cnt); cudaFree(h->bk.off); cudaFree(h->bk.rows); cudaFree(h->bk.n_stray);
   if (h->own_stream) cudaStreamDestroy(h->own_stream);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
@@ -753,15 +777,24 @@ extern "C" int alz_submit_l7_raw(alz_handle* h, const void* raw, size_t n) {
 }
 
 // ---- window result ---------------------------------------------------------------------------
-// Resolve + sort of the live edge keys (no reset). After it h->n_live edges sit in d_keys[1]/d_rows[1].
-// The edge count is final once fold_resolve_kernel has run, so the counters are copied out right there and
-// the host waits on an event for THAT copy only. What does not need the count is enqueued before the wait and
-// keeps the GPU busy while the host sizes and enqueues the sort:
+// Resolve + sort of the live edge keys (no reset). After it the live edges sit in d_keys[1]/d_rows[1], in key order.
+// The edge count is final once fold_resolve_kernel has run, so the counters are copied out right there (ev_count);
+// the sort reads the count on the device and needs no host wait:
 //  - one rank: the pair rows are bucketed by edge row and the pair dictionaries cleared (nothing probes them
 //    after the resolve); finish_flush sums each bucket straight into its output row;
 //  - several ranks: the rest of the fold into the edge table, which the merge reads (alz_comm.cu).
-// *overflow: the window lost rows (pair or edge table full); the flush still emits what it has.
-static int prepare_flush(alz_handle* h, bool* overflow) {
+// wait: the host waits for the counters here and sets n_live and *overflow; otherwise read_flush_count does, once
+// the whole flush is enqueued. *overflow: the window lost rows (pair or edge table full); the flush still emits what
+// it has.
+static int read_flush_count(alz_handle* h, bool* overflow) {
+  CK(cudaEventSynchronize(h->ev_count));
+  h->n_live = h->h_ctr->edge_rows;
+  if (h->n_live > h->cfg.max_edges) { h->n_live = h->cfg.max_edges; *overflow = true; }
+  // events the pair table could not take during this window's ingest launches
+  if (h->h_ctr->capacity_events != h->lost_reported) { h->lost_reported = h->h_ctr->capacity_events; *overflow = true; }
+  return ALZ_OK;
+}
+static int prepare_flush(alz_handle* h, bool wait, bool* overflow) {
   *overflow = false;
   const bool fold = !(h->cfg.flags & ALZ_CFG_EAGER_JOIN) && h->pending_since_fold != 0;
   int rc = ALZ_OK;
@@ -777,38 +810,27 @@ static int prepare_flush(alz_handle* h, bool* overflow) {
   } else if (fold && (rc = fold_second_half(h)) != ALZ_OK) {
     return rc;
   }
-  CK(cudaEventSynchronize(h->ev_count));
-  h->n_live = h->h_ctr->edge_rows;
-  if (h->n_live > h->cfg.max_edges) { h->n_live = h->cfg.max_edges; *overflow = true; }
-  // events the pair table could not take during this window's ingest launches
-  if (h->h_ctr->capacity_events != h->lost_reported) { h->lost_reported = h->h_ctr->capacity_events; *overflow = true; }
-  if (h->n_live) {
-    launch_iota(h->d_rows[0], h->n_live, h->sms, h->stream);
-    h->launches += 1;
-    sort_pairs(h->d_sort_tmp, h->sort_tmp_bytes, h->edges.row_key, h->d_keys[1], h->d_rows[0], h->d_rows[1],
-               h->n_live, h->stream);
-    CK(cudaGetLastError());
-  }
-  return ALZ_OK;
+  CK(edge_sort(h->edges, h->es, h->d_keys[1], h->d_rows[1], h->sms, h->stream));
+  h->launches += kEdgeSortKernels;
+  return wait ? read_flush_count(h, overflow) : ALZ_OK;
 }
 
 // Single rank: the output rows in key order, each the sum of its edge's pair rows (and of the edge accumulators
 // when a fold already ran in this window); the edge table and the pair rows are left zeroed for the next window.
+// Every launch here reads the edge count on the device; last_n_edges is set by the caller once the count is read.
 static int finish_flush(alz_handle* h) {
   const FlushBuckets* b = nullptr;
   if (h->bucketed) {
-    // cnt[n_live] is zero (every edge row of a pair row is below n_live), so off[n_live] ends the last bucket
-    exclusive_scan_u32(h->d_sort_tmp, h->sort_tmp_bytes, h->bk.cnt, h->bk.off, h->n_live + 1, h->stream);
+    // cnt[e] is zero from the edge count on (every edge row of a pair row is below it), so off[e + 1] ends bucket e
+    exclusive_scan_u32(h->d_sort_tmp, h->sort_tmp_bytes, h->bk.cnt, h->bk.off, h->cfg.max_edges + 1, h->stream);
     launch_bucket_fill(h->pairs, h->cfg.max_edges, h->bk, h->sms, h->stream);
     h->launches += 1;
     b = &h->bk;
   }
   const bool with_edges = h->edges_dirty || (h->cfg.flags & ALZ_CFG_EAGER_JOIN);
-  if (b || h->n_live) {
-    launch_emit_edges(h->pairs, h->edges, h->d_ctr, h->d_hot, h->d_keys[1], h->d_rows[1], h->n_live, b, with_edges,
-                      h->d_out, h->sms, h->stream);
-    h->launches += 1;
-  }
+  launch_emit_edges(h->pairs, h->edges, h->d_ctr, h->d_hot, h->d_keys[1], h->d_rows[1], b, with_edges, h->d_out,
+                    h->sms, h->stream);
+  h->launches += 1;
   CK(cudaGetLastError());
   if (h->bucketed) {
     CK(cudaMemsetAsync(h->bk.n_stray, 0, 4, h->stream));
@@ -819,9 +841,9 @@ static int finish_flush(alz_handle* h) {
     h->bucketed = false;
     h->pending_since_fold = 0;
   }
-  CK(edge_table_clear(h->edges, h->stream));
+  CK(edge_table_clear(h->edges, h->sms, h->stream));
+  h->launches += 1;
   h->edges_dirty = false;
-  h->last_n_edges = h->n_live;
   h->windows++;
   return ALZ_OK;
 }
@@ -860,8 +882,8 @@ static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, si
   bool overflow = false;
   const bool ranks = h->comm_nranks > 1;
   CK(cudaEventRecord(h->ev_t[0], h->stream));
-  int rc = prepare_flush(h, &overflow);
-  *n_out = ranks ? 0u : h->n_live;
+  int rc = prepare_flush(h, ranks, &overflow);
+  *n_out = 0;
   CK(cudaEventRecord(h->ev_t[1], h->stream));
   int mrc;
   bool roll = true;
@@ -870,7 +892,8 @@ static int flush_device_locked(alz_handle* h, const alz_edge_out** dev_edges, si
     if (mrc != ALZ_OK && overflow && rc == ALZ_OK) h->lost_reported = ~0ull;   // window kept: report the loss again
   } else {
     if (rc != ALZ_OK) return rc;
-    mrc = finish_flush(h);
+    if ((mrc = finish_flush(h)) == ALZ_OK && (mrc = read_flush_count(h, &overflow)) == ALZ_OK)
+      h->last_n_edges = h->n_live;
   }
   CK(cudaEventRecord(h->ev_t[2], h->stream));
   h->ev_t_valid = true;
@@ -895,12 +918,15 @@ extern "C" int alz_window_flush(alz_handle* h, alz_edge_out* out, size_t cap, si
   std::lock_guard<std::mutex> g(h->mu);
   CK(cudaSetDevice(h->device));
   if (h->comm_nranks <= 1) {
-    // size check first so that a too-small buffer keeps the window intact
+    // size check first so that a too-small buffer keeps the window intact: only a buffer smaller than max_edges
+    // needs the edge count before the rows are emitted
     bool overflow = false;
-    int rc = prepare_flush(h, &overflow);
-    *n_out = h->n_live;
+    const bool wait = cap < h->cfg.max_edges;
+    int rc = prepare_flush(h, wait, &overflow);
+    *n_out = 0;
     if (rc != ALZ_OK) return rc;
-    if (h->n_live > cap) {
+    if (wait) *n_out = h->n_live;
+    if (wait && h->n_live > cap) {
       if (overflow) h->lost_reported = ~0ull;   // report the loss again next time
       if (h->bucketed) {                        // keep the window: the bucketed pair rows go into the edge table
         CK(cudaMemsetAsync(h->bk.cnt, 0, ((size_t)h->cfg.max_edges + 1) * 4, h->stream));
@@ -912,6 +938,8 @@ extern "C" int alz_window_flush(alz_handle* h, alz_edge_out* out, size_t cap, si
     }
     rc = finish_flush(h);
     if (rc != ALZ_OK) return rc;
+    if (!wait && (rc = read_flush_count(h, &overflow)) != ALZ_OK) return rc;
+    *n_out = h->last_n_edges = h->n_live;
     if (h->n_live) CK(cudaMemcpyAsync(out, h->d_out, (size_t)h->n_live * sizeof(alz_edge_out),
                                       cudaMemcpyDeviceToHost, h->stream));
     if ((rc = alz_internal_history_append(h, h->win_on ? h->d_win : nullptr)) != ALZ_OK) return rc;

@@ -302,7 +302,7 @@ __global__ void __launch_bounds__(256) consume_window_kernel(const MergeInfo* __
   uint4* dict = reinterpret_cast<uint4*>(edges.dict);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < dict_words; i += (size_t)gridDim.x * blockDim.x)
     dict[i] = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
-  if (blockIdx.x == 0 && threadIdx.x == 0) *edges.n_rows = 0u;
+  if (blockIdx.x == 0 && threadIdx.x == 0) { *edges.n_rows = 0u; edges.log.n[0] = 0u; }
   for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 3; i < n; i += groups) edge_row_zero(edges, rows[i], sl);
 }
 
@@ -435,7 +435,8 @@ static int drop_window(alz_handle* h, bool* lost, bool at_e) {
     consume_window_kernel<<<grid, 256, 0, s>>>(c->d_info, h->edges, h->d_rows[1], h->n_live);
     h->launches += 2;
   } else if (at_e) {
-    CK(edge_table_clear(h->edges, s));
+    CK(edge_table_clear(h->edges, h->sms, s));
+    h->launches += 1;
   }
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(c->h_info, c->d_info, sizeof(MergeInfo), cudaMemcpyDeviceToHost, s));
@@ -467,7 +468,7 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   if (total == 0) {
     h->last_n_edges = 0;
     h->windows++;
-    if (at_e) CK(edge_table_clear(h->edges, s));
+    if (at_e) { CK(edge_table_clear(h->edges, h->sms, s)); h->launches += 1; }
     return ALZ_OK;
   }
   if ((uint64_t)pad * R > c->gather_cap) return drop_window(h, lost, at_e);
@@ -510,7 +511,7 @@ static int merge_allreduce(alz_handle* h, bool* lost, bool at_e) {
   // 5. unpack; local edge table back to empty
   unpack_canonical_kernel<<<grid * 2, 256, 0, s>>>(c->d_can_keys, c->d_can, n_can, h->d_out);
   CK(cudaGetLastError());
-  if (at_e) CK(edge_table_clear(h->edges, s));
+  if (at_e) { CK(edge_table_clear(h->edges, h->sms, s)); h->launches += 1; }
   h->last_n_edges = n_can;
   h->windows++;
   return ALZ_OK;

@@ -189,6 +189,20 @@ constexpr uint32_t kClaimRow = 0xFFFFFFFCu; // pair table: a thread is allocatin
 
 constexpr uint32_t kPairFwd = 0u, kPairRev = 1u, kPairHost = 2u, kPairKinds = 3u;
 
+// Claimed-slot log of a table's dictionaries: every CAS that takes a slot from kEmptyKey appends the slot, so a clear
+// resets the slots a window used instead of the whole capacity (dict_clear_kernel, alz_kernels.cu). A table with two
+// dictionaries logs the second one's slots after the first one's (index dict_mask + 1 + slot). A log that overflowed
+// (n[0] > cap) makes the clear take the whole capacity. n[1] counts the clear's finished blocks.
+struct SlotLog {
+  uint32_t* slot;   // [cap]
+  uint32_t* n;      // [2]: slots claimed since the last clear (counted past cap), blocks done
+  uint32_t cap;
+};
+__device__ __forceinline__ void log_claim(const SlotLog& l, uint32_t idx) {
+  const uint32_t i = atomicAdd(l.n, 1u);
+  if (i < l.cap) l.slot[i] = idx;
+}
+
 // The pair table: socket pairs -> rows of the sectored layout below. One dictionary slot serves both directions of
 // a pair (kPairFwd, kPairRev); the host-keyed outbound events (kind kPairHost: the key's high word is a Host-header
 // id, not a daddr; ALZ_PROTO_F_HOSTKEY) have a dictionary of their own, a key space of its own. Both dictionaries
@@ -218,6 +232,7 @@ struct PairTable {
   // partials (take_pair_row, alz_kernels.cu). A cell pair is added to as a u64: cells are u32 and a fold runs before any cell
   // could reach 2^31 (alz_api.cu), so nothing carries from the low cell into the high one.
   uint64_t* sect;     // [(max_rows + 3) * kSectPerRow * 4]
+  SlotLog log;        // slots of dict, then of dict_host
 };
 constexpr uint32_t kSectPerRow = 16;
 __device__ __forceinline__ uint64_t* pair_sect(const PairTable& t, uint32_t row, uint32_t bucket) {
@@ -239,6 +254,7 @@ struct EdgeTable {
   uint64_t* lat_sum;  // [max_rows + 1]
   uint64_t* err5xx;   // [max_rows + 1]
   uint32_t* hist;     // [(max_rows + 1) * ALZ_NB]
+  SlotLog log;
 };
 
 // one event into an edge row
@@ -264,11 +280,9 @@ __device__ __forceinline__ void edge_row_zero(const EdgeTable& t, uint32_t row, 
   cells[1] = make_uint4(0u, 0u, 0u, 0u);
   if (sl == 0) { t.count[row] = 0ull; t.lat_sum[row] = 0ull; t.err5xx[row] = 0ull; }
 }
-// all keys out of the dictionary and the row allocator back to zero, in stream order (whoever took the rows zeroed them)
-inline cudaError_t edge_table_clear(const EdgeTable& t, cudaStream_t s) {
-  const cudaError_t e = cudaMemsetAsync(t.dict, 0xFF, ((size_t)t.dict_mask + 1) * sizeof(DictEnt), s);
-  return e != cudaSuccess ? e : cudaMemsetAsync(t.n_rows, 0, 4, s);
-}
+// all keys out of the dictionary and the row allocator back to zero, in stream order (whoever took the rows zeroed
+// them); one dict_clear_kernel launch (alz_kernels.cu)
+cudaError_t edge_table_clear(const EdgeTable& t, int sms, cudaStream_t s);
 
 // row of `key`, inserting it if absent; >= kLostRow when capacity is exhausted
 __device__ __forceinline__ uint32_t find_or_insert(const EdgeTable& t, uint64_t key) {
@@ -283,6 +297,7 @@ __device__ __forceinline__ uint32_t find_or_insert(const EdgeTable& t, uint64_t 
       const uint64_t old = atomicCAS((unsigned long long*)&t.dict[slot].key, (unsigned long long)kEmptyKey,
                                      (unsigned long long)key);
       if (old == kEmptyKey) {
+        log_claim(t.log, slot);
         row = atomicAdd(t.n_rows, 1u);
         if (row >= t.max_rows) row = kLostRow; else t.row_key[row] = key;
         *reinterpret_cast<volatile uint32_t*>(&t.dict[slot].row[0]) = row;
@@ -345,7 +360,7 @@ __device__ __forceinline__ uint32_t find_or_insert_pair(const PairTable& t, uint
     if (k == kEmptyKey) {
       if (!is_pod()) return kDropRow;
       k = atomicCAS((unsigned long long*)&dict[slot].key, (unsigned long long)kEmptyKey, (unsigned long long)key);
-      if (k == kEmptyKey) k = key;
+      if (k == kEmptyKey) { log_claim(t.log, kind == kPairHost ? t.dict_mask + 1u + slot : slot); k = key; }
       row = *reinterpret_cast<volatile uint32_t*>(&dict[slot].row[w]);
     }
     if (k == key) {

@@ -101,6 +101,7 @@ struct alz_handle {
   void* d_sort_tmp = nullptr;
   size_t sort_tmp_bytes = 0;
   alz_edge_out* d_out = nullptr;
+  alz::EdgeSortScratch es{};              // the edge-key sort (alz_sort.cu): keys/rows are d_keys[0] / d_rows[0]
   uint32_t n_live = 0, last_n_edges = 0;
   alz::FlushBuckets bk{};                 // single-rank flush: pair rows by edge row (not with ALZ_CFG_EAGER_JOIN)
   bool bucketed = false;                  // prepare_flush bucketed the pair rows; finish_flush emits them

@@ -361,7 +361,7 @@ __global__ void __launch_bounds__(256) bucket_fill_kernel(PairTable pairs, uint3
 // no pair rows to take (nothing was ingested since the last fold, or ALZ_CFG_EAGER_JOIN).
 __global__ void __launch_bounds__(256) emit_edges_kernel(PairTable pairs, EdgeTable edges, Counters* ctr,
                                                          uint32_t* __restrict__ hot_bins, const uint64_t* __restrict__ keys,
-                                                         const uint32_t* __restrict__ rows, uint32_t n_live,
+                                                         const uint32_t* __restrict__ rows,
                                                          const uint32_t* __restrict__ off,
                                                          const uint32_t* __restrict__ row_list, uint32_t list_cap,
                                                          const uint32_t* __restrict__ n_stray, bool with_edges,
@@ -369,6 +369,7 @@ __global__ void __launch_bounds__(256) emit_edges_kernel(PairTable pairs, EdgeTa
   const uint32_t lane = threadIdx.x & 31u, sl = lane & 7u;
   const uint32_t gmask = 0xFFu << (lane & ~7u);
   const uint32_t groups_per_grid = (gridDim.x * blockDim.x) >> 3;
+  const uint32_t n_live = min(*edges.n_rows, edges.max_rows);
   const uint32_t n_groups = n_live + (off != nullptr ? *n_stray : 0u);
   __shared__ uint32_t s_bins[128];
   block_bins_begin(s_bins);
@@ -478,6 +479,37 @@ __global__ void __launch_bounds__(256) synth_owned_kernel(alz_synth_view v, uint
   }
 }
 
+// Empties a table's dictionaries (a, then b; b_mask + 1 slots of b, or none) from its claimed-slot log: the logged
+// slots go back to kEmptyKey, or every slot of both when the log overflowed. The last block to finish resets the log
+// and, when n_rows is given, the row allocator; every block has read the log count before any block finishes.
+__global__ void __launch_bounds__(256) dict_clear_kernel(DictEnt* __restrict__ a, uint32_t a_mask, DictEnt* __restrict__ b,
+                                                         uint32_t b_slots, SlotLog log, uint32_t* __restrict__ n_rows) {
+  const uint32_t n = *reinterpret_cast<volatile uint32_t*>(log.n);
+  const uint4 empty = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t first = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n <= log.cap) {
+    for (size_t i = first; i < n; i += stride) {
+      const uint32_t v = log.slot[i];
+      DictEnt* e = v <= a_mask ? &a[v] : &b[v - a_mask - 1u];
+      *reinterpret_cast<uint4*>(e) = empty;
+    }
+  } else {
+    const size_t total = (size_t)a_mask + 1u + b_slots;
+    for (size_t i = first; i < total; i += stride)
+      *reinterpret_cast<uint4*>(i <= a_mask ? &a[i] : &b[i - a_mask - 1u]) = empty;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    if (atomicAdd(&log.n[1], 1u) == gridDim.x - 1u) {
+      log.n[0] = 0u;
+      log.n[1] = 0u;
+      if (n_rows) *n_rows = 0u;
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------
 // launchers
 // ---------------------------------------------------------------------------
@@ -538,11 +570,19 @@ void launch_bucket_fill(const PairTable& pairs, uint32_t max_edges, const FlushB
   bucket_fill_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs, max_edges, b.cnt, b.off, b.rows);
 }
 void launch_emit_edges(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
-                       const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
-                       int sms, cudaStream_t s) {
-  emit_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot->bins, keys, rows, n_live,
+                       const uint32_t* rows, const FlushBuckets* b, bool with_edges, alz_edge_out* out, int sms,
+                       cudaStream_t s) {
+  emit_edges_kernel<<<grid_for(sms, 8), 256, 0, s>>>(pairs, edges, ctr, hot->bins, keys, rows,
                                                      b ? b->off : nullptr, b ? b->rows : nullptr, b ? b->cap : 0u,
                                                      b ? b->n_stray : nullptr, with_edges, out);
+}
+void launch_pair_dict_clear(const PairTable& pairs, bool reset_rows, int sms, cudaStream_t s) {
+  dict_clear_kernel<<<grid_for(sms, 4), 256, 0, s>>>(pairs.dict, pairs.dict_mask, pairs.dict_host, pairs.dict_host_mask + 1u,
+                                                     pairs.log, reset_rows ? pairs.n_rows : nullptr);
+}
+cudaError_t edge_table_clear(const EdgeTable& t, int sms, cudaStream_t s) {
+  dict_clear_kernel<<<grid_for(sms, 4), 256, 0, s>>>(t.dict, t.dict_mask, nullptr, 0u, t.log, t.n_rows);
+  return cudaGetLastError();
 }
 void launch_compact_raw(const uint8_t* raw, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s) {
   if (n == 0) return;

@@ -59,10 +59,12 @@ struct FlushBuckets {
 };
 void launch_bucket_count(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
 void launch_bucket_fill(const PairTable& pairs, uint32_t max_edges, const FlushBuckets& b, int sms, cudaStream_t s);
-// b == nullptr: no pair rows to take
+// b == nullptr: no pair rows to take. Emits the edge table's live rows, as many as its allocator counts.
 void launch_emit_edges(const PairTable& pairs, const EdgeTable& edges, Counters* ctr, HotState* hot, const uint64_t* keys,
-                       const uint32_t* rows, uint32_t n_live, const FlushBuckets* b, bool with_edges, alz_edge_out* out,
-                       int sms, cudaStream_t s);
+                       const uint32_t* rows, const FlushBuckets* b, bool with_edges, alz_edge_out* out, int sms,
+                       cudaStream_t s);
+// the pair dictionaries emptied from their claimed-slot log; reset_rows: the row allocator back to zero too
+void launch_pair_dict_clear(const PairTable& pairs, bool reset_rows, int sms, cudaStream_t s);
 void launch_compact_raw(const uint8_t* raw, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s);
 void launch_synth(const alz_synth_view& v, uint64_t first, uint64_t n, alz_l7_rec* out, int sms, cudaStream_t s);
 void launch_synth_owned(const alz_synth_view& v, uint64_t first, uint64_t n, uint32_t nranks, uint32_t rank,
@@ -75,4 +77,22 @@ cudaError_t sort_pairs(void* temp, size_t temp_bytes, const uint64_t* keys_in, u
 size_t scan_temp_bytes(uint32_t n);
 cudaError_t exclusive_scan_u32(void* temp, size_t temp_bytes, const uint32_t* in, uint32_t* out, uint32_t n,
                                cudaStream_t s);
+// single-rank flush: the live edge rows of a table sorted by key, sized on the device (alz_sort.cu). pods bounds the
+// pod ids that get a segment of their own (any larger id still sorts right, in one shared segment).
+struct EdgeSortScratch {
+  uint32_t pods;
+  uint32_t* cnt;       // [8 * pods + 1] all zero between sorts
+  uint32_t* off;       // [8 * pods + 1]
+  uint64_t* keys;      // [max_edges] keys bucketed by their high word
+  uint32_t* rows;      // [max_edges]
+  uint32_t* large;     // [max_edges / 257 + 1] buckets of segments too large for a thread per key
+  uint32_t* n_large;   // [2] large segments listed, most 4096-key chunks in one of them
+  void* temp;          // the scan's
+  size_t temp_bytes;
+};
+size_t edge_sort_temp_bytes(uint32_t pods);
+// kEdgeSortKernels launches of its own and a CUB scan; the scan's status, or the launches'
+constexpr int kEdgeSortKernels = 5;
+cudaError_t edge_sort(const EdgeTable& t, const EdgeSortScratch& x, uint64_t* keys_out, uint32_t* rows_out, int sms,
+                      cudaStream_t s);
 }  // namespace alz
