@@ -24,6 +24,7 @@ AMQP_PUBLISH, AMQP_DELIVER = 1, 2
 REDIS_COMMAND, REDIS_PUSHED_EVENT, REDIS_PING = 1, 2, 3
 MF_METHOD_MASK, MF_PAYLOAD_REJECT, MF_TLS = 0x3F, 0x40, 0x80
 NODE_POD, NODE_SVC, NODE_OUTBOUND, NODE_OUTBOUND_HOST = 0, 1, 2, 3
+NODE_GROUP = 4                                                      # a caller-defined group (§24)
 PROTO_F_HOSTKEY = 0x40
 TABLE_POD, TABLE_SVC = 0, 1
 CFG_EAGER_JOIN = 0x1
@@ -248,6 +249,17 @@ NODE_CHANGE = np.dtype([
 assert NODE_CHANGE.itemsize == 48
 assert all(NODE_CHANGE.fields[f][1] == EDGE_CHANGE.fields[f][1]
            for f in ("presence", "index", "base_index", "value", "base_value", "change"))   # EDGE_CHANGE's offsets
+
+
+class GroupInfo(C.Structure):
+    """alz_group_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("source_rows", "mapped_ends", "edges", "internal")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
+GROUP_INFO = GroupInfo
 
 
 class SpanInfo(C.Structure):

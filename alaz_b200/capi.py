@@ -37,7 +37,10 @@ EXPORTS = [
     "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
     "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device",
     "alz_node_changes", "alz_node_changes_device", "alz_node_changes_top", "alz_node_changes_top_device",
-    "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_group_set", "alz_group_edges", "alz_group_edges_device", "alz_group_edge_metrics",
+    "alz_group_edge_metrics_device", "alz_group_edge_top", "alz_group_edge_top_device", "alz_group_nodes",
+    "alz_group_nodes_device", "alz_group_node_metrics", "alz_group_node_metrics_device", "alz_group_node_top",
+    "alz_group_node_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -167,6 +170,24 @@ def load(rebuild=False):
                                          C.POINTER(abi.ChangeInfo)], i),
         "alz_debug_node_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
                                          C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_set": ([vp, vp, vp, sz], i),
+        "alz_group_edges": ([vp, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.GroupInfo)], i),
+        "alz_group_edges_device": ([vp, u32, pp, C.POINTER(sz), C.POINTER(abi.GroupInfo)], i),
+        "alz_group_edge_metrics": ([vp, u32, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_group_edge_metrics_device": ([vp, u32, vp, u32, pp, C.POINTER(sz)], i),
+        "alz_group_edge_top": ([vp, u32, vp, u32, C.c_double, vp, vp, vp, sz, C.POINTER(sz), C.POINTER(abi.TopInfo)],
+                               i),
+        "alz_group_edge_top_device": ([vp, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
+                                       C.POINTER(abi.TopInfo)], i),
+        "alz_group_nodes": ([vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_group_nodes_device": ([vp, u32, pp, C.POINTER(sz)], i),
+        "alz_group_node_metrics": ([vp, u32, u32, vp, u32, vp, sz, C.POINTER(sz)], i),
+        "alz_group_node_metrics_device": ([vp, u32, u32, vp, u32, pp, C.POINTER(sz)], i),
+        "alz_group_node_top": ([vp, u32, u32, vp, u32, C.c_double, vp, vp, vp, sz, C.POINTER(sz),
+                                C.POINTER(abi.TopInfo)], i),
+        "alz_group_node_top_device": ([vp, u32, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
+                                       C.POINTER(abi.TopInfo)], i),
+        "alz_debug_group_edges": ([vp, vp, sz, vp, sz, C.POINTER(sz), C.POINTER(abi.GroupInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -214,7 +235,11 @@ def load(rebuild=False):
                   "alz_node_series", "alz_node_series_device", "alz_node_series_keys", "alz_node_series_keys_device",
                   "alz_node_trends", "alz_node_trends_device", "alz_node_trends_top", "alz_node_trends_top_device",
                   "alz_node_changes", "alz_node_changes_device", "alz_node_changes_top",
-                  "alz_node_changes_top_device", "alz_debug_node_changes_rows"):
+                  "alz_node_changes_top_device", "alz_debug_node_changes_rows", "alz_group_set", "alz_group_edges",
+                  "alz_group_edges_device", "alz_group_edge_metrics", "alz_group_edge_metrics_device",
+                  "alz_group_edge_top", "alz_group_edge_top_device", "alz_group_nodes", "alz_group_nodes_device",
+                  "alz_group_node_metrics", "alz_group_node_metrics_device", "alz_group_node_top",
+                  "alz_group_node_top_device", "alz_debug_group_edges"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -883,6 +908,106 @@ class Handle:
             if len(rows):
                 self.h2d(p, rows)
             return self._node_rows("alz_debug_node_rows", (C.c_void_p(p), len(rows)))
+        finally:
+            self.dev_free(p)
+
+    # ---- groups (alz_groups.cu, docs/SPEC.md §24)
+    def group_set(self, nodes, groups):
+        """alz_group_set: node nodes[i] (see node_ends) is a member of group groups[i]; empty lists clear the map."""
+        keys = np.ascontiguousarray(self.node_ends(nodes))
+        g = np.ascontiguousarray(groups, dtype=np.uint32)
+        if len(keys) != len(g):
+            raise ValueError("one group per node")
+        self._ck(self.L.alz_group_set(self.h, _ptr(keys), _ptr(g), len(keys)), "alz_group_set")
+
+    def _group_edges(self, fn, args):
+        """fn(h, *args, out, cap, &n, &info): (EDGE_OUT group-edge rows, info dict); a first call with cap 0 sizes it."""
+        f, n, info = getattr(self.L, fn), C.c_size_t(0), abi.GroupInfo()
+        if self._ck(f(self.h, *args, None, 0, C.byref(n), C.byref(info)), fn, allow=(abi.E_CAPACITY,)) == 0:
+            return np.zeros(0, dtype=abi.EDGE_OUT), info.as_dict()
+        out = np.zeros(n.value, dtype=abi.EDGE_OUT)
+        self._ck(f(self.h, *args, _ptr(out), n.value, C.byref(n), C.byref(info)), fn)
+        return out, info.as_dict()
+
+    def group_edges(self, source=abi.SOURCE_WINDOW):
+        """alz_group_edges: the group-edge rows of `source` (abi.SOURCE_WINDOW or abi.ROLLUP_*) as EDGE_OUT rows in
+        (from key, to key) order, and the info dict."""
+        return self._group_edges("alz_group_edges", (int(source),))
+
+    def group_edges_device(self, source=abi.SOURCE_WINDOW):
+        """alz_group_edges_device: (device pointer, rows, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.GroupInfo()
+        self._ck(self.L.alz_group_edges_device(self.h, int(source), C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_group_edges_device")
+        return p.value, n.value, info.as_dict()
+
+    def group_edge_metrics(self, source, *specs):
+        """alz_group_edge_metrics: values [group-edge rows x len(specs)]."""
+        return self._edge_metrics("alz_group_edge_metrics", (int(source),), specs)
+
+    def group_edge_metrics_device(self, source, *specs):
+        """alz_group_edge_metrics_device: (device pointer, rows)."""
+        return self._edge_metrics_device("alz_group_edge_metrics_device", (int(source),), specs)
+
+    def group_edge_top(self, source, spec, k, min_value=0.0):
+        """alz_group_edge_top: (group-edge rows, values, row indices, info dict), rank order."""
+        return self._edge_top("alz_group_edge_top", (int(source),), spec, k, min_value)
+
+    def group_edge_top_device(self, source, spec, k, min_value=0.0):
+        """alz_group_edge_top_device: (rows, values, index device pointers, results, info dict)."""
+        return self._edge_top_device("alz_group_edge_top_device", (int(source),), spec, k, min_value)
+
+    def group_nodes(self, source=abi.SOURCE_WINDOW):
+        """alz_group_nodes: the §21 NODE_OUT rows of the group-edge rows of `source`, node order."""
+        return self._node_rows("alz_group_nodes", (int(source),))
+
+    def group_nodes_device(self, source=abi.SOURCE_WINDOW):
+        """alz_group_nodes_device: (device pointer, nodes)."""
+        p, n = C.c_void_p(), C.c_size_t(0)
+        self._ck(self.L.alz_group_nodes_device(self.h, int(source), C.byref(p), C.byref(n)), "alz_group_nodes_device")
+        return p.value, n.value
+
+    def group_node_metrics(self, source, side, *specs):
+        """alz_group_node_metrics: values [group nodes x len(specs)] of side abi.SIDE_IN / SIDE_OUT."""
+        return self._edge_metrics("alz_group_node_metrics", (int(source), int(side)), specs)
+
+    def group_node_metrics_device(self, source, side, *specs):
+        """alz_group_node_metrics_device: (device pointer, nodes)."""
+        return self._edge_metrics_device("alz_group_node_metrics_device", (int(source), int(side)), specs)
+
+    def group_node_top(self, source, side, spec, k, min_value=0.0):
+        """alz_group_node_top: (NODE_OUT rows, values, node indices, info dict), rank order."""
+        f, n, info, m = self.L.alz_group_node_top, C.c_size_t(0), abi.TopInfo(), abi.metrics(spec)
+        cap = min(int(k), 1 << 16)
+        while True:
+            nodes = np.zeros(cap, dtype=abi.NODE_OUT)
+            values = np.zeros(cap, dtype=np.float64)
+            index = np.zeros(cap, dtype=np.uint32)
+            rc = self._ck(f(self.h, int(source), int(side), m, int(k), float(min_value), _ptr(nodes), _ptr(values),
+                            _ptr(index), cap, C.byref(n), C.byref(info)), "alz_group_node_top",
+                          allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                r = n.value
+                return nodes[:r].copy(), values[:r].copy(), index[:r].copy(), info.as_dict()
+            cap = n.value
+
+    def group_node_top_device(self, source, side, spec, k, min_value=0.0):
+        """alz_group_node_top_device: (nodes, values, index device pointers, results, info dict)."""
+        pn, pv, pi, n, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), abi.TopInfo()
+        self._ck(self.L.alz_group_node_top_device(self.h, int(source), int(side), abi.metrics(spec), int(k),
+                                                  float(min_value), C.byref(pn), C.byref(pv), C.byref(pi), C.byref(n),
+                                                  C.byref(info)), "alz_group_node_top_device")
+        return pn.value, pv.value, pi.value, n.value, info.as_dict()
+
+    def debug_group_edges(self, rows):
+        """alz_debug_group_edges over a host EDGE_OUT array (copied to the device) with the handle's map: (group-edge
+        rows, info dict)."""
+        rows = np.ascontiguousarray(rows, dtype=abi.EDGE_OUT)
+        p = self.dev_alloc(max(rows.nbytes, 1))
+        try:
+            if len(rows):
+                self.h2d(p, rows)
+            return self._group_edges("alz_debug_group_edges", (C.c_void_p(p), len(rows)))
         finally:
             self.dev_free(p)
 

@@ -39,6 +39,7 @@ struct alz_trend_state;   // alz_trends.cu
 struct alz_node_state;    // alz_nodes.cu
 struct alz_node_series_state;   // alz_node_series.cu
 struct alz_node_changes_state;  // alz_node_changes.cu
+struct alz_group_state;         // alz_groups.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -141,6 +142,8 @@ struct alz_handle {
   alz_trend_state* node_trends = nullptr;         // the node trends' buffers (alz_node_trends*); null until the first
   alz_node_changes_state* node_changes = nullptr; // the node changes' buffers and the baseline's node rows
                                                   // (alz_node_changes*); null until the first
+  alz_group_state* groups = nullptr;      // the group map and the group calls' buffers (alz_group_*); null until the
+                                          // first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -195,4 +198,5 @@ void alz_internal_free_nodes(alz_handle* h);
 void alz_internal_free_node_series(alz_handle* h);
 void alz_internal_free_node_trends(alz_handle* h);
 void alz_internal_free_node_changes(alz_handle* h);
+void alz_internal_free_groups(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

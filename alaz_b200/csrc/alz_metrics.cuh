@@ -1,9 +1,9 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
 // (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
-// (alz_node_series.cu) and the node changes (alz_node_changes.cu): the §17 metric values of a row list, of node rows
-// or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node group-by, a source's edge or
-// node series into given buffers, the 64-bit top selection with its own scratch, and the pinned baseline with the
-// §18 change arithmetic.
+// (alz_node_series.cu), the node changes (alz_node_changes.cu) and the groups (alz_groups.cu): the §17 metric values
+// of a row list, of node rows or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node
+// group-by, a source's edge or node series into given buffers, the 64-bit top selection with its own scratch, and the
+// pinned baseline with the §18 change arithmetic.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -128,6 +128,11 @@ int node_group_reduce(alz_handle* h, const NodeGroup& g, const alz_edge_out* row
 int node_gather(alz_handle* h, const uint32_t* idx, uint32_t m, const alz_node_out* nodes, alz_node_out* out);
 // The rows of `source`, checked against kMaxNodeSourceRows (ALZ_E_CAPACITY). Caller holds h->mu.
 int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_t* n);
+// The §21 node rows of n rows into `out`, grown to hold them, with g as the group-by's scratch: node_group_keys,
+// node_group_runs (one wait), then node_group_reduce on the stream. *n_nodes = the nodes; more than cap:
+// ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device; n <= kMaxNodeSourceRows.
+int node_rows_of(alz_handle* h, NodeGroup& g, DevBuf& out, const alz_edge_out* rows, size_t n, size_t cap,
+                 size_t* n_nodes);
 
 // The pinned baseline of the change calls (alz_changes.cu): its rows, their count, what its source reported, and the
 // generation of its pin, which every alz_baseline_pin moves on. ALZ_E_STATE when none is pinned. Caller holds h->mu.

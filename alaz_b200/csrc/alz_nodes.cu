@@ -311,6 +311,24 @@ int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_
   return *n > kMaxNodeSourceRows ? ALZ_E_CAPACITY : ALZ_OK;
 }
 
+int node_rows_of(alz_handle* h, NodeGroup& g, DevBuf& out, const alz_edge_out* rows, size_t n, size_t cap,
+                 size_t* n_nodes) {
+  *n_nodes = 0;
+  const uint32_t n2 = 2u * (uint32_t)n;
+  if (n == 0) return reserve(h, {{&out, sizeof(alz_node_out)}});
+  int rc = node_group_reserve(h, g, n2);
+  if (rc != ALZ_OK) return rc;
+  node_group_keys(h, g, rows, (uint32_t)n);
+  rc = node_group_runs(h, g, n2, kNodeKeyBits);
+  if (rc != ALZ_OK) return rc;
+  const size_t nodes = g.h_words[0];
+  *n_nodes = nodes;
+  if (nodes > cap) return ALZ_E_CAPACITY;
+  rc = reserve(h, {{&out, nodes * sizeof(alz_node_out)}});
+  if (rc != ALZ_OK) return rc;
+  return node_group_reduce(h, g, rows, n2, static_cast<alz_node_out*>(out.p));
+}
+
 }  // namespace metrics
 }  // namespace alz
 
@@ -320,22 +338,8 @@ namespace {
 // nodes than cap: ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device;
 // n <= kMaxNodeSourceRows.
 int group_nodes(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_nodes) {
-  *n_nodes = 0;
   if (!h->nodes) h->nodes = new alz_node_state();
-  alz_node_state* s = h->nodes;
-  const uint32_t n2 = 2u * (uint32_t)n;
-  if (n == 0) return reserve(h, {{&s->rows, sizeof(alz_node_out)}});
-  int rc = node_group_reserve(h, s->g, n2);
-  if (rc != ALZ_OK) return rc;
-  node_group_keys(h, s->g, rows, (uint32_t)n);
-  rc = node_group_runs(h, s->g, n2, kNodeKeyBits);
-  if (rc != ALZ_OK) return rc;
-  const size_t nodes = s->g.h_words[0];
-  *n_nodes = nodes;
-  if (nodes > cap) return ALZ_E_CAPACITY;
-  rc = reserve(h, {{&s->rows, nodes * sizeof(alz_node_out)}});
-  if (rc != ALZ_OK) return rc;
-  return node_group_reduce(h, s->g, rows, n2, static_cast<alz_node_out*>(s->rows.p));
+  return node_rows_of(h, h->nodes->g, h->nodes->rows, rows, n, cap, n_nodes);
 }
 
 bool valid_source(uint32_t source) { return source == ALZ_SOURCE_WINDOW || source <= ALZ_ROLLUP_SPAN; }

@@ -41,7 +41,7 @@ uint8_t MethodEnum(uint8_t proto, const std::string& m) {
   }
 }
 const char* NodeTypeName(uint8_t t) {   // aggregator/data.go:42-44 (a Host-header keyed destination is OUTBOUND too)
-  return t == ALZ_NODE_POD ? "pod" : t == ALZ_NODE_SVC ? "service" : "outbound";
+  return t == ALZ_NODE_POD ? "pod" : t == ALZ_NODE_SVC ? "service" : t == ALZ_NODE_GROUP ? "group" : "outbound";
 }
 }  // namespace
 
@@ -123,6 +123,7 @@ uint32_t Aggregator::Interner::Acquire(const std::string& uid) {
     names.push_back(uid); refs.push_back(0); unmapped_in.push_back(0); reused_after.push_back(0);
   }
   ids.emplace(uid, id);
+  changes += 1;
   return id;
 }
 void Aggregator::Interner::Map(uint32_t ip, uint32_t id, uint64_t open_window) {
@@ -150,12 +151,13 @@ void Aggregator::Interner::EndWindow(uint64_t flushed, uint64_t hold, uint64_t p
     if (pinned_from && unmapped_in[id] >= pinned_from) { pending_free[keep++] = id; continue; }   // in the baseline
     ids.erase(it);
     free_ids.push_back(id);
+    changes += 1;
   }
   pending_free.resize(keep);
   keep = 0;
   for (uint32_t id : held) {
     if (pinned_from && unmapped_in[id] >= pinned_from) held[keep++] = id;
-    else free_ids.push_back(id);
+    else { free_ids.push_back(id); changes += 1; }
   }
   held.resize(keep);
 }
@@ -293,6 +295,7 @@ std::string Aggregator::UidOf(uint8_t t, uint32_t v) const {
   if (t == ALZ_NODE_POD) return v < pods_.names.size() ? pods_.names[v] : std::string("?");
   if (t == ALZ_NODE_SVC) return v < svcs_.names.size() ? svcs_.names[v] : std::string("?");
   if (t == ALZ_NODE_OUTBOUND_HOST) return v < host_names_.size() ? host_names_[v] : std::string("?");   // data.go:852
+  if (t == ALZ_NODE_GROUP) return v < group_names_.size() ? group_names_[v] : std::string("?");
   return FormatIPv4(v);   // outbound: the raw daddr string (data.go:862)
 }
 
@@ -693,6 +696,111 @@ int Aggregator::TopNodes(uint32_t source, uint32_t side, const alz_metric& metri
   size_t n = 0;
   node_values_.resize(nodes_.size());
   int rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > nodes_.size()) {
+    nodes_.resize(n);
+    node_values_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToNodes(nodes_.data(), n, node_values_.data(), 1);
+  return ALZ_OK;
+}
+
+int Aggregator::SetGroups(const std::vector<GroupMember>& members) {
+  if (!h_) return ALZ_E_STATE;
+  std::lock_guard<std::mutex> g(mu_);
+  members_ = members;
+  for (const GroupMember& m : members_) {
+    if (group_ids_.count(m.Group)) continue;
+    if (group_names_.size() >= (1u << 29)) return ALZ_E_CAPACITY;
+    group_ids_.emplace(m.Group, (uint32_t)group_names_.size());
+    group_names_.push_back(m.Group);
+  }
+  groups_sent_ = false;
+  return ALZ_OK;
+}
+
+int Aggregator::SyncGroups() {
+  const uint64_t changes = pods_.changes + svcs_.changes + host_names_.size();
+  if (groups_sent_ && changes == groups_changes_) return ALZ_OK;
+  std::vector<alz_node_ends> nodes;
+  std::vector<uint32_t> groups;
+  std::unordered_map<uint64_t, bool> seen;
+  for (const GroupMember& m : members_) {
+    alz_node_ends e{};
+    if (!EndOf(m.Type, m.UID, &e.type, &e.value)) continue;   // no id now: not in any row the library holds
+    if (!seen.emplace(((uint64_t)e.type << 32) | e.value, true).second) continue;
+    nodes.push_back(e);
+    groups.push_back(group_ids_.at(m.Group));
+  }
+  const int rc = alz_group_set(h_, nodes.data(), groups.data(), nodes.size());
+  if (rc != ALZ_OK) return rc;
+  groups_sent_ = true;
+  groups_changes_ = changes;
+  return ALZ_OK;
+}
+
+int Aggregator::GroupEdges(uint32_t source, std::vector<EdgeWindow>* out, alz_group_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into roll_, grown once when the rows do not fit (ALZ_E_CAPACITY with n = the rows; nothing written)
+  size_t n = 0;
+  rc = alz_group_edges(h_, src, roll_.data(), roll_.size(), &n, info);
+  if (rc == ALZ_E_CAPACITY && n > roll_.size()) {
+    roll_.resize(n);
+    rc = alz_group_edges(h_, src, roll_.data(), roll_.size(), &n, info);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToEdges(roll_.data(), n, nullptr);
+  return ALZ_OK;
+}
+
+int Aggregator::GroupNodes(uint32_t source, uint32_t side, const std::vector<alz_metric>& metrics,
+                           std::vector<NodeWindow>* out) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const uint32_t nm = (uint32_t)metrics.size();
+  // the node count (ALZ_E_CAPACITY with n = the nodes; nothing written), then the rows and the values
+  size_t n = 0;
+  rc = alz_group_nodes(h_, src, nullptr, 0, &n);
+  if (rc == ALZ_E_CAPACITY) {
+    nodes_.resize(n);
+    rc = alz_group_nodes(h_, src, nodes_.data(), n, &n);
+  }
+  if (rc != ALZ_OK) return rc;
+  node_values_.assign(n * nm, 0.0);
+  size_t nv = 0;
+  rc = alz_group_node_metrics(h_, src, side, metrics.data(), nm, node_values_.data(), n, &nv);
+  if (rc != ALZ_OK) return rc;
+  if (nv != n) return ALZ_E_STATE;
+  *out = ToNodes(nodes_.data(), n, node_values_.data(), nm);
+  return ALZ_OK;
+}
+
+int Aggregator::TopGroupNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
+                              std::vector<NodeWindow>* out, alz_top_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into nodes_ / node_values_, grown once when the results do not fit (ALZ_E_CAPACITY with n = the results)
+  auto call = [&](size_t* n) {
+    return alz_group_node_top(h_, src, side, &metric, k, min_value, nodes_.data(), node_values_.data(), nullptr,
+                              nodes_.size(), n, info);
+  };
+  size_t n = 0;
+  node_values_.resize(nodes_.size());
+  rc = call(&n);
   if (rc == ALZ_E_CAPACITY && n > nodes_.size()) {
     nodes_.resize(n);
     node_values_.resize(n);

@@ -117,6 +117,12 @@ struct NodeRef {
   std::string Type, UID;
 };
 
+// a member of a caller-defined group (docs/SPEC.md §24): the node by Type ("pod" | "service" | "outbound") and UID as
+// NodeRef names it, and its group's name (a deployment, a namespace)
+struct GroupMember {
+  std::string Type, UID, Group;
+};
+
 // one node's series (docs/SPEC.md §22): per point, oldest first, whether that entry holds a row on the side of the
 // node and the metrics' values of the side's sums there (every value 0 where it does not)
 struct NodeSeriesRow {
@@ -279,6 +285,22 @@ class Aggregator {
   int NodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
                  const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
                  std::vector<alz_rollup_info>* points = nullptr);
+  // Groups (docs/SPEC.md §24). SetGroups replaces the group map: each member's node goes to its group, named by a
+  // string the adapter interns; an empty list clears the map. A member is resolved by UID whenever the map is sent:
+  // before the next group call after SetGroups, and again before a group call whenever an id was handed out or freed
+  // since the last send. A member whose UID has no id then is skipped, and the first of repeated members counts.
+  // SetHistory's hold keeps a deleted pod's id, and so its membership, for every retained row that carries it.
+  int SetGroups(const std::vector<GroupMember>& members);
+  // the group-edge rows of `source` (kLastWindow or a rollup kind, as in Anomalies) into *out, in the library's order:
+  // a group end is Type "group", UID the group's name; an unmapped end is named as ToEdges names it. info may be null.
+  // Returns 0 or an alz_status.
+  int GroupEdges(uint32_t source, std::vector<EdgeWindow>* out, alz_group_info* info = nullptr);
+  // the §21 nodes of the group-edge rows with `metrics` of side `side`, in node order (groups last), named as
+  // GroupEdges names the ends: "what is deployment checkout's inbound p99 over the last hour"
+  int GroupNodes(uint32_t source, uint32_t side, const std::vector<alz_metric>& metrics, std::vector<NodeWindow>* out);
+  // the k group nodes with the highest values of `metric` on side `side` >= min_value, as TopNodes ranks nodes
+  int TopGroupNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
+                    std::vector<NodeWindow>* out, alz_top_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -310,6 +332,9 @@ class Aggregator {
   // row's Present and Values in *out (EdgeSeries or NodeSeriesRow; the names are the caller's); requires mu_
   template <class Row, class Call>
   int RunSeries(size_t nm, std::vector<Row>* out, std::vector<alz_rollup_info>* points, Call call);
+  // the group map resolved by UID sent to the library when SetGroups changed it or an interner handed out or freed an
+  // id since the last send; requires mu_
+  int SyncGroups();
   // UID <-> dense id (< 2^29). An id whose last IP mapping went away while window w was open may be carried by
   // window w, and by every retained entry and open block that covers w: it is recycled once `hold` more windows
   // have been flushed after w (hold 0: when w is flushed).
@@ -322,6 +347,7 @@ class Aggregator {
     std::vector<uint32_t> free_ids, pending_free;
     std::vector<uint32_t> held;                       // freed ids taken back while a pinned baseline may carry them
     std::vector<uint64_t> reused_after;               // unmapped_in of the id when another UID last took it (0: never)
+    uint64_t changes = 0;                             // ids handed out or freed so far
     uint32_t Acquire(const std::string& uid);
     void Map(uint32_t ip, uint32_t id, uint64_t open_window);
     void Unmap(uint32_t ip, uint64_t open_window);
@@ -366,6 +392,11 @@ class Aggregator {
   std::vector<alz_node_change> node_changes_;   // records of the last NodeChanges
   std::vector<alz_node_trend> node_trends_;   // records, node rows, series and presence of the last NodeTrends
   std::vector<alz_node_out> node_trend_rows_;
+  std::vector<GroupMember> members_;                    // the group map as SetGroups gave it
+  std::unordered_map<std::string, uint32_t> group_ids_;  // group name -> dense id (ALZ_NODE_GROUP)
+  std::vector<std::string> group_names_;
+  bool groups_sent_ = true;                             // the library holds members_ as resolved at groups_changes_
+  uint64_t groups_changes_ = 0;                         // the interners' changes at the last send
 };
 
 }  // namespace alaz

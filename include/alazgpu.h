@@ -71,7 +71,9 @@ enum { ALZ_REDIS_COMMAND = 1, ALZ_REDIS_PUSHED_EVENT = 2, ALZ_REDIS_PING = 3 };
 /* node kinds of an edge end (aggregator/data.go POD/SVC/OUTBOUND) */
 enum { ALZ_NODE_POD = 0, ALZ_NODE_SVC = 1, ALZ_NODE_OUTBOUND = 2,
        ALZ_NODE_OUTBOUND_HOST = 3 /* outbound destination keyed by the HTTP Host header (aggregator/data.go:851-854);
-                                     value = the caller's dense id of the header string */ };
+                                     value = the caller's dense id of the header string */,
+       ALZ_NODE_GROUP = 4 /* a caller-defined group of nodes (docs/SPEC.md §24), value = the caller's dense id of the
+                             group; only the group calls produce it, never a flush */ };
 /* tables of the join's build side (aggregator/cluster.go:15-16) */
 enum { ALZ_TABLE_POD = 0, ALZ_TABLE_SVC = 1 };
 
@@ -831,6 +833,72 @@ int alz_node_changes_top(alz_handle* h, uint32_t source, uint32_t side, const al
 int alz_node_changes_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
                                 uint32_t presence, uint32_t k, double min_change,
                                 const alz_node_change** dev_out, size_t* n_out, alz_change_info* info);
+
+/* ---- groups (docs/SPEC.md §24) --------------------------------------------------------------------------------------
+ * The group map sends nodes to caller-defined groups (a deployment, a namespace): node nodes[i] is a member of group
+ * groups[i], the node (ALZ_NODE_GROUP, groups[i]). Any of the four flushed node types may be mapped. alz_group_set
+ * replaces the whole map; n = 0 clears it, and a handle starts with it empty. A malformed key (a type above
+ * ALZ_NODE_OUTBOUND_HOST, a pod or service value >= 2^29), a group >= 2^29, one node twice in one call, or null arrays
+ * with n > 0: ALZ_E_INVAL. More than 2^30 - 1 entries: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. Every failure leaves
+ * the previous map in force. The map lives on the device; it survives flushes, rollups, pins and every other call and
+ * goes with the next alz_group_set or alz_destroy. On several ranks, every rank sets the same map: no collective runs.
+ *
+ * The group edges of a source (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability rule of §15): each row's from
+ * end and to end is replaced by its group when the map holds it and kept otherwise; rows equal in (from_type, from,
+ * to_type, to) after that are summed by the §3 rule (count, err5xx, lat_sum_ns mod 2^64, hist cells mod 2^32). Rows
+ * come out in ascending (node key of from, node key of to), node key (type << 32) | value: with an empty map, the
+ * source's rows in that order. Each row keeps its orientation; a row whose two ends land in one group is an internal
+ * row (g -> g) and is kept. Padding is zero. Group edge metrics and top: §17 over the group-edge rows, the index being
+ * the group-edge row's position. Group nodes, their metrics and top: §21 over the group-edge rows, so a group's side IN
+ * sums every row into any of its members, and a group node (type 4) is listed after every other node.
+ * *n_out is always set; a host call whose cap is below it returns ALZ_E_CAPACITY and writes nothing. An unknown source
+ * or side, a bad metric list (§17), k = 0, a NaN min_value or a null required pointer: ALZ_E_INVAL. No rows of a rollup
+ * source: ALZ_E_STATE. More than 2^29 - 1 source rows: ALZ_E_CAPACITY, before anything runs; no memory: ALZ_E_NOMEM. A
+ * 0-row source: 0 rows, ALZ_OK. info (may be NULL): the source's rows, the row ends the map held, the group-edge rows,
+ * and the source rows whose two ends are one node after the mapping. Reads only: the window, every ring, the open
+ * blocks, every rollup's rows, the baseline and every other family's results, device pointers included, are unchanged.
+ * Device results stay valid until the next group call on the handle. Every rank holds the same rows and the same map,
+ * so every rank gets the same result. */
+typedef struct alz_group_info {
+  uint64_t source_rows;   /* rows of the source */
+  uint64_t mapped_ends;   /* row ends (two per row) the map held */
+  uint64_t edges;         /* group-edge rows */
+  uint64_t internal;      /* source rows whose from and to are one node after the mapping */
+} alz_group_info;
+int alz_group_set(alz_handle* h, const alz_node_ends* nodes, const uint32_t* groups, size_t n);
+/* every group-edge row of a source, in (from key, to key) order; cap counts rows */
+int alz_group_edges(alz_handle* h, uint32_t source, alz_edge_out* out, size_t cap, size_t* n_out, alz_group_info* info);
+int alz_group_edges_device(alz_handle* h, uint32_t source, const alz_edge_out** dev_out, size_t* n_out,
+                           alz_group_info* info);
+/* values[i * nm + j]: metric j of group-edge row i; cap counts rows */
+int alz_group_edge_metrics(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t nm, double* values, size_t cap,
+                           size_t* n_out);
+int alz_group_edge_metrics_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t nm,
+                                  const double** dev_values, size_t* n_out);
+/* the first min(k, above) group-edge rows by one metric, ranked as alz_edge_top; rows, values, index and info may each
+ * be NULL. info->scored = the group-edge rows. */
+int alz_group_edge_top(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t k, double min_value,
+                       alz_edge_out* rows, double* values, uint32_t* index, size_t cap, size_t* n_out,
+                       alz_top_info* info);
+int alz_group_edge_top_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t k, double min_value,
+                              const alz_edge_out** dev_rows, const double** dev_values, const uint32_t** dev_index,
+                              size_t* n_out, alz_top_info* info);
+/* the §21 node rows of the group-edge rows, in node order; cap counts nodes */
+int alz_group_nodes(alz_handle* h, uint32_t source, alz_node_out* out, size_t cap, size_t* n_out);
+int alz_group_nodes_device(alz_handle* h, uint32_t source, const alz_node_out** dev_out, size_t* n_out);
+/* values[i * nm + j]: metric j of group node i's side `side` (ALZ_SIDE_*); cap counts nodes */
+int alz_group_node_metrics(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t nm,
+                           double* values, size_t cap, size_t* n_out);
+int alz_group_node_metrics_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t nm,
+                                  const double** dev_values, size_t* n_out);
+/* the first min(k, above) group nodes by one metric of one side, ranked as alz_node_top; nodes, values, index and info
+ * may each be NULL (dev_nodes, dev_values and dev_index too). info->scored = the group nodes. */
+int alz_group_node_top(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t k,
+                       double min_value, alz_node_out* nodes, double* values, uint32_t* index, size_t cap,
+                       size_t* n_out, alz_top_info* info);
+int alz_group_node_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t k,
+                              double min_value, const alz_node_out** dev_nodes, const double** dev_values,
+                              const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
 
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +

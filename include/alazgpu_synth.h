@@ -65,6 +65,11 @@ int alz_debug_node_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size
                                 const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows, uint32_t side,
                                 const alz_metric* m, uint32_t mode, uint32_t presence, alz_node_change* out,
                                 size_t cap, size_t* n_out, alz_change_info* info);
+/* test/debug: the group edges of alz_group_edges (docs/SPEC.md §24) of n caller rows in device memory with the
+ * handle's group map, which may hold layouts ingest cannot make (any row order, repeated edges, one group edge on 2^20
+ * rows, cells of 2^32 - 1); the rules of alz_group_edges otherwise. Uses the group calls' buffers. */
+int alz_debug_group_edges(alz_handle* h, const alz_edge_out* dev_rows, size_t n, alz_edge_out* out, size_t cap,
+                          size_t* n_out, alz_group_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
