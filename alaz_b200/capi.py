@@ -40,7 +40,10 @@ EXPORTS = [
     "alz_group_set", "alz_group_edges", "alz_group_edges_device", "alz_group_edge_metrics",
     "alz_group_edge_metrics_device", "alz_group_edge_top", "alz_group_edge_top_device", "alz_group_nodes",
     "alz_group_nodes_device", "alz_group_node_metrics", "alz_group_node_metrics_device", "alz_group_node_top",
-    "alz_group_node_top_device", "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
+    "alz_group_node_top_device", "alz_group_edge_changes", "alz_group_edge_changes_device",
+    "alz_group_edge_changes_top", "alz_group_edge_changes_top_device", "alz_group_node_changes",
+    "alz_group_node_changes_device", "alz_group_node_changes_top", "alz_group_node_changes_top_device",
+    "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
 ]
@@ -188,6 +191,22 @@ def load(rebuild=False):
         "alz_group_node_top_device": ([vp, u32, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
                                        C.POINTER(abi.TopInfo)], i),
         "alz_debug_group_edges": ([vp, vp, sz, vp, sz, C.POINTER(sz), C.POINTER(abi.GroupInfo)], i),
+        "alz_group_edge_changes": ([vp, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_edge_changes_device": ([vp, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_edge_changes_top": ([vp, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
+                                        C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_edge_changes_top_device": ([vp, u32, vp, u32, u32, u32, C.c_double, pp, C.POINTER(sz),
+                                               C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_node_changes": ([vp, u32, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)],
+                                   i),
+        "alz_group_node_changes_device": ([vp, u32, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)],
+                                          i),
+        "alz_group_node_changes_top": ([vp, u32, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
+                                        C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_node_changes_top_device": ([vp, u32, u32, vp, u32, u32, u32, C.c_double, pp, C.POINTER(sz),
+                                               C.POINTER(abi.ChangeInfo)], i),
+        "alz_debug_group_edge_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
+                                               C.POINTER(abi.ChangeInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -239,7 +258,10 @@ def load(rebuild=False):
                   "alz_group_edges_device", "alz_group_edge_metrics", "alz_group_edge_metrics_device",
                   "alz_group_edge_top", "alz_group_edge_top_device", "alz_group_nodes", "alz_group_nodes_device",
                   "alz_group_node_metrics", "alz_group_node_metrics_device", "alz_group_node_top",
-                  "alz_group_node_top_device", "alz_debug_group_edges"):
+                  "alz_group_node_top_device", "alz_debug_group_edges", "alz_group_edge_changes",
+                  "alz_group_edge_changes_device", "alz_group_edge_changes_top", "alz_group_edge_changes_top_device",
+                  "alz_group_node_changes", "alz_group_node_changes_device", "alz_group_node_changes_top",
+                  "alz_group_node_changes_top_device", "alz_debug_group_edge_changes_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -1114,6 +1136,92 @@ class Handle:
                                  (C.c_void_p(ps), len(src), int(src_windows), C.c_void_p(pb), len(base),
                                   int(base_windows), int(side), abi.metrics(spec), int(mode), int(presence)),
                                  abi.NODE_CHANGE)
+        finally:
+            self.dev_free(ps)
+            self.dev_free(pb)
+
+    # ---- group changes against the pinned baseline (alz_group_changes.cu, docs/SPEC.md §25)
+    def group_edge_changes(self, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
+        """alz_group_edge_changes of the group edges of `source` against the pinned baseline's, both grouped by the
+        current map, by one metric: (EDGE_CHANGE records in ascending (from key, to key) order, info dict)."""
+        return self._changes("alz_group_edge_changes", (int(source), abi.metrics(spec), int(mode), int(presence)))
+
+    def group_edge_changes_device(self, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                  source=abi.SOURCE_WINDOW):
+        """alz_group_edge_changes_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_group_edge_changes_device(self.h, int(source), abi.metrics(spec), int(mode), int(presence),
+                                                      C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_group_edge_changes_device")
+        return p.value, n.value, info.as_dict()
+
+    def group_edge_changes_top(self, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                               source=abi.SOURCE_WINDOW):
+        """alz_group_edge_changes_top: (the first min(k, above) EDGE_CHANGE records by change, rank order; info
+        dict)."""
+        return self._changes("alz_group_edge_changes_top", (int(source), abi.metrics(spec), int(mode), int(presence),
+                                                            int(k), float(min_change)))
+
+    def group_edge_changes_top_device(self, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                      source=abi.SOURCE_WINDOW):
+        """alz_group_edge_changes_top_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_group_edge_changes_top_device(self.h, int(source), abi.metrics(spec), int(mode),
+                                                          int(presence), int(k), float(min_change), C.byref(p),
+                                                          C.byref(n), C.byref(info)),
+                 "alz_group_edge_changes_top_device")
+        return p.value, n.value, info.as_dict()
+
+    def group_node_changes(self, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                           source=abi.SOURCE_WINDOW):
+        """alz_group_node_changes of side `side` (abi.SIDE_*) of the group nodes of `source` against the pinned
+        baseline's by one metric: (NODE_CHANGE records in ascending node key order, info dict)."""
+        return self._changes("alz_group_node_changes", (int(source), int(side), abi.metrics(spec), int(mode),
+                                                        int(presence)), abi.NODE_CHANGE)
+
+    def group_node_changes_device(self, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                  source=abi.SOURCE_WINDOW):
+        """alz_group_node_changes_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_group_node_changes_device(self.h, int(source), int(side), abi.metrics(spec), int(mode),
+                                                      int(presence), C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_group_node_changes_device")
+        return p.value, n.value, info.as_dict()
+
+    def group_node_changes_top(self, side, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                               source=abi.SOURCE_WINDOW):
+        """alz_group_node_changes_top: (the first min(k, above) NODE_CHANGE records by change, rank order; info
+        dict)."""
+        return self._changes("alz_group_node_changes_top", (int(source), int(side), abi.metrics(spec), int(mode),
+                                                            int(presence), int(k), float(min_change)),
+                             abi.NODE_CHANGE)
+
+    def group_node_changes_top_device(self, side, spec, k, min_change=0.0, mode=abi.CHANGE_DELTA,
+                                      presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
+        """alz_group_node_changes_top_device: (device pointer, records, info dict)."""
+        p, n, info = C.c_void_p(), C.c_size_t(0), abi.ChangeInfo()
+        self._ck(self.L.alz_group_node_changes_top_device(self.h, int(source), int(side), abi.metrics(spec),
+                                                          int(mode), int(presence), int(k), float(min_change),
+                                                          C.byref(p), C.byref(n), C.byref(info)),
+                 "alz_group_node_changes_top_device")
+        return p.value, n.value, info.as_dict()
+
+    def debug_group_edge_changes_rows(self, src, base, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL,
+                                      src_windows=1, base_windows=1):
+        """alz_debug_group_edge_changes_rows over two host row arrays (copied to the device, any order, repeats
+        allowed) with the handle's map: (EDGE_CHANGE records, info dict)."""
+        src = np.ascontiguousarray(src, dtype=abi.EDGE_OUT)
+        base = np.ascontiguousarray(base, dtype=abi.EDGE_OUT)
+        ps = self.dev_alloc(max(src.nbytes, 1))
+        pb = self.dev_alloc(max(base.nbytes, 1))
+        try:
+            if len(src):
+                self.h2d(ps, src)
+            if len(base):
+                self.h2d(pb, base)
+            return self._changes("alz_debug_group_edge_changes_rows",
+                                 (C.c_void_p(ps), len(src), int(src_windows), C.c_void_p(pb), len(base),
+                                  int(base_windows), abi.metrics(spec), int(mode), int(presence)))
         finally:
             self.dev_free(ps)
             self.dev_free(pb)

@@ -268,6 +268,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_node_trends(h);
   alz_internal_free_node_changes(h);
   alz_internal_free_groups(h);
+  alz_internal_free_group_changes(h);
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);

@@ -13,12 +13,15 @@
 //   emit    one 48-byte record per listed row, and for the top call its change into an 8-byte array, which the §17
 //           selection ranks; the selected records are gathered by position
 // One host wait per call reads the union's counts; the top call's selection adds its own (alz_top.cu). The node
-// changes (alz_node_changes.cu) read the baseline through pinned_baseline and share change_of and the gather.
+// changes (alz_node_changes.cu) read the baseline through pinned_baseline and share change_of, the gather and the
+// list-or-top tail; the group changes (alz_group_changes.cu) run this join on (from node key, to node key) keys, the
+// 16-byte instantiation of the keys and match kernels, into buffers of their own.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <mutex>
 #include <string>
+#include <tuple>
 
 #include "alz_metrics.cuh"
 
@@ -32,18 +35,47 @@ namespace {
 constexpr uint32_t kAbsent = 0xFFFFFFFFu;
 constexpr uint32_t kMatched = 0x80000000u;   // in a lower bound: the other side holds the key (bounds are < 2^30)
 
-// the row's packed keys
+// A group-edge row's join key (docs/SPEC.md §25): the node keys of its from and to ends, compared in that order. A
+// pair of ends needs 70 bits (a 3-bit type and any 32-bit value each), so it does not pack into one word.
+struct __align__(16) EndsKey {
+  uint64_t from, to;
+};
+__device__ __forceinline__ bool operator==(const EndsKey& x, const EndsKey& y) { return x.from == y.from && x.to == y.to; }
+__device__ __forceinline__ bool operator<(const EndsKey& x, const EndsKey& y) {
+  return x.from < y.from || (x.from == y.from && x.to < y.to);
+}
+
+// a row's key: its packed key (§3), or its ends (from the 16-byte head: types, pad | from, to)
+template <class Key> __device__ __forceinline__ Key key_of(const alz_edge_out* r);
+template <> __device__ __forceinline__ uint64_t key_of<uint64_t>(const alz_edge_out* r) { return row_key_of(r); }
+template <> __device__ __forceinline__ EndsKey key_of<EndsKey>(const alz_edge_out* r) {
+  const uint2 ty = reinterpret_cast<const uint2*>(r)[0], ft = reinterpret_cast<const uint2*>(r)[1];
+  return EndsKey{node_key(ty.x & 0xFFu, ft.x), node_key((ty.x >> 8) & 0xFFu, ft.y)};
+}
+
+__device__ __forceinline__ uint32_t lower_bound_key(const uint64_t* __restrict__ a, uint32_t n, uint64_t k) {
+  return lower_bound_u64(a, n, k);
+}
+__device__ __forceinline__ uint32_t lower_bound_key(const EndsKey* __restrict__ a, uint32_t n, EndsKey k) {
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < k) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+
+// the rows' keys
+template <class Key>
 __global__ void __launch_bounds__(256) change_keys_kernel(const alz_edge_out* __restrict__ rows, uint32_t n,
-                                                          uint64_t* __restrict__ keys) {
+                                                          Key* __restrict__ keys) {
   const uint32_t stride = gridDim.x * blockDim.x;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) keys[i] = row_key_of(rows + i);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) keys[i] = key_of<Key>(rows + i);
 }
 
 // Thread t < n_a: source row t; t >= n_a: baseline row t - n_a. lb_*: the lower bound into the other side's keys, with
 // kMatched when that side holds the key; keep_*: the row is listed by its own thread (keep_*[n] = 0 closes each
 // scan); *both: the matched source rows.
-__global__ void __launch_bounds__(256) change_match_kernel(const uint64_t* __restrict__ ka, uint32_t n_a,
-                                                           const uint64_t* __restrict__ kb, uint32_t n_b,
+template <class Key>
+__global__ void __launch_bounds__(256) change_match_kernel(const Key* __restrict__ ka, uint32_t n_a,
+                                                           const Key* __restrict__ kb, uint32_t n_b,
                                                            uint32_t presence, uint32_t* __restrict__ lb_a,
                                                            uint32_t* __restrict__ lb_b, uint32_t* __restrict__ keep_a,
                                                            uint32_t* __restrict__ keep_b, uint32_t* __restrict__ both) {
@@ -52,16 +84,16 @@ __global__ void __launch_bounds__(256) change_match_kernel(const uint64_t* __res
   uint32_t matched = 0;
   for (uint32_t t = t0; t < n_a + n_b; t += stride) {
     if (t < n_a) {
-      const uint64_t key = ka[t];
-      const uint32_t p = lower_bound_u64(kb, n_b, key);
+      const Key key = ka[t];
+      const uint32_t p = lower_bound_key(kb, n_b, key);
       const bool m = p < n_b && kb[p] == key;
       lb_a[t] = p | (m ? kMatched : 0u);
       keep_a[t] = (presence & (m ? ALZ_PRESENT_BOTH : ALZ_PRESENT_NEW)) ? 1u : 0u;
       matched += m;
     } else {
       const uint32_t j = t - n_a;
-      const uint64_t key = kb[j];
-      const uint32_t p = lower_bound_u64(ka, n_a, key);
+      const Key key = kb[j];
+      const uint32_t p = lower_bound_key(ka, n_a, key);
       const bool m = p < n_a && ka[p] == key;
       lb_b[j] = p | (m ? kMatched : 0u);
       keep_b[j] = (!m && (presence & ALZ_PRESENT_GONE)) ? 1u : 0u;
@@ -139,15 +171,6 @@ __global__ void __launch_bounds__(256) change_gather_kernel(const uint32_t* __re
   }
 }
 
-// one side of a join: n rows in ascending key order, their keys (null: derived into the side's key buffer), and the
-// windows its values are divided by
-struct Side {
-  const alz_edge_out* rows;
-  const uint64_t* keys;
-  uint32_t n;
-  uint32_t windows;
-};
-
 }  // namespace
 
 // The pinned baseline and the buffers of the change calls, each grown on demand and never shrunk; freed in alz_destroy
@@ -155,20 +178,22 @@ struct alz_changes_state {
   DevBuf base_rows, base_keys;   // the baseline: its rows and their packed keys
   size_t base_n = 0;
   bool pinned = false;
-  uint64_t generation = 0;       // pins so far: tells the node changes' cached baseline nodes from a later pin's
+  uint64_t generation = 0;       // pins so far: tells the node and group changes' cached baseline from a later pin's
   alz_rollup_info base_info{};
-  DevBuf keys_a, keys_b;         // the sides' keys when derived
-  DevBuf lb_a, lb_b, keep_a, keep_b, scan_a, scan_b, val_a, val_b, both, tmp;   // the join's scratch
-  DevBuf list, chg, top_list;    // the results: the filtered union, its changes, the top records
-  Selection sel;                 // the top call's selection
+  ChangeBufs j;                  // the join's scratch and results
 };
+
+void alz::metrics::ChangeBufs::free() {
+  free_bufs({&keys_a, &keys_b, &member_a, &member_b, &lb_a, &lb_b, &keep_a, &keep_b, &scan_a, &scan_b, &val_a, &val_b,
+             &counts, &tmp, &list, &chg, &top_list});
+  sel.free();
+}
 
 void alz_internal_free_changes(alz_handle* h) {
   alz_changes_state* s = h->changes;
   if (!s) return;
-  free_bufs({&s->base_rows, &s->base_keys, &s->keys_a, &s->keys_b, &s->lb_a, &s->lb_b, &s->keep_a, &s->keep_b,
-             &s->scan_a, &s->scan_b, &s->val_a, &s->val_b, &s->both, &s->tmp, &s->list, &s->chg, &s->top_list});
-  s->sel.free();
+  free_bufs({&s->base_rows, &s->base_keys});
+  s->j.free();
   delete s;
   h->changes = nullptr;
 }
@@ -197,7 +222,8 @@ int alz::metrics::source_rows(alz_handle* h, uint32_t source, const alz_edge_out
 
 void alz::metrics::launch_row_keys(alz_handle* h, const alz_edge_out* rows, uint32_t n, uint64_t* keys) {
   if (n == 0) return;
-  change_keys_kernel<<<std::min<unsigned>((n + 255) / 256, (unsigned)h->sms * 8), 256, 0, h->stream>>>(rows, n, keys);
+  change_keys_kernel<uint64_t><<<std::min<unsigned>((n + 255) / 256, (unsigned)h->sms * 8), 256, 0, h->stream>>>(rows, n,
+                                                                                                        keys);
   h->launches += 1;
 }
 
@@ -226,47 +252,57 @@ template int alz::metrics::gather_changes(alz_handle*, const uint32_t*, uint32_t
 template int alz::metrics::gather_changes(alz_handle*, const uint32_t*, uint32_t, const alz_node_change*,
                                           alz_node_change*);
 
-namespace {
-
-// The join of a and b (docs/SPEC.md §18) into s->list, *listed records, and with top their changes into s->chg.
-// One wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
-int join(alz_handle* h, Side a, Side b, const MetricSet& ms, uint32_t mode, uint32_t presence, bool top,
-         uint64_t* listed, alz_change_info* ci) {
-  alz_changes_state* s = h->changes;
+int alz::metrics::edge_change_join(alz_handle* h, ChangeBufs& cb, EdgeChangeSide a, EdgeChangeSide b, bool ends,
+                                   const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
+                                   alz_change_info* ci) {
   cudaStream_t st = h->stream;
   const size_t na = a.n, nb = b.n;
-  int rc = reserve(h, {{&s->keys_a, a.keys ? 0 : std::max<size_t>(na, 1) * 8},
-                       {&s->keys_b, b.keys ? 0 : std::max<size_t>(nb, 1) * 8},
-                       {&s->lb_a, std::max<size_t>(na, 1) * 4},
-                       {&s->lb_b, std::max<size_t>(nb, 1) * 4},
-                       {&s->keep_a, (na + 1) * 4},
-                       {&s->keep_b, (nb + 1) * 4},
-                       {&s->scan_a, (na + 1) * 4},
-                       {&s->scan_b, (nb + 1) * 4},
-                       {&s->val_a, std::max<size_t>(na, 1) * 8},
-                       {&s->val_b, std::max<size_t>(nb, 1) * 8},
-                       {&s->both, 4},
-                       {&s->tmp, scan_temp_bytes((uint32_t)std::max(na, nb) + 1)}});
+  const size_t key_bytes = ends ? sizeof(EndsKey) : 8;
+  int rc = reserve(h, {{&cb.keys_a, a.keys ? 0 : std::max<size_t>(na, 1) * key_bytes},
+                       {&cb.keys_b, b.keys ? 0 : std::max<size_t>(nb, 1) * key_bytes},
+                       {&cb.lb_a, std::max<size_t>(na, 1) * 4},
+                       {&cb.lb_b, std::max<size_t>(nb, 1) * 4},
+                       {&cb.keep_a, (na + 1) * 4},
+                       {&cb.keep_b, (nb + 1) * 4},
+                       {&cb.scan_a, (na + 1) * 4},
+                       {&cb.scan_b, (nb + 1) * 4},
+                       {&cb.val_a, std::max<size_t>(na, 1) * 8},
+                       {&cb.val_b, std::max<size_t>(nb, 1) * 8},
+                       {&cb.counts, 4},
+                       {&cb.tmp, scan_temp_bytes((uint32_t)std::max(na, nb) + 1)}});
   if (rc != ALZ_OK) return rc;
-  if (!a.keys) { launch_row_keys(h, a.rows, a.n, static_cast<uint64_t*>(s->keys_a.p)); a.keys = static_cast<uint64_t*>(s->keys_a.p); }
-  if (!b.keys) { launch_row_keys(h, b.rows, b.n, static_cast<uint64_t*>(s->keys_b.p)); b.keys = static_cast<uint64_t*>(s->keys_b.p); }
-  uint32_t* lb_a = static_cast<uint32_t*>(s->lb_a.p);
-  uint32_t* lb_b = static_cast<uint32_t*>(s->lb_b.p);
-  uint32_t* keep_a = static_cast<uint32_t*>(s->keep_a.p);
-  uint32_t* keep_b = static_cast<uint32_t*>(s->keep_b.p);
-  uint32_t* scan_a = static_cast<uint32_t*>(s->scan_a.p);
-  uint32_t* scan_b = static_cast<uint32_t*>(s->scan_b.p);
-  uint32_t* both = static_cast<uint32_t*>(s->both.p);
+  uint32_t* lb_a = static_cast<uint32_t*>(cb.lb_a.p);
+  uint32_t* lb_b = static_cast<uint32_t*>(cb.lb_b.p);
+  uint32_t* keep_a = static_cast<uint32_t*>(cb.keep_a.p);
+  uint32_t* keep_b = static_cast<uint32_t*>(cb.keep_b.p);
+  uint32_t* scan_a = static_cast<uint32_t*>(cb.scan_a.p);
+  uint32_t* scan_b = static_cast<uint32_t*>(cb.scan_b.p);
+  uint32_t* both = static_cast<uint32_t*>(cb.counts.p);
   CK(cudaMemsetAsync(both, 0, 4, st));
   const uint32_t n_ab = a.n + b.n;   // each side is below 2^30
   const unsigned grid = std::max<unsigned>(1u, std::min<unsigned>((n_ab + 255) / 256, (unsigned)h->sms * 8));
-  change_match_kernel<<<grid, 256, 0, st>>>(a.keys, a.n, b.keys, b.n, presence, lb_a, lb_b, keep_a, keep_b, both);
+  if (ends) {
+    EndsKey* ka = static_cast<EndsKey*>(cb.keys_a.p);
+    EndsKey* kb = static_cast<EndsKey*>(cb.keys_b.p);
+    for (auto [rows, n, keys] : {std::make_tuple(a.rows, a.n, ka), std::make_tuple(b.rows, b.n, kb)}) {
+      if (n == 0) continue;
+      change_keys_kernel<EndsKey><<<std::min<unsigned>((n + 255) / 256, (unsigned)h->sms * 8), 256, 0, st>>>(rows, n,
+                                                                                                             keys);
+      h->launches += 1;
+    }
+    change_match_kernel<EndsKey><<<grid, 256, 0, st>>>(ka, a.n, kb, b.n, presence, lb_a, lb_b, keep_a, keep_b, both);
+  } else {
+    if (!a.keys) { launch_row_keys(h, a.rows, a.n, static_cast<uint64_t*>(cb.keys_a.p)); a.keys = static_cast<uint64_t*>(cb.keys_a.p); }
+    if (!b.keys) { launch_row_keys(h, b.rows, b.n, static_cast<uint64_t*>(cb.keys_b.p)); b.keys = static_cast<uint64_t*>(cb.keys_b.p); }
+    change_match_kernel<uint64_t><<<grid, 256, 0, st>>>(a.keys, a.n, b.keys, b.n, presence, lb_a, lb_b, keep_a,
+                                                        keep_b, both);
+  }
   h->launches += 1;
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, keep_a, scan_a, a.n + 1, st));
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, keep_b, scan_b, b.n + 1, st));
-  rc = run_metrics(h, a.rows, a.n, ms, static_cast<double*>(s->val_a.p));
+  CK(exclusive_scan_u32(cb.tmp.p, cb.tmp.bytes, keep_a, scan_a, a.n + 1, st));
+  CK(exclusive_scan_u32(cb.tmp.p, cb.tmp.bytes, keep_b, scan_b, b.n + 1, st));
+  rc = run_metrics(h, a.rows, a.n, ms, static_cast<double*>(cb.val_a.p));
   if (rc != ALZ_OK) return rc;
-  rc = run_metrics(h, b.rows, b.n, ms, static_cast<double*>(s->val_b.p));
+  rc = run_metrics(h, b.rows, b.n, ms, static_cast<double*>(cb.val_b.p));
   if (rc != ALZ_OK) return rc;
   CK(cudaGetLastError());
   uint32_t cnt[3];   // listed source rows, listed gone rows, matched source rows
@@ -286,24 +322,54 @@ int join(alz_handle* h, Side a, Side b, const MetricSet& ms, uint32_t mode, uint
   ci->base_windows = b.windows;
   *listed = ci->listed;
   if (na + nb - n_both > kMaxRows) return ALZ_E_CAPACITY;
-  rc = reserve(h, {{&s->list, std::max<size_t>(*listed, 1) * sizeof(alz_edge_change)},
-                   {&s->chg, top ? std::max<size_t>(*listed, 1) * 8 : 0}});
+  rc = reserve(h, {{&cb.list, std::max<size_t>(*listed, 1) * sizeof(alz_edge_change)},
+                   {&cb.chg, top ? std::max<size_t>(*listed, 1) * 8 : 0}});
   if (rc != ALZ_OK) return rc;
   if (*listed) {
     const bool divide = ms.kind[0] == ALZ_METRIC_COUNT || ms.kind[0] == ALZ_METRIC_ERR5XX;
     const EmitArgs ea{a.rows, b.rows, a.n, b.n, lb_a, lb_b, keep_a, keep_b, scan_a, scan_b,
-                      static_cast<const double*>(s->val_a.p), static_cast<const double*>(s->val_b.p),
+                      static_cast<const double*>(cb.val_a.p), static_cast<const double*>(cb.val_b.p),
                       (double)a.windows, (double)b.windows, divide, mode};
-    change_emit_kernel<<<grid, 256, 0, st>>>(ea, static_cast<alz_edge_change*>(s->list.p),
-                                             top ? static_cast<uint64_t*>(s->chg.p) : nullptr);
+    change_emit_kernel<<<grid, 256, 0, st>>>(ea, static_cast<alz_edge_change*>(cb.list.p),
+                                             top ? static_cast<uint64_t*>(cb.chg.p) : nullptr);
     h->launches += 1;
     CK(cudaGetLastError());
   }
   return ALZ_OK;
 }
 
-// The change list of `source` against the baseline (top: its first min(k, above) records by change) into s->list or
-// s->top_list; *n = records. Caller holds h->mu.
+template <class Record>
+int alz::metrics::change_results(alz_handle* h, ChangeBufs& cb, bool top, uint64_t listed, uint32_t k,
+                                 double min_change, const Record** res, size_t* n, alz_change_info* ci) {
+  if (!top) {
+    *res = static_cast<const Record*>(cb.list.p);
+    *n = listed;
+    return ALZ_OK;
+  }
+  size_t m = 0;
+  uint64_t above = 0;
+  int rc = select_top(h, cb.sel, static_cast<const uint64_t*>(cb.chg.p), (uint32_t)listed, k, min_change, nullptr,
+                      &m, &above);
+  if (rc != ALZ_OK) return rc;
+  ci->above = above;
+  rc = reserve(h, {{&cb.top_list, std::max<size_t>(m, 1) * sizeof(Record)}});
+  if (rc != ALZ_OK) return rc;
+  rc = gather_changes(h, static_cast<const uint32_t*>(cb.sel.top_index.p), (uint32_t)m,
+                      static_cast<const Record*>(cb.list.p), static_cast<Record*>(cb.top_list.p));
+  if (rc != ALZ_OK) return rc;
+  *res = static_cast<const Record*>(cb.top_list.p);
+  *n = m;
+  return ALZ_OK;
+}
+template int alz::metrics::change_results(alz_handle*, ChangeBufs&, bool, uint64_t, uint32_t, double,
+                                          const alz_edge_change**, size_t*, alz_change_info*);
+template int alz::metrics::change_results(alz_handle*, ChangeBufs&, bool, uint64_t, uint32_t, double,
+                                          const alz_node_change**, size_t*, alz_change_info*);
+
+namespace {
+
+// The change list of `source` against the baseline (top: its first min(k, above) records by change) into s->j.list or
+// s->j.top_list; *n = records. Caller holds h->mu.
 int changes_locked(alz_handle* h, uint32_t source, const MetricSet& ms, uint32_t mode, uint32_t presence, bool top,
                    uint32_t k, double min_change, const alz_edge_change** res, size_t* n, alz_change_info* ci) {
   CK(cudaSetDevice(h->device));
@@ -316,30 +382,13 @@ int changes_locked(alz_handle* h, uint32_t source, const MetricSet& ms, uint32_t
   if (!s || !s->pinned) return ALZ_E_STATE;
   if (n_src > kMaxRows || s->base_n > kMaxRows) return ALZ_E_CAPACITY;
   uint64_t listed = 0;
-  rc = join(h, Side{rows, nullptr, (uint32_t)n_src, ri.windows},
-            Side{static_cast<const alz_edge_out*>(s->base_rows.p), static_cast<const uint64_t*>(s->base_keys.p),
-                 (uint32_t)s->base_n, s->base_info.windows},
-            ms, mode, presence, top, &listed, ci);
+  rc = edge_change_join(h, s->j, EdgeChangeSide{rows, nullptr, (uint32_t)n_src, ri.windows},
+                        EdgeChangeSide{static_cast<const alz_edge_out*>(s->base_rows.p),
+                                       static_cast<const uint64_t*>(s->base_keys.p), (uint32_t)s->base_n,
+                                       s->base_info.windows},
+                        false, ms, mode, presence, top, &listed, ci);
   if (rc != ALZ_OK) return rc;
-  if (!top) {
-    *res = static_cast<const alz_edge_change*>(s->list.p);
-    *n = listed;
-    return ALZ_OK;
-  }
-  size_t m = 0;
-  uint64_t above = 0;
-  rc = select_top(h, s->sel, static_cast<const uint64_t*>(s->chg.p), (uint32_t)listed, k, min_change, nullptr, &m,
-                  &above);
-  if (rc != ALZ_OK) return rc;
-  ci->above = above;
-  rc = reserve(h, {{&s->top_list, std::max<size_t>(m, 1) * sizeof(alz_edge_change)}});
-  if (rc != ALZ_OK) return rc;
-  rc = gather_changes(h, static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)m,
-                      static_cast<const alz_edge_change*>(s->list.p), static_cast<alz_edge_change*>(s->top_list.p));
-  if (rc != ALZ_OK) return rc;
-  *res = static_cast<const alz_edge_change*>(s->top_list.p);
-  *n = m;
-  return ALZ_OK;
+  return change_results(h, s->j, top, listed, k, min_change, res, n, ci);
 }
 
 bool valid_change(const alz_metric* m, uint32_t mode, uint32_t presence, MetricSet* ms) {
@@ -462,13 +511,14 @@ extern "C" int alz_debug_edge_changes_rows(alz_handle* h, const alz_edge_out* de
   alz_changes_state* s = changes_state(h);
   uint64_t listed = 0;
   alz_change_info ci{};
-  const int rc = join(h, Side{dev_src, nullptr, (uint32_t)n_src, src_windows},
-                      Side{dev_base, nullptr, (uint32_t)n_base, base_windows}, ms, mode, presence, false, &listed, &ci);
+  const int rc = edge_change_join(h, s->j, EdgeChangeSide{dev_src, nullptr, (uint32_t)n_src, src_windows},
+                                  EdgeChangeSide{dev_base, nullptr, (uint32_t)n_base, base_windows}, false, ms, mode,
+                                  presence, false, &listed, &ci);
   if (info) *info = ci;
   if (rc != ALZ_OK) return rc;
   *n_out = listed;
   if (listed > cap) return ALZ_E_CAPACITY;
-  if (listed) CK(cudaMemcpyAsync(out, s->list.p, listed * sizeof(alz_edge_change), cudaMemcpyDeviceToHost, h->stream));
+  if (listed) CK(cudaMemcpyAsync(out, s->j.list.p, listed * sizeof(alz_edge_change), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }

@@ -296,6 +296,7 @@ __global__ void __launch_bounds__(kWarps * 32) group_reduce_kernel(const alz_edg
 struct alz_group_state {
   DevBuf map_keys, map_groups;   // the map: node keys ascending, each one's group
   uint32_t map_n = 0;
+  uint64_t map_gen = 0;          // successful alz_group_set calls: tells the group changes' cached baseline groups stale
   NodeGroup ends, edge_keys;     // the group-by of the mapped ends, then of the group-edge keys; ends also serves the
                                  // group nodes' group-by once the group edges are enqueued
   DevBuf end_idx, nkeys, ctr;    // each end's node index, each node's key, the ends kernel's two counters
@@ -339,15 +340,18 @@ uint32_t index_bits(uint64_t u) {
   return b;
 }
 
-// The group-edge rows of n rows into s->edges, on the stream after two waits: *n_out = their count, *info what §24
+}  // namespace
+
+// The group-edge rows of n rows into `out`, on the stream after two waits: *n_out = their count, *info what §24
 // reports. More than cap: ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device;
 // n <= kMaxNodeSourceRows.
-int group_edges(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_out, alz_group_info* info) {
+int alz::metrics::group_edges_into(alz_handle* h, DevBuf& out_buf, const alz_edge_out* rows, size_t n, size_t cap,
+                                   size_t* n_out, alz_group_info* info) {
   *n_out = 0;
   *info = alz_group_info{};
   info->source_rows = n;
   alz_group_state* s = state(h);
-  if (n == 0) return reserve(h, {{&s->edges, sizeof(alz_edge_out)}});
+  if (n == 0) return reserve(h, {{&out_buf, sizeof(alz_edge_out)}});
   if (!s->h_ctr) {
     void* p = nullptr;
     if (cudaMallocHost(&p, 2 * sizeof(uint64_t)) != cudaSuccess) {
@@ -391,9 +395,9 @@ int group_edges(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, s
   info->edges = edges;
   *n_out = edges;
   if (edges > cap) return ALZ_E_CAPACITY;
-  rc = reserve(h, {{&s->edges, edges * sizeof(alz_edge_out)}});
+  rc = reserve(h, {{&out_buf, edges * sizeof(alz_edge_out)}});
   if (rc != ALZ_OK) return rc;
-  alz_edge_out* out = static_cast<alz_edge_out*>(s->edges.p);
+  alz_edge_out* out = static_cast<alz_edge_out*>(out_buf.p);
   const uint64_t* keys = static_cast<const uint64_t*>(s->edge_keys.keys_out.p);
   const uint32_t* idx = static_cast<const uint32_t*>(s->edge_keys.idx.p);
   if (n1 > kBlockRows) {
@@ -407,6 +411,19 @@ int group_edges(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, s
   h->launches += 1;
   CK(cudaGetLastError());
   return ALZ_OK;
+}
+
+int alz::metrics::group_nodes_into(alz_handle* h, DevBuf& out, const alz_edge_out* edges, size_t n, size_t* n_nodes) {
+  return node_rows_of(h, state(h)->ends, out, edges, n, SIZE_MAX, n_nodes);
+}
+
+uint64_t alz::metrics::group_map_generation(const alz_handle* h) { return h->groups ? h->groups->map_gen : 0; }
+
+namespace {
+
+// The group-edge rows of n rows into s->edges (group_edges_into)
+int group_edges(alz_handle* h, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_out, alz_group_info* info) {
+  return group_edges_into(h, state(h)->edges, rows, n, cap, n_out, info);
 }
 
 // The rows of a source (node_source's rules) or of the hook's caller rows
@@ -575,6 +592,7 @@ int set_map(alz_handle* h, const alz_node_ends* nodes, const uint32_t* groups, s
   if (n == 0) {
     free_bufs({&s->map_keys, &s->map_groups});
     s->map_n = 0;
+    s->map_gen += 1;
     return ALZ_OK;
   }
   std::vector<uint64_t> keys(n);
@@ -622,6 +640,7 @@ int set_map(alz_handle* h, const alz_node_ends* nodes, const uint32_t* groups, s
   s->map_keys = k_out;
   s->map_groups = g_out;
   s->map_n = m;
+  s->map_gen += 1;
   return ALZ_OK;
 }
 

@@ -40,6 +40,7 @@ struct alz_node_state;    // alz_nodes.cu
 struct alz_node_series_state;   // alz_node_series.cu
 struct alz_node_changes_state;  // alz_node_changes.cu
 struct alz_group_state;         // alz_groups.cu
+struct alz_group_changes_state; // alz_group_changes.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -144,6 +145,8 @@ struct alz_handle {
                                                   // (alz_node_changes*); null until the first
   alz_group_state* groups = nullptr;      // the group map and the group calls' buffers (alz_group_*); null until the
                                           // first
+  alz_group_changes_state* group_changes = nullptr;   // the group changes' buffers and the baseline's groups
+                                                      // (alz_group_*_changes*); null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -199,4 +202,5 @@ void alz_internal_free_node_series(alz_handle* h);
 void alz_internal_free_node_trends(alz_handle* h);
 void alz_internal_free_node_changes(alz_handle* h);
 void alz_internal_free_groups(alz_handle* h);
+void alz_internal_free_group_changes(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -1,9 +1,10 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
 // (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
-// (alz_node_series.cu), the node changes (alz_node_changes.cu) and the groups (alz_groups.cu): the §17 metric values
-// of a row list, of node rows or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node
-// group-by, a source's edge or node series into given buffers, the 64-bit top selection with its own scratch, and the
-// pinned baseline with the §18 change arithmetic.
+// (alz_node_series.cu), the node changes (alz_node_changes.cu), the groups (alz_groups.cu) and the group changes
+// (alz_group_changes.cu): the §17 metric values of a row list, of node rows or of series slots, the rows' packed keys,
+// the grow-on-demand device buffers, the node group-by, a source's edge or node series into given buffers, the 64-bit
+// top selection with its own scratch, the pinned baseline with the §18 change arithmetic and the §18 and §23 joins
+// into given buffers, and the §24 group-by into given buffers.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -204,6 +205,56 @@ struct Selection {
 // null. *m_out results in s.top_index / s.top_values (/ s.top_rows), *above eligible values.
 int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,
                const alz_edge_out* rows, size_t* m_out, uint64_t* above);
+
+// The scratch and the results of change joins, grown on demand: the edge changes, the node changes and the group
+// changes (alz_group_changes.cu) each own one set, so none clobbers another's device results
+struct ChangeBufs {
+  DevBuf keys_a, keys_b, member_a, member_b;   // the sides' keys when derived; the node sides' membership
+  DevBuf lb_a, lb_b, keep_a, keep_b, scan_a, scan_b, val_a, val_b, counts, tmp;   // the join's scratch
+  DevBuf list, chg, top_list;                  // the results: the filtered union, its changes, the top records
+  Selection sel;                               // the top call's selection
+  void free();
+};
+// One side of an edge change join: n rows strictly ascending in the join's key, their packed keys (null: derived),
+// and the windows its values are divided by
+struct EdgeChangeSide {
+  const alz_edge_out* rows;
+  const uint64_t* keys;
+  uint32_t n;
+  uint32_t windows;
+};
+// The §18 join of a and b into b.list, *listed records, and with top their changes into b.chg. ends: the rows are
+// matched by (node key of from, node key of to), the §24 order, on keys derived here (a.keys and b.keys null); else
+// by packed key. One wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
+int edge_change_join(alz_handle* h, ChangeBufs& cb, EdgeChangeSide a, EdgeChangeSide b, bool ends,
+                     const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
+                     alz_change_info* ci);
+// One node list of a node change join: n node rows in ascending key order, and the windows its values are divided by
+struct NodeChangeSide {
+  const alz_node_out* nodes;
+  uint32_t n;
+  uint32_t windows;
+};
+// The §23 join of a and b on side `side` into cb.list, *listed records, and with top their changes into cb.chg. One
+// wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
+int node_change_join(alz_handle* h, ChangeBufs& cb, NodeChangeSide a, NodeChangeSide b, uint32_t side,
+                     const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
+                     alz_change_info* ci);
+// After a join into cb: the listed records in cb.list (top false), or the first min(k, above) of them by change
+// gathered into cb.top_list (top, ci->above set). *res, *n = the records. Caller holds h->mu.
+template <class Record>
+int change_results(alz_handle* h, ChangeBufs& cb, bool top, uint64_t listed, uint32_t k, double min_change,
+                   const Record** res, size_t* n, alz_change_info* ci);
+
+// The §24 group-edge rows of n rows under the handle's map into `out`, grown to hold them, with the group calls'
+// scratch (alz_groups.cu): two waits, then the reduce on the stream. *n_out = the rows; more than cap: ALZ_E_CAPACITY
+// before the reduce is enqueued. Caller holds h->mu and has set the device; n <= kMaxNodeSourceRows.
+int group_edges_into(alz_handle* h, DevBuf& out, const alz_edge_out* rows, size_t n, size_t cap, size_t* n_out,
+                     alz_group_info* info);
+// The §21 node rows of n group-edge rows into `out` with the group calls' scratch, as node_rows_of
+int group_nodes_into(alz_handle* h, DevBuf& out, const alz_edge_out* edges, size_t n, size_t* n_nodes);
+// The map's generation: every alz_group_set that succeeds moves it on (0 before the first)
+uint64_t group_map_generation(const alz_handle* h);
 
 }  // namespace metrics
 }  // namespace alz

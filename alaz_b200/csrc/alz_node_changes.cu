@@ -161,13 +161,6 @@ unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
   return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
 }
 
-// one node list of a join: n node rows in ascending key order, and the windows its values are divided by
-struct Side {
-  const alz_node_out* nodes;
-  uint32_t n;
-  uint32_t windows;
-};
-
 }  // namespace
 
 // Buffers of the node change calls, each grown on demand and never shrunk; freed in alz_destroy
@@ -177,21 +170,102 @@ struct alz_node_changes_state {
   size_t base_n = 0;               // base_nodes' rows
   bool base_cached = false;        // base_nodes hold the baseline of pin base_gen
   uint64_t base_gen = 0;
-  DevBuf keys_a, keys_b, member_a, member_b, lb_a, lb_b, keep_a, keep_b, scan_a, scan_b, val_a, val_b, counts, tmp;
-  DevBuf list, chg, top_list;      // the results: the filtered union, its changes, the top records
-  Selection sel;                   // the top call's selection
+  ChangeBufs j;                    // the join's scratch and results
 };
 
 void alz_internal_free_node_changes(alz_handle* h) {
   alz_node_changes_state* s = h->node_changes;
   if (!s) return;
   s->g.free();
-  free_bufs({&s->src_nodes, &s->base_nodes, &s->keys_a, &s->keys_b, &s->member_a, &s->member_b, &s->lb_a, &s->lb_b,
-             &s->keep_a, &s->keep_b, &s->scan_a, &s->scan_b, &s->val_a, &s->val_b, &s->counts, &s->tmp, &s->list,
-             &s->chg, &s->top_list});
-  s->sel.free();
+  free_bufs({&s->src_nodes, &s->base_nodes});
+  s->j.free();
   delete s;
   h->node_changes = nullptr;
+}
+
+int alz::metrics::node_change_join(alz_handle* h, ChangeBufs& cb, NodeChangeSide a, NodeChangeSide b, uint32_t side,
+                                   const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
+                                   alz_change_info* ci) {
+  cudaStream_t st = h->stream;
+  const size_t na = a.n, nb = b.n;
+  int rc = reserve(h, {{&cb.keys_a, std::max<size_t>(na, 1) * 8},
+                       {&cb.keys_b, std::max<size_t>(nb, 1) * 8},
+                       {&cb.member_a, std::max<size_t>(na, 1)},
+                       {&cb.member_b, std::max<size_t>(nb, 1)},
+                       {&cb.lb_a, std::max<size_t>(na, 1) * 4},
+                       {&cb.lb_b, std::max<size_t>(nb, 1) * 4},
+                       {&cb.keep_a, (na + 1) * 4},
+                       {&cb.keep_b, (nb + 1) * 4},
+                       {&cb.scan_a, (na + 1) * 4},
+                       {&cb.scan_b, (nb + 1) * 4},
+                       {&cb.val_a, std::max<size_t>(na, 1) * 8},
+                       {&cb.val_b, std::max<size_t>(nb, 1) * 8},
+                       {&cb.counts, 3 * 4},
+                       {&cb.tmp, scan_temp_bytes((uint32_t)std::max(na, nb) + 1)}});
+  if (rc != ALZ_OK) return rc;
+  uint64_t* keys_a = static_cast<uint64_t*>(cb.keys_a.p);
+  uint64_t* keys_b = static_cast<uint64_t*>(cb.keys_b.p);
+  uint8_t* member_a = static_cast<uint8_t*>(cb.member_a.p);
+  uint8_t* member_b = static_cast<uint8_t*>(cb.member_b.p);
+  uint32_t* lb_a = static_cast<uint32_t*>(cb.lb_a.p);
+  uint32_t* lb_b = static_cast<uint32_t*>(cb.lb_b.p);
+  uint32_t* keep_a = static_cast<uint32_t*>(cb.keep_a.p);
+  uint32_t* keep_b = static_cast<uint32_t*>(cb.keep_b.p);
+  uint32_t* scan_a = static_cast<uint32_t*>(cb.scan_a.p);
+  uint32_t* scan_b = static_cast<uint32_t*>(cb.scan_b.p);
+  uint32_t* counts = static_cast<uint32_t*>(cb.counts.p);   // members of a, members of b, matched members
+  CK(cudaMemsetAsync(counts, 0, 3 * 4, st));
+  if (na) {
+    node_change_keys_kernel<<<grid_for(h, na, 8), 256, 0, st>>>(a.nodes, a.n, side, keys_a, member_a, counts);
+    h->launches += 1;
+  }
+  if (nb) {
+    node_change_keys_kernel<<<grid_for(h, nb, 8), 256, 0, st>>>(b.nodes, b.n, side, keys_b, member_b, counts + 1);
+    h->launches += 1;
+  }
+  const uint32_t n_ab = a.n + b.n;   // each list is below 2^30
+  const unsigned grid = grid_for(h, n_ab, 8);
+  node_change_match_kernel<<<grid, 256, 0, st>>>(keys_a, member_a, a.n, keys_b, member_b, b.n, presence, lb_a, lb_b,
+                                                 keep_a, keep_b, counts + 2);
+  h->launches += 1;
+  CK(exclusive_scan_u32(cb.tmp.p, cb.tmp.bytes, keep_a, scan_a, a.n + 1, st));
+  CK(exclusive_scan_u32(cb.tmp.p, cb.tmp.bytes, keep_b, scan_b, b.n + 1, st));
+  rc = run_metrics_nodes(h, NodeRows{a.nodes, side}, a.n, ms, static_cast<double*>(cb.val_a.p));
+  if (rc != ALZ_OK) return rc;
+  rc = run_metrics_nodes(h, NodeRows{b.nodes, side}, b.n, ms, static_cast<double*>(cb.val_b.p));
+  if (rc != ALZ_OK) return rc;
+  CK(cudaGetLastError());
+  uint32_t cnt[5];   // listed source nodes, listed gone nodes, members of a, members of b, matched members
+  CK(cudaMemcpyAsync(&cnt[0], scan_a + a.n, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&cnt[1], scan_b + b.n, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&cnt[2], counts, 3 * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));   // the one wait: the union's counts
+  const uint64_t mem_a = cnt[2], mem_b = cnt[3], n_both = cnt[4];
+  *ci = alz_change_info{};
+  ci->source_rows = mem_a;
+  ci->base_rows = mem_b;
+  ci->both = n_both;
+  ci->added = mem_a - n_both;
+  ci->gone = mem_b - n_both;
+  ci->listed = (uint64_t)cnt[0] + cnt[1];
+  ci->source_windows = a.windows;
+  ci->base_windows = b.windows;
+  *listed = ci->listed;
+  if (mem_a + mem_b - n_both > kMaxRows) return ALZ_E_CAPACITY;
+  rc = reserve(h, {{&cb.list, std::max<size_t>(*listed, 1) * sizeof(alz_node_change)},
+                   {&cb.chg, top ? std::max<size_t>(*listed, 1) * 8 : 0}});
+  if (rc != ALZ_OK) return rc;
+  if (*listed) {
+    const bool divide = ms.kind[0] == ALZ_METRIC_COUNT || ms.kind[0] == ALZ_METRIC_ERR5XX;
+    const EmitArgs ea{a.nodes, b.nodes, a.n, b.n, lb_a, lb_b, keep_a, keep_b, scan_a, scan_b,
+                      static_cast<const double*>(cb.val_a.p), static_cast<const double*>(cb.val_b.p),
+                      (double)a.windows, (double)b.windows, divide, mode};
+    node_change_emit_kernel<<<grid, 256, 0, st>>>(ea, static_cast<alz_node_change*>(cb.list.p),
+                                                  top ? static_cast<uint64_t*>(cb.chg.p) : nullptr);
+    h->launches += 1;
+    CK(cudaGetLastError());
+  }
+  return ALZ_OK;
 }
 
 namespace {
@@ -213,95 +287,8 @@ int group(alz_handle* h, NodeGroup& g, DevBuf* out, const alz_edge_out* rows, si
   return node_group_reduce(h, g, rows, n2, static_cast<alz_node_out*>(out->p));
 }
 
-// The join of a and b on side `side` (docs/SPEC.md §23) into s->list, *listed records, and with top their changes
-// into s->chg. One wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
-int join(alz_handle* h, Side a, Side b, uint32_t side, const MetricSet& ms, uint32_t mode, uint32_t presence, bool top,
-         uint64_t* listed, alz_change_info* ci) {
-  alz_node_changes_state* s = h->node_changes;
-  cudaStream_t st = h->stream;
-  const size_t na = a.n, nb = b.n;
-  int rc = reserve(h, {{&s->keys_a, std::max<size_t>(na, 1) * 8},
-                       {&s->keys_b, std::max<size_t>(nb, 1) * 8},
-                       {&s->member_a, std::max<size_t>(na, 1)},
-                       {&s->member_b, std::max<size_t>(nb, 1)},
-                       {&s->lb_a, std::max<size_t>(na, 1) * 4},
-                       {&s->lb_b, std::max<size_t>(nb, 1) * 4},
-                       {&s->keep_a, (na + 1) * 4},
-                       {&s->keep_b, (nb + 1) * 4},
-                       {&s->scan_a, (na + 1) * 4},
-                       {&s->scan_b, (nb + 1) * 4},
-                       {&s->val_a, std::max<size_t>(na, 1) * 8},
-                       {&s->val_b, std::max<size_t>(nb, 1) * 8},
-                       {&s->counts, 3 * 4},
-                       {&s->tmp, scan_temp_bytes((uint32_t)std::max(na, nb) + 1)}});
-  if (rc != ALZ_OK) return rc;
-  uint64_t* keys_a = static_cast<uint64_t*>(s->keys_a.p);
-  uint64_t* keys_b = static_cast<uint64_t*>(s->keys_b.p);
-  uint8_t* member_a = static_cast<uint8_t*>(s->member_a.p);
-  uint8_t* member_b = static_cast<uint8_t*>(s->member_b.p);
-  uint32_t* lb_a = static_cast<uint32_t*>(s->lb_a.p);
-  uint32_t* lb_b = static_cast<uint32_t*>(s->lb_b.p);
-  uint32_t* keep_a = static_cast<uint32_t*>(s->keep_a.p);
-  uint32_t* keep_b = static_cast<uint32_t*>(s->keep_b.p);
-  uint32_t* scan_a = static_cast<uint32_t*>(s->scan_a.p);
-  uint32_t* scan_b = static_cast<uint32_t*>(s->scan_b.p);
-  uint32_t* counts = static_cast<uint32_t*>(s->counts.p);   // members of a, members of b, matched members
-  CK(cudaMemsetAsync(counts, 0, 3 * 4, st));
-  if (na) {
-    node_change_keys_kernel<<<grid_for(h, na, 8), 256, 0, st>>>(a.nodes, a.n, side, keys_a, member_a, counts);
-    h->launches += 1;
-  }
-  if (nb) {
-    node_change_keys_kernel<<<grid_for(h, nb, 8), 256, 0, st>>>(b.nodes, b.n, side, keys_b, member_b, counts + 1);
-    h->launches += 1;
-  }
-  const uint32_t n_ab = a.n + b.n;   // each list is below 2^30
-  const unsigned grid = grid_for(h, n_ab, 8);
-  node_change_match_kernel<<<grid, 256, 0, st>>>(keys_a, member_a, a.n, keys_b, member_b, b.n, presence, lb_a, lb_b,
-                                                 keep_a, keep_b, counts + 2);
-  h->launches += 1;
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, keep_a, scan_a, a.n + 1, st));
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, keep_b, scan_b, b.n + 1, st));
-  rc = run_metrics_nodes(h, NodeRows{a.nodes, side}, a.n, ms, static_cast<double*>(s->val_a.p));
-  if (rc != ALZ_OK) return rc;
-  rc = run_metrics_nodes(h, NodeRows{b.nodes, side}, b.n, ms, static_cast<double*>(s->val_b.p));
-  if (rc != ALZ_OK) return rc;
-  CK(cudaGetLastError());
-  uint32_t cnt[5];   // listed source nodes, listed gone nodes, members of a, members of b, matched members
-  CK(cudaMemcpyAsync(&cnt[0], scan_a + a.n, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&cnt[1], scan_b + b.n, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&cnt[2], counts, 3 * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));   // the one wait: the union's counts
-  const uint64_t mem_a = cnt[2], mem_b = cnt[3], n_both = cnt[4];
-  *ci = alz_change_info{};
-  ci->source_rows = mem_a;
-  ci->base_rows = mem_b;
-  ci->both = n_both;
-  ci->added = mem_a - n_both;
-  ci->gone = mem_b - n_both;
-  ci->listed = (uint64_t)cnt[0] + cnt[1];
-  ci->source_windows = a.windows;
-  ci->base_windows = b.windows;
-  *listed = ci->listed;
-  if (mem_a + mem_b - n_both > kMaxRows) return ALZ_E_CAPACITY;
-  rc = reserve(h, {{&s->list, std::max<size_t>(*listed, 1) * sizeof(alz_node_change)},
-                   {&s->chg, top ? std::max<size_t>(*listed, 1) * 8 : 0}});
-  if (rc != ALZ_OK) return rc;
-  if (*listed) {
-    const bool divide = ms.kind[0] == ALZ_METRIC_COUNT || ms.kind[0] == ALZ_METRIC_ERR5XX;
-    const EmitArgs ea{a.nodes, b.nodes, a.n, b.n, lb_a, lb_b, keep_a, keep_b, scan_a, scan_b,
-                      static_cast<const double*>(s->val_a.p), static_cast<const double*>(s->val_b.p),
-                      (double)a.windows, (double)b.windows, divide, mode};
-    node_change_emit_kernel<<<grid, 256, 0, st>>>(ea, static_cast<alz_node_change*>(s->list.p),
-                                                  top ? static_cast<uint64_t*>(s->chg.p) : nullptr);
-    h->launches += 1;
-    CK(cudaGetLastError());
-  }
-  return ALZ_OK;
-}
-
 // The node change list of `source` against the baseline (top: its first min(k, above) records by change) into
-// s->list or s->top_list; *n = records. Caller holds h->mu.
+// s->j.list or s->j.top_list; *n = records. Caller holds h->mu.
 int node_changes_locked(alz_handle* h, uint32_t source, uint32_t side, const MetricSet& ms, uint32_t mode,
                         uint32_t presence, bool top, uint32_t k, double min_change, const alz_node_change** res,
                         size_t* n, alz_change_info* ci) {
@@ -330,29 +317,13 @@ int node_changes_locked(alz_handle* h, uint32_t source, uint32_t side, const Met
     s->base_gen = gen;
   }
   uint64_t listed = 0;
-  rc = join(h, Side{static_cast<const alz_node_out*>(s->src_nodes.p), (uint32_t)nodes_a, ri.windows},
-            Side{static_cast<const alz_node_out*>(s->base_nodes.p), (uint32_t)s->base_n, bi.windows}, side, ms, mode,
-            presence, top, &listed, ci);
+  rc = node_change_join(h, s->j, NodeChangeSide{static_cast<const alz_node_out*>(s->src_nodes.p), (uint32_t)nodes_a,
+                                                 ri.windows},
+                        NodeChangeSide{static_cast<const alz_node_out*>(s->base_nodes.p), (uint32_t)s->base_n,
+                                       bi.windows},
+                        side, ms, mode, presence, top, &listed, ci);
   if (rc != ALZ_OK) return rc;
-  if (!top) {
-    *res = static_cast<const alz_node_change*>(s->list.p);
-    *n = listed;
-    return ALZ_OK;
-  }
-  size_t m = 0;
-  uint64_t above = 0;
-  rc = select_top(h, s->sel, static_cast<const uint64_t*>(s->chg.p), (uint32_t)listed, k, min_change, nullptr, &m,
-                  &above);
-  if (rc != ALZ_OK) return rc;
-  ci->above = above;
-  rc = reserve(h, {{&s->top_list, std::max<size_t>(m, 1) * sizeof(alz_node_change)}});
-  if (rc != ALZ_OK) return rc;
-  rc = gather_changes(h, static_cast<const uint32_t*>(s->sel.top_index.p), (uint32_t)m,
-                      static_cast<const alz_node_change*>(s->list.p), static_cast<alz_node_change*>(s->top_list.p));
-  if (rc != ALZ_OK) return rc;
-  *res = static_cast<const alz_node_change*>(s->top_list.p);
-  *n = m;
-  return ALZ_OK;
+  return change_results(h, s->j, top, listed, k, min_change, res, n, ci);
 }
 
 bool valid_node_change(uint32_t side, const alz_metric* m, uint32_t mode, uint32_t presence, MetricSet* ms) {
@@ -448,14 +419,17 @@ extern "C" int alz_debug_node_changes_rows(alz_handle* h, const alz_edge_out* de
   if (rc != ALZ_OK) return rc;
   uint64_t listed = 0;
   alz_change_info ci{};
-  rc = join(h, Side{static_cast<const alz_node_out*>(s->src_nodes.p), (uint32_t)nodes_a, src_windows},
-            Side{static_cast<const alz_node_out*>(s->base_nodes.p), (uint32_t)s->base_n, base_windows}, side, ms,
-            mode, presence, false, &listed, &ci);
+  rc = node_change_join(h, s->j,
+                        NodeChangeSide{static_cast<const alz_node_out*>(s->src_nodes.p), (uint32_t)nodes_a,
+                                       src_windows},
+                        NodeChangeSide{static_cast<const alz_node_out*>(s->base_nodes.p), (uint32_t)s->base_n,
+                                       base_windows},
+                        side, ms, mode, presence, false, &listed, &ci);
   if (info) *info = ci;
   if (rc != ALZ_OK) return rc;
   *n_out = listed;
   if (listed > cap) return ALZ_E_CAPACITY;
-  if (listed) CK(cudaMemcpyAsync(out, s->list.p, listed * sizeof(alz_node_change), cudaMemcpyDeviceToHost, h->stream));
+  if (listed) CK(cudaMemcpyAsync(out, s->j.list.p, listed * sizeof(alz_node_change), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return ALZ_OK;
 }

@@ -442,17 +442,22 @@ int Aggregator::Changes(uint32_t source, const alz_metric& metric, uint32_t mode
     rc = call(&n);
   }
   if (rc != ALZ_OK) return rc;
-  out->assign(n, EdgeChange{});
+  *out = ToChanges(changes_.data(), n);
+  return ALZ_OK;
+}
+
+std::vector<EdgeChange> Aggregator::ToChanges(const alz_edge_change* recs, size_t n) const {
+  std::vector<EdgeChange> out(n);
   for (size_t i = 0; i < n; ++i) {
-    const alz_edge_change& c = changes_[i];
+    const alz_edge_change& c = recs[i];
     alz_edge_out row{};
     row.from_type = c.from_type; row.to_type = c.to_type; row.from = c.from; row.to = c.to;
     const EdgeWindow w = ToEdges(&row, 1, nullptr)[0];
-    EdgeChange& e = (*out)[i];
+    EdgeChange& e = out[i];
     e.FromType = w.FromType; e.FromUID = w.FromUID; e.ToType = w.ToType; e.ToUID = w.ToUID;
     e.Presence = c.presence; e.Value = c.value; e.BaseValue = c.base_value; e.Change = c.change;
   }
-  return ALZ_OK;
+  return out;
 }
 
 bool Aggregator::EndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const {
@@ -671,15 +676,20 @@ int Aggregator::NodeChanges(uint32_t source, uint32_t side, const alz_metric& me
     rc = call(&n);
   }
   if (rc != ALZ_OK) return rc;
-  out->assign(n, NodeChange{});
+  *out = ToNodeChanges(node_changes_.data(), n);
+  return ALZ_OK;
+}
+
+std::vector<NodeChange> Aggregator::ToNodeChanges(const alz_node_change* recs, size_t n) const {
+  std::vector<NodeChange> out(n);
   for (size_t i = 0; i < n; ++i) {
-    const alz_node_change& c = node_changes_[i];
-    NodeChange& e = (*out)[i];
+    const alz_node_change& c = recs[i];
+    NodeChange& e = out[i];
     e.Type = NodeTypeName(c.type);
     e.UID = UidOf(c.type, c.node);
     e.Presence = c.presence; e.Value = c.value; e.BaseValue = c.base_value; e.Change = c.change;
   }
-  return ALZ_OK;
+  return out;
 }
 
 int Aggregator::TopNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
@@ -808,6 +818,58 @@ int Aggregator::TopGroupNodes(uint32_t source, uint32_t side, const alz_metric& 
   }
   if (rc != ALZ_OK) return rc;
   *out = ToNodes(nodes_.data(), n, node_values_.data(), 1);
+  return ALZ_OK;
+}
+
+int Aggregator::GroupChanges(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
+                             double min_change, std::vector<EdgeChange>* out, alz_change_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
+  auto call = [&](size_t* n) {
+    return k == 0 ? alz_group_edge_changes(h_, src, &metric, mode, presence, changes_.data(), changes_.size(), n, info)
+                  : alz_group_edge_changes_top(h_, src, &metric, mode, presence, k, min_change, changes_.data(),
+                                               changes_.size(), n, info);
+  };
+  size_t n = 0;
+  rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > changes_.size()) {
+    changes_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToChanges(changes_.data(), n);
+  return ALZ_OK;
+}
+
+int Aggregator::GroupNodeChanges(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t mode,
+                                 uint32_t presence, uint32_t k, double min_change, std::vector<NodeChange>* out,
+                                 alz_change_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // into node_changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
+  auto call = [&](size_t* n) {
+    return k == 0 ? alz_group_node_changes(h_, src, side, &metric, mode, presence, node_changes_.data(),
+                                           node_changes_.size(), n, info)
+                  : alz_group_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change,
+                                               node_changes_.data(), node_changes_.size(), n, info);
+  };
+  size_t n = 0;
+  rc = call(&n);
+  if (rc == ALZ_E_CAPACITY && n > node_changes_.size()) {
+    node_changes_.resize(n);
+    rc = call(&n);
+  }
+  if (rc != ALZ_OK) return rc;
+  *out = ToNodeChanges(node_changes_.data(), n);
   return ALZ_OK;
 }
 

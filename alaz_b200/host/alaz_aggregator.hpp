@@ -301,6 +301,18 @@ class Aggregator {
   // the k group nodes with the highest values of `metric` on side `side` >= min_value, as TopNodes ranks nodes
   int TopGroupNodes(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t k, double min_value,
                     std::vector<NodeWindow>* out, alz_top_info* info = nullptr);
+  // Group changes (docs/SPEC.md §25): Changes and NodeChanges over the group-edge rows and group nodes of `source` and
+  // of the baseline, both grouped by the map SetGroups gave, resolved by UID as for every group call: "what changed
+  // since the deploy, per deployment". A rolling deploy's pods are NEW and GONE under their own UIDs; their group is
+  // BOTH, with quantiles of the summed histograms on each side. GroupChanges names ends as GroupEdges does,
+  // GroupNodeChanges nodes as GroupNodes does. The map is the current one on both sides: a baseline pod stays
+  // resolvable by UID after its deletion through PinBaseline's hold, but a member dropped from the list since the pin
+  // no longer maps, and its baseline rows then show under the pod's own UID. info may be null. Returns 0 or an
+  // alz_status.
+  int GroupChanges(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
+                   double min_change, std::vector<EdgeChange>* out, alz_change_info* info = nullptr);
+  int GroupNodeChanges(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t mode, uint32_t presence,
+                       uint32_t k, double min_change, std::vector<NodeChange>* out, alz_change_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -322,6 +334,9 @@ class Aggregator {
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
   // the UID of an edge end or node (type, id) as the interners and the Host table hold it
   std::string UidOf(uint8_t type, uint32_t id) const;
+  // change records -> EdgeChange / NodeChange with the UIDs the interners and the group names hold
+  std::vector<EdgeChange> ToChanges(const alz_edge_change* recs, size_t n) const;
+  std::vector<NodeChange> ToNodeChanges(const alz_node_change* recs, size_t n) const;
   // node rows -> NodeWindow (values: nm per row, or null)
   std::vector<NodeWindow> ToNodes(const alz_node_out* rows, size_t n, const double* values, size_t nm) const;
   // the library's (type, id) of an edge end or node named by UID; false when the UID has no id

@@ -900,6 +900,57 @@ int alz_group_node_top_device(alz_handle* h, uint32_t source, uint32_t side, con
                               double min_value, const alz_node_out** dev_nodes, const double** dev_values,
                               const uint32_t** dev_index, size_t* n_out, alz_top_info* info);
 
+/* ---- group changes against a pinned baseline (docs/SPEC.md §25) -----------------------------------------------------
+ * §18 and §23 over groups: a source (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, availability rule of §15) against the baseline
+ * alz_baseline_pin holds, both sides grouped by the map in force at the call (§24; an empty map is allowed). Each side's
+ * group-edge rows are what alz_group_edges gives for a source holding that side's rows, and its group nodes what
+ * alz_group_nodes gives. Rows and nodes a rollout replaces (pods) are NEW and GONE; the groups they belong to are
+ * BOTH, with a quantile of the summed histograms on each side.
+ *
+ * Group edge changes: the union of the two group-edge lists, matched by (node key of from, node key of to), in that
+ * ascending order (§24), filtered by presence; index / base_index: the row's position in each side's group-edge list.
+ * Group node changes: §23 over the two group-node lists, with its side-membership rule; index / base_index: positions
+ * in each side's full group-node list, and a group node (type 4) sorts after every other type. value, base_value,
+ * change and the top calls' ranking and eligibility: as §18 (COUNT and ERR5XX per window, one rounding each).
+ * info->source_rows / base_rows count group-edge rows (edge calls) or member group nodes (node calls). Unknown metric,
+ * mode, side or source, presence 0 or above 7, k = 0, a NaN min_change or a null required pointer: ALZ_E_INVAL. No
+ * baseline, or no rows of a rollup source: ALZ_E_STATE. A side of more than 2^29 - 1 rows (before anything runs) or a
+ * union of more than 2^30 - 1 entries: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. *n_out is always set; a host call whose
+ * cap (in records) is below it returns ALZ_E_CAPACITY and writes nothing. info may be NULL.
+ *
+ * Reads only: the window, every ring, the open blocks, every rollup's rows, the baseline and the map are unchanged, and
+ * so are every other family's results (groups, edge and node changes, node, metric, top, series, trend, GNN), device
+ * pointers included. The baseline's group edges, and its group nodes once a node call needs them, are grouped on the
+ * first call that needs them and kept until the next pin or the next alz_group_set that succeeds. Device results stay
+ * valid until the next group change call. Every rank holds the same rows, map and baseline, so every rank gets the
+ * same result with no collective. */
+/* every listed group edge, in ascending (from key, to key) order */
+int alz_group_edge_changes(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                           alz_edge_change* out, size_t cap, size_t* n_out, alz_change_info* info);
+int alz_group_edge_changes_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode,
+                                  uint32_t presence, const alz_edge_change** dev_out, size_t* n_out,
+                                  alz_change_info* info);
+/* the first min(k, above) listed group edges by change, in rank order; info->above = the eligible ones */
+int alz_group_edge_changes_top(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode, uint32_t presence,
+                               uint32_t k, double min_change, alz_edge_change* out, size_t cap, size_t* n_out,
+                               alz_change_info* info);
+int alz_group_edge_changes_top_device(alz_handle* h, uint32_t source, const alz_metric* m, uint32_t mode,
+                                      uint32_t presence, uint32_t k, double min_change,
+                                      const alz_edge_change** dev_out, size_t* n_out, alz_change_info* info);
+/* every listed group node of side `side` (ALZ_SIDE_*), in ascending node key order */
+int alz_group_node_changes(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                           uint32_t presence, alz_node_change* out, size_t cap, size_t* n_out, alz_change_info* info);
+int alz_group_node_changes_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                                  uint32_t presence, const alz_node_change** dev_out, size_t* n_out,
+                                  alz_change_info* info);
+/* the first min(k, above) listed group nodes by change, in rank order; info->above = the eligible ones */
+int alz_group_node_changes_top(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m, uint32_t mode,
+                               uint32_t presence, uint32_t k, double min_change, alz_node_change* out, size_t cap,
+                               size_t* n_out, alz_change_info* info);
+int alz_group_node_changes_top_device(alz_handle* h, uint32_t source, uint32_t side, const alz_metric* m,
+                                      uint32_t mode, uint32_t presence, uint32_t k, double min_change,
+                                      const alz_node_change** dev_out, size_t* n_out, alz_change_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

@@ -70,6 +70,16 @@ int alz_debug_node_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size
  * rows, cells of 2^32 - 1); the rules of alz_group_edges otherwise. Uses the group calls' buffers. */
 int alz_debug_group_edges(alz_handle* h, const alz_edge_out* dev_rows, size_t n, alz_edge_out* out, size_t cap,
                           size_t* n_out, alz_group_info* info);
+/* test/debug: alz_group_edge_changes (docs/SPEC.md §25) between the group edges of two caller row lists in device
+ * memory under the handle's map, each in any order with repeats allowed and covering src_windows / base_windows (>= 1)
+ * windows, which may hold layouts ingest cannot make (ends whose node keys collide when packed into 64 bits, one group
+ * edge on 2^20 rows, cells of 2^32 - 1); the pinned baseline and its cached groups are neither used nor touched. More
+ * than 2^29 - 1 rows in a list: ALZ_E_CAPACITY. The rules of alz_group_edge_changes otherwise. Uses the group change
+ * calls' buffers. */
+int alz_debug_group_edge_changes_rows(alz_handle* h, const alz_edge_out* dev_src, size_t n_src, uint32_t src_windows,
+                                      const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows,
+                                      const alz_metric* m, uint32_t mode, uint32_t presence, alz_edge_change* out,
+                                      size_t cap, size_t* n_out, alz_change_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
