@@ -43,6 +43,12 @@ EXPORTS = [
     "alz_group_node_top_device", "alz_group_edge_changes", "alz_group_edge_changes_device",
     "alz_group_edge_changes_top", "alz_group_edge_changes_top_device", "alz_group_node_changes",
     "alz_group_node_changes_device", "alz_group_node_changes_top", "alz_group_node_changes_top_device",
+    "alz_group_edge_series", "alz_group_edge_series_device", "alz_group_edge_series_keys",
+    "alz_group_edge_series_keys_device", "alz_group_node_series", "alz_group_node_series_device",
+    "alz_group_node_series_keys", "alz_group_node_series_keys_device", "alz_group_edge_trends",
+    "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
+    "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
+    "alz_group_node_trends_top_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -207,6 +213,39 @@ def load(rebuild=False):
                                                C.POINTER(abi.ChangeInfo)], i),
         "alz_debug_group_edge_changes_rows": ([vp, vp, sz, u32, vp, sz, u32, vp, u32, u32, vp, sz, C.POINTER(sz),
                                                C.POINTER(abi.ChangeInfo)], i),
+        "alz_group_edge_series": ([vp, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                                   C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_edge_series_device": ([vp, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                          C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_edge_series_keys": ([vp, vp, sz, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                                        C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_edge_series_keys_device": ([vp, vp, sz, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32),
+                                               vp, C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_node_series": ([vp, u32, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+                                   C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_node_series_device": ([vp, u32, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                          C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_node_series_keys": ([vp, vp, sz, u32, u32, u32, vp, u32, vp, vp, sz, C.POINTER(sz), C.POINTER(u32),
+                                        vp, C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_node_series_keys_device": ([vp, vp, sz, u32, u32, u32, vp, u32, pp, pp, C.POINTER(sz),
+                                               C.POINTER(u32), vp, C.POINTER(abi.SeriesInfo)], i),
+        "alz_group_edge_trends": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), vp, sz, C.POINTER(sz), C.POINTER(u32),
+                                   vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_edge_trends_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), pp, C.POINTER(sz),
+                                          C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_edge_trends_top": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, vp, vp, vp, vp,
+                                       sz, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_edge_trends_top_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp, pp,
+                                              pp, pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_node_trends": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), vp, sz, C.POINTER(sz),
+                                   C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_node_trends_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), pp, C.POINTER(sz),
+                                          C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_node_trends_top": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, vp, vp, vp,
+                                       vp, sz, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.TrendInfo)], i),
+        "alz_group_node_trends_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp,
+                                              pp, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
+                                              C.POINTER(abi.TrendInfo)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -261,7 +300,13 @@ def load(rebuild=False):
                   "alz_group_node_top_device", "alz_debug_group_edges", "alz_group_edge_changes",
                   "alz_group_edge_changes_device", "alz_group_edge_changes_top", "alz_group_edge_changes_top_device",
                   "alz_group_node_changes", "alz_group_node_changes_device", "alz_group_node_changes_top",
-                  "alz_group_node_changes_top_device", "alz_debug_group_edge_changes_rows"):
+                  "alz_group_node_changes_top_device", "alz_debug_group_edge_changes_rows",
+                  "alz_group_edge_series", "alz_group_edge_series_device", "alz_group_edge_series_keys",
+                  "alz_group_edge_series_keys_device", "alz_group_node_series", "alz_group_node_series_device",
+                  "alz_group_node_series_keys", "alz_group_node_series_keys_device", "alz_group_edge_trends",
+                  "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
+                  "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
+                  "alz_group_node_trends_top_device"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -1225,6 +1270,95 @@ class Handle:
         finally:
             self.dev_free(ps)
             self.dev_free(pb)
+
+    # ---- group series and trends (alz_group_series.cu, alz_trends.cu, docs/SPEC.md §26)
+    def group_edge_series(self, source, tier, k, *specs):
+        """alz_group_edge_series: every group edge of `source` (alz_group_edges order) over the last k entries of
+        `tier`, each entry grouped by the map in force: (values [rows, P, nm], present [rows, P], points, info)."""
+        return self._series("alz_group_edge_series", (int(source),), (int(tier), int(k)), specs)
+
+    def group_edge_series_device(self, source, tier, k, *specs):
+        """alz_group_edge_series_device: (values and present device pointers, rows, P, points, info dict)."""
+        return self._series_device("alz_group_edge_series_device", (int(source),), (int(tier), int(k)), specs)
+
+    def group_edge_series_keys(self, edges, tier, k, *specs):
+        """alz_group_edge_series_keys: the caller's group edges (see edge_ends; a type may be abi.NODE_GROUP), in
+        their order: (values [n, P, nm], present [n, P], points, info dict)."""
+        keys = np.ascontiguousarray(self.edge_ends(edges))
+        return self._series("alz_group_edge_series_keys", (_ptr(keys), len(keys)), (int(tier), int(k)), specs)
+
+    def group_edge_series_keys_device(self, edges, tier, k, *specs):
+        """alz_group_edge_series_keys_device: (values and present device pointers, n, P, points, info dict)."""
+        keys = np.ascontiguousarray(self.edge_ends(edges))
+        return self._series_device("alz_group_edge_series_keys_device", (_ptr(keys), len(keys)), (int(tier), int(k)),
+                                   specs)
+
+    def group_node_series(self, source, side, tier, k, *specs):
+        """alz_group_node_series: every group node of `source` (alz_group_nodes order), side `side`: (values
+        [nodes, P, nm], present [nodes, P], points, info dict)."""
+        return self._series("alz_group_node_series", (int(source), int(side)), (int(tier), int(k)), specs)
+
+    def group_node_series_device(self, source, side, tier, k, *specs):
+        """alz_group_node_series_device: (values and present device pointers, nodes, P, points, info dict)."""
+        return self._series_device("alz_group_node_series_device", (int(source), int(side)), (int(tier), int(k)),
+                                   specs)
+
+    def group_node_series_keys(self, nodes, side, tier, k, *specs):
+        """alz_group_node_series_keys: the caller's nodes (see node_ends; a type may be abi.NODE_GROUP), in their
+        order: (values [n, P, nm], present [n, P], points, info dict)."""
+        keys = np.ascontiguousarray(self.node_ends(nodes))
+        return self._series("alz_group_node_series_keys", (_ptr(keys), len(keys), int(side)), (int(tier), int(k)),
+                            specs)
+
+    def group_node_series_keys_device(self, nodes, side, tier, k, *specs):
+        """alz_group_node_series_keys_device: (values and present device pointers, n, P, points, info dict)."""
+        keys = np.ascontiguousarray(self.node_ends(nodes))
+        return self._series_device("alz_group_node_series_keys_device", (_ptr(keys), len(keys), int(side)),
+                                   (int(tier), int(k)), specs)
+
+    def group_edge_trends(self, source, tier, k, spec, trend):
+        """alz_group_edge_trends: every group edge of `source` by one metric and an abi.Trend: (EDGE_TREND records in
+        alz_group_edges order, points, info dict)."""
+        return self._trends("alz_group_edge_trends", (int(source), int(tier)), k, spec, trend, abi.EDGE_TREND)
+
+    def group_edge_trends_device(self, source, tier, k, spec, trend):
+        """alz_group_edge_trends_device: (device pointer to the records, rows, P, points, info dict)."""
+        return self._trends_device("alz_group_edge_trends_device", (int(source), int(tier)), k, spec, trend)
+
+    def group_edge_trends_top(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_group_edge_trends_top: the first min(top, above) valid group edges by trend, rank order: (records,
+        EDGE_OUT group-edge rows, series [m, P], present [m, P], points, info dict)."""
+        return self._trends_top("alz_group_edge_trends_top", (int(source), int(tier)), k, spec, trend, top, min_trend,
+                                abi.EDGE_TREND, abi.EDGE_OUT)
+
+    def group_edge_trends_top_device(self, source, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_group_edge_trends_top_device: (records, rows, series and present device pointers, results, P, points,
+        info dict)."""
+        return self._trends_top_device("alz_group_edge_trends_top_device", (int(source), int(tier)), k, spec, trend,
+                                       top, min_trend)
+
+    def group_node_trends(self, source, side, tier, k, spec, trend):
+        """alz_group_node_trends: every group node of `source`, side `side`, by one metric and an abi.Trend:
+        (NODE_TREND records in alz_group_nodes order, points, info dict)."""
+        return self._trends("alz_group_node_trends", (int(source), int(side), int(tier)), k, spec, trend,
+                            abi.NODE_TREND)
+
+    def group_node_trends_device(self, source, side, tier, k, spec, trend):
+        """alz_group_node_trends_device: (device pointer to the records, nodes, P, points, info dict)."""
+        return self._trends_device("alz_group_node_trends_device", (int(source), int(side), int(tier)), k, spec,
+                                   trend)
+
+    def group_node_trends_top(self, source, side, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_group_node_trends_top: the first min(top, above) valid group nodes by trend, rank order: (records,
+        NODE_OUT rows, series [m, P], present [m, P], points, info dict)."""
+        return self._trends_top("alz_group_node_trends_top", (int(source), int(side), int(tier)), k, spec, trend, top,
+                                min_trend, abi.NODE_TREND, abi.NODE_OUT)
+
+    def group_node_trends_top_device(self, source, side, tier, k, spec, trend, top, min_trend=-np.inf):
+        """alz_group_node_trends_top_device: (records, node rows, series and present device pointers, results, P,
+        points, info dict)."""
+        return self._trends_top_device("alz_group_node_trends_top_device", (int(source), int(side), int(tier)), k,
+                                       spec, trend, top, min_trend)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -269,6 +269,8 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_node_changes(h);
   alz_internal_free_groups(h);
   alz_internal_free_group_changes(h);
+  alz_internal_free_group_series(h);
+  alz_internal_free_group_trends(h);
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);

@@ -41,7 +41,6 @@ constexpr uint32_t kWarpRows = 64;                     // sorted rows per warp
 constexpr uint32_t kBlockRows = kWarps * kWarpRows;    // sorted rows per block
 constexpr uint32_t kSlotWords = 3 + ALZ_NB / 2;        // a run's partial sums: the three u64 sums, 32 cell pairs
 constexpr uint32_t kMaxMap = (1u << 30) - 1u;          // map entries: the CUB item counts are ints
-constexpr uint64_t kGroupType = ALZ_NODE_GROUP;
 
 static_assert(sizeof(alz_group_info) == 32, "alz_group_info is four u64");
 static_assert(offsetof(alz_edge_out, count) == 16 && offsetof(alz_edge_out, hist) == 40 && sizeof(alz_edge_out) == 296,
@@ -57,21 +56,6 @@ __global__ void __launch_bounds__(256) map_dup_kernel(const uint64_t* __restrict
   const uint32_t stride = gridDim.x * blockDim.x;
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x + 1; j < n; j += stride)
     if (keys[j] == keys[j - 1]) *flag = 1u;
-}
-
-// the group node of a node key when the map holds it, the key itself otherwise
-__device__ __forceinline__ uint64_t map_end(uint64_t key, const uint64_t* __restrict__ mk,
-                                            const uint32_t* __restrict__ mg, uint32_t m, uint32_t* hit) {
-  uint32_t lo = 0, hi = m;
-  while (lo < hi) {
-    const uint32_t mid = (lo + hi) >> 1;
-    if (mk[mid] < key) lo = mid + 1; else hi = mid;
-  }
-  if (lo < m && mk[lo] == key) {
-    *hit += 1u;
-    return (kGroupType << 32) | mg[lo];
-  }
-  return key;
 }
 
 // Pair 2i + side: row i's mapped to end (IN) or from end (OUT) and its own position; ctr[0] += ends the map held,
@@ -418,6 +402,15 @@ int alz::metrics::group_nodes_into(alz_handle* h, DevBuf& out, const alz_edge_ou
 }
 
 uint64_t alz::metrics::group_map_generation(const alz_handle* h) { return h->groups ? h->groups->map_gen : 0; }
+
+GroupMap alz::metrics::group_map(const alz_handle* h) {
+  GroupMap m;
+  if (!h->groups) return m;
+  m.keys = static_cast<const uint64_t*>(h->groups->map_keys.p);
+  m.groups = static_cast<const uint32_t*>(h->groups->map_groups.p);
+  m.n = h->groups->map_n;
+  return m;
+}
 
 namespace {
 

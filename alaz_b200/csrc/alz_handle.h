@@ -41,6 +41,7 @@ struct alz_node_series_state;   // alz_node_series.cu
 struct alz_node_changes_state;  // alz_node_changes.cu
 struct alz_group_state;         // alz_groups.cu
 struct alz_group_changes_state; // alz_group_changes.cu
+struct alz_group_series_state;  // alz_group_series.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -147,6 +148,10 @@ struct alz_handle {
                                           // first
   alz_group_changes_state* group_changes = nullptr;   // the group changes' buffers and the baseline's groups
                                                       // (alz_group_*_changes*); null until the first
+  alz_group_series_state* group_series = nullptr;     // the group series' buffers (alz_group_*_series*); null until
+                                                      // the first
+  alz_trend_state* group_trends = nullptr;            // the group trends' buffers (alz_group_*_trends*); null until
+                                                      // the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -203,4 +208,6 @@ void alz_internal_free_node_trends(alz_handle* h);
 void alz_internal_free_node_changes(alz_handle* h);
 void alz_internal_free_groups(alz_handle* h);
 void alz_internal_free_group_changes(alz_handle* h);
+void alz_internal_free_group_series(alz_handle* h);
+void alz_internal_free_group_trends(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -1,10 +1,11 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
 // (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
-// (alz_node_series.cu), the node changes (alz_node_changes.cu), the groups (alz_groups.cu) and the group changes
-// (alz_group_changes.cu): the §17 metric values of a row list, of node rows or of series slots, the rows' packed keys,
-// the grow-on-demand device buffers, the node group-by, a source's edge or node series into given buffers, the 64-bit
-// top selection with its own scratch, the pinned baseline with the §18 change arithmetic and the §18 and §23 joins
-// into given buffers, and the §24 group-by into given buffers.
+// (alz_node_series.cu), the node changes (alz_node_changes.cu), the groups (alz_groups.cu), the group changes
+// (alz_group_changes.cu) and the group series (alz_group_series.cu): the §17 metric values of a row list, of node rows
+// or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node group-by, a source's edge,
+// node or group series into given buffers, the 64-bit top selection with its own scratch, the pinned baseline with the
+// §18 change arithmetic and the §18 and §23 joins into given buffers, the §24 group-by into given buffers and the map
+// lookup.
 #pragma once
 #include <cstdint>
 #include <initializer_list>
@@ -194,6 +195,68 @@ struct NodeSeriesBufs {
 int run_node_series_rows(alz_handle* h, NodeSeriesBufs& b, const alz_edge_out* rows, size_t n, uint32_t side,
                          uint32_t tier, uint32_t k, const MetricSet& ms, bool with_rows, size_t cap, size_t* n_out,
                          uint32_t* n_points, uint64_t* rows_in);
+
+// The group map (alz_groups.cu): n node keys ascending and each one's group
+struct GroupMap {
+  const uint64_t* keys = nullptr;
+  const uint32_t* groups = nullptr;
+  uint32_t n = 0;
+};
+GroupMap group_map(const alz_handle* h);
+#ifdef __CUDACC__
+// the group node of a node key when the map holds it, the key itself otherwise; *hit += 1 when it held it
+__device__ __forceinline__ uint64_t map_end(uint64_t key, const uint64_t* __restrict__ mk,
+                                            const uint32_t* __restrict__ mg, uint32_t m, uint32_t* hit) {
+  uint32_t lo = 0, hi = m;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (mk[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  if (lo < m && mk[lo] == key) {
+    *hit += 1u;
+    return ((uint64_t)ALZ_NODE_GROUP << 32) | mg[lo];
+  }
+  return key;
+}
+// map_end for callers that do not count the keys the map held
+__device__ __forceinline__ uint64_t map_end(uint64_t key, const uint64_t* __restrict__ mk,
+                                            const uint32_t* __restrict__ mg, uint32_t m) {
+  uint32_t held = 0;   // dropped: the compiler removes the count
+  return map_end(key, mk, mg, m, &held);
+}
+#endif
+
+// A node series whose entry rows' ends pass through the group map `map` before the lookup (group node series,
+// alz_group_series.cu): of the nodes of the n rows `rows` (by_source, as run_node_series_rows; the group-edge rows of a
+// source give its group nodes), or of the caller's n_keys keys (each already checked). *waited as run_node_series_rows'
+// waits happened after the ring's clocks were enqueued.
+int run_mapped_node_series(alz_handle* h, NodeSeriesBufs& b, bool by_source, const alz_edge_out* rows, size_t n,
+                           const alz_node_ends* keys, size_t n_keys, const GroupMap& map, uint32_t side,
+                           uint32_t tier, uint32_t k, const MetricSet& ms, bool with_rows, size_t cap, size_t* n_out,
+                           uint32_t* n_points, uint64_t* rows_in, bool* waited);
+// The entries of a ring view as one virtual row space: runs = first[P] then vbase[P + 1]; returns the entries' rows
+uint64_t entry_runs(const alz_ring_view& v, std::vector<uint32_t>* runs);
+// The slot group-by of a node series once its R pairs (slot key, 2 x arena row + side) are in b.g.keys_in /
+// b.g.vals_in, slot keys below n_slots and n_slots for a row that names no queried key, those counted in b.miss: one
+// node row per present slot into b.slot_rows and b.slot[slot key] = its row (the caller set b.slot to kSlotAbsent).
+// One wait. Caller holds h->mu and has set the device.
+int node_series_slots(alz_handle* h, NodeSeriesBufs& b, const alz_edge_out* arena, uint32_t R, uint64_t n_slots);
+
+// The buffers one group series fills (alz_group_series.cu): the source's group-edge rows and the series over them.
+// The group series calls own one set, the group trend calls (alz_trends.cu) another.
+struct GroupSeriesBufs {
+  NodeSeriesBufs s;   // the series (for group edges, keys holds 16-byte (from key, to key) pairs)
+  DevBuf edges;       // the source's §24 group-edge rows
+  void free();
+};
+// The group series of the n source rows `rows` into b (s.values / s.present), on the stream: nodes false, every group
+// edge of the rows (series rows in b.edges, *n_out of them); nodes true, every group node on side `side` (keys in
+// b.s.keys; with_rows: their node rows in b.s.src_rows). *n_points = P, *rows_in = the entries' rows. ALZ_E_CAPACITY
+// for more than 2^30 - 1 slots or series rows > cap. Caller holds h->mu and has set the device; n <=
+// kMaxNodeSourceRows.
+int run_group_series_rows(alz_handle* h, GroupSeriesBufs& b, const alz_edge_out* rows, size_t n, bool nodes,
+                          uint32_t side, uint32_t tier, uint32_t k, const MetricSet& ms, bool with_rows, size_t cap,
+                          size_t* n_out, uint32_t* n_points, uint64_t* rows_in);
 
 // The scratch and the results of one top selection over 64-bit values, grown on demand
 struct Selection {

@@ -33,7 +33,10 @@ static_assert(offsetof(alz_node_ends, value) == offsetof(alz_node_out, value), "
 namespace {
 
 // Thread t: row t of the entries' virtual row space (entry j holds arena rows [first[j], first[j] + vbase[j + 1] -
-// vbase[j]), n_rows = vbase[points]): its pair, and a warp-reduced count of the rows that name no queried node
+// vbase[j]), n_rows = vbase[points]): its pair, and a warp-reduced count of the rows that name no queried node.
+// kMapped: the row's end passes through the group map (mk, mg, m) first (group node series, alz_group_series.cu); the
+// map's arguments come last, so the unmapped kernel reads its arguments where it always did.
+template <bool kMapped>
 __global__ void __launch_bounds__(256) node_series_pairs_kernel(const alz_edge_out* __restrict__ arena,
                                                                 const uint32_t* __restrict__ first,
                                                                 const uint32_t* __restrict__ vbase, uint32_t points,
@@ -41,7 +44,9 @@ __global__ void __launch_bounds__(256) node_series_pairs_kernel(const alz_edge_o
                                                                 const uint64_t* __restrict__ keys, uint32_t n_keys,
                                                                 uint64_t* __restrict__ pair_keys,
                                                                 uint32_t* __restrict__ pair_vals,
-                                                                uint32_t* __restrict__ misses) {
+                                                                uint32_t* __restrict__ misses,
+                                                                const uint64_t* __restrict__ mk,
+                                                                const uint32_t* __restrict__ mg, uint32_t m) {
   const uint32_t stride = gridDim.x * blockDim.x;
   const uint64_t miss_key = (uint64_t)n_keys * points;
   uint32_t n_miss = 0;
@@ -54,7 +59,8 @@ __global__ void __launch_bounds__(256) node_series_pairs_kernel(const alz_edge_o
     const uint32_t row = first[lo] + (t - vbase[lo]);
     const uint2* r = reinterpret_cast<const uint2*>(arena + row);   // rows are 296 bytes apart: 8-byte aligned
     const uint2 ty = r[0], ft = r[1];                               // from_type, to_type, pad | from, to
-    const uint64_t key = side == ALZ_SIDE_IN ? node_key((ty.x >> 8) & 0xFFu, ft.y) : node_key(ty.x & 0xFFu, ft.x);
+    uint64_t key = side == ALZ_SIDE_IN ? node_key((ty.x >> 8) & 0xFFu, ft.y) : node_key(ty.x & 0xFFu, ft.x);
+    if (kMapped) key = map_end(key, mk, mg, m);
     const uint32_t u = lower_bound_u64(keys, n_keys, key);
     const bool hit = u < n_keys && keys[u] == key;
     pair_keys[t] = hit ? (uint64_t)u * points + lo : miss_key;
@@ -145,10 +151,11 @@ void caller_nodes(Nodes* q) {
 
 // The series of `q` over the last min(k, retained) entries of tier `tier` into b, on the stream: *n_out series rows,
 // *n_points = P, *rows_in entry rows read, *waited when the call has waited since the ring's clocks were enqueued.
-// n_out > cap: ALZ_E_CAPACITY before the entries are read. Caller holds h->mu and has set the device.
+// map: the entry rows' ends pass through it before the lookup (null: they do not). n_out > cap: ALZ_E_CAPACITY before
+// the entries are read. Caller holds h->mu and has set the device.
 int node_series_enqueue(alz_handle* h, NodeSeriesBufs& b, Nodes& q, uint32_t side, uint32_t tier, uint32_t k,
-                        const MetricSet& ms, bool with_rows, size_t cap, size_t* n_out, uint32_t* n_points,
-                        uint64_t* rows_in_out, bool* waited) {
+                        const MetricSet& ms, bool with_rows, size_t cap, const GroupMap* map, size_t* n_out,
+                        uint32_t* n_points, uint64_t* rows_in_out, bool* waited) {
   *waited = false;
   int rc = alz_internal_ring_view(h, tier, k, &b.view);
   if (rc != ALZ_OK) return rc;
@@ -174,14 +181,8 @@ int node_series_enqueue(alz_handle* h, NodeSeriesBufs& b, Nodes& q, uint32_t sid
   if (!q.by_source) caller_nodes(&q);   // sorted once the sizes are known to fit
   const size_t n_keys = q.by_source ? n : q.keys.size();
   const size_t slots = n * P;
-  uint64_t rows_in = 0;
-  std::vector<uint32_t> runs(2 * (size_t)P + 1);   // first[P], vbase[P + 1]
-  for (uint32_t j = 0; j < P; ++j) {
-    runs[j] = (uint32_t)v.first_row[j];   // arena rows are below 2^31
-    runs[P + j] = (uint32_t)rows_in;      // entries do not overlap: their rows add up to at most the arena's
-    rows_in += v.n[j];
-  }
-  runs[2 * (size_t)P] = (uint32_t)rows_in;
+  std::vector<uint32_t> runs;
+  const uint64_t rows_in = entry_runs(v, &runs);
   *rows_in_out = rows_in;
   rc = reserve(h, {{&b.keys, std::max<size_t>(n_keys, 1) * 8},
                    {&b.map, q.by_source ? 0 : std::max<size_t>(n, 1) * 4},
@@ -220,27 +221,19 @@ int node_series_enqueue(alz_handle* h, NodeSeriesBufs& b, Nodes& q, uint32_t sid
     if (rc != ALZ_OK) return rc;
     uint32_t* d_miss = static_cast<uint32_t*>(b.miss.p);
     CK(cudaMemsetAsync(d_miss, 0, 4, st));
-    node_series_pairs_kernel<<<grid_for(h, R, 8), 256, 0, st>>>(
-        v.arena, d_runs, d_runs + P, P, R, side, d_keys, (uint32_t)n_keys, static_cast<uint64_t*>(g.keys_in.p),
-        static_cast<uint32_t*>(g.vals_in.p), d_miss);
+    uint64_t* pk = static_cast<uint64_t*>(g.keys_in.p);
+    uint32_t* pv = static_cast<uint32_t*>(g.vals_in.p);
+    if (map)
+      node_series_pairs_kernel<true><<<grid_for(h, R, 8), 256, 0, st>>>(
+          v.arena, d_runs, d_runs + P, P, R, side, d_keys, (uint32_t)n_keys, pk, pv, d_miss, map->keys, map->groups,
+          map->n);
+    else
+      node_series_pairs_kernel<false><<<grid_for(h, R, 8), 256, 0, st>>>(
+          v.arena, d_runs, d_runs + P, P, R, side, d_keys, (uint32_t)n_keys, pk, pv, d_miss, nullptr, nullptr, 0);
     h->launches += 1;
-    CK(cudaMemcpyAsync(g.h_words + 1, d_miss, 4, cudaMemcpyDeviceToHost, st));   // read after the runs' wait
-    rc = node_group_runs(h, g, R, key_bits_of((uint64_t)n_keys * P));
+    rc = node_series_slots(h, b, v.arena, R, (uint64_t)n_keys * P);
     if (rc != ALZ_OK) return rc;
     *waited = true;
-    const uint32_t misses = g.h_words[1];
-    const uint32_t present = g.h_words[0] - (misses ? 1u : 0u), hits = R - misses;
-    rc = reserve(h, {{&b.slot_rows, (size_t)present * sizeof(alz_node_out)}});
-    if (rc != ALZ_OK) return rc;
-    if (hits) {
-      rc = node_group_reduce(h, g, v.arena, hits, static_cast<alz_node_out*>(b.slot_rows.p));
-      if (rc != ALZ_OK) return rc;
-      node_slot_kernel<<<grid_for(h, hits, 8), 256, 0, st>>>(static_cast<const uint64_t*>(g.keys_out.p),
-                                                             static_cast<const uint32_t*>(g.heads.p),
-                                                             static_cast<const uint32_t*>(g.idx.p), hits, d_slot);
-      h->launches += 1;
-      CK(cudaGetLastError());
-    }
   }
   const NodeSeriesRows sr{static_cast<const alz_node_out*>(b.slot_rows.p), d_slot,
                           q.by_source ? nullptr : static_cast<const uint32_t*>(b.map.p), P, side,
@@ -285,8 +278,8 @@ int series_entry(alz_handle* h, bool by_source, uint32_t source, const alz_node_
   NodeSeriesBufs& b = h->node_series->b;
   uint64_t rows_in = 0;
   bool waited = false;
-  const int rc = node_series_enqueue(h, b, q, side, tier, k, ms, false, device ? SIZE_MAX : cap, n_out, n_points,
-                                     &rows_in, &waited);
+  const int rc = node_series_enqueue(h, b, q, side, tier, k, ms, false, device ? SIZE_MAX : cap, nullptr, n_out,
+                                     n_points, &rows_in, &waited);
   if (rc != ALZ_OK) return rc;
   const size_t slots = *n_out * *n_points;
   if (info) {
@@ -315,6 +308,56 @@ int series_entry(alz_handle* h, bool by_source, uint32_t source, const alz_node_
 
 }  // namespace
 
+uint64_t alz::metrics::entry_runs(const alz_ring_view& v, std::vector<uint32_t>* runs) {
+  const uint32_t P = (uint32_t)v.n.size();
+  runs->assign(2 * (size_t)P + 1, 0u);   // first[P], vbase[P + 1]
+  uint64_t rows_in = 0;
+  for (uint32_t j = 0; j < P; ++j) {
+    (*runs)[j] = (uint32_t)v.first_row[j];   // arena rows are below 2^31
+    (*runs)[P + j] = (uint32_t)rows_in;      // entries do not overlap: their rows add up to at most the arena's
+    rows_in += v.n[j];
+  }
+  (*runs)[2 * (size_t)P] = (uint32_t)rows_in;
+  return rows_in;
+}
+
+int alz::metrics::node_series_slots(alz_handle* h, NodeSeriesBufs& b, const alz_edge_out* arena, uint32_t R,
+                                    uint64_t n_slots) {
+  NodeGroup& g = b.g;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(g.h_words + 1, b.miss.p, 4, cudaMemcpyDeviceToHost, h->stream));   // read after the runs' wait
+  int rc = node_group_runs(h, g, R, key_bits_of(n_slots));
+  if (rc != ALZ_OK) return rc;
+  const uint32_t misses = g.h_words[1];
+  const uint32_t present = g.h_words[0] - (misses ? 1u : 0u), hits = R - misses;
+  rc = reserve(h, {{&b.slot_rows, (size_t)present * sizeof(alz_node_out)}});
+  if (rc != ALZ_OK) return rc;
+  if (!hits) return ALZ_OK;
+  rc = node_group_reduce(h, g, arena, hits, static_cast<alz_node_out*>(b.slot_rows.p));
+  if (rc != ALZ_OK) return rc;
+  node_slot_kernel<<<grid_for(h, hits, 8), 256, 0, h->stream>>>(static_cast<const uint64_t*>(g.keys_out.p),
+                                                                static_cast<const uint32_t*>(g.heads.p),
+                                                                static_cast<const uint32_t*>(g.idx.p), hits,
+                                                                static_cast<uint32_t*>(b.slot.p));
+  h->launches += 1;
+  CK(cudaGetLastError());
+  return ALZ_OK;
+}
+
+int alz::metrics::run_mapped_node_series(alz_handle* h, NodeSeriesBufs& b, bool by_source, const alz_edge_out* rows,
+                                         size_t n, const alz_node_ends* keys, size_t n_keys, const GroupMap& map,
+                                         uint32_t side, uint32_t tier, uint32_t k, const MetricSet& ms,
+                                         bool with_rows, size_t cap, size_t* n_out, uint32_t* n_points,
+                                         uint64_t* rows_in, bool* waited) {
+  Nodes q;
+  q.by_source = by_source;
+  q.rows = rows;
+  q.n_rows = n;
+  q.ends = keys;
+  q.n = by_source ? 0 : n_keys;
+  return node_series_enqueue(h, b, q, side, tier, k, ms, with_rows, cap, &map, n_out, n_points, rows_in, waited);
+}
+
 int alz::metrics::run_node_series_rows(alz_handle* h, NodeSeriesBufs& b, const alz_edge_out* rows, size_t n,
                                        uint32_t side, uint32_t tier, uint32_t k, const MetricSet& ms, bool with_rows,
                                        size_t cap, size_t* n_out, uint32_t* n_points, uint64_t* rows_in) {
@@ -323,7 +366,7 @@ int alz::metrics::run_node_series_rows(alz_handle* h, NodeSeriesBufs& b, const a
   q.rows = rows;
   q.n_rows = n;
   bool waited = false;
-  return node_series_enqueue(h, b, q, side, tier, k, ms, with_rows, cap, n_out, n_points, rows_in, &waited);
+  return node_series_enqueue(h, b, q, side, tier, k, ms, with_rows, cap, nullptr, n_out, n_points, rows_in, &waited);
 }
 
 extern "C" int alz_node_series(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,

@@ -1,9 +1,12 @@
 // alz_trends.cu — edge trends (docs/SPEC.md §20): one statistic per source row over its §19 series of one metric,
-// and the top rows by it with their series; node trends (§22): the same per source node over its node series.
+// and the top rows by it with their series; node trends (§22): the same per source node over its node series; group
+// trends (§26): the same per group edge or group node of the source over its group series.
 //
 //   series  the §19 path (alz_series.cu: keys, match, the §17 metric kernels over the slots) with nm = 1, into the
 //           trend state's own SeriesBufs, so a trend call leaves the series calls' device results alone; for nodes
-//           the §22 path (alz_node_series.cu) into the node trend state's own NodeSeriesBufs
+//           the §22 path (alz_node_series.cu) into the node trend state's own NodeSeriesBufs; for groups the §26
+//           path (alz_group_series.cu) into the group trend state's own GroupSeriesBufs, whose group-edge rows are the
+//           edge records' heads and the selection's rows
 //   trend   one thread per series row walks its P values and presence bytes in the SPEC's order: the sums of the
 //           used, recent and earlier points, then a second pass for Sxy / Sxx or the squared deviations. It writes
 //           the 48-byte record and, for a top call, an 8-byte selection value: the trend's bits for a valid row, all
@@ -196,10 +199,12 @@ __global__ void __launch_bounds__(256) trend_gather_kernel(const uint32_t* __res
 }  // namespace
 
 // Buffers of the trend calls, each grown on demand and never shrunk; freed in alz_destroy. The edge trend calls own
-// one (h->trends), the node trend calls another (h->node_trends), each using its own series buffers.
+// one (h->trends), the node trend calls another (h->node_trends), the group trend calls a third (h->group_trends), each
+// using its own series buffers.
 struct alz_trend_state {
   SeriesBufs ser;                      // edges: the series of the source's rows, one metric
   NodeSeriesBufs nser;                 // nodes: the series of the source's nodes, one metric, and their node rows
+  GroupSeriesBufs gser;                // groups: the source's group-edge rows and their or their group nodes' series
   DevBuf rec, sel_val, valid_cnt;      // the records, the selection values, the valid count
   DevBuf top_rec, top_values, top_present, top_nodes;   // the top call's records, series and node rows
   Selection sel;                       // the top call's selection (and, for edges, its gathered source rows)
@@ -212,6 +217,7 @@ void free_trend_state(alz_trend_state*& s) {
   if (!s) return;
   s->ser.free();
   s->nser.free();
+  s->gser.free();
   free_bufs({&s->rec, &s->sel_val, &s->valid_cnt, &s->top_rec, &s->top_values, &s->top_present, &s->top_nodes});
   s->sel.free();
   if (s->h_valid) cudaFreeHost(s->h_valid);
@@ -223,11 +229,12 @@ void free_trend_state(alz_trend_state*& s) {
 
 void alz_internal_free_trends(alz_handle* h) { free_trend_state(h->trends); }
 void alz_internal_free_node_trends(alz_handle* h) { free_trend_state(h->node_trends); }
+void alz_internal_free_group_trends(alz_handle* h) { free_trend_state(h->group_trends); }
 
 namespace {
 
 struct TrendCall {
-  bool device = false, top = false, node = false;
+  bool device = false, top = false, node = false, group = false;
   uint32_t source = 0, side = 0, tier = 0, k = 0, n_top = 0;
   double min_trend = 0.0;
   MetricSet ms{};
@@ -252,7 +259,7 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
   CK(cudaSetDevice(h->device));
   const alz_edge_out* rows = h->d_out;
   size_t n = h->last_n_edges;
-  if (c.node) {
+  if (c.node || c.group) {
     const int rc = node_source(h, c.source, &rows, &n);
     if (rc != ALZ_OK) return rc;
   } else {
@@ -262,13 +269,14 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
     }
     if (n > kMaxRows) return ALZ_E_CAPACITY;
   }
-  alz_trend_state*& sp = c.node ? h->node_trends : h->trends;
+  alz_trend_state*& sp = c.group ? h->group_trends : c.node ? h->node_trends : h->trends;
   if (!sp) sp = new alz_trend_state();
   alz_trend_state* s = sp;
   if (!s->h_valid) {
     void* p = nullptr;
     if (cudaMallocHost(&p, sizeof(uint32_t)) != cudaSuccess) {
-      h->last_err = std::string(c.node ? "node trends: " : "edge trends: ") + cudaGetErrorString(cudaGetLastError());
+      h->last_err = std::string(c.group ? "group trends: " : c.node ? "node trends: " : "edge trends: ") +
+                    cudaGetErrorString(cudaGetLastError());
       return ALZ_E_NOMEM;
     }
     s->h_valid = static_cast<uint32_t*>(p);
@@ -276,15 +284,19 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
   size_t n_rows = 0;   // series rows: the source's rows, or its nodes
   uint64_t rows_in = 0;
   const size_t room = c.top ? SIZE_MAX : cap;
-  int rc = c.node ? run_node_series_rows(h, s->nser, rows, n, c.side, c.tier, c.k, c.ms, c.top, room, &n_rows,
-                                         n_points, &rows_in)
-                  : run_series_rows(h, s->ser, rows, n, c.tier, c.k, c.ms, room, &n_rows, n_points, &rows_in);
+  int rc = c.group  ? run_group_series_rows(h, s->gser, rows, n, c.node, c.side, c.tier, c.k, c.ms, c.top, room,
+                                             &n_rows, n_points, &rows_in)
+           : c.node ? run_node_series_rows(h, s->nser, rows, n, c.side, c.tier, c.k, c.ms, c.top, room, &n_rows,
+                                           n_points, &rows_in)
+                    : run_series_rows(h, s->ser, rows, n, c.tier, c.k, c.ms, room, &n_rows, n_points, &rows_in);
   res->m = c.top ? 0 : n_rows;
   if (rc != ALZ_OK) return rc;
   const uint32_t P = *n_points;
   const size_t N = n_rows;
-  const double* values = static_cast<const double*>(c.node ? s->nser.values.p : s->ser.values.p);
-  const uint8_t* present = static_cast<const uint8_t*>(c.node ? s->nser.present.p : s->ser.present.p);
+  const NodeSeriesBufs& nser = c.group ? s->gser.s : s->nser;   // node or group series
+  if (c.group && !c.node) rows = static_cast<const alz_edge_out*>(s->gser.edges.p);   // the series rows
+  const double* values = static_cast<const double*>(c.node || c.group ? nser.values.p : s->ser.values.p);
+  const uint8_t* present = static_cast<const uint8_t*>(c.node || c.group ? nser.present.p : s->ser.present.p);
   rc = reserve(h, {{&s->rec, std::max<size_t>(N, 1) * sizeof(alz_edge_trend)},
                    {&s->sel_val, c.top ? std::max<size_t>(N, 1) * 8 : 0},
                    {&s->valid_cnt, 4}});
@@ -299,7 +311,7 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
     const unsigned grid = std::min<unsigned>((unsigned)((N + 255) / 256), (unsigned)h->sms * 8);
     uint64_t* sel = c.top ? static_cast<uint64_t*>(s->sel_val.p) : nullptr;
     if (c.node)
-      trend_kernel<<<grid, 256, 0, st>>>(ta, NodeHead{static_cast<const uint64_t*>(s->nser.keys.p)}, d_rec, sel,
+      trend_kernel<<<grid, 256, 0, st>>>(ta, NodeHead{static_cast<const uint64_t*>(nser.keys.p)}, d_rec, sel,
                                          d_valid);
     else
       trend_kernel<<<grid, 256, 0, st>>>(ta, EdgeHead{rows}, d_rec, sel, d_valid);
@@ -329,7 +341,7 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
       h->launches += 1;
       CK(cudaGetLastError());
       if (c.node) {
-        rc = node_gather(h, top_index, (uint32_t)m, static_cast<const alz_node_out*>(s->nser.src_rows.p),
+        rc = node_gather(h, top_index, (uint32_t)m, static_cast<const alz_node_out*>(nser.src_rows.p),
                          static_cast<alz_node_out*>(s->top_nodes.p));
         if (rc != ALZ_OK) return rc;
       }
@@ -442,6 +454,14 @@ TrendCall node_call_of(bool device, bool top, uint32_t source, uint32_t side, ui
   return c;
 }
 
+TrendCall group_call_of(bool node, bool device, bool top, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                        uint32_t n_top, double min_trend) {
+  TrendCall c = node ? node_call_of(device, top, source, side, tier, k, n_top, min_trend)
+                     : call_of(device, top, source, tier, k, n_top, min_trend);
+  c.group = true;
+  return c;
+}
+
 }  // namespace
 
 extern "C" int alz_edge_trends(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
@@ -507,4 +527,75 @@ extern "C" int alz_node_trends_top_device(alz_handle* h, uint32_t source, uint32
                                           uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info) {
   return trends_device(h, node_call_of(true, true, source, side, tier, k, top, min_trend), m, t, dev_out, dev_nodes,
                        dev_series, dev_present, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_edge_trends(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                     const alz_trend* t, alz_edge_trend* out, size_t cap, size_t* n_out,
+                                     uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info) {
+  return trends_entry(h, group_call_of(false, false, false, source, 0, tier, k, 0, 0.0), m, t, out, nullptr, nullptr,
+                      nullptr, cap, nullptr, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_edge_trends_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k,
+                                            const alz_metric* m, const alz_trend* t, const alz_edge_trend** dev_out,
+                                            size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                                            alz_trend_info* info) {
+  return trends_device<alz_edge_trend, alz_edge_out>(h, group_call_of(false, true, false, source, 0, tier, k, 0, 0.0),
+                                                     m, t, dev_out, nullptr, nullptr, nullptr, n_out, n_points, points,
+                                                     info);
+}
+
+extern "C" int alz_group_edge_trends_top(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k,
+                                         const alz_metric* m, const alz_trend* t, uint32_t top, double min_trend,
+                                         alz_edge_trend* out, alz_edge_out* rows, double* series, uint8_t* present,
+                                         size_t cap, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                                         alz_trend_info* info) {
+  return trends_entry(h, group_call_of(false, false, true, source, 0, tier, k, top, min_trend), m, t, out, rows,
+                      series, present, cap, nullptr, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_edge_trends_top_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k,
+                                                const alz_metric* m, const alz_trend* t, uint32_t top,
+                                                double min_trend, const alz_edge_trend** dev_out,
+                                                const alz_edge_out** dev_rows, const double** dev_series,
+                                                const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                                alz_rollup_info* points, alz_trend_info* info) {
+  return trends_device(h, group_call_of(false, true, true, source, 0, tier, k, top, min_trend), m, t, dev_out,
+                       dev_rows, dev_series, dev_present, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_node_trends(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                     const alz_metric* m, const alz_trend* t, alz_node_trend* out, size_t cap,
+                                     size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                                     alz_trend_info* info) {
+  return trends_entry(h, group_call_of(true, false, false, source, side, tier, k, 0, 0.0), m, t, out, nullptr,
+                      nullptr, nullptr, cap, nullptr, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_node_trends_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                            const alz_metric* m, const alz_trend* t, const alz_node_trend** dev_out,
+                                            size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                                            alz_trend_info* info) {
+  return trends_device<alz_node_trend, alz_node_out>(
+      h, group_call_of(true, true, false, source, side, tier, k, 0, 0.0), m, t, dev_out, nullptr, nullptr, nullptr,
+      n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_node_trends_top(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                         const alz_metric* m, const alz_trend* t, uint32_t top, double min_trend,
+                                         alz_node_trend* out, alz_node_out* nodes, double* series, uint8_t* present,
+                                         size_t cap, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                                         alz_trend_info* info) {
+  return trends_entry(h, group_call_of(true, false, true, source, side, tier, k, top, min_trend), m, t, out, nodes,
+                      series, present, cap, nullptr, n_out, n_points, points, info);
+}
+
+extern "C" int alz_group_node_trends_top_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier,
+                                                uint32_t k, const alz_metric* m, const alz_trend* t, uint32_t top,
+                                                double min_trend, const alz_node_trend** dev_out,
+                                                const alz_node_out** dev_nodes, const double** dev_series,
+                                                const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                                alz_rollup_info* points, alz_trend_info* info) {
+  return trends_device(h, group_call_of(true, true, true, source, side, tier, k, top, min_trend), m, t, dev_out,
+                       dev_nodes, dev_series, dev_present, n_out, n_points, points, info);
 }

@@ -582,20 +582,26 @@ int Aggregator::Trends(uint32_t source, uint32_t tier, uint32_t k, const alz_met
   if (!h_) return ALZ_E_STATE;
   if (!out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(mu_);
+  return RunEdgeTrends(alz_edge_trends_top, source, tier, k, metric, trend, top, min_trend, out, points);
+}
+
+int Aggregator::RunEdgeTrends(EdgeTrendsTop fn, uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                              const alz_trend& trend, uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+                              std::vector<alz_rollup_info>* points) {
   const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
   // a first call sizes the results (ALZ_E_CAPACITY with n = the results, P = the points; nothing written)
   size_t n = 0;
   uint32_t P = 0;
-  int rc = alz_edge_trends_top(h_, src, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr, nullptr,
-                               0, &n, &P, nullptr, nullptr);
+  int rc = fn(h_, src, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr, nullptr, 0, &n, &P,
+              nullptr, nullptr);
   std::vector<alz_rollup_info> pts(P);
   if (rc == ALZ_E_CAPACITY && n > 0) {
     trends_.resize(n);
     trend_rows_.resize(n);
     trend_values_.resize(n * P);
     trend_present_.resize(n * P);
-    rc = alz_edge_trends_top(h_, src, tier, k, &metric, &trend, top, min_trend, trends_.data(), trend_rows_.data(),
-                             trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
+    rc = fn(h_, src, tier, k, &metric, &trend, top, min_trend, trends_.data(), trend_rows_.data(),
+            trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
   }
   if (rc != ALZ_OK) return rc;
   const std::vector<EdgeWindow> names = ToEdges(trend_rows_.data(), n, nullptr);
@@ -943,21 +949,26 @@ int Aggregator::NodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32
   if (!h_) return ALZ_E_STATE;
   if (!out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(mu_);
+  return RunNodeTrends(alz_node_trends_top, source, side, tier, k, metric, trend, top, min_trend, out, points);
+}
+
+int Aggregator::RunNodeTrends(NodeTrendsTop fn, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                              const alz_metric& metric, const alz_trend& trend, uint32_t top, double min_trend,
+                              std::vector<NodeTrend>* out, std::vector<alz_rollup_info>* points) {
   const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
   // a first call sizes the results (ALZ_E_CAPACITY with n = the results, P = the points; nothing written)
   size_t n = 0;
   uint32_t P = 0;
-  int rc = alz_node_trends_top(h_, src, side, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr,
-                               nullptr, 0, &n, &P, nullptr, nullptr);
+  int rc = fn(h_, src, side, tier, k, &metric, &trend, top, min_trend, nullptr, nullptr, nullptr, nullptr, 0, &n,
+              &P, nullptr, nullptr);
   std::vector<alz_rollup_info> pts(P);
   if (rc == ALZ_E_CAPACITY && n > 0) {
     node_trends_.resize(n);
     node_trend_rows_.resize(n);
     trend_values_.resize(n * P);
     trend_present_.resize(n * P);
-    rc = alz_node_trends_top(h_, src, side, tier, k, &metric, &trend, top, min_trend, node_trends_.data(),
-                             node_trend_rows_.data(), trend_values_.data(), trend_present_.data(), n, &n, &P,
-                             pts.data(), nullptr);
+    rc = fn(h_, src, side, tier, k, &metric, &trend, top, min_trend, node_trends_.data(), node_trend_rows_.data(),
+            trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
   }
   if (rc != ALZ_OK) return rc;
   const std::vector<NodeWindow> names = ToNodes(node_trend_rows_.data(), n, nullptr, 0);
@@ -974,6 +985,177 @@ int Aggregator::NodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32
   }
   if (points) *points = pts;
   return ALZ_OK;
+}
+
+bool Aggregator::GroupEndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const {
+  if (type != "group") return EndOf(type, uid, t, v);
+  const auto it = group_ids_.find(uid);
+  if (it == group_ids_.end()) return false;
+  *t = ALZ_NODE_GROUP;
+  *v = it->second;
+  return true;
+}
+
+int Aggregator::GroupSeries(uint32_t source, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                            std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const uint32_t nm = (uint32_t)metrics.size();
+  rc = RunSeries(nm, out, points, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                      alz_rollup_info* pts) {
+    return alz_group_edge_series(h_, src, tier, k, metrics.data(), nm, v, p, cap, n, P, pts, nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  // the names: the source's group-edge rows, in the same order
+  const size_t n = out->size();
+  if (n == 0) return ALZ_OK;
+  roll_.resize(n);
+  size_t m = 0;
+  rc = alz_group_edges(h_, src, roll_.data(), n, &m, nullptr);
+  if (rc != ALZ_OK) return rc;
+  if (m != n) return ALZ_E_STATE;
+  const std::vector<EdgeWindow> names = ToEdges(roll_.data(), n, nullptr);
+  for (size_t i = 0; i < n; ++i) {
+    EdgeSeries& e = (*out)[i];
+    e.FromType = names[i].FromType; e.FromUID = names[i].FromUID; e.ToType = names[i].ToType; e.ToUID = names[i].ToUID;
+  }
+  return ALZ_OK;
+}
+
+int Aggregator::GroupSeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint32_t k,
+                               const std::vector<alz_metric>& metrics, std::vector<EdgeSeries>* out,
+                               std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  // the edges whose ends resolve go to the library; the others are absent at every point
+  std::vector<alz_edge_ends> keys;
+  std::vector<size_t> row_of;   // edge -> row of keys, or SIZE_MAX
+  for (const EdgeRef& e : edges) {
+    alz_edge_ends k_{};
+    if (GroupEndOf(e.FromType, e.FromUID, &k_.from_type, &k_.from) &&
+        GroupEndOf(e.ToType, e.ToUID, &k_.to_type, &k_.to)) {
+      row_of.push_back(keys.size());
+      keys.push_back(k_);
+    } else {
+      row_of.push_back(SIZE_MAX);
+    }
+  }
+  const uint32_t nm = (uint32_t)metrics.size();
+  std::vector<EdgeSeries> known;
+  std::vector<alz_rollup_info> pts;
+  rc = RunSeries(nm, &known, &pts, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                       alz_rollup_info* pp) {
+    return alz_group_edge_series_keys(h_, keys.data(), keys.size(), tier, k, metrics.data(), nm, v, p, cap, n, P, pp,
+                                      nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  const size_t P = pts.size();
+  out->assign(edges.size(), EdgeSeries{});
+  for (size_t i = 0; i < edges.size(); ++i) {
+    EdgeSeries& e = (*out)[i];
+    if (row_of[i] != SIZE_MAX) e = known[row_of[i]];
+    else { e.Present.assign(P, 0); e.Values.assign(P * nm, 0.0); }
+    e.FromType = edges[i].FromType; e.FromUID = edges[i].FromUID; e.ToType = edges[i].ToType; e.ToUID = edges[i].ToUID;
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::GroupNodeSeries(uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                                std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const uint32_t nm = (uint32_t)metrics.size();
+  rc = RunSeries(nm, out, points, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                      alz_rollup_info* pts) {
+    return alz_group_node_series(h_, src, side, tier, k, metrics.data(), nm, v, p, cap, n, P, pts, nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  // the names: the source's group nodes, in the same node order
+  const size_t n = out->size();
+  if (n == 0) return ALZ_OK;
+  nodes_.resize(n);
+  size_t m = 0;
+  rc = alz_group_nodes(h_, src, nodes_.data(), n, &m);
+  if (rc != ALZ_OK) return rc;
+  if (m != n) return ALZ_E_STATE;
+  for (size_t i = 0; i < n; ++i) {
+    (*out)[i].Type = NodeTypeName(nodes_[i].type);
+    (*out)[i].UID = UidOf(nodes_[i].type, nodes_[i].value);
+  }
+  return ALZ_OK;
+}
+
+int Aggregator::GroupNodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
+                                   const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                                   std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  // the nodes that resolve go to the library; the others are absent at every point
+  std::vector<alz_node_ends> keys;
+  std::vector<size_t> row_of;   // node -> row of keys, or SIZE_MAX
+  for (const NodeRef& r : nodes) {
+    alz_node_ends k_{};
+    if (GroupEndOf(r.Type, r.UID, &k_.type, &k_.value)) { row_of.push_back(keys.size()); keys.push_back(k_); }
+    else row_of.push_back(SIZE_MAX);
+  }
+  const uint32_t nm = (uint32_t)metrics.size();
+  std::vector<NodeSeriesRow> known;
+  std::vector<alz_rollup_info> pts;
+  rc = RunSeries(nm, &known, &pts, [&](double* v, uint8_t* p, size_t cap, size_t* n, uint32_t* P,
+                                       alz_rollup_info* pp) {
+    return alz_group_node_series_keys(h_, keys.data(), keys.size(), side, tier, k, metrics.data(), nm, v, p, cap, n,
+                                      P, pp, nullptr);
+  });
+  if (rc != ALZ_OK) return rc;
+  const size_t P = pts.size();
+  out->assign(nodes.size(), NodeSeriesRow{});
+  for (size_t i = 0; i < nodes.size(); ++i) {
+    NodeSeriesRow& e = (*out)[i];
+    if (row_of[i] != SIZE_MAX) e = known[row_of[i]];
+    else { e.Present.assign(P, 0); e.Values.assign(P * nm, 0.0); }
+    e.Type = nodes[i].Type;
+    e.UID = nodes[i].UID;
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::GroupTrends(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                            const alz_trend& trend, uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+                            std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunEdgeTrends(alz_group_edge_trends_top, source, tier, k, metric, trend, top, min_trend, out, points);
+}
+
+int Aggregator::GroupNodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                                const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
+                                std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunNodeTrends(alz_group_node_trends_top, source, side, tier, k, metric, trend, top, min_trend, out, points);
 }
 
 int Aggregator::SetHistory(uint32_t depth, uint64_t arena_rows, const std::vector<alz_history_tier>& tiers) {

@@ -313,6 +313,31 @@ class Aggregator {
                    double min_change, std::vector<EdgeChange>* out, alz_change_info* info = nullptr);
   int GroupNodeChanges(uint32_t source, uint32_t side, const alz_metric& metric, uint32_t mode, uint32_t presence,
                        uint32_t k, double min_change, std::vector<NodeChange>* out, alz_change_info* info = nullptr);
+  // Group series and trends (docs/SPEC.md §26): Series, SeriesFor, NodeSeries, NodeSeriesFor, Trends and NodeTrends
+  // over groups, with every retained entry grouped by the map SetGroups gave, resolved by UID as for every group call:
+  // "what was deployment checkout's inbound p99, minute by minute", "which deployments are getting worse". GroupSeries
+  // and GroupTrends name ends as GroupEdges does, GroupNodeSeries and GroupNodeTrends nodes as GroupNodes does. In the
+  // For forms a ref of Type "group" names a group by the name SetGroups gave it; a name SetGroups never gave, like a
+  // UID with no id, is absent at every point. The map is the current one for every point: a rolled-out pod keeps
+  // contributing to its deployment's earlier points only while it stays in the member list, and SetHistory's hold
+  // keeps its id resolvable for as long as a retained entry carries it. *points (may be null) as in Series. Returns 0
+  // or an alz_status.
+  int GroupSeries(uint32_t source, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                  std::vector<EdgeSeries>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int GroupSeriesFor(const std::vector<EdgeRef>& edges, uint32_t tier, uint32_t k,
+                     const std::vector<alz_metric>& metrics, std::vector<EdgeSeries>* out,
+                     std::vector<alz_rollup_info>* points = nullptr);
+  int GroupNodeSeries(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const std::vector<alz_metric>& metrics,
+                      std::vector<NodeSeriesRow>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int GroupNodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
+                         const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
+                         std::vector<alz_rollup_info>* points = nullptr);
+  int GroupTrends(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_trend& trend,
+                  uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+                  std::vector<alz_rollup_info>* points = nullptr);
+  int GroupNodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                      const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
+                      std::vector<alz_rollup_info>* points = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -341,12 +366,28 @@ class Aggregator {
   std::vector<NodeWindow> ToNodes(const alz_node_out* rows, size_t n, const double* values, size_t nm) const;
   // the library's (type, id) of an edge end or node named by UID; false when the UID has no id
   bool EndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const;
+  // EndOf, and a group (Type "group") by the name SetGroups gave it; false for a name it never gave
+  bool GroupEndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const;
   // ends -> the library's key of an edge named by UID; false when a UID has no id
   bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
   // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then each series
   // row's Present and Values in *out (EdgeSeries or NodeSeriesRow; the names are the caller's); requires mu_
   template <class Row, class Call>
   int RunSeries(size_t nm, std::vector<Row>* out, std::vector<alz_rollup_info>* points, Call call);
+  // the edge trends_top call `fn` (alz_edge_trends_top, alz_group_edge_trends_top) into trends_ and its rows named,
+  // and the node one (alz_node_trends_top, alz_group_node_trends_top) into node_trends_; require mu_
+  using EdgeTrendsTop = int (*)(alz_handle*, uint32_t, uint32_t, uint32_t, const alz_metric*, const alz_trend*,
+                                uint32_t, double, alz_edge_trend*, alz_edge_out*, double*, uint8_t*, size_t, size_t*,
+                                uint32_t*, alz_rollup_info*, alz_trend_info*);
+  using NodeTrendsTop = int (*)(alz_handle*, uint32_t, uint32_t, uint32_t, uint32_t, const alz_metric*,
+                                const alz_trend*, uint32_t, double, alz_node_trend*, alz_node_out*, double*, uint8_t*,
+                                size_t, size_t*, uint32_t*, alz_rollup_info*, alz_trend_info*);
+  int RunEdgeTrends(EdgeTrendsTop fn, uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                    const alz_trend& trend, uint32_t top, double min_trend, std::vector<EdgeTrend>* out,
+                    std::vector<alz_rollup_info>* points);
+  int RunNodeTrends(NodeTrendsTop fn, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                    const alz_metric& metric, const alz_trend& trend, uint32_t top, double min_trend,
+                    std::vector<NodeTrend>* out, std::vector<alz_rollup_info>* points);
   // the group map resolved by UID sent to the library when SetGroups changed it or an interner handed out or freed an
   // id since the last send; requires mu_
   int SyncGroups();

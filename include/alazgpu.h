@@ -951,6 +951,94 @@ int alz_group_node_changes_top_device(alz_handle* h, uint32_t source, uint32_t s
                                       uint32_t mode, uint32_t presence, uint32_t k, double min_change,
                                       const alz_node_change** dev_out, size_t* n_out, alz_change_info* info);
 
+/* ---- group series and trends (docs/SPEC.md §26) ---------------------------------------------------------------------
+ * §19, §20 and §22 over groups: the map in force at the call (§24; an empty map is allowed) groups the source and every
+ * entry the call reads. Series rows: the group-edge rows of alz_group_edges(source), or the group nodes of
+ * alz_group_nodes(source) (type 4 last), in that order; or the caller's keys in the caller's order, duplicates giving
+ * identical rows. Point j of a group edge is present when entry j holds a row that maps onto it, and its values are
+ * then bit for bit what alz_group_edge_metrics* gives for a source holding entry j alone; point j of a group node is
+ * present when entry j holds a row whose mapped end on the side is the node (§22's rule: a group seen only on the other
+ * side is absent), with the values alz_group_node_metrics* gives for such a source. An absent point is +0.0 in every
+ * value, present 0. With an empty map, the group node series are alz_node_series* byte for byte, and the group edge
+ * series alz_edge_series* up to row order.
+ * Keys: a node key is one §22 accepts or (ALZ_NODE_GROUP, g) with g < 2^29; a group-edge key with no group end follows
+ * §19's rules, one with a group end needs two valid node keys. A key naming a node the map holds is absent at every
+ * point. Malformed keys are ALZ_E_INVAL, checked before any size; §19's and §22's own key rules do not change.
+ * Trends (by source only): §20's statistics, directions, absent modes, validity rules and roundings over those series.
+ * Records are alz_edge_trend (the head is the group-edge row's ends: from_type / to_type may be 4) and alz_node_trend;
+ * index is the position in alz_group_edges(source) / alz_group_nodes(source), and a top result's rows / nodes entry is
+ * byte for byte what those calls give at that index.
+ * Errors, outputs and waits as §19, §20 and §22, plus ALZ_E_CAPACITY for a source of more than 2^29 - 1 rows, checked
+ * before anything runs; *n_out and *n_points are always set; no retained entry gives P = 0, ALZ_OK. Reads only: the
+ * window, every ring, the open blocks, every rollup's rows, the baseline, the map, the group changes' baseline groups
+ * and every other family's device results are unchanged. Device results stay valid until the next call of the same
+ * family (group series, group trends). Each family's buffers grow to its largest call and are kept until alz_destroy:
+ * a group edge series holds a 576-byte node row per present slot, several GB for 60 points of 200,000 group edges. Every rank holds the same history and map, so every rank gets the same result
+ * with no collective. */
+/* every group edge of a source; cap counts series rows */
+int alz_group_edge_series(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m, uint32_t nm,
+                          double* values, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                          alz_rollup_info* points, alz_series_info* info);
+int alz_group_edge_series_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                 uint32_t nm, const double** dev_values, const uint8_t** dev_present, size_t* n_out,
+                                 uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+/* the caller's group edges (from_type / to_type may be ALZ_NODE_GROUP), keys in host memory */
+int alz_group_edge_series_keys(alz_handle* h, const alz_edge_ends* keys, size_t n_keys, uint32_t tier, uint32_t k,
+                               const alz_metric* m, uint32_t nm, double* values, uint8_t* present, size_t cap,
+                               size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+int alz_group_edge_series_keys_device(alz_handle* h, const alz_edge_ends* keys, size_t n_keys, uint32_t tier,
+                                      uint32_t k, const alz_metric* m, uint32_t nm, const double** dev_values,
+                                      const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                      alz_rollup_info* points, alz_series_info* info);
+/* every group node of a source, side `side` (ALZ_SIDE_*) */
+int alz_group_node_series(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                          const alz_metric* m, uint32_t nm, double* values, uint8_t* present, size_t cap,
+                          size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+int alz_group_node_series_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                 const alz_metric* m, uint32_t nm, const double** dev_values,
+                                 const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                 alz_rollup_info* points, alz_series_info* info);
+/* the caller's nodes (type may be ALZ_NODE_GROUP), keys in host memory */
+int alz_group_node_series_keys(alz_handle* h, const alz_node_ends* keys, size_t n_keys, uint32_t side, uint32_t tier,
+                               uint32_t k, const alz_metric* m, uint32_t nm, double* values, uint8_t* present,
+                               size_t cap, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                               alz_series_info* info);
+int alz_group_node_series_keys_device(alz_handle* h, const alz_node_ends* keys, size_t n_keys, uint32_t side,
+                                      uint32_t tier, uint32_t k, const alz_metric* m, uint32_t nm,
+                                      const double** dev_values, const uint8_t** dev_present, size_t* n_out,
+                                      uint32_t* n_points, alz_rollup_info* points, alz_series_info* info);
+/* one record per group edge / group node of the source; the top calls as alz_edge_trends_top / alz_node_trends_top */
+int alz_group_edge_trends(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                          const alz_trend* t, alz_edge_trend* out, size_t cap, size_t* n_out, uint32_t* n_points,
+                          alz_rollup_info* points, alz_trend_info* info);
+int alz_group_edge_trends_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                 const alz_trend* t, const alz_edge_trend** dev_out, size_t* n_out,
+                                 uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_edge_trends_top(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                              const alz_trend* t, uint32_t top, double min_trend, alz_edge_trend* out,
+                              alz_edge_out* rows, double* series, uint8_t* present, size_t cap, size_t* n_out,
+                              uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_edge_trends_top_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                     const alz_trend* t, uint32_t top, double min_trend,
+                                     const alz_edge_trend** dev_out, const alz_edge_out** dev_rows,
+                                     const double** dev_series, const uint8_t** dev_present, size_t* n_out,
+                                     uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_node_trends(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                          const alz_metric* m, const alz_trend* t, alz_node_trend* out, size_t cap, size_t* n_out,
+                          uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_node_trends_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                 const alz_metric* m, const alz_trend* t, const alz_node_trend** dev_out,
+                                 size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_node_trends_top(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                              const alz_metric* m, const alz_trend* t, uint32_t top, double min_trend,
+                              alz_node_trend* out, alz_node_out* nodes, double* series, uint8_t* present, size_t cap,
+                              size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+int alz_group_node_trends_top_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                     const alz_metric* m, const alz_trend* t, uint32_t top, double min_trend,
+                                     const alz_node_trend** dev_out, const alz_node_out** dev_nodes,
+                                     const double** dev_series, const uint8_t** dev_present, size_t* n_out,
+                                     uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces
