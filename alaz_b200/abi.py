@@ -261,6 +261,23 @@ class GroupInfo(C.Structure):
 
 GROUP_INFO = GroupInfo
 
+REACH_DOWN, REACH_UP, REACH_ANY = 0, 1, 2                           # alz_reach* directions (§27)
+REACH_MAX_HOPS = 64
+REACH_NONE = 0xFFFFFFFF                                             # parent / row of a seed
+REACH_NODE = np.dtype([
+    ("type", "u1"), ("_pad", "u1", (3,)), ("value", "<u4"), ("hops", "<u4"), ("index", "<u4"), ("parent", "<u4"),
+    ("row", "<u4"),
+])
+assert REACH_NODE.itemsize == 24 and REACH_NODE.fields["value"][1] == NODE_ENDS.fields["value"][1]
+
+
+class ReachInfo(C.Structure):
+    """alz_reach_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("rows", "traversable", "seeds_found", "nodes", "levels", "cut")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
 
 class SpanInfo(C.Structure):
     """alz_span_info."""

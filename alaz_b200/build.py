@@ -13,7 +13,7 @@ SOURCES = ["alz_api.cu", "alz_kernels.cu", "alz_ingest.cu", "alz_sort.cu", "alz_
            "alz_rollup.cu", "alz_top.cu", "alz_metrics.cu", "alz_changes.cu",
            "alz_series.cu", "alz_trends.cu", "alz_nodes.cu", "alz_node_series.cu",
            "alz_node_changes.cu", "alz_groups.cu", "alz_group_changes.cu",
-           "alz_group_series.cu"]
+           "alz_group_series.cu", "alz_reach.cu"]
 EXTRA = [os.path.join(HERE, "synth", "alz_synth_topo.c")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

@@ -48,7 +48,7 @@ EXPORTS = [
     "alz_group_node_series_keys", "alz_group_node_series_keys_device", "alz_group_edge_trends",
     "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
     "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
-    "alz_group_node_trends_top_device",
+    "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach", "alz_group_reach_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -197,6 +197,16 @@ def load(rebuild=False):
         "alz_group_node_top_device": ([vp, u32, u32, vp, u32, C.c_double, pp, pp, pp, C.POINTER(sz),
                                        C.POINTER(abi.TopInfo)], i),
         "alz_debug_group_edges": ([vp, vp, sz, vp, sz, C.POINTER(sz), C.POINTER(abi.GroupInfo)], i),
+        "alz_reach": ([vp, u32, vp, sz, u32, u32, vp, C.c_double, vp, sz, C.POINTER(sz), vp, vp, sz, C.POINTER(sz),
+                       C.POINTER(abi.ReachInfo)], i),
+        "alz_reach_device": ([vp, u32, vp, sz, u32, u32, vp, C.c_double, pp, C.POINTER(sz), pp, pp, C.POINTER(sz),
+                              C.POINTER(abi.ReachInfo)], i),
+        "alz_group_reach": ([vp, u32, vp, sz, u32, u32, vp, C.c_double, vp, sz, C.POINTER(sz), vp, vp, sz,
+                             C.POINTER(sz), C.POINTER(abi.ReachInfo)], i),
+        "alz_group_reach_device": ([vp, u32, vp, sz, u32, u32, vp, C.c_double, pp, C.POINTER(sz), pp, pp,
+                                    C.POINTER(sz), C.POINTER(abi.ReachInfo)], i),
+        "alz_debug_reach_rows": ([vp, vp, sz, vp, sz, u32, u32, vp, C.c_double, vp, sz, C.POINTER(sz), vp, vp, sz,
+                                  C.POINTER(sz), C.POINTER(abi.ReachInfo)], i),
         "alz_group_edge_changes": ([vp, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
         "alz_group_edge_changes_device": ([vp, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
         "alz_group_edge_changes_top": ([vp, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
@@ -306,7 +316,8 @@ def load(rebuild=False):
                   "alz_group_node_series_keys", "alz_group_node_series_keys_device", "alz_group_edge_trends",
                   "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
                   "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
-                  "alz_group_node_trends_top_device"):
+                  "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach",
+                  "alz_group_reach_device", "alz_debug_reach_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -1359,6 +1370,68 @@ class Handle:
         points, info dict)."""
         return self._trends_top_device("alz_group_node_trends_top_device", (int(source), int(side), int(tier)), k,
                                        spec, trend, top, min_trend)
+
+    # ---- reach (alz_reach.cu, docs/SPEC.md §27)
+    def _reach(self, fn, head, seeds, direction, max_hops, spec, min_value):
+        """fn(h, *head, seeds, n_seeds, dir, max_hops, m, min_value, nodes, node_cap, &n_nodes, row_index, rows,
+        row_cap, &n_rows, &info): (REACH_NODE records, row_index, EDGE_OUT rows, info dict); a first call without
+        arrays sizes them."""
+        f, nn, nr, info = getattr(self.L, fn), C.c_size_t(0), C.c_size_t(0), abi.ReachInfo()
+        keys = np.ascontiguousarray(self.node_ends(seeds))
+        m = abi.metrics(spec) if spec is not None else None
+        args = (self.h, *head, _ptr(keys), len(keys), int(direction), int(max_hops), m, float(min_value))
+        self._ck(f(*args, None, 0, C.byref(nn), None, None, 0, C.byref(nr), C.byref(info)), fn)
+        nodes = np.zeros(nn.value, dtype=abi.REACH_NODE)
+        index = np.zeros(nr.value, dtype=np.uint32)
+        rows = np.zeros(nr.value, dtype=abi.EDGE_OUT)
+        self._ck(f(*args, _ptr(nodes), len(nodes), C.byref(nn), _ptr(index), _ptr(rows), len(rows), C.byref(nr),
+                   C.byref(info)), fn)
+        return nodes, index, rows, info.as_dict()
+
+    def _reach_device(self, fn, source, seeds, direction, max_hops, spec, min_value):
+        pn, pi, pr, nn, nr, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), C.c_size_t(0), \
+            abi.ReachInfo()
+        keys = np.ascontiguousarray(self.node_ends(seeds))
+        m = abi.metrics(spec) if spec is not None else None
+        self._ck(getattr(self.L, fn)(self.h, int(source), _ptr(keys), len(keys), int(direction), int(max_hops), m,
+                                     float(min_value), C.byref(pn), C.byref(nn), C.byref(pi), C.byref(pr),
+                                     C.byref(nr), C.byref(info)), fn)
+        return pn.value, nn.value, pi.value, pr.value, nr.value, info.as_dict()
+
+    def reach(self, source, seeds, direction=abi.REACH_DOWN, max_hops=abi.REACH_MAX_HOPS, spec=None, min_value=0.0):
+        """alz_reach: the nodes of `source` within max_hops rows of the seeds (see node_ends) in abi.REACH_DOWN / UP /
+        ANY, following only rows whose metric `spec` is at least min_value when spec is given: (REACH_NODE records,
+        row positions, EDGE_OUT rows, info dict)."""
+        return self._reach("alz_reach", (int(source),), seeds, direction, max_hops, spec, min_value)
+
+    def reach_device(self, source, seeds, direction=abi.REACH_DOWN, max_hops=abi.REACH_MAX_HOPS, spec=None,
+                     min_value=0.0):
+        """alz_reach_device: (records pointer, nodes, row_index pointer, rows pointer, rows, info dict)."""
+        return self._reach_device("alz_reach_device", source, seeds, direction, max_hops, spec, min_value)
+
+    def group_reach(self, source, seeds, direction=abi.REACH_DOWN, max_hops=abi.REACH_MAX_HOPS, spec=None,
+                    min_value=0.0):
+        """alz_group_reach: reach over the group-edge rows of `source` under the handle's map; seeds may be
+        (abi.NODE_GROUP, g)."""
+        return self._reach("alz_group_reach", (int(source),), seeds, direction, max_hops, spec, min_value)
+
+    def group_reach_device(self, source, seeds, direction=abi.REACH_DOWN, max_hops=abi.REACH_MAX_HOPS, spec=None,
+                           min_value=0.0):
+        """alz_group_reach_device: (records pointer, nodes, row_index pointer, rows pointer, rows, info dict)."""
+        return self._reach_device("alz_group_reach_device", source, seeds, direction, max_hops, spec, min_value)
+
+    def debug_reach_rows(self, rows, seeds, direction=abi.REACH_DOWN, max_hops=abi.REACH_MAX_HOPS, spec=None,
+                         min_value=0.0):
+        """alz_debug_reach_rows over a host EDGE_OUT array (copied to the device): as reach."""
+        rows = np.ascontiguousarray(rows, dtype=abi.EDGE_OUT)
+        p = self.dev_alloc(max(rows.nbytes, 1))
+        try:
+            if len(rows):
+                self.h2d(p, rows)
+            return self._reach("alz_debug_reach_rows", (C.c_void_p(p), len(rows)), seeds, direction, max_hops, spec,
+                               min_value)
+        finally:
+            self.dev_free(p)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -114,11 +114,7 @@ void alz_internal_free_group_series(alz_handle* h) {
 namespace {
 
 // a node key of §26: one §22 accepts, or a group below 2^29
-bool valid_group_node(uint32_t type, uint32_t value) {
-  if (type == ALZ_NODE_GROUP) return value < (1u << 29);
-  if (type > ALZ_NODE_OUTBOUND_HOST) return false;
-  return (type != ALZ_NODE_POD && type != ALZ_NODE_SVC) || value < (1u << 29);
-}
+bool valid_group_node(uint32_t type, uint32_t value) { return valid_group_node_key(type, value); }
 
 // a group-edge key of §26: §19's rules when neither end is a group, else two valid node keys
 bool valid_group_edge(const alz_edge_ends& e) {

@@ -312,10 +312,7 @@ alz_group_state* state(alz_handle* h) {
 bool valid_source(uint32_t source) { return source == ALZ_SOURCE_WINDOW || source <= ALZ_ROLLUP_SPAN; }
 
 // a node a flush can produce: a type up to ALZ_NODE_OUTBOUND_HOST, a pod or service value below 2^29
-bool valid_member(const alz_node_ends& e) {
-  if (e.type > ALZ_NODE_OUTBOUND_HOST) return false;
-  return (e.type != ALZ_NODE_POD && e.type != ALZ_NODE_SVC) || e.value < (1u << 29);
-}
+bool valid_member(const alz_node_ends& e) { return valid_node_key(e.type, e.value); }
 
 // ceil(log2(u)), at least 1
 uint32_t index_bits(uint64_t u) {

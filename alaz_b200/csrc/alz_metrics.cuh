@@ -19,6 +19,17 @@ namespace metrics {
 // the CUB item counts are ints and the selection's tile counts pack two 32-bit counts: at most 2^30 - 1 rows
 constexpr uint32_t kMaxRows = (1u << 30) - 1u;
 
+// a node key a flush can produce (§22's key rule): a type up to ALZ_NODE_OUTBOUND_HOST, a pod or service value below
+// 2^29
+inline bool valid_node_key(uint32_t type, uint32_t value) {
+  if (type > ALZ_NODE_OUTBOUND_HOST) return false;
+  return (type != ALZ_NODE_POD && type != ALZ_NODE_SVC) || value < (1u << 29);
+}
+// a node key of §26: one valid_node_key accepts, or a group below 2^29
+inline bool valid_group_node_key(uint32_t type, uint32_t value) {
+  return type == ALZ_NODE_GROUP ? value < (1u << 29) : valid_node_key(type, value);
+}
+
 struct MetricSet {
   uint32_t nm;
   uint32_t kind[ALZ_MAX_METRICS];

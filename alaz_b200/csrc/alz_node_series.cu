@@ -132,10 +132,7 @@ struct Nodes {
 
 // whether a caller's key names a node a flush can produce: a type up to ALZ_NODE_OUTBOUND_HOST, a pod or service
 // value below 2^29
-bool valid_node(const alz_node_ends& e) {
-  if (e.type > ALZ_NODE_OUTBOUND_HOST) return false;
-  return (e.type != ALZ_NODE_POD && e.type != ALZ_NODE_SVC) || e.value < (1u << 29);
-}
+bool valid_node(const alz_node_ends& e) { return valid_node_key(e.type, e.value); }
 
 // q->keys and q->map from the caller's keys, every one valid_node
 void caller_nodes(Nodes* q) {

@@ -24,11 +24,6 @@ namespace alz {
 namespace top {
 namespace {
 
-template <class U> __host__ __device__ __forceinline__ U order_key(U u) {
-  constexpr U kSign = (U)1 << (sizeof(U) * 8 - 1);
-  return (u & kSign) ? (U)~u : (U)(u ^ kSign);
-}
-
 // pass P: digit = (ik >> kShift[P]) & (2^kBits[P] - 1), prefix = ik >> (kShift[P] + kBits[P])
 template <class U> struct Digits;
 template <> struct Digits<uint32_t> {
@@ -284,8 +279,14 @@ template <class U> int select_results(alz_handle* h, const U* vals, uint32_t n, 
   size_t tmp_bytes = s.tmp_bytes;
   CK(cub::DeviceRadixSort::SortPairs(s.tmp, tmp_bytes, (const U*)s.cand_key, (U*)s.sorted_key, s.cand_idx,
                                      s.sorted_idx, (int)c.m, 0, bits_for((uint64_t)(U)(c.prefix - ik_min)), st));
-  top_gather_kernel<U><<<std::min<unsigned>((c.m + kWarps - 1) / kWarps, (unsigned)h->sms * 4), kThreads, 0, st>>>(
-      s.sorted_idx, c.m, vals, rows, out_index, out_vals, out_rows);
+  return gather<U>(h, s.sorted_idx, c.m, vals, rows, out_index, out_vals, out_rows);
+}
+
+template <class U> int gather(alz_handle* h, const uint32_t* idx, uint32_t m, const U* vals, const alz_edge_out* rows,
+                              uint32_t* out_index, U* out_vals, alz_edge_out* out_rows) {
+  if (m == 0) return ALZ_OK;
+  top_gather_kernel<U><<<std::min<unsigned>((m + kWarps - 1) / kWarps, (unsigned)h->sms * 4), kThreads, 0,
+                         h->stream>>>(idx, m, vals, rows, out_index, out_vals, out_rows);
   h->launches += 1;
   CK(cudaGetLastError());
   return ALZ_OK;
@@ -295,7 +296,9 @@ template <class U> int select_results(alz_handle* h, const U* vals, uint32_t n, 
   template size_t tmp_bytes<U>(uint32_t, uint32_t);                                                                 \
   template int select_candidates<U>(alz_handle*, const U*, uint32_t, uint32_t, U, const Scratch&, Ctl<U>*);        \
   template int select_results<U>(alz_handle*, const U*, uint32_t, const Ctl<U>&, const alz_edge_out*,              \
-                                 const Scratch&, uint32_t*, U*, alz_edge_out*);
+                                 const Scratch&, uint32_t*, U*, alz_edge_out*);                                     \
+  template int gather<U>(alz_handle*, const uint32_t*, uint32_t, const U*, const alz_edge_out*, uint32_t*, U*,      \
+                         alz_edge_out*);
 ALZ_TOP_INSTANTIATE(uint32_t)
 ALZ_TOP_INSTANTIATE(uint64_t)
 #undef ALZ_TOP_INSTANTIATE

@@ -25,6 +25,12 @@ constexpr size_t kWordsBytes = kHistWords * 4 + sizeof(Ctl<uint64_t>);
 
 inline uint32_t tiles(uint32_t n) { return (n + kTile - 1) / kTile; }
 
+// the IEEE total-order key of a value's bits: ascending keys are ascending values
+template <class U> __host__ __device__ __forceinline__ U order_key(U u) {
+  constexpr U kSign = (U)1 << (sizeof(U) * 8 - 1);
+  return (u & kSign) ? (U)~u : (U)(u ^ kSign);
+}
+
 // Device scratch for a selection over n values with at most m_max = min(n, k) results
 struct Scratch {
   uint32_t* words;        // kWordsBytes
@@ -47,5 +53,9 @@ template <class U> int select_candidates(alz_handle* h, const U* vals, uint32_t 
 template <class U> int select_results(alz_handle* h, const U* vals, uint32_t n, const Ctl<U>& c,
                                       const alz_edge_out* rows, const Scratch& s, uint32_t* out_index, U* out_vals,
                                       alz_edge_out* out_rows);
+// The gather of select_results on its own, on the stream: for j < m, i = idx[j]: out_index[j] = i, out_vals[j] = vals[i]
+// and, with rows, out_rows[j] = rows[i]
+template <class U> int gather(alz_handle* h, const uint32_t* idx, uint32_t m, const U* vals, const alz_edge_out* rows,
+                              uint32_t* out_index, U* out_vals, alz_edge_out* out_rows);
 }  // namespace top
 }  // namespace alz

@@ -1098,6 +1098,77 @@ int Aggregator::GroupNodeSeries(uint32_t source, uint32_t side, uint32_t tier, u
   return ALZ_OK;
 }
 
+int Aggregator::Reach(uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
+                      const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
+                      std::vector<EdgeWindow>* rows, alz_reach_info* info) {
+  return RunReach(false, source, seeds, dir, max_hops, filter, min_value, nodes, rows, info);
+}
+
+int Aggregator::GroupReach(uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
+                           const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
+                           std::vector<EdgeWindow>* rows, alz_reach_info* info) {
+  return RunReach(true, source, seeds, dir, max_hops, filter, min_value, nodes, rows, info);
+}
+
+int Aggregator::RunReach(bool group, uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir,
+                         uint32_t max_hops, const alz_metric* filter, double min_value,
+                         std::vector<ReachNode>* nodes, std::vector<EdgeWindow>* rows, alz_reach_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!nodes || !rows) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  if (info) *info = alz_reach_info{};
+  nodes->clear();
+  rows->clear();
+  if (group) {
+    const int rc = SyncGroups();
+    if (rc != ALZ_OK) return rc;
+  }
+  std::vector<alz_node_ends> keys;
+  for (const NodeRef& r : seeds) {
+    alz_node_ends k_{};
+    if (group ? GroupEndOf(r.Type, r.UID, &k_.type, &k_.value) : EndOf(r.Type, r.UID, &k_.type, &k_.value))
+      keys.push_back(k_);
+  }
+  if (keys.empty()) return ALZ_OK;
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // never empty: a null array would not be written (and its cap not checked)
+  if (reach_nodes_.empty()) reach_nodes_.resize(1);
+  if (reach_index_.empty()) reach_index_.resize(1);
+  if (roll_.empty()) roll_.resize(1);
+  auto call = [&](size_t* nn, size_t* nr) {
+    return (group ? alz_group_reach : alz_reach)(h_, src, keys.data(), keys.size(), dir, max_hops, filter, min_value,
+                                                 reach_nodes_.data(), reach_nodes_.size(), nn, reach_index_.data(),
+                                                 roll_.data(), std::min(reach_index_.size(), roll_.size()), nr, info);
+  };
+  // into reach_nodes_ / reach_index_ / roll_, grown once when the results do not fit (ALZ_E_CAPACITY with the counts
+  // set; nothing written)
+  size_t nn = 0, nr = 0;
+  int rc = call(&nn, &nr);
+  if (rc == ALZ_E_CAPACITY && (nn > reach_nodes_.size() || nr > reach_index_.size() || nr > roll_.size())) {
+    reach_nodes_.resize(std::max(nn, reach_nodes_.size()));
+    reach_index_.resize(std::max(nr, reach_index_.size()));
+    roll_.resize(std::max(nr, roll_.size()));
+    rc = call(&nn, &nr);
+  }
+  if (rc != ALZ_OK) return rc;
+  *rows = ToEdges(roll_.data(), nr, nullptr);
+  nodes->resize(nn);
+  for (size_t i = 0; i < nn; ++i) {
+    const alz_reach_node& r = reach_nodes_[i];
+    ReachNode& o = (*nodes)[i];
+    o.Type = NodeTypeName(r.type);
+    o.UID = UidOf(r.type, r.value);
+    o.Hops = r.hops;
+    o.Parent = r.parent;
+    o.Row = kReachNone;
+    if (r.row != kReachNone) {   // the parent's row is listed: its tail is the parent, at hops < max_hops
+      o.Row = (uint32_t)(std::lower_bound(reach_index_.begin(), reach_index_.begin() + nr, r.row) -
+                         reach_index_.begin());
+    }
+  }
+  return ALZ_OK;
+}
+
 int Aggregator::GroupNodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
                                    const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
                                    std::vector<alz_rollup_info>* points) {

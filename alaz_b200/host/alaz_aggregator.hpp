@@ -123,6 +123,14 @@ struct GroupMember {
   std::string Type, UID, Group;
 };
 
+// one node a reach (docs/SPEC.md §27) listed: named as Nodes / GroupNodes name it, its hops from the nearest seed, the
+// position in the result of its parent on one shortest path and the position in the rows of the row used from that
+// parent (both kReachNone for a seed)
+struct ReachNode {
+  std::string Type, UID;
+  uint32_t Hops = 0, Parent = 0, Row = 0;
+};
+
 // one node's series (docs/SPEC.md §22): per point, oldest first, whether that entry holds a row on the side of the
 // node and the metrics' values of the side's sums there (every value 0 where it does not)
 struct NodeSeriesRow {
@@ -338,6 +346,23 @@ class Aggregator {
   int GroupNodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
                       const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
                       std::vector<alz_rollup_info>* points = nullptr);
+  // Reach (docs/SPEC.md §27): the nodes of `source` within max_hops rows of the seeds, in direction dir
+  // (ALZ_REACH_DOWN: what the seeds call; ALZ_REACH_UP: who calls them; ALZ_REACH_ANY), in (hops, node key) order, and
+  // the rows crossed, in the source's order, named as ToEdges names ends. filter (may be null): only rows whose value
+  // of that metric is >= min_value are followed ("follow the calls that return 5xx"). A seed whose UID has no id is
+  // skipped like a seed no row holds; when no seed resolves, *nodes and *rows are empty and info counts nothing. info
+  // may be null. Returns 0 or an alz_status.
+  int Reach(uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
+            const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes, std::vector<EdgeWindow>* rows,
+            alz_reach_info* info = nullptr);
+  // Reach over the group-edge rows of `source` under the map SetGroups gave (sent first, as for every group call):
+  // "which deployments does checkout depend on". A seed of Type "group" names a group by its SetGroups name; a name
+  // SetGroups never gave is skipped like a UID with no id. Nodes and rows are named as GroupNodes / GroupEdges name
+  // them.
+  int GroupReach(uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
+                 const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
+                 std::vector<EdgeWindow>* rows, alz_reach_info* info = nullptr);
+  static constexpr uint32_t kReachNone = 0xFFFFFFFFu;   // ReachNode.Parent / Row of a seed
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -368,6 +393,10 @@ class Aggregator {
   bool EndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const;
   // EndOf, and a group (Type "group") by the name SetGroups gave it; false for a name it never gave
   bool GroupEndOf(const std::string& type, const std::string& uid, uint8_t* t, uint32_t* v) const;
+  // Reach and GroupReach: the seeds resolved by EndOf (group false) or GroupEndOf, the call, the results named
+  int RunReach(bool group, uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
+               const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
+               std::vector<EdgeWindow>* rows, alz_reach_info* info);
   // ends -> the library's key of an edge named by UID; false when a UID has no id
   bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
   // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then each series
@@ -448,6 +477,8 @@ class Aggregator {
   std::vector<alz_node_change> node_changes_;   // records of the last NodeChanges
   std::vector<alz_node_trend> node_trends_;   // records, node rows, series and presence of the last NodeTrends
   std::vector<alz_node_out> node_trend_rows_;
+  std::vector<alz_reach_node> reach_nodes_;   // the records and row positions of the last Reach / GroupReach
+  std::vector<uint32_t> reach_index_;
   std::vector<GroupMember> members_;                    // the group map as SetGroups gave it
   std::unordered_map<std::string, uint32_t> group_ids_;  // group name -> dense id (ALZ_NODE_GROUP)
   std::vector<std::string> group_names_;

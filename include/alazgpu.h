@@ -1039,6 +1039,79 @@ int alz_group_node_trends_top_device(alz_handle* h, uint32_t source, uint32_t si
                                      const double** dev_series, const uint8_t** dev_present, size_t* n_out,
                                      uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info);
 
+/* ---- reach (docs/SPEC.md §27) ---------------------------------------------------------------------------------------
+ * A breadth-first search of a source's graph (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability rule of §15)
+ * from chosen seed nodes, up to max_hops (1 .. ALZ_REACH_MAX_HOPS) rows away. alz_reach* traverses the source's rows
+ * and its nodes are alz_node_rows(source); alz_group_reach* traverses the source's group-edge rows under the map in
+ * force at the call (§24; an empty map is allowed) and its nodes are alz_group_nodes(source). A node's index is its
+ * position in that node list. ALZ_REACH_DOWN: a row leads from its from end to its to end (dependencies); ALZ_REACH_UP:
+ * from its to end to its from end (callers); ALZ_REACH_ANY: both ways. With m NULL every row is traversable and
+ * min_value is ignored; otherwise m is one §17 metric and a row is traversable when the IEEE total-order key of its
+ * value (bit for bit alz_edge_metrics* / alz_group_edge_metrics*) is at least key(min_value): ERR5XX >= 1 follows failing
+ * calls only. hops(v) is the fewest traversable rows on a path from a seed to v. A seed that is no node of the traversed
+ * rows is skipped (info->seeds_found counts the distinct ones that are); duplicates are allowed.
+ * Nodes: every node with hops <= max_hops, ordered by (hops, node key (type << 32) | value). A record's parent is the
+ * position in this result of the node with the smallest index among the listed nodes at hops - 1 that have a
+ * traversable row leading to it, and its row the smallest position among the traversable rows leading from that parent
+ * to it (under ANY, either orientation counts); seeds have parent = row = 0xFFFFFFFF. The bytes do not depend on thread
+ * order, and parent and row rebuild one shortest path with the row of every hop.
+ * Rows: every traversable row whose tail (from for DOWN, to for UP, either end for ANY) has hops < max_hops, in
+ * traversed-list order: row_index[j] its position there, rows[j] the row byte for byte (a source row, or a group-edge
+ * row for the group form). Their heads are listed nodes.
+ * Seeds: the node form takes §22's keys (a type above ALZ_NODE_OUTBOUND_HOST or a pod or service value >= 2^29 is
+ * malformed), the group form §26's (also (ALZ_NODE_GROUP, g) with g < 2^29); malformed seeds are checked before any
+ * size. An unknown source or dir, max_hops 0 or above 64, n_seeds 0, a null seeds, n_nodes or n_rows, a bad metric
+ * (§17) or a NaN min_value with a metric: ALZ_E_INVAL. No rows of a rollup source: ALZ_E_STATE. More than 2^29 - 1
+ * source rows (before anything runs) or more than 2^30 - 1 seeds: ALZ_E_CAPACITY; no memory: ALZ_E_NOMEM. No seed
+ * found, or a 0-row source: 0 nodes, 0 rows, ALZ_OK. *n_nodes and *n_rows are always set. Host forms: nodes, row_index
+ * and rows may each be NULL; node_cap is checked when nodes is not NULL and row_cap when row_index or rows is not; a
+ * failed check returns ALZ_E_CAPACITY and writes none of the three. Device forms: dev_nodes, dev_row_index and dev_rows
+ * may each be NULL; the results stay valid until the next reach call of either form. info may be NULL.
+ * Waits: one for the node count (§21), one for the seeds found, one per level expanded (min(levels + 1, max_hops) of
+ * them), one for the listed rows, and a host call one more for its copies; the group form adds §24's two. Reads only:
+ * the window, every ring, the open blocks, every rollup's rows and info, the baseline and its caches, the map and every
+ * other family's device results are unchanged; reach keeps its buffers in a state of its own, grown on demand and freed
+ * in alz_destroy. Every rank holds the same rows and the same map, so every rank returns the same bytes with no
+ * collective. */
+#define ALZ_REACH_DOWN 0u   /* from end -> to end: what the seeds call */
+#define ALZ_REACH_UP   1u   /* to end -> from end: who calls the seeds */
+#define ALZ_REACH_ANY  2u   /* both ways */
+#define ALZ_REACH_MAX_HOPS 64u
+typedef struct alz_reach_node {   /* 24 B; the first 8 bytes are an alz_node_ends */
+  uint8_t type;                   /* ALZ_NODE_* */
+  uint8_t _pad[3];                /* zero */
+  uint32_t value;
+  uint32_t hops;
+  uint32_t index;                 /* the node's position in the traversed rows' node list */
+  uint32_t parent;                /* the predecessor's position in this result; 0xFFFFFFFF for a seed */
+  uint32_t row;                   /* the traversed row used from the parent; 0xFFFFFFFF for a seed */
+} alz_reach_node;
+typedef struct alz_reach_info {
+  uint64_t rows;          /* traversed rows */
+  uint64_t traversable;   /* of which traversable */
+  uint64_t seeds_found;   /* distinct seeds that are nodes */
+  uint64_t nodes;         /* nodes listed */
+  uint64_t levels;        /* the largest hops listed */
+  uint64_t cut;           /* traversable rows from a node at hops = max_hops to a node not listed; 0: a larger
+                             max_hops lists no more nodes */
+} alz_reach_info;
+int alz_reach(alz_handle* h, uint32_t source, const alz_node_ends* seeds, size_t n_seeds, uint32_t dir,
+              uint32_t max_hops, const alz_metric* m, double min_value, alz_reach_node* nodes, size_t node_cap,
+              size_t* n_nodes, uint32_t* row_index, alz_edge_out* rows, size_t row_cap, size_t* n_rows,
+              alz_reach_info* info);
+int alz_reach_device(alz_handle* h, uint32_t source, const alz_node_ends* seeds, size_t n_seeds, uint32_t dir,
+                     uint32_t max_hops, const alz_metric* m, double min_value, const alz_reach_node** dev_nodes,
+                     size_t* n_nodes, const uint32_t** dev_row_index, const alz_edge_out** dev_rows, size_t* n_rows,
+                     alz_reach_info* info);
+int alz_group_reach(alz_handle* h, uint32_t source, const alz_node_ends* seeds, size_t n_seeds, uint32_t dir,
+                    uint32_t max_hops, const alz_metric* m, double min_value, alz_reach_node* nodes, size_t node_cap,
+                    size_t* n_nodes, uint32_t* row_index, alz_edge_out* rows, size_t row_cap, size_t* n_rows,
+                    alz_reach_info* info);
+int alz_group_reach_device(alz_handle* h, uint32_t source, const alz_node_ends* seeds, size_t n_seeds, uint32_t dir,
+                           uint32_t max_hops, const alz_metric* m, double min_value, const alz_reach_node** dev_nodes,
+                           size_t* n_nodes, const uint32_t** dev_row_index, const alz_edge_out** dev_rows,
+                           size_t* n_rows, alz_reach_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

@@ -80,6 +80,14 @@ int alz_debug_group_edge_changes_rows(alz_handle* h, const alz_edge_out* dev_src
                                       const alz_edge_out* dev_base, size_t n_base, uint32_t base_windows,
                                       const alz_metric* m, uint32_t mode, uint32_t presence, alz_edge_change* out,
                                       size_t cap, size_t* n_out, alz_change_info* info);
+/* test/debug: alz_reach (docs/SPEC.md §27) over n caller rows in device memory, which may hold layouts ingest cannot
+ * make (any row order, any type byte, long chains, one node on 2^20 rows); the traversed rows are the caller's rows and
+ * the node list their §21 node list. More than 2^29 - 1 rows: ALZ_E_CAPACITY. The rules of alz_reach otherwise. Uses
+ * the reach calls' buffers. */
+int alz_debug_reach_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, const alz_node_ends* seeds,
+                         size_t n_seeds, uint32_t dir, uint32_t max_hops, const alz_metric* m, double min_value,
+                         alz_reach_node* nodes, size_t node_cap, size_t* n_nodes, uint32_t* row_index,
+                         alz_edge_out* rows, size_t row_cap, size_t* n_rows, alz_reach_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
