@@ -1144,7 +1144,7 @@ class Handle:
         return self._trends_top_device("alz_node_trends_top_device", (int(source), int(side), int(tier)), k, spec,
                                        trend, top, min_trend)
 
-    # ---- node changes against the pinned baseline (alz_node_changes.cu, docs/SPEC.md §23)
+    # ---- node changes against the pinned baseline (alz_changes.cu, docs/SPEC.md §23)
     def node_changes(self, side, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
         """alz_node_changes of side `side` (abi.SIDE_*) of the nodes of `source` against the pinned baseline by one
         metric: (NODE_CHANGE records in ascending node key order, info dict)."""
@@ -1196,7 +1196,7 @@ class Handle:
             self.dev_free(ps)
             self.dev_free(pb)
 
-    # ---- group changes against the pinned baseline (alz_group_changes.cu, docs/SPEC.md §25)
+    # ---- group changes against the pinned baseline (alz_changes.cu, docs/SPEC.md §25)
     def group_edge_changes(self, spec, mode=abi.CHANGE_DELTA, presence=abi.PRESENT_ALL, source=abi.SOURCE_WINDOW):
         """alz_group_edge_changes of the group edges of `source` against the pinned baseline's, both grouped by the
         current map, by one metric: (EDGE_CHANGE records in ascending (from key, to key) order, info dict)."""

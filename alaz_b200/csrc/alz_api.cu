@@ -266,9 +266,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_nodes(h);
   alz_internal_free_node_series(h);
   alz_internal_free_node_trends(h);
-  alz_internal_free_node_changes(h);
   alz_internal_free_groups(h);
-  alz_internal_free_group_changes(h);
   alz_internal_free_group_series(h);
   alz_internal_free_group_trends(h);
   alz_internal_free_reach(h);

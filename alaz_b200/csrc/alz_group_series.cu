@@ -87,10 +87,6 @@ __global__ void __launch_bounds__(256) group_edge_pairs_kernel(const alz_edge_ou
   if ((threadIdx.x & 31u) == 0 && n_miss) atomicAdd(misses, n_miss);
 }
 
-unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
-  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
-}
-
 }  // namespace
 
 void alz::metrics::GroupSeriesBufs::free() {

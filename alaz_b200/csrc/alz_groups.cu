@@ -46,10 +46,6 @@ static_assert(sizeof(alz_group_info) == 32, "alz_group_info is four u64");
 static_assert(offsetof(alz_edge_out, count) == 16 && offsetof(alz_edge_out, hist) == 40 && sizeof(alz_edge_out) == 296,
               "the reduce stores a row as 37 8-byte words: head (2), sums (3), cell pairs (32)");
 
-unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
-  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
-}
-
 // flag[0] = 1 when two adjacent sorted keys are equal
 __global__ void __launch_bounds__(256) map_dup_kernel(const uint64_t* __restrict__ keys, uint32_t n,
                                                       uint32_t* __restrict__ flag) {

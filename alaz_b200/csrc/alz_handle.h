@@ -38,9 +38,7 @@ struct alz_series_state;  // alz_series.cu
 struct alz_trend_state;   // alz_trends.cu
 struct alz_node_state;    // alz_nodes.cu
 struct alz_node_series_state;   // alz_node_series.cu
-struct alz_node_changes_state;  // alz_node_changes.cu
 struct alz_group_state;         // alz_groups.cu
-struct alz_group_changes_state; // alz_group_changes.cu
 struct alz_group_series_state;  // alz_group_series.cu
 struct alz_reach_state;         // alz_reach.cu
 
@@ -143,12 +141,8 @@ struct alz_handle {
   alz_node_state* nodes = nullptr;        // the node calls' buffers (alz_node_*); null until the first
   alz_node_series_state* node_series = nullptr;   // the node series' buffers (alz_node_series*); null until the first
   alz_trend_state* node_trends = nullptr;         // the node trends' buffers (alz_node_trends*); null until the first
-  alz_node_changes_state* node_changes = nullptr; // the node changes' buffers and the baseline's node rows
-                                                  // (alz_node_changes*); null until the first
   alz_group_state* groups = nullptr;      // the group map and the group calls' buffers (alz_group_*); null until the
                                           // first
-  alz_group_changes_state* group_changes = nullptr;   // the group changes' buffers and the baseline's groups
-                                                      // (alz_group_*_changes*); null until the first
   alz_group_series_state* group_series = nullptr;     // the group series' buffers (alz_group_*_series*); null until
                                                       // the first
   alz_trend_state* group_trends = nullptr;            // the group trends' buffers (alz_group_*_trends*); null until
@@ -208,9 +202,7 @@ void alz_internal_free_trends(alz_handle* h);
 void alz_internal_free_nodes(alz_handle* h);
 void alz_internal_free_node_series(alz_handle* h);
 void alz_internal_free_node_trends(alz_handle* h);
-void alz_internal_free_node_changes(alz_handle* h);
 void alz_internal_free_groups(alz_handle* h);
-void alz_internal_free_group_changes(alz_handle* h);
 void alz_internal_free_group_series(alz_handle* h);
 void alz_internal_free_group_trends(alz_handle* h);
 void alz_internal_free_reach(alz_handle* h);

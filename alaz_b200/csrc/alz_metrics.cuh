@@ -1,12 +1,12 @@
-// alz_metrics.cuh — what alz_metrics.cu shares with the change list (alz_changes.cu), the edge series
-// (alz_series.cu), the edge and node trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
-// (alz_node_series.cu), the node changes (alz_node_changes.cu), the groups (alz_groups.cu), the group changes
-// (alz_group_changes.cu) and the group series (alz_group_series.cu): the §17 metric values of a row list, of node rows
-// or of series slots, the rows' packed keys, the grow-on-demand device buffers, the node group-by, a source's edge,
-// node or group series into given buffers, the 64-bit top selection with its own scratch, the pinned baseline with the
-// §18 change arithmetic and the §18 and §23 joins into given buffers, the §24 group-by into given buffers and the map
-// lookup.
+// alz_metrics.cuh — what alz_metrics.cu shares with the changes (alz_changes.cu), the edge series (alz_series.cu),
+// the edge, node and group trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
+// (alz_node_series.cu), the groups (alz_groups.cu), the group series (alz_group_series.cu) and the reach calls
+// (alz_reach.cu): the §17 metric values of a row list, of node rows or of series slots, a source's rows, the rows'
+// packed keys, the grow-on-demand device buffers and launch grids, the node group-by, a source's edge, node or group
+// series into given buffers, the 64-bit top selection with its own scratch, the §24 group-by into given buffers and
+// the map lookup.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <initializer_list>
 #include <utility>
@@ -47,6 +47,11 @@ void free_bufs(std::initializer_list<DevBuf*> bufs);
 // Every buffer in `need` holds at least its bytes. The last calls may still read them: one wait before the first
 // buffer is replaced. A failed allocation leaves that buffer empty and returns ALZ_E_NOMEM.
 int reserve(alz_handle* h, std::initializer_list<std::pair<DevBuf*, size_t>> need);
+
+// The blocks of a 256-thread grid-stride launch over `threads` items: one per 256, at least 1, at most per_sm per SM
+inline unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
+  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
+}
 
 // The metrics of n rows into out[n * ms.nm], on the stream; no wait
 int run_metrics(alz_handle* h, const alz_edge_out* rows, uint32_t n, const MetricSet& ms, double* out);
@@ -146,27 +151,6 @@ int node_source(alz_handle* h, uint32_t source, const alz_edge_out** rows, size_
 // ALZ_E_CAPACITY before the reduce is enqueued. Caller holds h->mu and has set the device; n <= kMaxNodeSourceRows.
 int node_rows_of(alz_handle* h, NodeGroup& g, DevBuf& out, const alz_edge_out* rows, size_t n, size_t cap,
                  size_t* n_nodes);
-
-// The pinned baseline of the change calls (alz_changes.cu): its rows, their count, what its source reported, and the
-// generation of its pin, which every alz_baseline_pin moves on. ALZ_E_STATE when none is pinned. Caller holds h->mu.
-int pinned_baseline(alz_handle* h, const alz_edge_out** rows, size_t* n, alz_rollup_info* info, uint64_t* generation);
-// out[j] = list[idx[j]] for j < m, on the stream: 48-byte change records (alz_edge_change, alz_node_change)
-template <class Record>
-int gather_changes(alz_handle* h, const uint32_t* idx, uint32_t m, const Record* list, Record* out);
-
-#ifdef __CUDACC__
-// A §18 side's value: COUNT and ERR5XX per window (one rounding), the others as they are
-__device__ __forceinline__ double per_window(double v, bool divide, double windows) {
-  return divide ? __ddiv_rn(v, windows) : v;
-}
-// The §18 change of mode from a source value and a baseline value, one rounding
-__device__ __forceinline__ double change_of(uint32_t mode, double cur, double base) {
-  if (mode == ALZ_CHANGE_DELTA) return __dsub_rn(cur, base);
-  if (mode == ALZ_CHANGE_DROP) return __dsub_rn(base, cur);
-  if (base > 0.0) return __ddiv_rn(cur, base);   // ALZ_CHANGE_RATIO
-  return cur > 0.0 ? __longlong_as_double(0x7FF0000000000000ll) : 1.0;
-}
-#endif
 
 // The rows of a source and its windows (ALZ_SOURCE_WINDOW: the last flushed window, 1), or of the last rollup of a
 // kind with what it reported (alz_changes.cu). Caller holds h->mu.
@@ -279,46 +263,6 @@ struct Selection {
 // null. *m_out results in s.top_index / s.top_values (/ s.top_rows), *above eligible values.
 int select_top(alz_handle* h, Selection& s, const uint64_t* vals, uint32_t n, uint32_t k, double min_value,
                const alz_edge_out* rows, size_t* m_out, uint64_t* above);
-
-// The scratch and the results of change joins, grown on demand: the edge changes, the node changes and the group
-// changes (alz_group_changes.cu) each own one set, so none clobbers another's device results
-struct ChangeBufs {
-  DevBuf keys_a, keys_b, member_a, member_b;   // the sides' keys when derived; the node sides' membership
-  DevBuf lb_a, lb_b, keep_a, keep_b, scan_a, scan_b, val_a, val_b, counts, tmp;   // the join's scratch
-  DevBuf list, chg, top_list;                  // the results: the filtered union, its changes, the top records
-  Selection sel;                               // the top call's selection
-  void free();
-};
-// One side of an edge change join: n rows strictly ascending in the join's key, their packed keys (null: derived),
-// and the windows its values are divided by
-struct EdgeChangeSide {
-  const alz_edge_out* rows;
-  const uint64_t* keys;
-  uint32_t n;
-  uint32_t windows;
-};
-// The §18 join of a and b into b.list, *listed records, and with top their changes into b.chg. ends: the rows are
-// matched by (node key of from, node key of to), the §24 order, on keys derived here (a.keys and b.keys null); else
-// by packed key. One wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
-int edge_change_join(alz_handle* h, ChangeBufs& cb, EdgeChangeSide a, EdgeChangeSide b, bool ends,
-                     const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
-                     alz_change_info* ci);
-// One node list of a node change join: n node rows in ascending key order, and the windows its values are divided by
-struct NodeChangeSide {
-  const alz_node_out* nodes;
-  uint32_t n;
-  uint32_t windows;
-};
-// The §23 join of a and b on side `side` into cb.list, *listed records, and with top their changes into cb.chg. One
-// wait. ci: the counts (above left 0). Caller holds h->mu and has set the device.
-int node_change_join(alz_handle* h, ChangeBufs& cb, NodeChangeSide a, NodeChangeSide b, uint32_t side,
-                     const MetricSet& ms, uint32_t mode, uint32_t presence, bool top, uint64_t* listed,
-                     alz_change_info* ci);
-// After a join into cb: the listed records in cb.list (top false), or the first min(k, above) of them by change
-// gathered into cb.top_list (top, ci->above set). *res, *n = the records. Caller holds h->mu.
-template <class Record>
-int change_results(alz_handle* h, ChangeBufs& cb, bool top, uint64_t listed, uint32_t k, double min_change,
-                   const Record** res, size_t* n, alz_change_info* ci);
 
 // The §24 group-edge rows of n rows under the handle's map into `out`, grown to hold them, with the group calls'
 // scratch (alz_groups.cu): two waits, then the reduce on the stream. *n_out = the rows; more than cap: ALZ_E_CAPACITY

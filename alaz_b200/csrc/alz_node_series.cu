@@ -91,10 +91,6 @@ __global__ void __launch_bounds__(256) node_slot_kernel(const uint64_t* __restri
     if (heads[j]) slot[sorted[j]] = idx[j];
 }
 
-unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
-  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
-}
-
 int key_bits_of(uint64_t max_key) { return 64 - __builtin_clzll(max_key); }
 
 }  // namespace

@@ -226,14 +226,6 @@ void alz_internal_free_nodes(alz_handle* h) {
   h->nodes = nullptr;
 }
 
-namespace {
-
-unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
-  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
-}
-
-}  // namespace
-
 namespace alz {
 namespace metrics {
 

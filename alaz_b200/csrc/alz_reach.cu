@@ -49,10 +49,6 @@ constexpr uint32_t kUnreached = 0xFFFFFFFFu;
 constexpr uint64_t kNoBest = ~0ull;
 constexpr uint32_t kMaxSeeds = (1u << 30) - 1u;
 
-unsigned grid_for(alz_handle* h, uint64_t threads, unsigned per_sm) {
-  return (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((threads + 255) / 256, (uint64_t)h->sms * per_sm));
-}
-
 // j over the n2 sorted ends: end_node[vals[j]] = the node index of j's run; node_keys[index] = its key at a run head
 __global__ void __launch_bounds__(256) reach_index_kernel(const uint64_t* __restrict__ keys,
                                                           const uint32_t* __restrict__ vals,

@@ -424,23 +424,26 @@ int Aggregator::ClearBaseline() {
   return ALZ_OK;
 }
 
+template <class Rec, class Call>
+int Aggregator::RunChanges(std::vector<Rec>* recs, size_t* n, Call call) {
+  int rc = call(recs->data(), recs->size(), n);
+  if (rc == ALZ_E_CAPACITY && *n > recs->size()) {
+    recs->resize(*n);
+    rc = call(recs->data(), recs->size(), n);
+  }
+  return rc;
+}
+
 int Aggregator::Changes(uint32_t source, const alz_metric& metric, uint32_t mode, uint32_t presence, uint32_t k,
                         double min_change, std::vector<EdgeChange>* out, alz_change_info* info) {
   if (!h_) return ALZ_E_STATE;
   if (!out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(mu_);
-  // into changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
-  auto call = [&](size_t* n) {
-    return k == 0 ? alz_edge_changes(h_, source, &metric, mode, presence, changes_.data(), changes_.size(), n, info)
-                  : alz_edge_changes_top(h_, source, &metric, mode, presence, k, min_change, changes_.data(),
-                                         changes_.size(), n, info);
-  };
   size_t n = 0;
-  int rc = call(&n);
-  if (rc == ALZ_E_CAPACITY && n > changes_.size()) {
-    changes_.resize(n);
-    rc = call(&n);
-  }
+  const int rc = RunChanges(&changes_, &n, [&](alz_edge_change* recs, size_t cap, size_t* n_out) {
+    return k == 0 ? alz_edge_changes(h_, source, &metric, mode, presence, recs, cap, n_out, info)
+                  : alz_edge_changes_top(h_, source, &metric, mode, presence, k, min_change, recs, cap, n_out, info);
+  });
   if (rc != ALZ_OK) return rc;
   *out = ToChanges(changes_.data(), n);
   return ALZ_OK;
@@ -668,19 +671,11 @@ int Aggregator::NodeChanges(uint32_t source, uint32_t side, const alz_metric& me
   if (!out) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(mu_);
   const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
-  // into node_changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
-  auto call = [&](size_t* n) {
-    return k == 0 ? alz_node_changes(h_, src, side, &metric, mode, presence, node_changes_.data(),
-                                     node_changes_.size(), n, info)
-                  : alz_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change, node_changes_.data(),
-                                         node_changes_.size(), n, info);
-  };
   size_t n = 0;
-  int rc = call(&n);
-  if (rc == ALZ_E_CAPACITY && n > node_changes_.size()) {
-    node_changes_.resize(n);
-    rc = call(&n);
-  }
+  const int rc = RunChanges(&node_changes_, &n, [&](alz_node_change* recs, size_t cap, size_t* n_out) {
+    return k == 0 ? alz_node_changes(h_, src, side, &metric, mode, presence, recs, cap, n_out, info)
+                  : alz_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change, recs, cap, n_out, info);
+  });
   if (rc != ALZ_OK) return rc;
   *out = ToNodeChanges(node_changes_.data(), n);
   return ALZ_OK;
@@ -835,18 +830,11 @@ int Aggregator::GroupChanges(uint32_t source, const alz_metric& metric, uint32_t
   int rc = SyncGroups();
   if (rc != ALZ_OK) return rc;
   const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
-  // into changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
-  auto call = [&](size_t* n) {
-    return k == 0 ? alz_group_edge_changes(h_, src, &metric, mode, presence, changes_.data(), changes_.size(), n, info)
-                  : alz_group_edge_changes_top(h_, src, &metric, mode, presence, k, min_change, changes_.data(),
-                                               changes_.size(), n, info);
-  };
   size_t n = 0;
-  rc = call(&n);
-  if (rc == ALZ_E_CAPACITY && n > changes_.size()) {
-    changes_.resize(n);
-    rc = call(&n);
-  }
+  rc = RunChanges(&changes_, &n, [&](alz_edge_change* recs, size_t cap, size_t* n_out) {
+    return k == 0 ? alz_group_edge_changes(h_, src, &metric, mode, presence, recs, cap, n_out, info)
+                  : alz_group_edge_changes_top(h_, src, &metric, mode, presence, k, min_change, recs, cap, n_out, info);
+  });
   if (rc != ALZ_OK) return rc;
   *out = ToChanges(changes_.data(), n);
   return ALZ_OK;
@@ -861,19 +849,12 @@ int Aggregator::GroupNodeChanges(uint32_t source, uint32_t side, const alz_metri
   int rc = SyncGroups();
   if (rc != ALZ_OK) return rc;
   const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
-  // into node_changes_, grown once when the records do not fit (ALZ_E_CAPACITY with n = the records; nothing written)
-  auto call = [&](size_t* n) {
-    return k == 0 ? alz_group_node_changes(h_, src, side, &metric, mode, presence, node_changes_.data(),
-                                           node_changes_.size(), n, info)
-                  : alz_group_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change,
-                                               node_changes_.data(), node_changes_.size(), n, info);
-  };
   size_t n = 0;
-  rc = call(&n);
-  if (rc == ALZ_E_CAPACITY && n > node_changes_.size()) {
-    node_changes_.resize(n);
-    rc = call(&n);
-  }
+  rc = RunChanges(&node_changes_, &n, [&](alz_node_change* recs, size_t cap, size_t* n_out) {
+    return k == 0 ? alz_group_node_changes(h_, src, side, &metric, mode, presence, recs, cap, n_out, info)
+                  : alz_group_node_changes_top(h_, src, side, &metric, mode, presence, k, min_change, recs, cap,
+                                               n_out, info);
+  });
   if (rc != ALZ_OK) return rc;
   *out = ToNodeChanges(node_changes_.data(), n);
   return ALZ_OK;

@@ -384,6 +384,10 @@ class Aggregator {
   std::vector<EdgeWindow> ToEdges(const alz_edge_out* rows, size_t n, const float* scores) const;
   // the UID of an edge end or node (type, id) as the interners and the Host table hold it
   std::string UidOf(uint8_t type, uint32_t id) const;
+  // a change call(recs, cap, &n) into *recs (changes_ or node_changes_), grown once when the records do not fit
+  // (ALZ_E_CAPACITY with n = the records; nothing written); requires mu_
+  template <class Rec, class Call>
+  int RunChanges(std::vector<Rec>* recs, size_t* n, Call call);
   // change records -> EdgeChange / NodeChange with the UIDs the interners and the group names hold
   std::vector<EdgeChange> ToChanges(const alz_edge_change* recs, size_t n) const;
   std::vector<NodeChange> ToNodeChanges(const alz_node_change* recs, size_t n) const;
