@@ -279,6 +279,22 @@ class ReachInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+CYCLE_NODE = np.dtype([                                             # alz_cycle_node (§28)
+    ("type", "u1"), ("_pad", "u1", (3,)), ("value", "<u4"), ("index", "<u4"), ("component", "<u4"), ("size", "<u4"),
+    ("depth", "<u4"), ("height", "<u4"),
+])
+assert CYCLE_NODE.itemsize == 28 and CYCLE_NODE.fields["value"][1] == NODE_ENDS.fields["value"][1]
+
+
+class CycleInfo(C.Structure):
+    """alz_cycle_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("rows", "traversable", "self_rows", "nodes", "components", "cyclic",
+                                          "cyclic_nodes", "largest", "cycle_rows", "depth")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

@@ -49,6 +49,7 @@ EXPORTS = [
     "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
     "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
     "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach", "alz_group_reach_device",
+    "alz_cycles", "alz_cycles_device", "alz_group_cycles", "alz_group_cycles_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -207,6 +208,16 @@ def load(rebuild=False):
                                     C.POINTER(sz), C.POINTER(abi.ReachInfo)], i),
         "alz_debug_reach_rows": ([vp, vp, sz, vp, sz, u32, u32, vp, C.c_double, vp, sz, C.POINTER(sz), vp, vp, sz,
                                   C.POINTER(sz), C.POINTER(abi.ReachInfo)], i),
+        "alz_cycles": ([vp, u32, vp, C.c_double, u32, vp, sz, C.POINTER(sz), vp, vp, sz, C.POINTER(sz),
+                        C.POINTER(abi.CycleInfo)], i),
+        "alz_cycles_device": ([vp, u32, vp, C.c_double, u32, pp, C.POINTER(sz), pp, pp, C.POINTER(sz),
+                               C.POINTER(abi.CycleInfo)], i),
+        "alz_group_cycles": ([vp, u32, vp, C.c_double, u32, vp, sz, C.POINTER(sz), vp, vp, sz, C.POINTER(sz),
+                              C.POINTER(abi.CycleInfo)], i),
+        "alz_group_cycles_device": ([vp, u32, vp, C.c_double, u32, pp, C.POINTER(sz), pp, pp, C.POINTER(sz),
+                                     C.POINTER(abi.CycleInfo)], i),
+        "alz_debug_cycles_rows": ([vp, vp, sz, vp, C.c_double, u32, vp, sz, C.POINTER(sz), vp, vp, sz, C.POINTER(sz),
+                                   C.POINTER(abi.CycleInfo)], i),
         "alz_group_edge_changes": ([vp, u32, vp, u32, u32, vp, sz, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
         "alz_group_edge_changes_device": ([vp, u32, vp, u32, u32, pp, C.POINTER(sz), C.POINTER(abi.ChangeInfo)], i),
         "alz_group_edge_changes_top": ([vp, u32, vp, u32, u32, u32, C.c_double, vp, sz, C.POINTER(sz),
@@ -317,7 +328,8 @@ def load(rebuild=False):
                   "alz_group_edge_trends_device", "alz_group_edge_trends_top", "alz_group_edge_trends_top_device",
                   "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
                   "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach",
-                  "alz_group_reach_device", "alz_debug_reach_rows"):
+                  "alz_group_reach_device", "alz_debug_reach_rows", "alz_cycles", "alz_cycles_device",
+                  "alz_group_cycles", "alz_group_cycles_device", "alz_debug_cycles_rows"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -1430,6 +1442,58 @@ class Handle:
                 self.h2d(p, rows)
             return self._reach("alz_debug_reach_rows", (C.c_void_p(p), len(rows)), seeds, direction, max_hops, spec,
                                min_value)
+        finally:
+            self.dev_free(p)
+
+    # ---- cycles (alz_cycles.cu, docs/SPEC.md §28)
+    def _cycles(self, fn, head, spec, min_value, min_size):
+        """fn(h, *head, m, min_value, min_size, nodes, node_cap, &n_nodes, row_index, rows, row_cap, &n_rows, &info):
+        (CYCLE_NODE records, row_index, EDGE_OUT rows, info dict); a first call without arrays sizes them."""
+        f, nn, nr, info = getattr(self.L, fn), C.c_size_t(0), C.c_size_t(0), abi.CycleInfo()
+        m = abi.metrics(spec) if spec is not None else None
+        args = (self.h, *head, m, float(min_value), int(min_size))
+        self._ck(f(*args, None, 0, C.byref(nn), None, None, 0, C.byref(nr), C.byref(info)), fn)
+        nodes = np.zeros(nn.value, dtype=abi.CYCLE_NODE)
+        index = np.zeros(nr.value, dtype=np.uint32)
+        rows = np.zeros(nr.value, dtype=abi.EDGE_OUT)
+        self._ck(f(*args, _ptr(nodes), len(nodes), C.byref(nn), _ptr(index), _ptr(rows), len(rows), C.byref(nr),
+                   C.byref(info)), fn)
+        return nodes, index, rows, info.as_dict()
+
+    def _cycles_device(self, fn, source, spec, min_value, min_size):
+        pn, pi, pr, nn, nr, info = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_size_t(0), C.c_size_t(0), \
+            abi.CycleInfo()
+        m = abi.metrics(spec) if spec is not None else None
+        self._ck(getattr(self.L, fn)(self.h, int(source), m, float(min_value), int(min_size), C.byref(pn), C.byref(nn),
+                                     C.byref(pi), C.byref(pr), C.byref(nr), C.byref(info)), fn)
+        return pn.value, nn.value, pi.value, pr.value, nr.value, info.as_dict()
+
+    def cycles(self, source, spec=None, min_value=0.0, min_size=1):
+        """alz_cycles: the strongly connected components of `source`'s nodes, following only rows whose metric `spec`
+        is at least min_value when spec is given, listing the nodes of components of at least min_size nodes:
+        (CYCLE_NODE records, row positions, EDGE_OUT rows, info dict)."""
+        return self._cycles("alz_cycles", (int(source),), spec, min_value, min_size)
+
+    def cycles_device(self, source, spec=None, min_value=0.0, min_size=1):
+        """alz_cycles_device: (records pointer, nodes, row_index pointer, rows pointer, rows, info dict)."""
+        return self._cycles_device("alz_cycles_device", source, spec, min_value, min_size)
+
+    def group_cycles(self, source, spec=None, min_value=0.0, min_size=1):
+        """alz_group_cycles: cycles over the group-edge rows of `source` under the handle's map."""
+        return self._cycles("alz_group_cycles", (int(source),), spec, min_value, min_size)
+
+    def group_cycles_device(self, source, spec=None, min_value=0.0, min_size=1):
+        """alz_group_cycles_device: (records pointer, nodes, row_index pointer, rows pointer, rows, info dict)."""
+        return self._cycles_device("alz_group_cycles_device", source, spec, min_value, min_size)
+
+    def debug_cycles_rows(self, rows, spec=None, min_value=0.0, min_size=1):
+        """alz_debug_cycles_rows over a host EDGE_OUT array (copied to the device): as cycles."""
+        rows = np.ascontiguousarray(rows, dtype=abi.EDGE_OUT)
+        p = self.dev_alloc(max(rows.nbytes, 1))
+        try:
+            if len(rows):
+                self.h2d(p, rows)
+            return self._cycles("alz_debug_cycles_rows", (C.c_void_p(p), len(rows)), spec, min_value, min_size)
         finally:
             self.dev_free(p)
 

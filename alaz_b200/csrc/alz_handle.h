@@ -41,6 +41,7 @@ struct alz_node_series_state;   // alz_node_series.cu
 struct alz_group_state;         // alz_groups.cu
 struct alz_group_series_state;  // alz_group_series.cu
 struct alz_reach_state;         // alz_reach.cu
+struct alz_cycle_state;         // alz_cycles.cu
 
 // One host->device staging slot: pinned host buffer + device buffer. A submitting thread owns the slot
 // (mu) from the copy into the pinned buffer until its H2D and kernel are enqueued.
@@ -149,6 +150,8 @@ struct alz_handle {
                                                       // the first
   alz_reach_state* reach = nullptr;                   // the reach calls' buffers (alz_reach*, alz_group_reach*); null
                                                       // until the first
+  alz_cycle_state* cycles = nullptr;                  // the cycles calls' buffers (alz_cycles*, alz_group_cycles*);
+                                                      // null until the first
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -206,4 +209,5 @@ void alz_internal_free_groups(alz_handle* h);
 void alz_internal_free_group_series(alz_handle* h);
 void alz_internal_free_group_trends(alz_handle* h);
 void alz_internal_free_reach(alz_handle* h);
+void alz_internal_free_cycles(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

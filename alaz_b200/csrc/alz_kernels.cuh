@@ -74,6 +74,10 @@ size_t sort_pairs_temp_bytes(uint32_t n);
 // both return CUB's status: cudaErrorInvalidValue, with nothing enqueued, when temp_bytes is too small
 cudaError_t sort_pairs(void* temp, size_t temp_bytes, const uint64_t* keys_in, uint64_t* keys_out,
                        const uint32_t* vals_in, uint32_t* vals_out, uint32_t n, cudaStream_t s, int end_bit = 64);
+// radix sort of 64-bit keys alone, on bits [0, end_bit) (alz_sort.cu)
+size_t sort_keys_temp_bytes(uint32_t n);
+cudaError_t sort_keys(void* temp, size_t temp_bytes, const uint64_t* keys_in, uint64_t* keys_out, uint32_t n,
+                      cudaStream_t s, int end_bit);
 size_t scan_temp_bytes(uint32_t n);
 cudaError_t exclusive_scan_u32(void* temp, size_t temp_bytes, const uint32_t* in, uint32_t* out, uint32_t n,
                                cudaStream_t s);

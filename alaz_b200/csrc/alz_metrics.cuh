@@ -1,10 +1,10 @@
 // alz_metrics.cuh — what alz_metrics.cu shares with the changes (alz_changes.cu), the edge series (alz_series.cu),
 // the edge, node and group trends (alz_trends.cu), the node calls (alz_nodes.cu), the node series
-// (alz_node_series.cu), the groups (alz_groups.cu), the group series (alz_group_series.cu) and the reach calls
-// (alz_reach.cu): the §17 metric values of a row list, of node rows or of series slots, a source's rows, the rows'
-// packed keys, the grow-on-demand device buffers and launch grids, the node group-by, a source's edge, node or group
-// series into given buffers, the 64-bit top selection with its own scratch, the §24 group-by into given buffers and
-// the map lookup.
+// (alz_node_series.cu), the groups (alz_groups.cu), the group series (alz_group_series.cu), the reach calls
+// (alz_reach.cu) and the cycles calls (alz_cycles.cu): the §17 metric values of a row list, of node rows or of series
+// slots, a source's rows, the rows' packed keys, the grow-on-demand device buffers and launch grids, the node
+// group-by, a source's edge, node or group series into given buffers, the 64-bit top selection with its own scratch,
+// the §24 group-by into given buffers, the map lookup and the graph of a row list.
 #pragma once
 #include <algorithm>
 #include <cstdint>
@@ -273,6 +273,28 @@ int group_edges_into(alz_handle* h, DevBuf& out, const alz_edge_out* rows, size_
 int group_nodes_into(alz_handle* h, DevBuf& out, const alz_edge_out* edges, size_t n, size_t* n_nodes);
 // The map's generation: every alz_group_set that succeeds moves it on (0 before the first)
 uint64_t group_map_generation(const alz_handle* h);
+
+// The graph of a traversed row list (alz_reach.cu), which the reach and cycles calls (alz_cycles.cu) search: each row
+// end's node index (§21 node list order), each node's key, which rows are traversable, and CSRs by tail
+struct Graph {
+  NodeGroup g;                  // the §21 group-by of the rows' ends
+  DevBuf end_node, node_keys;   // end_node[2r] row r's to end's index, [2r + 1] its from end's; node_keys[index]
+  DevBuf values, trav;          // the filter's metric values, each row traversable (1) or not (0)
+  DevBuf tmp;                   // CUB scratch: a scan of max(nodes, rows) + 1 words
+  uint32_t nodes = 0;
+  void free();
+};
+// A CSR by tail: off[nodes + 1], and adj[off[u] ..] = (head << 32) | row for each orientation of a traversable row
+// with tail u that the direction follows (ALZ_REACH_DOWN: from -> to; UP: to -> from; ANY: both)
+struct Csr {
+  DevBuf off, cursor, adj;
+  void free();
+};
+// gr over n rows: the §21 sort of the ends (one wait, for the node count), the index scatter, with ms the metric
+// filter (a row is traversable when key(value) >= key(min_value)), then one CSR per (direction, csr) pair, on the
+// stream. Caller holds h->mu and has set the device; 0 < n <= kMaxNodeSourceRows.
+int graph_build(alz_handle* h, Graph& gr, const alz_edge_out* rows, uint32_t n, const MetricSet* ms, double min_value,
+                std::initializer_list<std::pair<uint32_t, Csr*>> csrs);
 
 }  // namespace metrics
 }  // namespace alz

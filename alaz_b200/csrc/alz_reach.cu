@@ -247,15 +247,85 @@ __global__ void __launch_bounds__(256) reach_emit_kernel(const uint32_t* __restr
 
 }  // namespace
 
+namespace alz {
+namespace metrics {
+
+void Graph::free() {
+  g.free();
+  free_bufs({&end_node, &node_keys, &values, &trav, &tmp});
+}
+
+void Csr::free() { free_bufs({&off, &cursor, &adj}); }
+
+int graph_build(alz_handle* h, Graph& gr, const alz_edge_out* rows, uint32_t n, const MetricSet* ms, double min_value,
+                std::initializer_list<std::pair<uint32_t, Csr*>> csrs) {
+  cudaStream_t st = h->stream;
+  const uint32_t n2 = 2u * n;
+  NodeGroup& g = gr.g;
+  int rc = node_group_reserve(h, g, n2);
+  if (rc != ALZ_OK) return rc;
+  node_group_keys(h, g, rows, n);
+  rc = node_group_runs(h, g, n2, kNodeKeyBits);   // the wait for the node count
+  if (rc != ALZ_OK) return rc;
+  const uint32_t N = g.h_words[0];
+  gr.nodes = N;
+  rc = reserve(h, {{&gr.end_node, (size_t)n2 * 4},
+                   {&gr.node_keys, (size_t)N * 8},
+                   {&gr.values, ms ? (size_t)n * 8 : 0},
+                   {&gr.trav, n},
+                   {&gr.tmp, scan_temp_bytes(std::max(N, n) + 1u)}});
+  if (rc != ALZ_OK) return rc;
+  for (const auto& c : csrs) {
+    const uint32_t entries_max = c.first == ALZ_REACH_ANY ? n2 : n;
+    rc = reserve(h, {{&c.second->off, ((size_t)N + 1) * 4},
+                     {&c.second->cursor, ((size_t)N + 1) * 4},
+                     {&c.second->adj, (size_t)entries_max * 8}});
+    if (rc != ALZ_OK) return rc;
+  }
+  uint32_t* end_node = static_cast<uint32_t*>(gr.end_node.p);
+  uint8_t* trav = static_cast<uint8_t*>(gr.trav.p);
+  reach_index_kernel<<<grid_for(h, n2, 8), 256, 0, st>>>(static_cast<const uint64_t*>(g.keys_out.p),
+                                                         static_cast<const uint32_t*>(g.vals_out.p),
+                                                         static_cast<const uint32_t*>(g.heads.p),
+                                                         static_cast<const uint32_t*>(g.idx.p), n2, end_node,
+                                                         static_cast<uint64_t*>(gr.node_keys.p));
+  h->launches += 1;
+  const uint64_t* vals = nullptr;
+  uint64_t min_key = 0;
+  if (ms) {
+    rc = run_metrics(h, rows, n, *ms, static_cast<double*>(gr.values.p));
+    if (rc != ALZ_OK) return rc;
+    vals = static_cast<const uint64_t*>(gr.values.p);
+    uint64_t bits;
+    memcpy(&bits, &min_value, 8);
+    min_key = top::order_key(bits);
+  }
+  for (const auto& c : csrs) {
+    uint32_t* adj_off = static_cast<uint32_t*>(c.second->off.p);
+    uint32_t* cursor = static_cast<uint32_t*>(c.second->cursor.p);
+    CK(cudaMemsetAsync(cursor, 0, ((size_t)N + 1) * 4, st));
+    reach_count_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(end_node, n, c.first, vals, min_key, trav, cursor);
+    CK(cudaGetLastError());
+    CK(exclusive_scan_u32(gr.tmp.p, gr.tmp.bytes, cursor, adj_off, N + 1, st));
+    CK(cudaMemcpyAsync(cursor, adj_off, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
+    reach_fill_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(end_node, n, c.first, trav, cursor,
+                                                         static_cast<uint64_t*>(c.second->adj.p));
+    h->launches += 2;
+  }
+  return ALZ_OK;
+}
+
+}  // namespace metrics
+}  // namespace alz
+
 // Buffers of the reach calls, each grown on demand and never shrunk; freed in alz_destroy
 struct alz_reach_state {
-  NodeGroup g;                         // the §21 group-by of the traversed rows' ends
+  Graph gr;                            // the traversed rows' nodes, traversable rows and scan scratch
+  Csr csr;                             // by tail, in the call's direction
   DevBuf edges;                        // group form: the source's group-edge rows
-  DevBuf end_node, node_keys, seeds;   // each row end's node index, each node's key, the packed seeds
-  DevBuf values, trav;                 // the filter's metric values, each row traversable or not
-  DevBuf adj_off, cursor, adj;         // the CSR by tail
+  DevBuf seeds;                        // the packed seeds
   DevBuf hops, best, flag, scan;       // per node (flag and scan also per row)
-  DevBuf pos, deg, dscan, ctr, tmp;    // node -> result position, the frontier's degrees, the cut, CUB scratch
+  DevBuf pos, deg, dscan, ctr;         // node -> result position, the frontier's degrees, the cut
   DevBuf row_pos, row_vals;            // the listed rows' positions, the gather's value scratch
   DevBuf order, row_index, rows;       // the results: nodes in result order (then the records), rows
   DevBuf rec;
@@ -265,9 +335,9 @@ struct alz_reach_state {
 void alz_internal_free_reach(alz_handle* h) {
   alz_reach_state* s = h->reach;
   if (!s) return;
-  s->g.free();
-  free_bufs({&s->edges, &s->end_node, &s->node_keys, &s->seeds, &s->values, &s->trav, &s->adj_off, &s->cursor,
-             &s->adj, &s->hops, &s->best, &s->flag, &s->scan, &s->pos, &s->deg, &s->dscan, &s->ctr, &s->tmp,
+  s->gr.free();
+  s->csr.free();
+  free_bufs({&s->edges, &s->seeds, &s->hops, &s->best, &s->flag, &s->scan, &s->pos, &s->deg, &s->dscan, &s->ctr,
              &s->row_pos, &s->row_vals, &s->order, &s->row_index, &s->rows, &s->rec});
   if (s->h_words) cudaFreeHost(s->h_words);
   delete s;
@@ -308,24 +378,12 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
   res->info.rows = n_rows;
   if (n_rows == 0) return ALZ_OK;
   cudaStream_t st = h->stream;
-  const uint32_t n = (uint32_t)n_rows, n2 = 2u * n;
-  NodeGroup& g = s->g;
-  int rc = node_group_reserve(h, g, n2);
+  const uint32_t n = (uint32_t)n_rows;
+  int rc = graph_build(h, s->gr, rows, n, q.filter ? &q.ms : nullptr, q.min_value, {{q.dir, &s->csr}});
   if (rc != ALZ_OK) return rc;
-  node_group_keys(h, g, rows, n);
-  rc = node_group_runs(h, g, n2, kNodeKeyBits);   // the wait for the node count
-  if (rc != ALZ_OK) return rc;
-  const uint32_t N = g.h_words[0];
-  const uint32_t entries_max = q.dir == ALZ_REACH_ANY ? n2 : n;
+  const uint32_t N = s->gr.nodes;
   const uint32_t flags = std::max(N, n) + 1u;
-  rc = reserve(h, {{&s->end_node, (size_t)n2 * 4},
-                   {&s->node_keys, (size_t)N * 8},
-                   {&s->seeds, q.n_seeds * 8},
-                   {&s->values, q.filter ? (size_t)n * 8 : 0},
-                   {&s->trav, n},
-                   {&s->adj_off, ((size_t)N + 1) * 4},
-                   {&s->cursor, ((size_t)N + 1) * 4},
-                   {&s->adj, (size_t)entries_max * 8},
+  rc = reserve(h, {{&s->seeds, q.n_seeds * 8},
                    {&s->hops, (size_t)N * 4},
                    {&s->best, (size_t)N * 8},
                    {&s->flag, (size_t)flags * 4},
@@ -335,8 +393,7 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
                    {&s->dscan, ((size_t)N + 1) * 4},
                    {&s->ctr, 16},
                    {&s->order, (size_t)N * 4},
-                   {&s->row_pos, (size_t)n * 4},
-                   {&s->tmp, scan_temp_bytes(flags)}});
+                   {&s->row_pos, (size_t)n * 4}});
   if (rc != ALZ_OK) return rc;
   if (!s->h_words) {
     void* p = nullptr;
@@ -346,25 +403,21 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
     }
     s->h_words = static_cast<uint64_t*>(p);
   }
-  uint32_t* end_node = static_cast<uint32_t*>(s->end_node.p);
-  uint64_t* node_keys = static_cast<uint64_t*>(s->node_keys.p);
-  uint32_t* adj_off = static_cast<uint32_t*>(s->adj_off.p);
-  uint32_t* cursor = static_cast<uint32_t*>(s->cursor.p);
-  uint64_t* adj = static_cast<uint64_t*>(s->adj.p);
+  const uint32_t* end_node = static_cast<const uint32_t*>(s->gr.end_node.p);
+  const uint64_t* node_keys = static_cast<const uint64_t*>(s->gr.node_keys.p);
+  const uint32_t* adj_off = static_cast<const uint32_t*>(s->csr.off.p);
+  const uint64_t* adj = static_cast<const uint64_t*>(s->csr.adj.p);
+  const uint8_t* trav = static_cast<const uint8_t*>(s->gr.trav.p);
+  void* tmp = s->gr.tmp.p;
+  const size_t tmp_bytes = s->gr.tmp.bytes;
   uint32_t* hops = static_cast<uint32_t*>(s->hops.p);
   uint64_t* best = static_cast<uint64_t*>(s->best.p);
   uint32_t* flag = static_cast<uint32_t*>(s->flag.p);
   uint32_t* scan = static_cast<uint32_t*>(s->scan.p);
   uint32_t* pos = static_cast<uint32_t*>(s->pos.p);
   uint32_t* order = static_cast<uint32_t*>(s->order.p);
-  uint8_t* trav = static_cast<uint8_t*>(s->trav.p);
   unsigned long long* cut = static_cast<unsigned long long*>(s->ctr.p);
   uint32_t* entries = reinterpret_cast<uint32_t*>(cut + 1);   // the next frontier's adjacency entries
-  reach_index_kernel<<<grid_for(h, n2, 8), 256, 0, st>>>(static_cast<const uint64_t*>(g.keys_out.p),
-                                                         static_cast<const uint32_t*>(g.vals_out.p),
-                                                         static_cast<const uint32_t*>(g.heads.p),
-                                                         static_cast<const uint32_t*>(g.idx.p), n2, end_node,
-                                                         node_keys);
   // seeds
   std::vector<uint64_t> packed(q.n_seeds);
   for (size_t i = 0; i < q.n_seeds; ++i) packed[i] = ((uint64_t)q.seeds[i].type << 32) | q.seeds[i].value;
@@ -373,31 +426,13 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
   CK(cudaMemsetAsync(best, 0xFF, (size_t)N * 8, st));
   reach_seed_kernel<<<grid_for(h, q.n_seeds, 8), 256, 0, st>>>(static_cast<const uint64_t*>(s->seeds.p),
                                                                 (uint32_t)q.n_seeds, node_keys, N, hops);
-  h->launches += 2;
-  // filter and adjacency
-  const uint64_t* vals = nullptr;
-  uint64_t min_key = 0;
-  if (q.filter) {
-    rc = run_metrics(h, rows, n, q.ms, static_cast<double*>(s->values.p));
-    if (rc != ALZ_OK) return rc;
-    vals = static_cast<const uint64_t*>(s->values.p);
-    uint64_t bits;
-    memcpy(&bits, &q.min_value, 8);
-    min_key = top::order_key(bits);
-  }
-  CK(cudaMemsetAsync(cursor, 0, ((size_t)N + 1) * 4, st));
-  reach_count_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(end_node, n, q.dir, vals, min_key, trav, cursor);
-  CK(cudaGetLastError());
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, cursor, adj_off, N + 1, st));
-  CK(cudaMemcpyAsync(cursor, adj_off, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
-  reach_fill_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(end_node, n, q.dir, trav, cursor, adj);
-  h->launches += 2;
+  h->launches += 1;
   // level 0: the seeds found
   uint32_t off = 0, size = 0;
   CK(cudaMemsetAsync(entries, 0, 4, st));
   reach_discover_kernel<<<grid_for(h, N, 8), 256, 0, st>>>(best, N, 0, adj_off, hops, flag, entries);
   CK(cudaGetLastError());
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, flag, scan, N + 1, st));
+  CK(exclusive_scan_u32(tmp, tmp_bytes, flag, scan, N + 1, st));
   reach_scatter_kernel<<<grid_for(h, N, 8), 256, 0, st>>>(flag, scan, N, 0, order, pos);
   h->launches += 2;
   REACH_READ(0, scan + N, 4);
@@ -414,14 +449,14 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
     uint32_t* dscan = static_cast<uint32_t*>(s->dscan.p);
     reach_degree_kernel<<<grid_for(h, size, 8), 256, 0, st>>>(frontier, size, adj_off, deg);
     CK(cudaGetLastError());
-    CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, deg, dscan, size + 1, st));
+    CK(exclusive_scan_u32(tmp, tmp_bytes, deg, dscan, size + 1, st));
     const uint32_t frontier_entries = (uint32_t)s->h_words[3];   // read with the frontier's size
     reach_expand_kernel<<<grid_for(h, frontier_entries, 8), 256, 0, st>>>(frontier, size, dscan, adj_off, adj, hops,
                                                                           reinterpret_cast<unsigned long long*>(best));
     CK(cudaMemsetAsync(entries, 0, 4, st));
     reach_discover_kernel<<<grid_for(h, N, 8), 256, 0, st>>>(best, N, level + 1, adj_off, hops, flag, entries);
     CK(cudaGetLastError());
-    CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, flag, scan, N + 1, st));
+    CK(exclusive_scan_u32(tmp, tmp_bytes, flag, scan, N + 1, st));
     reach_scatter_kernel<<<grid_for(h, N, 8), 256, 0, st>>>(flag, scan, N, off + size, order, pos);
     h->launches += 4;
     REACH_READ(0, scan + N, 4);
@@ -439,7 +474,7 @@ int run_reach(alz_handle* h, alz_reach_state* s, const alz_edge_out* rows, size_
   CK(cudaMemsetAsync(cut, 0, 8, st));
   reach_rows_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(end_node, n, q.dir, trav, hops, q.max_hops, flag, cut);
   CK(cudaGetLastError());
-  CK(exclusive_scan_u32(s->tmp.p, s->tmp.bytes, flag, scan, n + 1, st));
+  CK(exclusive_scan_u32(tmp, tmp_bytes, flag, scan, n + 1, st));
   reach_scatter_kernel<<<grid_for(h, n, 8), 256, 0, st>>>(flag, scan, n, 0, static_cast<uint32_t*>(s->row_pos.p),
                                                           nullptr);
   h->launches += 2;

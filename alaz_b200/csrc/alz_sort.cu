@@ -20,6 +20,15 @@ cudaError_t sort_pairs(void* temp, size_t temp_bytes, const uint64_t* keys_in, u
   // end_bit: only key bits [0, end_bit) differ between keys (each 8 bits less is one pass over the data less)
   return cub::DeviceRadixSort::SortPairs(temp, temp_bytes, keys_in, keys_out, vals_in, vals_out, (int)n, 0, end_bit, s);
 }
+size_t sort_keys_temp_bytes(uint32_t n) {
+  size_t bytes = 0;
+  cub::DeviceRadixSort::SortKeys(nullptr, bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)n);
+  return bytes;
+}
+cudaError_t sort_keys(void* temp, size_t temp_bytes, const uint64_t* keys_in, uint64_t* keys_out, uint32_t n,
+                      cudaStream_t s, int end_bit) {
+  return cub::DeviceRadixSort::SortKeys(temp, temp_bytes, keys_in, keys_out, (int)n, 0, end_bit, s);
+}
 size_t scan_temp_bytes(uint32_t n) {
   size_t bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n);

@@ -1150,6 +1150,64 @@ int Aggregator::RunReach(bool group, uint32_t source, const std::vector<NodeRef>
   return ALZ_OK;
 }
 
+int Aggregator::Cycles(uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+                       std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info) {
+  return RunCycles(false, source, filter, min_value, min_size, nodes, rows, info);
+}
+
+int Aggregator::GroupCycles(uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+                            std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info) {
+  return RunCycles(true, source, filter, min_value, min_size, nodes, rows, info);
+}
+
+int Aggregator::RunCycles(bool group, uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+                          std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info) {
+  if (!h_) return ALZ_E_STATE;
+  if (!nodes || !rows) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  if (info) *info = alz_cycle_info{};
+  nodes->clear();
+  rows->clear();
+  if (group) {
+    const int rc = SyncGroups();
+    if (rc != ALZ_OK) return rc;
+  }
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  // never empty: a null array would not be written (and its cap not checked)
+  if (cycle_nodes_.empty()) cycle_nodes_.resize(1);
+  if (cycle_index_.empty()) cycle_index_.resize(1);
+  if (roll_.empty()) roll_.resize(1);
+  auto call = [&](size_t* nn, size_t* nr) {
+    return (group ? alz_group_cycles : alz_cycles)(h_, src, filter, min_value, min_size, cycle_nodes_.data(),
+                                                   cycle_nodes_.size(), nn, cycle_index_.data(), roll_.data(),
+                                                   std::min(cycle_index_.size(), roll_.size()), nr, info);
+  };
+  // into cycle_nodes_ / cycle_index_ / roll_, grown once when the results do not fit (ALZ_E_CAPACITY with the counts
+  // set; nothing written)
+  size_t nn = 0, nr = 0;
+  int rc = call(&nn, &nr);
+  if (rc == ALZ_E_CAPACITY && (nn > cycle_nodes_.size() || nr > cycle_index_.size() || nr > roll_.size())) {
+    cycle_nodes_.resize(std::max(nn, cycle_nodes_.size()));
+    cycle_index_.resize(std::max(nr, cycle_index_.size()));
+    roll_.resize(std::max(nr, roll_.size()));
+    rc = call(&nn, &nr);
+  }
+  if (rc != ALZ_OK) return rc;
+  *rows = ToEdges(roll_.data(), nr, nullptr);
+  nodes->resize(nn);
+  for (size_t i = 0; i < nn; ++i) {
+    const alz_cycle_node& r = cycle_nodes_[i];
+    CycleNode& o = (*nodes)[i];
+    o.Type = NodeTypeName(r.type);
+    o.UID = UidOf(r.type, r.value);
+    o.Component = r.component;
+    o.Size = r.size;
+    o.Depth = r.depth;
+    o.Height = r.height;
+  }
+  return ALZ_OK;
+}
+
 int Aggregator::GroupNodeSeriesFor(const std::vector<NodeRef>& nodes, uint32_t side, uint32_t tier, uint32_t k,
                                    const std::vector<alz_metric>& metrics, std::vector<NodeSeriesRow>* out,
                                    std::vector<alz_rollup_info>* points) {

@@ -131,6 +131,13 @@ struct ReachNode {
   uint32_t Hops = 0, Parent = 0, Row = 0;
 };
 
+// one node of a cycles call (docs/SPEC.md §28): named as Nodes / GroupNodes name it, its component's number, node
+// count, depth (the most rows between components on a path that ends at it) and height (on a path that starts at it)
+struct CycleNode {
+  std::string Type, UID;
+  uint32_t Component = 0, Size = 0, Depth = 0, Height = 0;
+};
+
 // one node's series (docs/SPEC.md §22): per point, oldest first, whether that entry holds a row on the side of the
 // node and the metrics' values of the side's sums there (every value 0 where it does not)
 struct NodeSeriesRow {
@@ -363,6 +370,18 @@ class Aggregator {
                  const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
                  std::vector<EdgeWindow>* rows, alz_reach_info* info = nullptr);
   static constexpr uint32_t kReachNone = 0xFFFFFFFFu;   // ReachNode.Parent / Row of a seed
+  // Cycles (docs/SPEC.md §28): the strongly connected components of `source`'s nodes, following rows from caller to
+  // callee. *nodes lists the nodes of every component of at least min_size nodes (2: the services on a loop) in
+  // (component, node index) order; *rows the rows inside the listed loops, by component then source order, named as
+  // ToEdges names ends. filter (may be null): only rows whose value of that metric is >= min_value are followed
+  // ("loops of failing calls"). info may be null. Returns 0 or an alz_status.
+  int Cycles(uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+             std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info = nullptr);
+  // Cycles over the group-edge rows of `source` under the map SetGroups gave (sent first, as for every group call):
+  // "which deployments call each other in a loop". A group's internal rows never make it a loop. Nodes and rows are
+  // named as GroupNodes / GroupEdges name them.
+  int GroupCycles(uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+                  std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info = nullptr);
   int Stats(alz_stats* out);
   // one tick of clearSocketLines (aggregator/data.go:1681-1716, every 120 s there): with send_alive (the
   // reference's SEND_ALIVE_TCP_CONNECTIONS) every open connection with a pod at its source goes to
@@ -401,6 +420,9 @@ class Aggregator {
   int RunReach(bool group, uint32_t source, const std::vector<NodeRef>& seeds, uint32_t dir, uint32_t max_hops,
                const alz_metric* filter, double min_value, std::vector<ReachNode>* nodes,
                std::vector<EdgeWindow>* rows, alz_reach_info* info);
+  // Cycles and GroupCycles: the call, the results named
+  int RunCycles(bool group, uint32_t source, const alz_metric* filter, double min_value, uint32_t min_size,
+                std::vector<CycleNode>* nodes, std::vector<EdgeWindow>* rows, alz_cycle_info* info);
   // ends -> the library's key of an edge named by UID; false when a UID has no id
   bool ToEnds(const EdgeRef& e, alz_edge_ends* out) const;
   // a series call(values, present, cap, &n, &P, points) into series_values_ / series_present_, then each series
@@ -483,6 +505,8 @@ class Aggregator {
   std::vector<alz_node_out> node_trend_rows_;
   std::vector<alz_reach_node> reach_nodes_;   // the records and row positions of the last Reach / GroupReach
   std::vector<uint32_t> reach_index_;
+  std::vector<alz_cycle_node> cycle_nodes_;   // the records and row positions of the last Cycles / GroupCycles
+  std::vector<uint32_t> cycle_index_;
   std::vector<GroupMember> members_;                    // the group map as SetGroups gave it
   std::unordered_map<std::string, uint32_t> group_ids_;  // group name -> dense id (ALZ_NODE_GROUP)
   std::vector<std::string> group_names_;

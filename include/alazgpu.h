@@ -1112,6 +1112,74 @@ int alz_group_reach_device(alz_handle* h, uint32_t source, const alz_node_ends* 
                            size_t* n_nodes, const uint32_t** dev_row_index, const alz_edge_out** dev_rows,
                            size_t* n_rows, alz_reach_info* info);
 
+/* ---- cycles (docs/SPEC.md §28) --------------------------------------------------------------------------------------
+ * The strongly connected components of a source's graph (ALZ_SOURCE_WINDOW or ALZ_ROLLUP_*, with the availability
+ * rule of §15), with each component's depth and height. alz_cycles* traverses the source's rows and its nodes are
+ * alz_node_rows(source); alz_group_cycles* traverses the source's group-edge rows under the map in force at the call
+ * (§24; an empty map is allowed) and its nodes are alz_group_nodes(source). A node's index is its position in that node
+ * list. With m NULL every row is traversable and min_value is ignored; otherwise m is one §17 metric and a row is
+ * traversable when the IEEE total-order key of its value is at least key(min_value), as in §27.
+ * A self row is a traversable row whose from end and to end are one node (in the group form every internal row g -> g):
+ * it never makes a component cyclic, is never listed and is counted in info->self_rows.
+ * Components: two nodes are in one component when each reaches the other along traversable rows (from end -> to end).
+ * Every node is in exactly one, nodes without a traversable row included. Components are numbered from 0 in ascending
+ * order of their smallest node index; one of 2 or more nodes is cyclic. A traversable row between two components is a
+ * row of the condensation: depth(C) is the most condensation rows on a path that ends at C (0 without one into C),
+ * height(C) the most on a path that starts at C. Every node carries its component's number, size, depth and height.
+ * Nodes: the nodes of every component of at least min_size nodes (0 or 1: all; 2: the nodes on cycles), ordered by
+ * (component, index). Rows: every traversable row that is not a self row and whose two ends lie in one listed cyclic
+ * component, ordered by (component, row position): row_index[j] its position in the traversed list, rows[j] the row byte
+ * for byte (a source row, or a group-edge row for the group form). The components are unique, so every byte of the
+ * result follows from the rows whatever the order of the work.
+ * An unknown source, a null n_nodes or n_rows, a bad metric (§17) or a NaN min_value with a metric: ALZ_E_INVAL. No rows
+ * of a rollup source: ALZ_E_STATE. More than 2^29 - 1 source rows (before anything runs): ALZ_E_CAPACITY; no memory:
+ * ALZ_E_NOMEM. A 0-row source: 0 nodes, 0 rows, ALZ_OK. *n_nodes and *n_rows are always set. Host forms: nodes,
+ * row_index and rows may each be NULL; node_cap is checked when nodes is not NULL and row_cap when row_index or rows is
+ * not; a failed check returns ALZ_E_CAPACITY and writes none of the three. Device forms: dev_nodes, dev_row_index and
+ * dev_rows may each be NULL; the results stay valid until the next cycles call of either form. info may be NULL.
+ * Waits: one for the node count (§21), one for the totals that size the results, and a host call one more for its
+ * copies; the group form adds §24's two. The fixed-point phases run in cooperative launches with grid-wide barriers, so
+ * the waits do not grow with their rounds. The rounds are data-dependent: about one per node on a chain or a ring, and
+ * O(N^2) for N nodes in the worst case (each colouring iteration may take about N rounds and settle one component;
+ * iterations alternate direction, which settles a chain of loops in two, but layouts that defeat both may exist). Reads only: the window, every ring, the open blocks, every rollup's rows and info, the
+ * baseline and its caches, the map and every other family's device results are unchanged; cycles keeps its buffers in
+ * a state of its own, grown on demand and freed in alz_destroy. Every rank holds the same rows and the same map, so
+ * every rank returns the same bytes with no collective. */
+typedef struct alz_cycle_node {   /* 28 B; the first 8 bytes are an alz_node_ends */
+  uint8_t type;                   /* ALZ_NODE_* */
+  uint8_t _pad[3];                /* zero */
+  uint32_t value;
+  uint32_t index;                 /* the node's position in the traversed rows' node list */
+  uint32_t component;             /* its component's number */
+  uint32_t size;                  /* the component's node count */
+  uint32_t depth;                 /* the component's depth in the condensation */
+  uint32_t height;                /* the component's height in the condensation */
+} alz_cycle_node;
+typedef struct alz_cycle_info {
+  uint64_t rows;           /* traversed rows */
+  uint64_t traversable;    /* of which traversable */
+  uint64_t self_rows;      /* of which self rows */
+  uint64_t nodes;          /* nodes of the traversed rows */
+  uint64_t components;     /* components */
+  uint64_t cyclic;         /* components of 2 or more nodes */
+  uint64_t cyclic_nodes;   /* their nodes */
+  uint64_t largest;        /* the node count of the largest component */
+  uint64_t cycle_rows;     /* traversable rows that are not self rows inside cyclic components, whatever min_size */
+  uint64_t depth;          /* the largest depth (= the largest height) */
+} alz_cycle_info;
+int alz_cycles(alz_handle* h, uint32_t source, const alz_metric* m, double min_value, uint32_t min_size,
+               alz_cycle_node* nodes, size_t node_cap, size_t* n_nodes, uint32_t* row_index, alz_edge_out* rows,
+               size_t row_cap, size_t* n_rows, alz_cycle_info* info);
+int alz_cycles_device(alz_handle* h, uint32_t source, const alz_metric* m, double min_value, uint32_t min_size,
+                      const alz_cycle_node** dev_nodes, size_t* n_nodes, const uint32_t** dev_row_index,
+                      const alz_edge_out** dev_rows, size_t* n_rows, alz_cycle_info* info);
+int alz_group_cycles(alz_handle* h, uint32_t source, const alz_metric* m, double min_value, uint32_t min_size,
+                     alz_cycle_node* nodes, size_t node_cap, size_t* n_nodes, uint32_t* row_index, alz_edge_out* rows,
+                     size_t row_cap, size_t* n_rows, alz_cycle_info* info);
+int alz_group_cycles_device(alz_handle* h, uint32_t source, const alz_metric* m, double min_value, uint32_t min_size,
+                            const alz_cycle_node** dev_nodes, size_t* n_nodes, const uint32_t** dev_row_index,
+                            const alz_edge_out** dev_rows, size_t* n_rows, alz_cycle_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

@@ -88,6 +88,14 @@ int alz_debug_reach_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, 
                          size_t n_seeds, uint32_t dir, uint32_t max_hops, const alz_metric* m, double min_value,
                          alz_reach_node* nodes, size_t node_cap, size_t* n_nodes, uint32_t* row_index,
                          alz_edge_out* rows, size_t row_cap, size_t* n_rows, alz_reach_info* info);
+/* test/debug: alz_cycles (docs/SPEC.md §28) over n caller rows in device memory, which may hold layouts ingest cannot
+ * make (any row order, any type byte, repeated ends, long chains and rings, one node on 2^20 rows); the traversed rows
+ * are the caller's rows and the node list their §21 node list. More than 2^29 - 1 rows: ALZ_E_CAPACITY. The rules of
+ * alz_cycles otherwise. Uses the cycles calls' buffers. */
+int alz_debug_cycles_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n, const alz_metric* m, double min_value,
+                          uint32_t min_size, alz_cycle_node* nodes, size_t node_cap, size_t* n_nodes,
+                          uint32_t* row_index, alz_edge_out* rows, size_t row_cap, size_t* n_rows,
+                          alz_cycle_info* info);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
