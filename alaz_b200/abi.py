@@ -295,6 +295,45 @@ class CycleInfo(C.Structure):
         return {n: int(getattr(self, n)) for n, _ in self._fields_}
 
 
+CORR_POSITIVE, CORR_NEGATIVE, CORR_ABS = 0, 1, 2                     # alz_corr directions (§29)
+CORR_ABSENT_SKIP, CORR_ABSENT_ZERO = 0, 1                           # absent modes
+CORR_MAX_LAG = 32
+
+EDGE_CORR = np.dtype([                                              # alz_edge_corr
+    ("from_type", "u1"), ("to_type", "u1"), ("valid", "u1"), ("lag", "u1"), ("_pad", "u1", (4,)),
+    ("from", "<u4"), ("to", "<u4"), ("index", "<u4"), ("used", "<u4"),
+    ("r", "<f8"), ("score", "<f8"), ("r0", "<f8"),
+])
+assert EDGE_CORR.itemsize == 48
+NODE_CORR = np.dtype([                                              # alz_node_corr
+    ("type", "u1"), ("_pad0", "u1"), ("valid", "u1"), ("lag", "u1"), ("_pad1", "u1", (4,)),
+    ("value", "<u4"), ("_pad2", "<u4"), ("index", "<u4"), ("used", "<u4"),
+    ("r", "<f8"), ("score", "<f8"), ("r0", "<f8"),
+])
+assert NODE_CORR.itemsize == 48
+assert all(NODE_CORR.fields[f][1] == EDGE_CORR.fields[f][1]
+           for f in ("valid", "lag", "index", "used", "r", "score", "r0"))   # laid out as EDGE_CORR from valid on
+
+
+class Corr(C.Structure):
+    """alz_corr: direction CORR_*, absent CORR_ABSENT_*, lags 0 .. max_lag, a defined lag uses >= min_points pairs."""
+    _fields_ = [(n, C.c_uint32) for n in ("direction", "absent", "max_lag", "min_points")]
+
+
+class CorrTarget(C.Structure):
+    """alz_corr_target: n values (and presence bytes, or NULL) in host memory, the window_last of the newest point."""
+    _fields_ = [("values", C.c_void_p), ("present", C.c_void_p), ("n", C.c_size_t), ("window_last", C.c_uint64)]
+
+
+class CorrInfo(C.Structure):
+    """alz_corr_info."""
+    _fields_ = [(n, C.c_uint64) for n in ("rows", "rows_in", "valid", "above")] + \
+        [(n, C.c_uint32) for n in ("points", "tier", "target_used", "_pad")]
+
+    def as_dict(self):
+        return {n: int(getattr(self, n)) for n, _ in self._fields_ if n != "_pad"}
+
+
 class SpanInfo(C.Structure):
     """alz_span_info."""
     _fields_ = [("r", RollupInfo), ("entries", C.c_uint32 * (1 + MAX_TIERS)), ("open_blocks", C.c_uint32),

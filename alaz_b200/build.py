@@ -12,7 +12,7 @@ LIB = os.path.join(LIB_DIR, "libalazgpu.so")
 SOURCES = ["alz_api.cu", "alz_kernels.cu", "alz_ingest.cu", "alz_sort.cu", "alz_comm.cu", "alz_gnn.cu", "alz_sock.cu",
            "alz_rollup.cu", "alz_top.cu", "alz_metrics.cu", "alz_changes.cu",
            "alz_series.cu", "alz_trends.cu", "alz_nodes.cu", "alz_node_series.cu",
-           "alz_groups.cu", "alz_group_series.cu", "alz_reach.cu", "alz_cycles.cu"]
+           "alz_groups.cu", "alz_group_series.cu", "alz_reach.cu", "alz_cycles.cu", "alz_corr.cu"]
 EXTRA = [os.path.join(HERE, "synth", "alz_synth_topo.c")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

@@ -50,6 +50,12 @@ EXPORTS = [
     "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
     "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach", "alz_group_reach_device",
     "alz_cycles", "alz_cycles_device", "alz_group_cycles", "alz_group_cycles_device",
+    "alz_edge_correlations", "alz_edge_correlations_device", "alz_edge_correlations_top",
+    "alz_edge_correlations_top_device", "alz_node_correlations", "alz_node_correlations_device",
+    "alz_node_correlations_top", "alz_node_correlations_top_device", "alz_group_edge_correlations",
+    "alz_group_edge_correlations_device", "alz_group_edge_correlations_top", "alz_group_edge_correlations_top_device",
+    "alz_group_node_correlations", "alz_group_node_correlations_device", "alz_group_node_correlations_top",
+    "alz_group_node_correlations_top_device",
     "alz_edge_quantiles", "alz_submit_tcp", "alz_submit_tcp_raw", "alz_sock_lookup", "alz_sock_lookup_at",
     "alz_submit_l7_join", "alz_sock_gc", "alz_sock_alive", "alz_sock_stats", "alz_comm_unique_id", "alz_comm_init",
     "alz_owner_rank",
@@ -267,6 +273,40 @@ def load(rebuild=False):
         "alz_group_node_trends_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Trend), u32, C.c_double, pp,
                                               pp, pp, pp, C.POINTER(sz), C.POINTER(u32), vp,
                                               C.POINTER(abi.TrendInfo)], i),
+        "alz_edge_correlations": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+            C.POINTER(abi.CorrInfo)], i),
+        "alz_edge_correlations_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), pp, C.POINTER(sz), C.POINTER(u32),
+            vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_edge_correlations_top": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, vp, vp, vp, vp, sz,
+            C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_edge_correlations_top_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, pp, pp, pp,
+            pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_node_correlations": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+            C.POINTER(abi.CorrInfo)], i),
+        "alz_node_correlations_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), pp, C.POINTER(sz), C.POINTER(u32),
+            vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_node_correlations_top": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, vp, vp, vp, vp, sz,
+            C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_node_correlations_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, pp, pp, pp,
+            pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_edge_correlations": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+            C.POINTER(abi.CorrInfo)], i),
+        "alz_group_edge_correlations_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), pp, C.POINTER(sz), C.POINTER(u32),
+            vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_edge_correlations_top": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, vp, vp, vp, vp, sz,
+            C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_edge_correlations_top_device": ([vp, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, pp, pp, pp,
+            pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_node_correlations": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), vp, sz, C.POINTER(sz), C.POINTER(u32), vp,
+            C.POINTER(abi.CorrInfo)], i),
+        "alz_group_node_correlations_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), pp, C.POINTER(sz), C.POINTER(u32),
+            vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_node_correlations_top": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, vp, vp, vp, vp, sz,
+            C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_group_node_correlations_top_device": ([vp, u32, u32, u32, u32, vp, C.POINTER(abi.Corr), C.POINTER(abi.CorrTarget), u32, C.c_double, pp, pp, pp,
+            pp, C.POINTER(sz), C.POINTER(u32), vp, C.POINTER(abi.CorrInfo)], i),
+        "alz_debug_corr_series": ([vp, vp, vp, sz, u32, C.POINTER(abi.CorrTarget), C.POINTER(abi.Corr), u32,
+                                   C.c_double, vp, vp, sz, C.POINTER(sz), C.POINTER(u64), C.POINTER(u64)], i),
         "alz_edge_quantiles": ([vp, vp, sz, vp], i),
         "alz_submit_tcp": ([vp, vp, sz], i),
         "alz_sock_lookup": ([vp, vp, sz, vp], i),
@@ -329,7 +369,14 @@ def load(rebuild=False):
                   "alz_group_node_trends", "alz_group_node_trends_device", "alz_group_node_trends_top",
                   "alz_group_node_trends_top_device", "alz_reach", "alz_reach_device", "alz_group_reach",
                   "alz_group_reach_device", "alz_debug_reach_rows", "alz_cycles", "alz_cycles_device",
-                  "alz_group_cycles", "alz_group_cycles_device", "alz_debug_cycles_rows"):
+                  "alz_group_cycles", "alz_group_cycles_device", "alz_debug_cycles_rows", "alz_edge_correlations",
+                  "alz_edge_correlations_device", "alz_edge_correlations_top", "alz_edge_correlations_top_device",
+                  "alz_node_correlations", "alz_node_correlations_device", "alz_node_correlations_top",
+                  "alz_node_correlations_top_device", "alz_group_edge_correlations",
+                  "alz_group_edge_correlations_device", "alz_group_edge_correlations_top",
+                  "alz_group_edge_correlations_top_device", "alz_group_node_correlations",
+                  "alz_group_node_correlations_device", "alz_group_node_correlations_top",
+                  "alz_group_node_correlations_top_device", "alz_debug_corr_series"):
             sig.pop(k)
     for name, (args, res) in sig.items():
         f = getattr(L, name)   # AttributeError = header/library mismatch: loud
@@ -1496,6 +1543,144 @@ class Handle:
             return self._cycles("alz_debug_cycles_rows", (C.c_void_p(p), len(rows)), spec, min_value, min_size)
         finally:
             self.dev_free(p)
+
+    # ---- correlations (alz_corr.cu, docs/SPEC.md §29)
+    @staticmethod
+    def corr(direction=abi.CORR_POSITIVE, absent=abi.CORR_ABSENT_SKIP, max_lag=0, min_points=3):
+        """An alz_corr."""
+        return abi.Corr(int(direction), int(absent), int(max_lag), int(min_points))
+
+    class Target:
+        """An alz_corr_target over host arrays it keeps alive: values (float64), present (uint8, or None: every point
+        present), window_last; n = len(values) unless given."""
+
+        def __init__(self, values, present=None, window_last=0, n=None):
+            self.values = np.ascontiguousarray(values, dtype=np.float64)
+            self.present = None if present is None else np.ascontiguousarray(present, dtype=np.uint8)
+            self.s = abi.CorrTarget(_ptr(self.values) if len(self.values) else None,
+                                    None if self.present is None else _ptr(self.present),
+                                    len(self.values) if n is None else int(n), int(window_last))
+
+    @staticmethod
+    def _target_of(target):
+        return target if isinstance(target, Handle.Target) else Handle.Target(*target)
+
+    def _corrs(self, fn, head, k, spec, corr, target, dtype):
+        """fn(h, *head, k, m, &corr, &target, out, cap, &n, &P, points, &info): (records in source order, points, info
+        dict). A first call with cap 0 gives the records."""
+        f, n, p, info, m = getattr(self.L, fn), C.c_size_t(0), C.c_uint32(0), abi.CorrInfo(), abi.metrics(spec)
+        t = self._target_of(target)
+        self._ck(f(self.h, *head, int(k), m, C.byref(corr), C.byref(t.s), None, 0, C.byref(n), C.byref(p), None,
+                   C.byref(info)), fn, allow=(abi.E_CAPACITY,))
+        out = np.zeros(n.value, dtype=dtype)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(f(self.h, *head, int(k), m, C.byref(corr), C.byref(t.s), _ptr(out), len(out), C.byref(n), C.byref(p),
+                   points, C.byref(info)), fn)
+        return out, [points[j].as_dict() for j in range(p.value)], info.as_dict()
+
+    def _corrs_device(self, fn, head, k, spec, corr, target):
+        d, n, p, info = C.c_void_p(), C.c_size_t(0), C.c_uint32(0), abi.CorrInfo()
+        t = self._target_of(target)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(getattr(self.L, fn)(self.h, *head, int(k), abi.metrics(spec), C.byref(corr), C.byref(t.s), C.byref(d),
+                                     C.byref(n), C.byref(p), points, C.byref(info)), fn)
+        return d.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)], info.as_dict()
+
+    def _corrs_top(self, fn, head, k, spec, corr, target, top, min_score, rec_dtype, row_dtype):
+        """fn(h, *head, k, m, &corr, &target, top, min_score, out, rows, series, present, cap, &n, &P, points, &info).
+        The first call offers room for min(top, 4096) results; when more came out, it is repeated with room for all."""
+        f, n, p, info, m = getattr(self.L, fn), C.c_size_t(0), C.c_uint32(0), abi.CorrInfo(), abi.metrics(spec)
+        t = self._target_of(target)
+        cap = min(int(top), 1 << 12)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        while True:
+            out = np.zeros(cap, dtype=rec_dtype)
+            rows = np.zeros(cap, dtype=row_dtype)
+            series = np.zeros(cap * int(k))
+            present = np.zeros(cap * int(k), dtype=np.uint8)
+            rc = self._ck(f(self.h, *head, int(k), m, C.byref(corr), C.byref(t.s), int(top), float(min_score),
+                            _ptr(out), _ptr(rows), _ptr(series), _ptr(present), cap, C.byref(n), C.byref(p), points,
+                            C.byref(info)), fn, allow=(abi.E_CAPACITY,))
+            if rc == 0:
+                break
+            if n.value <= cap:   # a capacity error that no buffer cures: too many slots
+                raise AlzError(rc, fn)
+            cap = n.value
+        r, P = n.value, p.value
+        return (out[:r].copy(), rows[:r].copy(), series[: r * P].reshape(r, P).copy(),
+                present[: r * P].reshape(r, P).copy(), [points[j].as_dict() for j in range(P)], info.as_dict())
+
+    def _corrs_top_device(self, fn, head, k, spec, corr, target, top, min_score):
+        pr, pw, ps, pp_ = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+        n, p, info = C.c_size_t(0), C.c_uint32(0), abi.CorrInfo()
+        t = self._target_of(target)
+        points = (abi.RollupInfo * max(int(k), 1))()
+        self._ck(getattr(self.L, fn)(self.h, *head, int(k), abi.metrics(spec), C.byref(corr), C.byref(t.s), int(top),
+                                     float(min_score), C.byref(pr), C.byref(pw), C.byref(ps), C.byref(pp_), C.byref(n),
+                                     C.byref(p), points, C.byref(info)), fn)
+        return (pr.value, pw.value, ps.value, pp_.value, n.value, p.value, [points[j].as_dict() for j in range(p.value)],
+                info.as_dict())
+
+    _CORR_LEVELS = {"edge": (False, abi.EDGE_CORR, abi.EDGE_OUT), "node": (True, abi.NODE_CORR, abi.NODE_OUT),
+                    "group_edge": (False, abi.EDGE_CORR, abi.EDGE_OUT),
+                    "group_node": (True, abi.NODE_CORR, abi.NODE_OUT)}
+
+    def _corr_head(self, level, source, side, tier):
+        return (int(source), int(side), int(tier)) if self._CORR_LEVELS[level][0] else (int(source), int(tier))
+
+    def correlations(self, level, source, tier, k, spec, corr, target, side=abi.SIDE_IN):
+        """alz_{level}_correlations (level "edge", "node", "group_edge" or "group_node"): every candidate of `source`
+        against `target` (an Alz.Target or a (values, present, window_last) tuple) by one metric and an abi.Corr:
+        (EDGE_CORR / NODE_CORR records in source order, points, info dict). side: node levels only."""
+        return self._corrs(f"alz_{level}_correlations", self._corr_head(level, source, side, tier), k, spec, corr,
+                           target, self._CORR_LEVELS[level][1])
+
+    def correlations_device(self, level, source, tier, k, spec, corr, target, side=abi.SIDE_IN):
+        """alz_{level}_correlations_device: (device pointer to the records, rows, P, points, info dict)."""
+        return self._corrs_device(f"alz_{level}_correlations_device", self._corr_head(level, source, side, tier), k,
+                                  spec, corr, target)
+
+    def correlations_top(self, level, source, tier, k, spec, corr, target, top, min_score=-np.inf, side=abi.SIDE_IN):
+        """alz_{level}_correlations_top: the first min(top, above) valid candidates by score, rank order: (records,
+        EDGE_OUT or NODE_OUT rows, series [m, P], present [m, P], points, info dict)."""
+        _, rec, row = self._CORR_LEVELS[level]
+        return self._corrs_top(f"alz_{level}_correlations_top", self._corr_head(level, source, side, tier), k, spec,
+                               corr, target, top, min_score, rec, row)
+
+    def correlations_top_device(self, level, source, tier, k, spec, corr, target, top, min_score=-np.inf,
+                                side=abi.SIDE_IN):
+        """alz_{level}_correlations_top_device: (records, rows, series and present device pointers, results, P, points,
+        info dict)."""
+        return self._corrs_top_device(f"alz_{level}_correlations_top_device", self._corr_head(level, source, side, tier),
+                                      k, spec, corr, target, top, min_score)
+
+    def debug_corr_series(self, values, present, target, corr, top=0, min_score=-np.inf, offset=0):
+        """alz_debug_corr_series over host series values [n, P] float64 and present [n, P] uint8 (copied to the
+        device, `offset` elements past the start of their allocations): (EDGE_CORR records, top indices (top > 0) or
+        None, valid, above)."""
+        values = np.ascontiguousarray(values, dtype=np.float64)
+        present = np.ascontiguousarray(present, dtype=np.uint8)
+        n, P = values.shape
+        t = self._target_of(target)
+        pv, pp_ = self.dev_alloc(max(values.nbytes, 16) + 16), self.dev_alloc(max(present.nbytes, 16) + 16)
+        dv, dp = pv + 8 * int(offset), pp_ + int(offset)
+        try:
+            if values.size:
+                self.h2d(dv, values)
+                self.h2d(dp, present)
+            cap = n if not top else min(int(top), n)
+            out = np.zeros(cap, dtype=abi.EDGE_CORR)
+            idx = np.zeros(cap, dtype=np.uint32)
+            m, valid, above = C.c_size_t(0), C.c_uint64(0), C.c_uint64(0)
+            self._ck(self.L.alz_debug_corr_series(self.h, C.c_void_p(dv), C.c_void_p(dp), n, P, C.byref(t.s),
+                                                  C.byref(corr), int(top), float(min_score), _ptr(out), _ptr(idx), cap,
+                                                  C.byref(m), C.byref(valid), C.byref(above)),
+                     "alz_debug_corr_series")
+            r = m.value
+            return out[:r].copy(), (idx[:r].copy() if top else None), valid.value, above.value
+        finally:
+            self.dev_free(pv)
+            self.dev_free(pp_)
 
     def fold(self):
         self._ck(self.L.alz_fold(self.h), "alz_fold")

@@ -271,6 +271,7 @@ extern "C" int alz_destroy(alz_handle* h) {
   alz_internal_free_group_trends(h);
   alz_internal_free_reach(h);
   alz_internal_free_cycles(h);
+  alz_internal_free_corr(h);
   alz_internal_free_sock(h);
   alz_internal_free_rollup(h);
   alz_internal_free_tiers(h);

@@ -152,6 +152,10 @@ struct alz_handle {
                                                       // until the first
   alz_cycle_state* cycles = nullptr;                  // the cycles calls' buffers (alz_cycles*, alz_group_cycles*);
                                                       // null until the first
+  alz_trend_state* corr = nullptr;                    // the edge correlations' buffers (alz_edge_correlations*,
+                                                      // alz_debug_corr_series); null until the first
+  alz_trend_state* node_corr = nullptr;               // the node correlations' buffers (alz_node_correlations*)
+  alz_trend_state* group_corr = nullptr;              // the group correlations' buffers (alz_group_*_correlations*)
 };
 
 int alz_internal_fold(alz_handle* h);
@@ -193,6 +197,9 @@ int alz_internal_ring_view(alz_handle* h, uint32_t tier, uint32_t k, alz_ring_vi
 // points[j] = what a rollup of view entry j alone reports, for the view the last alz_internal_ring_view call gave
 // (same tier and k, no call on the handle in between), after a wait on the stream. Caller holds h->mu.
 void alz_internal_ring_points(alz_handle* h, uint32_t tier, uint32_t k, alz_rollup_info* points);
+// The alz_rollup_info.window_last of the newest closed entry of one ring (0 when it holds none), from the host's
+// records: no wait. The ring exists (an alz_internal_ring_view call for it succeeded). Caller holds h->mu.
+uint64_t alz_internal_ring_last(alz_handle* h, uint32_t tier);
 void alz_internal_free_rollup(alz_handle* h);
 void alz_internal_free_tiers(alz_handle* h);
 void alz_internal_free_span(alz_handle* h);
@@ -210,4 +217,5 @@ void alz_internal_free_group_series(alz_handle* h);
 void alz_internal_free_group_trends(alz_handle* h);
 void alz_internal_free_reach(alz_handle* h);
 void alz_internal_free_cycles(alz_handle* h);
+void alz_internal_free_corr(alz_handle* h);
 void alz_internal_free_sock(alz_handle* h);

@@ -296,5 +296,98 @@ struct Csr {
 int graph_build(alz_handle* h, Graph& gr, const alz_edge_out* rows, uint32_t n, const MetricSet* ms, double min_value,
                 std::initializer_list<std::pair<uint32_t, Csr*>> csrs);
 
+// Buffers of one family of scored calls (below), each grown on demand and never shrunk; freed in alz_destroy. The edge
+// trend calls own one (h->trends), the node trend calls another (h->node_trends), the group trend calls a third
+// (h->group_trends), and the edge, node and group correlation calls (alz_corr.cu) three more, each using its own
+// series buffers.
+}  // namespace metrics
+}  // namespace alz
+struct alz_trend_state {
+  alz::metrics::SeriesBufs ser;        // edges: the series of the source's rows, one metric
+  alz::metrics::NodeSeriesBufs nser;   // nodes: the series of the source's nodes, one metric, and their node rows
+  alz::metrics::GroupSeriesBufs gser;  // groups: the source's group-edge rows and their or their group nodes' series
+  alz::metrics::DevBuf rec, sel_val, valid_cnt;   // the records, the selection values, the valid count
+  alz::metrics::DevBuf top_rec, top_values, top_present, top_nodes;   // the top call's records, series and node rows
+  alz::metrics::Selection sel;         // the top call's selection (and, for edges, its gathered source rows)
+  uint32_t* h_valid = nullptr;         // pinned: the valid count, read after the call's wait
+  alz::metrics::DevBuf target;         // correlations: the target's values, then its presence bytes
+  void* h_target = nullptr;            // correlations: pinned staging of the same
+  size_t h_target_bytes = 0;
+};
+namespace alz {
+namespace metrics {
+
+// One call of a family that scores each series row of a source (alz_trends.cu: the trends; alz_corr.cu: the
+// correlations): the series of one metric, one 48-byte record per row, and for a top call the selection and a gather of
+// the top records with their series. The family's state is an alz_trend_state.
+struct ScoredCall {
+  bool top = false, node = false, group = false;
+  uint32_t source = 0, side = 0, tier = 0, k = 0, n_top = 0;
+  double min_value = 0.0;
+  MetricSet ms{};
+  // given: score these N x P device series (values[i * P + j], present[i * P + j]) instead of a source's; no rows,
+  // no ring
+  bool given = false;
+  const double* given_values = nullptr;
+  const uint8_t* given_present = nullptr;
+  size_t given_n = 0;
+  uint32_t given_points = 0;
+};
+// What the per-row pass reads: N series rows of P points, and what the records' heads come from (rows: the edge rows,
+// keys: the node keys; both null for given series)
+struct ScoredInput {
+  size_t n = 0;
+  uint32_t points = 0;
+  const double* values = nullptr;
+  const uint8_t* present = nullptr;
+  const alz_edge_out* rows = nullptr;
+  const uint64_t* keys = nullptr;
+};
+// The family's per-row pass: rec[i] (48 bytes) for every row and, with sel, the row's selection value (its score's
+// bits when valid, all ones otherwise); *valid_cnt += the valid rows. Enqueued on the stream, no wait.
+struct ScorePass {
+  virtual int launch(alz_handle* h, alz_trend_state& s, const ScoredInput& in, void* rec, uint64_t* sel,
+                     uint32_t* valid_cnt) = 0;
+};
+// A call's results, on the device: m records (and, for a top call, m source rows or node rows, their selection indices
+// and m x P series points)
+struct ScoredResult {
+  const void* rec = nullptr;
+  const void* rows = nullptr;
+  const uint32_t* index = nullptr;
+  const double* values = nullptr;
+  const uint8_t* present = nullptr;
+  size_t m = 0;
+};
+// The skeleton of one call into the state sp (created on first use; `what` names the family in errors): the source's
+// series, pass.launch, the selection and the gather, then the waits, after which *res, *n_points, points and *info
+// (points = P, edges = the series rows) are final. cap: a host full-list call's room (checked before the entries are
+// read); copy_out: where that call's records go, copied before its last wait. Caller holds h->mu.
+int scored_series_locked(alz_handle* h, alz_trend_state*& sp, const char* what, const ScoredCall& c, size_t cap,
+                         void* copy_out, ScorePass& pass, ScoredResult* res, uint32_t* n_points,
+                         alz_rollup_info* points, alz_trend_info* info);
+void free_scored_state(alz_trend_state*& s);
+
+#ifdef __CUDACC__
+// The first 16 bytes of an edge record: the source row's ends, with `valid` at byte 2
+struct EdgeHead {
+  const alz_edge_out* rows;
+  __device__ __forceinline__ uint4 operator()(uint32_t i, bool ok) const {
+    const uint2* row = reinterpret_cast<const uint2*>(rows + i);
+    const uint2 ty = row[0], ft = row[1];   // from_type, to_type, pad | from, to
+    return make_uint4((ty.x & 0xFFFFu) | ((ok ? 1u : 0u) << 16), 0u, ft.x, ft.y);
+  }
+};
+
+// The first 16 bytes of a node record: the node's type and value from its key (type << 32) | value
+struct NodeHead {
+  const uint64_t* keys;
+  __device__ __forceinline__ uint4 operator()(uint32_t i, bool ok) const {
+    const uint64_t k = keys[i];
+    return make_uint4((uint32_t)(k >> 32) | ((ok ? 1u : 0u) << 16), 0u, (uint32_t)k, 0u);
+  }
+};
+#endif
+
 }  // namespace metrics
 }  // namespace alz

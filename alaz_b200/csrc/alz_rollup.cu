@@ -697,6 +697,14 @@ void alz_internal_ring_points(alz_handle* h, uint32_t tier, uint32_t k, alz_roll
   });
 }
 
+uint64_t alz_internal_ring_last(alz_handle* h, uint32_t tier) {
+  uint64_t last = 0;
+  with_ring(h, tier, [&](auto& r) {
+    if (!r.entries.empty()) last = r.entries.back().window_last;
+  });
+  return last;
+}
+
 // A rollup entry point of a kind (ALZ_ROLLUP_*): lock, set the device and run the rollup (run(&rows, &info), which
 // sets *n_out and, with ALZ_OK, info). Into out (to_host): ALZ_E_CAPACITY when the rows do not fit, and nothing is
 // written; else *dev_rows (when not null) = the device rows. The kind's scratch holds rows to score, and their info,

@@ -15,6 +15,8 @@
 //           An edge record and a node record differ only in their first 16 bytes (EdgeHead, NodeHead).
 //   top     the §17 selection over those values, which gathers the source rows (for nodes, a gather of the source's
 //           node rows follows), then one gather of the selected records and their P-point series and presence
+// The orchestration (series, pass, selection, gather, waits) is scored_series_locked, which the correlations
+// (alz_corr.cu) share with their own pass.
 // Every SPEC operation is rounded on its own: nvcc would contract s + a * b into a fused multiply-add, so the
 // arithmetic is written with the round-to-nearest intrinsics. Waits: a full-list edge call waits once, at its end (the
 // ring's clocks and the valid count, and a host call's results); a top call adds the selection's wait. A node call
@@ -131,25 +133,6 @@ __device__ __forceinline__ Stat trend_of(const TrendArgs& a, uint32_t i) {
   return Stat{t, recent, before, nu, ok};
 }
 
-// The first 16 bytes of an edge record: the source row's ends, with `valid` at byte 2
-struct EdgeHead {
-  const alz_edge_out* rows;
-  __device__ __forceinline__ uint4 operator()(uint32_t i, bool ok) const {
-    const uint2* row = reinterpret_cast<const uint2*>(rows + i);
-    const uint2 ty = row[0], ft = row[1];   // from_type, to_type, pad | from, to
-    return make_uint4((ty.x & 0xFFFFu) | ((ok ? 1u : 0u) << 16), 0u, ft.x, ft.y);
-  }
-};
-
-// The first 16 bytes of a node record: the node's type and value from its key (type << 32) | value
-struct NodeHead {
-  const uint64_t* keys;
-  __device__ __forceinline__ uint4 operator()(uint32_t i, bool ok) const {
-    const uint64_t k = keys[i];
-    return make_uint4((uint32_t)(k >> 32) | ((ok ? 1u : 0u) << 16), 0u, (uint32_t)k, 0u);
-  }
-};
-
 // Thread i: series row i. rec[i] its record; with sel, sel[i] its selection value; *valid += the valid rows.
 template <class Head>
 __global__ void __launch_bounds__(256) trend_kernel(const __grid_constant__ TrendArgs a, const Head head,
@@ -198,68 +181,34 @@ __global__ void __launch_bounds__(256) trend_gather_kernel(const uint32_t* __res
 
 }  // namespace
 
-// Buffers of the trend calls, each grown on demand and never shrunk; freed in alz_destroy. The edge trend calls own
-// one (h->trends), the node trend calls another (h->node_trends), the group trend calls a third (h->group_trends), each
-// using its own series buffers.
-struct alz_trend_state {
-  SeriesBufs ser;                      // edges: the series of the source's rows, one metric
-  NodeSeriesBufs nser;                 // nodes: the series of the source's nodes, one metric, and their node rows
-  GroupSeriesBufs gser;                // groups: the source's group-edge rows and their or their group nodes' series
-  DevBuf rec, sel_val, valid_cnt;      // the records, the selection values, the valid count
-  DevBuf top_rec, top_values, top_present, top_nodes;   // the top call's records, series and node rows
-  Selection sel;                       // the top call's selection (and, for edges, its gathered source rows)
-  uint32_t* h_valid = nullptr;         // pinned: the valid count, read after the call's wait
-};
-
-namespace {
-
-void free_trend_state(alz_trend_state*& s) {
+void alz::metrics::free_scored_state(alz_trend_state*& s) {
   if (!s) return;
   s->ser.free();
   s->nser.free();
   s->gser.free();
-  free_bufs({&s->rec, &s->sel_val, &s->valid_cnt, &s->top_rec, &s->top_values, &s->top_present, &s->top_nodes});
+  free_bufs({&s->rec, &s->sel_val, &s->valid_cnt, &s->top_rec, &s->top_values, &s->top_present, &s->top_nodes,
+             &s->target});
   s->sel.free();
   if (s->h_valid) cudaFreeHost(s->h_valid);
+  if (s->h_target) cudaFreeHost(s->h_target);
   delete s;
   s = nullptr;
 }
 
-}  // namespace
+void alz_internal_free_trends(alz_handle* h) { free_scored_state(h->trends); }
+void alz_internal_free_node_trends(alz_handle* h) { free_scored_state(h->node_trends); }
+void alz_internal_free_group_trends(alz_handle* h) { free_scored_state(h->group_trends); }
 
-void alz_internal_free_trends(alz_handle* h) { free_trend_state(h->trends); }
-void alz_internal_free_node_trends(alz_handle* h) { free_trend_state(h->node_trends); }
-void alz_internal_free_group_trends(alz_handle* h) { free_trend_state(h->group_trends); }
-
-namespace {
-
-struct TrendCall {
-  bool device = false, top = false, node = false, group = false;
-  uint32_t source = 0, side = 0, tier = 0, k = 0, n_top = 0;
-  double min_trend = 0.0;
-  MetricSet ms{};
-  alz_trend t{};
-};
-
-// The results of one call, on the device: m records (and, for a top call, m source rows or node rows and m x P series
-// points)
-struct TrendResult {
-  const void* rec = nullptr;
-  const void* rows = nullptr;
-  const double* values = nullptr;
-  const uint8_t* present = nullptr;
-  size_t m = 0;
-};
-
-// The trends of a source (c.top: its top rows) into s; *res on the device, after the call's waits, so *info, the
-// points and the valid count are final. cap: a host full-list call's room (checked before the entries are read);
-// copy_out: where that call's records go, copied before its last wait. Caller holds h->mu.
-int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out, TrendResult* res,
-                  uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info) {
+int alz::metrics::scored_series_locked(alz_handle* h, alz_trend_state*& sp, const char* what, const ScoredCall& c,
+                                       size_t cap, void* copy_out, ScorePass& pass, ScoredResult* res,
+                                       uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info) {
   CK(cudaSetDevice(h->device));
   const alz_edge_out* rows = h->d_out;
   size_t n = h->last_n_edges;
-  if (c.node || c.group) {
+  if (c.given) {
+    n = c.given_n;
+    if (n > kMaxRows || (uint64_t)n * c.given_points > kMaxRows) return ALZ_E_CAPACITY;
+  } else if (c.node || c.group) {
     const int rc = node_source(h, c.source, &rows, &n);
     if (rc != ALZ_OK) return rc;
   } else {
@@ -269,14 +218,12 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
     }
     if (n > kMaxRows) return ALZ_E_CAPACITY;
   }
-  alz_trend_state*& sp = c.group ? h->group_trends : c.node ? h->node_trends : h->trends;
   if (!sp) sp = new alz_trend_state();
   alz_trend_state* s = sp;
   if (!s->h_valid) {
     void* p = nullptr;
     if (cudaMallocHost(&p, sizeof(uint32_t)) != cudaSuccess) {
-      h->last_err = std::string(c.group ? "group trends: " : c.node ? "node trends: " : "edge trends: ") +
-                    cudaGetErrorString(cudaGetLastError());
+      h->last_err = std::string(what) + ": " + cudaGetErrorString(cudaGetLastError());
       return ALZ_E_NOMEM;
     }
     s->h_valid = static_cast<uint32_t*>(p);
@@ -284,19 +231,29 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
   size_t n_rows = 0;   // series rows: the source's rows, or its nodes
   uint64_t rows_in = 0;
   const size_t room = c.top ? SIZE_MAX : cap;
-  int rc = c.group  ? run_group_series_rows(h, s->gser, rows, n, c.node, c.side, c.tier, c.k, c.ms, c.top, room,
-                                             &n_rows, n_points, &rows_in)
-           : c.node ? run_node_series_rows(h, s->nser, rows, n, c.side, c.tier, c.k, c.ms, c.top, room, &n_rows,
-                                           n_points, &rows_in)
-                    : run_series_rows(h, s->ser, rows, n, c.tier, c.k, c.ms, room, &n_rows, n_points, &rows_in);
+  int rc = ALZ_OK;
+  if (c.given) {
+    n_rows = n;
+    *n_points = c.given_points;
+    if (n > room) rc = ALZ_E_CAPACITY;
+  } else {
+    rc = c.group  ? run_group_series_rows(h, s->gser, rows, n, c.node, c.side, c.tier, c.k, c.ms, c.top, room,
+                                          &n_rows, n_points, &rows_in)
+         : c.node ? run_node_series_rows(h, s->nser, rows, n, c.side, c.tier, c.k, c.ms, c.top, room, &n_rows,
+                                         n_points, &rows_in)
+                  : run_series_rows(h, s->ser, rows, n, c.tier, c.k, c.ms, room, &n_rows, n_points, &rows_in);
+  }
   res->m = c.top ? 0 : n_rows;
   if (rc != ALZ_OK) return rc;
   const uint32_t P = *n_points;
   const size_t N = n_rows;
   const NodeSeriesBufs& nser = c.group ? s->gser.s : s->nser;   // node or group series
   if (c.group && !c.node) rows = static_cast<const alz_edge_out*>(s->gser.edges.p);   // the series rows
-  const double* values = static_cast<const double*>(c.node || c.group ? nser.values.p : s->ser.values.p);
-  const uint8_t* present = static_cast<const uint8_t*>(c.node || c.group ? nser.present.p : s->ser.present.p);
+  const double* values = c.given ? c.given_values
+                                 : static_cast<const double*>(c.node || c.group ? nser.values.p : s->ser.values.p);
+  const uint8_t* present = c.given ? c.given_present
+                                   : static_cast<const uint8_t*>(c.node || c.group ? nser.present.p
+                                                                                    : s->ser.present.p);
   rc = reserve(h, {{&s->rec, std::max<size_t>(N, 1) * sizeof(alz_edge_trend)},
                    {&s->sel_val, c.top ? std::max<size_t>(N, 1) * 8 : 0},
                    {&s->valid_cnt, 4}});
@@ -305,25 +262,22 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
   uint32_t* d_valid = static_cast<uint32_t*>(s->valid_cnt.p);
   CK(cudaMemsetAsync(d_valid, 0, 4, st));
   alz_edge_trend* d_rec = static_cast<alz_edge_trend*>(s->rec.p);
-  if (N) {
-    const TrendArgs ta{(uint32_t)N, P, values, present, c.t.stat, c.t.direction,
-                       c.t.absent == ALZ_TREND_ABSENT_ZERO ? 1u : 0u, c.t.recent, c.t.min_points};
-    const unsigned grid = std::min<unsigned>((unsigned)((N + 255) / 256), (unsigned)h->sms * 8);
-    uint64_t* sel = c.top ? static_cast<uint64_t*>(s->sel_val.p) : nullptr;
-    if (c.node)
-      trend_kernel<<<grid, 256, 0, st>>>(ta, NodeHead{static_cast<const uint64_t*>(nser.keys.p)}, d_rec, sel,
-                                         d_valid);
-    else
-      trend_kernel<<<grid, 256, 0, st>>>(ta, EdgeHead{rows}, d_rec, sel, d_valid);
-    h->launches += 1;
-    CK(cudaGetLastError());
-  }
+  ScoredInput in;
+  in.n = N;
+  in.points = P;
+  in.values = values;
+  in.present = present;
+  if (c.given) rows = nullptr;
+  else if (c.node) in.keys = static_cast<const uint64_t*>(nser.keys.p);
+  else in.rows = rows;
+  rc = pass.launch(h, *s, in, d_rec, c.top ? static_cast<uint64_t*>(s->sel_val.p) : nullptr, d_valid);
+  if (rc != ALZ_OK) return rc;
   CK(cudaMemcpyAsync(s->h_valid, d_valid, 4, cudaMemcpyDeviceToHost, st));   // read after the call's wait
   uint64_t above = 0;
   bool waited = false;
   if (c.top) {
     size_t m = 0;
-    rc = select_top(h, s->sel, static_cast<const uint64_t*>(s->sel_val.p), (uint32_t)N, c.n_top, c.min_trend,
+    rc = select_top(h, s->sel, static_cast<const uint64_t*>(s->sel_val.p), (uint32_t)N, c.n_top, c.min_value,
                     c.node ? nullptr : rows, &m, &above);
     if (rc != ALZ_OK) return rc;
     waited = N > 0;   // the selection waited for its control block
@@ -348,6 +302,7 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
     }
     res->rec = s->top_rec.p;
     res->rows = c.node ? s->top_nodes.p : s->sel.top_rows.p;
+    res->index = top_index;
     res->values = static_cast<const double*>(s->top_values.p);
     res->present = static_cast<const uint8_t*>(s->top_present.p);
     res->m = m;
@@ -356,7 +311,7 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
     if (N && copy_out) CK(cudaMemcpyAsync(copy_out, d_rec, N * sizeof(alz_edge_trend), cudaMemcpyDeviceToHost, st));
   }
   if (!waited) CK(cudaStreamSynchronize(st));   // a full-list call's last wait: its results, the clocks, the count
-  if (points) alz_internal_ring_points(h, c.tier, c.k, points);
+  if (points && !c.given) alz_internal_ring_points(h, c.tier, c.k, points);
   if (info) {
     *info = alz_trend_info{};
     info->edges = N;
@@ -369,6 +324,33 @@ int trends_locked(alz_handle* h, const TrendCall& c, size_t cap, void* copy_out,
   return ALZ_OK;
 }
 
+namespace {
+
+struct TrendCall : ScoredCall {
+  bool device = false;
+  alz_trend t{};
+};
+
+// The §20 pass: one trend_kernel thread per series row
+struct TrendPass final : ScorePass {
+  alz_trend t{};
+  int launch(alz_handle* h, alz_trend_state&, const ScoredInput& in, void* rec, uint64_t* sel,
+             uint32_t* valid_cnt) override {
+    if (!in.n) return ALZ_OK;
+    const TrendArgs ta{(uint32_t)in.n, in.points, in.values, in.present, t.stat, t.direction,
+                       t.absent == ALZ_TREND_ABSENT_ZERO ? 1u : 0u, t.recent, t.min_points};
+    const unsigned grid = std::min<unsigned>((unsigned)((in.n + 255) / 256), (unsigned)h->sms * 8);
+    alz_edge_trend* d_rec = static_cast<alz_edge_trend*>(rec);
+    if (in.keys)
+      trend_kernel<<<grid, 256, 0, h->stream>>>(ta, NodeHead{in.keys}, d_rec, sel, valid_cnt);
+    else
+      trend_kernel<<<grid, 256, 0, h->stream>>>(ta, EdgeHead{in.rows}, d_rec, sel, valid_cnt);
+    h->launches += 1;
+    CK(cudaGetLastError());
+    return ALZ_OK;
+  }
+};
+
 bool valid_trend(const alz_trend* t, uint32_t k) {
   return t && k >= 2 && t->stat <= ALZ_TREND_ZSCORE && t->direction <= ALZ_TREND_FALLING &&
          t->absent <= ALZ_TREND_ABSENT_ZERO && t->recent >= 1 && t->recent <= k - 1;
@@ -377,7 +359,7 @@ bool valid_trend(const alz_trend* t, uint32_t k) {
 // The eight entry points. A host full-list call's records are copied before its last wait; a host top call copies
 // its results after the selection, with one more wait. Device calls: *dev (required) gets the device results.
 int trends_entry(alz_handle* h, TrendCall c, const alz_metric* m, const alz_trend* t, void* out, void* rows,
-                 double* series, uint8_t* present, size_t cap, TrendResult* dev, size_t* n_out, uint32_t* n_points,
+                 double* series, uint8_t* present, size_t cap, ScoredResult* dev, size_t* n_out, uint32_t* n_points,
                  alz_rollup_info* points, alz_trend_info* info) {
   if (!h || !n_out || !n_points) {
     if (n_out) *n_out = 0;
@@ -391,13 +373,17 @@ int trends_entry(alz_handle* h, TrendCall c, const alz_metric* m, const alz_tren
   c.t = *t;
   if (c.source != ALZ_SOURCE_WINDOW && c.source > ALZ_ROLLUP_SPAN) return ALZ_E_INVAL;
   if (c.node && c.side > ALZ_SIDE_OUT) return ALZ_E_INVAL;
-  if (c.top && (c.n_top == 0 || std::isnan(c.min_trend))) return ALZ_E_INVAL;
+  if (c.top && (c.n_top == 0 || std::isnan(c.min_value))) return ALZ_E_INVAL;
   if (c.device ? !dev : (!c.top && !out && cap)) return ALZ_E_INVAL;
   std::lock_guard<std::mutex> g(h->mu);
-  TrendResult res;
+  ScoredResult res;
   alz_trend_info ti{};
-  const int rc = trends_locked(h, c, c.device ? SIZE_MAX : cap, c.device || c.top ? nullptr : out, &res, n_points,
-                               points, info ? &ti : nullptr);
+  TrendPass pass;
+  pass.t = c.t;
+  const int rc = scored_series_locked(h, c.group ? h->group_trends : c.node ? h->node_trends : h->trends,
+                                      c.group ? "group trends" : c.node ? "node trends" : "edge trends", c,
+                                      c.device ? SIZE_MAX : cap, c.device || c.top ? nullptr : out, pass, &res,
+                                      n_points, points, info ? &ti : nullptr);
   *n_out = res.m;
   if (rc != ALZ_OK) return rc;
   if (info) *info = ti;
@@ -423,7 +409,7 @@ template <class Rec, class Row>
 int trends_device(alz_handle* h, const TrendCall& c, const alz_metric* m, const alz_trend* t, const Rec** dev_out,
                   const Row** dev_rows, const double** dev_series, const uint8_t** dev_present, size_t* n_out,
                   uint32_t* n_points, alz_rollup_info* points, alz_trend_info* info) {
-  TrendResult r;
+  ScoredResult r;
   const int rc = trends_entry(h, c, m, t, nullptr, nullptr, nullptr, nullptr, 0, dev_out ? &r : nullptr, n_out,
                               n_points, points, info);
   if (rc != ALZ_OK) return rc;
@@ -442,7 +428,7 @@ TrendCall call_of(bool device, bool top, uint32_t source, uint32_t tier, uint32_
   c.tier = tier;
   c.k = k;
   c.n_top = n_top;
-  c.min_trend = min_trend;
+  c.min_value = min_trend;
   return c;
 }
 

@@ -1361,4 +1361,216 @@ int Aggregator::ClearSocketLines(bool send_alive, int64_t check_time_ms) {
   return alz_sock_gc(h_);
 }
 
+namespace {
+// the library's form of a CorrTarget; Present empty: every point present
+alz_corr_target CorrTargetOf(const CorrTarget& t) {
+  alz_corr_target c{};
+  c.values = t.Values.data();
+  c.present = t.Present.empty() ? nullptr : t.Present.data();
+  c.n = t.Values.size();
+  c.window_last = t.WindowLast;
+  return c;
+}
+// the target a one-row series call gave: its only row and its newest point's window_last
+template <class Row>
+CorrTarget TargetOfSeries(const std::vector<Row>& rows, const std::vector<alz_rollup_info>& pts) {
+  CorrTarget t;
+  if (!rows.empty()) {
+    t.Values = rows[0].Values;
+    t.Present = rows[0].Present;
+  }
+  t.WindowLast = pts.empty() ? 0 : pts.back().window_last;
+  return t;
+}
+}  // namespace
+
+int Aggregator::RunEdgeCorr(EdgeCorrTop fn, uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                            const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                            const EdgeRef* skip, std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points) {
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const alz_corr_target t = CorrTargetOf(target);
+  const uint32_t ask = skip && top ? top + 1 : top;   // room for the target's own row
+  // a first call sizes the results (ALZ_E_CAPACITY with n = the results, P = the points; nothing written)
+  size_t n = 0;
+  uint32_t P = 0;
+  int rc = fn(h_, src, tier, k, &metric, &corr, &t, ask, min_score, nullptr, nullptr, nullptr, nullptr, 0, &n, &P,
+              nullptr, nullptr);
+  std::vector<alz_rollup_info> pts(P);
+  if (rc == ALZ_E_CAPACITY && n > 0) {
+    corrs_.resize(n);
+    trend_rows_.resize(n);
+    trend_values_.resize(n * P);
+    trend_present_.resize(n * P);
+    rc = fn(h_, src, tier, k, &metric, &corr, &t, ask, min_score, corrs_.data(), trend_rows_.data(),
+            trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
+  }
+  if (rc != ALZ_OK) return rc;
+  const std::vector<EdgeWindow> names = ToEdges(trend_rows_.data(), n, nullptr);
+  out->clear();
+  for (size_t i = 0; i < n && out->size() < top; ++i) {
+    const EdgeWindow& w = names[i];
+    if (skip && w.FromType == skip->FromType && w.FromUID == skip->FromUID && w.ToType == skip->ToType &&
+        w.ToUID == skip->ToUID)
+      continue;
+    const alz_edge_corr& r = corrs_[i];
+    EdgeCorr e;
+    e.FromType = w.FromType; e.FromUID = w.FromUID; e.ToType = w.ToType; e.ToUID = w.ToUID;
+    e.Valid = r.valid != 0;
+    e.Lag = r.lag;
+    e.Used = r.used;
+    e.R = r.r; e.Score = r.score; e.R0 = r.r0;
+    e.Present.assign(trend_present_.begin() + i * P, trend_present_.begin() + (i + 1) * P);
+    e.Values.assign(trend_values_.begin() + i * P, trend_values_.begin() + (i + 1) * P);
+    out->push_back(std::move(e));
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::RunNodeCorr(NodeCorrTop fn, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                            const alz_metric& metric, const alz_corr& corr, const CorrTarget& target, uint32_t top,
+                            double min_score, const NodeRef* skip, std::vector<NodeCorr>* out,
+                            std::vector<alz_rollup_info>* points) {
+  const uint32_t src = source == kLastWindow ? ALZ_SOURCE_WINDOW : source;
+  const alz_corr_target t = CorrTargetOf(target);
+  const uint32_t ask = skip && top ? top + 1 : top;
+  size_t n = 0;
+  uint32_t P = 0;
+  int rc = fn(h_, src, side, tier, k, &metric, &corr, &t, ask, min_score, nullptr, nullptr, nullptr, nullptr, 0, &n,
+              &P, nullptr, nullptr);
+  std::vector<alz_rollup_info> pts(P);
+  if (rc == ALZ_E_CAPACITY && n > 0) {
+    node_corrs_.resize(n);
+    node_trend_rows_.resize(n);
+    trend_values_.resize(n * P);
+    trend_present_.resize(n * P);
+    rc = fn(h_, src, side, tier, k, &metric, &corr, &t, ask, min_score, node_corrs_.data(), node_trend_rows_.data(),
+            trend_values_.data(), trend_present_.data(), n, &n, &P, pts.data(), nullptr);
+  }
+  if (rc != ALZ_OK) return rc;
+  const std::vector<NodeWindow> names = ToNodes(node_trend_rows_.data(), n, nullptr, 0);
+  out->clear();
+  for (size_t i = 0; i < n && out->size() < top; ++i) {
+    if (skip && names[i].Type == skip->Type && names[i].UID == skip->UID) continue;
+    const alz_node_corr& r = node_corrs_[i];
+    NodeCorr e;
+    e.Node = names[i];
+    e.Valid = r.valid != 0;
+    e.Lag = r.lag;
+    e.Used = r.used;
+    e.R = r.r; e.Score = r.score; e.R0 = r.r0;
+    e.Present.assign(trend_present_.begin() + i * P, trend_present_.begin() + (i + 1) * P);
+    e.Values.assign(trend_values_.begin() + i * P, trend_values_.begin() + (i + 1) * P);
+    out->push_back(std::move(e));
+  }
+  if (points) *points = pts;
+  return ALZ_OK;
+}
+
+int Aggregator::Correlations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                             const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                             std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  return RunEdgeCorr(alz_edge_correlations_top, source, tier, k, metric, corr, target, top, min_score, nullptr, out,
+                     points);
+}
+
+int Aggregator::Correlations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                             const alz_corr& corr, const EdgeRef& target, uint32_t top, double min_score,
+                             std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::vector<EdgeSeries> ser;
+  std::vector<alz_rollup_info> pts;
+  int rc = SeriesFor({target}, tier, k, {metric}, &ser, &pts);
+  if (rc != ALZ_OK) return rc;
+  std::lock_guard<std::mutex> g(mu_);
+  return RunEdgeCorr(alz_edge_correlations_top, source, tier, k, metric, corr, TargetOfSeries(ser, pts), top,
+                     min_score, &target, out, points);
+}
+
+int Aggregator::NodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                                 const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                                 std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  return RunNodeCorr(alz_node_correlations_top, source, side, tier, k, metric, corr, target, top, min_score, nullptr,
+                     out, points);
+}
+
+int Aggregator::NodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                                 const alz_corr& corr, const NodeRef& target, uint32_t top, double min_score,
+                                 std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::vector<NodeSeriesRow> ser;
+  std::vector<alz_rollup_info> pts;
+  int rc = NodeSeriesFor({target}, side, tier, k, {metric}, &ser, &pts);
+  if (rc != ALZ_OK) return rc;
+  std::lock_guard<std::mutex> g(mu_);
+  return RunNodeCorr(alz_node_correlations_top, source, side, tier, k, metric, corr, TargetOfSeries(ser, pts), top,
+                     min_score, &target, out, points);
+}
+
+int Aggregator::GroupCorrelations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                                  const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                                  std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunEdgeCorr(alz_group_edge_correlations_top, source, tier, k, metric, corr, target, top, min_score, nullptr,
+                     out, points);
+}
+
+int Aggregator::GroupCorrelations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                                  const alz_corr& corr, const EdgeRef& target, uint32_t top, double min_score,
+                                  std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::vector<EdgeSeries> ser;
+  std::vector<alz_rollup_info> pts;
+  int rc = GroupSeriesFor({target}, tier, k, {metric}, &ser, &pts);
+  if (rc != ALZ_OK) return rc;
+  std::lock_guard<std::mutex> g(mu_);
+  rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunEdgeCorr(alz_group_edge_correlations_top, source, tier, k, metric, corr, TargetOfSeries(ser, pts), top,
+                     min_score, &target, out, points);
+}
+
+int Aggregator::GroupNodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                      const alz_metric& metric, const alz_corr& corr, const CorrTarget& target,
+                                      uint32_t top, double min_score, std::vector<NodeCorr>* out,
+                                      std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::lock_guard<std::mutex> g(mu_);
+  const int rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunNodeCorr(alz_group_node_correlations_top, source, side, tier, k, metric, corr, target, top, min_score,
+                     nullptr, out, points);
+}
+
+int Aggregator::GroupNodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                      const alz_metric& metric, const alz_corr& corr, const NodeRef& target,
+                                      uint32_t top, double min_score, std::vector<NodeCorr>* out,
+                                      std::vector<alz_rollup_info>* points) {
+  if (!h_) return ALZ_E_STATE;
+  if (!out) return ALZ_E_INVAL;
+  std::vector<NodeSeriesRow> ser;
+  std::vector<alz_rollup_info> pts;
+  int rc = GroupNodeSeriesFor({target}, side, tier, k, {metric}, &ser, &pts);
+  if (rc != ALZ_OK) return rc;
+  std::lock_guard<std::mutex> g(mu_);
+  rc = SyncGroups();
+  if (rc != ALZ_OK) return rc;
+  return RunNodeCorr(alz_group_node_correlations_top, source, side, tier, k, metric, corr, TargetOfSeries(ser, pts),
+                     top, min_score, &target, out, points);
+}
+
 }  // namespace alaz

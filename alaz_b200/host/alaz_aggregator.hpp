@@ -156,6 +156,36 @@ struct NodeTrend {
   std::vector<double> Values;         // [points]
 };
 
+// a target series for the correlation calls (docs/SPEC.md §29): per point, oldest first, its value and whether it is
+// present (empty Present: every point), aligned to the ring and k of the call; WindowLast is the window_last of its
+// newest point, as the *SeriesFor calls' points report it
+struct CorrTarget {
+  std::vector<double> Values;
+  std::vector<uint8_t> Present;
+  uint64_t WindowLast = 0;
+};
+
+// one edge's correlation with a target (docs/SPEC.md §29) and the series it was computed from
+struct EdgeCorr {
+  std::string FromType, FromUID, ToType, ToUID;
+  bool Valid = false;
+  uint32_t Lag = 0;                   // the best lag: the edge leads the target by this many points
+  uint32_t Used = 0;                  // pairs used at it
+  double R = 0.0, Score = 0.0, R0 = 0.0;   // r and the score at the best lag, r at lag 0
+  std::vector<uint8_t> Present;       // [points]
+  std::vector<double> Values;         // [points]
+};
+
+// one node's correlation with a target (docs/SPEC.md §29), its node row in the source and its series
+struct NodeCorr {
+  NodeWindow Node;                    // Type, UID, edge counts and both sides' sums in the source (Values empty)
+  bool Valid = false;
+  uint32_t Lag = 0, Used = 0;
+  double R = 0.0, Score = 0.0, R0 = 0.0;
+  std::vector<uint8_t> Present;       // [points]
+  std::vector<double> Values;         // [points]
+};
+
 // datastore/dto.go AliveConnection, as sendOpenConnection fills it (aggregator/data.go:1649-1675)
 struct AliveConnection {
   int64_t CheckTime = 0;   // unix ms
@@ -353,6 +383,38 @@ class Aggregator {
   int GroupNodeTrends(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
                       const alz_trend& trend, uint32_t top, double min_trend, std::vector<NodeTrend>* out,
                       std::vector<alz_rollup_info>* points = nullptr);
+  // Correlations (docs/SPEC.md §29): the `top` rows (Correlations), nodes of side `side` (NodeCorrelations), group
+  // edges (GroupCorrelations) or group nodes of side `side` (GroupNodeCorrelations) of `source` whose series of
+  // `metric` over the last k entries of `tier` followed a target most closely at the best lag up to corr.max_lag,
+  // valid scores >= min_score, largest first, ties in source order, each with its series; named as Trends,
+  // NodeTrends, GroupTrends and GroupNodeTrends name them. The target is a CorrTarget, or the series of one edge, node
+  // or group named as the matching *SeriesFor call names it; in that form the target's own row is left out of the
+  // result (top others are returned). "Who moved with checkout's inbound p99, and a point earlier?" A flush between the
+  // target's series and the call: ALZ_E_STATE. *points (may be null) as in Series. Returns 0 or an alz_status.
+  int Correlations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_corr& corr,
+                   const CorrTarget& target, uint32_t top, double min_score, std::vector<EdgeCorr>* out,
+                   std::vector<alz_rollup_info>* points = nullptr);
+  int Correlations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_corr& corr,
+                   const EdgeRef& target, uint32_t top, double min_score, std::vector<EdgeCorr>* out,
+                   std::vector<alz_rollup_info>* points = nullptr);
+  int NodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                       const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                       std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int NodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                       const alz_corr& corr, const NodeRef& target, uint32_t top, double min_score,
+                       std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int GroupCorrelations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_corr& corr,
+                        const CorrTarget& target, uint32_t top, double min_score, std::vector<EdgeCorr>* out,
+                        std::vector<alz_rollup_info>* points = nullptr);
+  int GroupCorrelations(uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric, const alz_corr& corr,
+                        const EdgeRef& target, uint32_t top, double min_score, std::vector<EdgeCorr>* out,
+                        std::vector<alz_rollup_info>* points = nullptr);
+  int GroupNodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                            const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                            std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points = nullptr);
+  int GroupNodeCorrelations(uint32_t source, uint32_t side, uint32_t tier, uint32_t k, const alz_metric& metric,
+                            const alz_corr& corr, const NodeRef& target, uint32_t top, double min_score,
+                            std::vector<NodeCorr>* out, std::vector<alz_rollup_info>* points = nullptr);
   // Reach (docs/SPEC.md §27): the nodes of `source` within max_hops rows of the seeds, in direction dir
   // (ALZ_REACH_DOWN: what the seeds call; ALZ_REACH_UP: who calls them; ALZ_REACH_ANY), in (hops, node key) order, and
   // the rows crossed, in the source's order, named as ToEdges names ends. filter (may be null): only rows whose value
@@ -443,6 +505,22 @@ class Aggregator {
   int RunNodeTrends(NodeTrendsTop fn, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
                     const alz_metric& metric, const alz_trend& trend, uint32_t top, double min_trend,
                     std::vector<NodeTrend>* out, std::vector<alz_rollup_info>* points);
+  // the edge correlations_top call `fn` (alz_edge_correlations_top, alz_group_edge_correlations_top) into corrs_ and
+  // its rows named, and the node one into node_corrs_; a row named `skip` (not null) is left out and top + 1 asked
+  // for; require mu_
+  using EdgeCorrTop = int (*)(alz_handle*, uint32_t, uint32_t, uint32_t, const alz_metric*, const alz_corr*,
+                              const alz_corr_target*, uint32_t, double, alz_edge_corr*, alz_edge_out*, double*,
+                              uint8_t*, size_t, size_t*, uint32_t*, alz_rollup_info*, alz_corr_info*);
+  using NodeCorrTop = int (*)(alz_handle*, uint32_t, uint32_t, uint32_t, uint32_t, const alz_metric*, const alz_corr*,
+                              const alz_corr_target*, uint32_t, double, alz_node_corr*, alz_node_out*, double*,
+                              uint8_t*, size_t, size_t*, uint32_t*, alz_rollup_info*, alz_corr_info*);
+  int RunEdgeCorr(EdgeCorrTop fn, uint32_t source, uint32_t tier, uint32_t k, const alz_metric& metric,
+                  const alz_corr& corr, const CorrTarget& target, uint32_t top, double min_score,
+                  const EdgeRef* skip, std::vector<EdgeCorr>* out, std::vector<alz_rollup_info>* points);
+  int RunNodeCorr(NodeCorrTop fn, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                  const alz_metric& metric, const alz_corr& corr, const CorrTarget& target, uint32_t top,
+                  double min_score, const NodeRef* skip, std::vector<NodeCorr>* out,
+                  std::vector<alz_rollup_info>* points);
   // the group map resolved by UID sent to the library when SetGroups changed it or an interner handed out or freed an
   // id since the last send; requires mu_
   int SyncGroups();
@@ -503,6 +581,8 @@ class Aggregator {
   std::vector<alz_node_change> node_changes_;   // records of the last NodeChanges
   std::vector<alz_node_trend> node_trends_;   // records, node rows, series and presence of the last NodeTrends
   std::vector<alz_node_out> node_trend_rows_;
+  std::vector<alz_edge_corr> corrs_;          // records of the last Correlations / GroupCorrelations (rows, series and
+  std::vector<alz_node_corr> node_corrs_;     // presence in trend_rows_ / node_trend_rows_ / trend_values_ / ...)
   std::vector<alz_reach_node> reach_nodes_;   // the records and row positions of the last Reach / GroupReach
   std::vector<uint32_t> reach_index_;
   std::vector<alz_cycle_node> cycle_nodes_;   // the records and row positions of the last Cycles / GroupCycles

@@ -1180,6 +1180,159 @@ int alz_group_cycles_device(alz_handle* h, uint32_t source, const alz_metric* m,
                             const alz_cycle_node** dev_nodes, size_t* n_nodes, const uint32_t** dev_row_index,
                             const alz_edge_out** dev_rows, size_t* n_rows, alz_cycle_info* info);
 
+/* ---- correlations (docs/SPEC.md §29) -------------------------------------------------------------------------------
+ * How closely each row's series of one metric followed a target series the caller supplies, at the best lag. The
+ * candidates are the series rows of §20 (alz_edge_correlations*: a source's rows), §22 (alz_node_correlations*: its
+ * nodes on one side) or §26 (alz_group_edge_correlations* / alz_group_node_correlations*: its group edges or group
+ * nodes under the map in force at the call) over the last P = min(k, retained) closed entries of one ring, oldest
+ * first. The target is aligned to the same ring and k: n = P points, and window_last the alz_rollup_info.window_last
+ * of its newest point (a one-key alz_*_series_keys call at the same tier and k gives both). n != P, or P > 0 and a
+ * window_last that is not the ring's newest entry's: ALZ_E_STATE (a flush came between). A present target value must be
+ * finite with |v| <= 2^64; an absent one is read as +0.0 whatever it holds.
+ * At lag L (0 .. max_lag) the candidate leads the target by L points: the pairs are (x[j - L], y[j]) for j in [L, P).
+ * ALZ_CORR_ABSENT_SKIP uses the pairs where both points are present, ALZ_CORR_ABSENT_ZERO every pair with an absent
+ * point as +0.0. With `used` the pairs used, the means, then Sxx, Syy and Sxy about them (sums from +0.0 in ascending
+ * j, each operation one float64 rounding), r = Sxy / (sqrt(Sxx) * sqrt(Syy)) clamped to [-1, 1]. A lag is defined when
+ * used >= min_points and the denominator is > 0; its score is r, 0.0 - r or |r| by direction. A row is valid when some
+ * lag is defined; its best lag is the defined lag with the largest score, the smallest on ties. An invalid row's record
+ * is all +0.0 but its head and `used`, which then counts the pairs of lag 0.
+ * The full-list calls give one record per candidate in source order; the top calls rank the valid rows as §20 does
+ * (64-bit key of the float64 score, descending, then row ascending; eligible when key(score) >= key(min_score)) and
+ * return the first min(top, above) with their source rows or node rows and their series (series[j * P + p],
+ * present[j * P + p]; room for cap x k each). k = 0, max_lag above ALZ_CORR_MAX_LAG or not below k, min_points below 3,
+ * an unknown direction or absent mode, a null target, a null target->values with n > 0, a bad target value, and
+ * everything the matching trend call refuses with ALZ_E_INVAL: ALZ_E_INVAL. The other errors, the waits, the
+ * availability rule, "reads only" (every other family's device results, trends and series included, are unchanged)
+ * and "every rank returns the same bytes with no collective" are §20's. Device results stay valid until the next
+ * correlation call of the same level. */
+#define ALZ_CORR_POSITIVE 0u   /* score r: the rows that rose and fell with the target rank first */
+#define ALZ_CORR_NEGATIVE 1u   /* score -r: the rows that moved against it */
+#define ALZ_CORR_ABS      2u   /* score |r|: either */
+#define ALZ_CORR_ABSENT_SKIP 0u   /* a pair with an absent point is left out */
+#define ALZ_CORR_ABSENT_ZERO 1u   /* an absent point counts as +0.0 */
+#define ALZ_CORR_MAX_LAG 32u
+typedef struct alz_corr {   /* 16 B */
+  uint32_t direction;    /* ALZ_CORR_POSITIVE / NEGATIVE / ABS */
+  uint32_t absent;       /* ALZ_CORR_ABSENT_SKIP / ABSENT_ZERO */
+  uint32_t max_lag;      /* lags 0 .. max_lag; max_lag <= ALZ_CORR_MAX_LAG and max_lag < k */
+  uint32_t min_points;   /* a defined lag uses at least this many pairs; >= 3 */
+} alz_corr;
+typedef struct alz_corr_target {   /* 32 B */
+  const double* values;    /* host memory, n values */
+  const uint8_t* present;  /* host memory, n bytes (nonzero: present), or NULL: every point present */
+  size_t n;                /* P */
+  uint64_t window_last;    /* alz_rollup_info.window_last of the newest point */
+} alz_corr_target;
+typedef struct alz_edge_corr {   /* 48 B; the head is laid out as alz_edge_trend's */
+  uint8_t from_type;     /* ALZ_NODE_* */
+  uint8_t to_type;
+  uint8_t valid;         /* 1: some lag is defined */
+  uint8_t lag;           /* the best lag */
+  uint8_t _pad[4];
+  uint32_t from;
+  uint32_t to;
+  uint32_t index;        /* row index in the source */
+  uint32_t used;         /* pairs used at the best lag (invalid: at lag 0) */
+  double r;              /* r at the best lag */
+  double score;          /* its score */
+  double r0;             /* r at lag 0, +0.0 when lag 0 is undefined */
+} alz_edge_corr;
+typedef struct alz_node_corr {   /* 48 B; from `valid` on, laid out as alz_edge_corr */
+  uint8_t type;          /* ALZ_NODE_* */
+  uint8_t _pad0;
+  uint8_t valid;
+  uint8_t lag;
+  uint8_t _pad1[4];
+  uint32_t value;
+  uint32_t _pad2;
+  uint32_t index;        /* node index in the source (§21 node order) */
+  uint32_t used;
+  double r;
+  double score;
+  double r0;
+} alz_node_corr;
+typedef struct alz_corr_info {
+  uint64_t rows;          /* candidates: the source's rows, nodes, group edges or group nodes */
+  uint64_t rows_in;       /* entry rows read: the sum of the P entries' rows */
+  uint64_t valid;         /* valid candidates */
+  uint64_t above;         /* top calls: eligible candidates before the cut; 0 otherwise */
+  uint32_t points;        /* P */
+  uint32_t tier;
+  uint32_t target_used;   /* the target's present points */
+  uint32_t _pad;
+} alz_corr_info;
+int alz_edge_correlations(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                          const alz_corr* corr, const alz_corr_target* target, alz_edge_corr* out, size_t cap,
+                          size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_corr_info* info);
+int alz_edge_correlations_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                 const alz_corr* corr, const alz_corr_target* target, const alz_edge_corr** dev_out,
+                                 size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_corr_info* info);
+int alz_edge_correlations_top(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                              const alz_corr* corr, const alz_corr_target* target, uint32_t top, double min_score,
+                              alz_edge_corr* out, alz_edge_out* rows, double* series, uint8_t* present, size_t cap,
+                              size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_corr_info* info);
+int alz_edge_correlations_top_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                     const alz_corr* corr, const alz_corr_target* target, uint32_t top,
+                                     double min_score, const alz_edge_corr** dev_out, const alz_edge_out** dev_rows,
+                                     const double** dev_series, const uint8_t** dev_present, size_t* n_out,
+                                     uint32_t* n_points, alz_rollup_info* points, alz_corr_info* info);
+int alz_node_correlations(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                          const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                          alz_node_corr* out, size_t cap, size_t* n_out, uint32_t* n_points, alz_rollup_info* points,
+                          alz_corr_info* info);
+int alz_node_correlations_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                 const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                 const alz_node_corr** dev_out, size_t* n_out, uint32_t* n_points,
+                                 alz_rollup_info* points, alz_corr_info* info);
+int alz_node_correlations_top(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                              const alz_metric* m, const alz_corr* corr, const alz_corr_target* target, uint32_t top,
+                              double min_score, alz_node_corr* out, alz_node_out* nodes, double* series,
+                              uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                              alz_rollup_info* points, alz_corr_info* info);
+int alz_node_correlations_top_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                     const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                     uint32_t top, double min_score, const alz_node_corr** dev_out,
+                                     const alz_node_out** dev_nodes, const double** dev_series,
+                                     const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                     alz_rollup_info* points, alz_corr_info* info);
+int alz_group_edge_correlations(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                const alz_corr* corr, const alz_corr_target* target, alz_edge_corr* out, size_t cap,
+                                size_t* n_out, uint32_t* n_points, alz_rollup_info* points, alz_corr_info* info);
+int alz_group_edge_correlations_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                       const alz_corr* corr, const alz_corr_target* target,
+                                       const alz_edge_corr** dev_out, size_t* n_out, uint32_t* n_points,
+                                       alz_rollup_info* points, alz_corr_info* info);
+int alz_group_edge_correlations_top(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k, const alz_metric* m,
+                                    const alz_corr* corr, const alz_corr_target* target, uint32_t top,
+                                    double min_score, alz_edge_corr* out, alz_edge_out* rows, double* series,
+                                    uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                                    alz_rollup_info* points, alz_corr_info* info);
+int alz_group_edge_correlations_top_device(alz_handle* h, uint32_t source, uint32_t tier, uint32_t k,
+                                           const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                           uint32_t top, double min_score, const alz_edge_corr** dev_out,
+                                           const alz_edge_out** dev_rows, const double** dev_series,
+                                           const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                           alz_rollup_info* points, alz_corr_info* info);
+int alz_group_node_correlations(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                alz_node_corr* out, size_t cap, size_t* n_out, uint32_t* n_points,
+                                alz_rollup_info* points, alz_corr_info* info);
+int alz_group_node_correlations_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                       const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                       const alz_node_corr** dev_out, size_t* n_out, uint32_t* n_points,
+                                       alz_rollup_info* points, alz_corr_info* info);
+int alz_group_node_correlations_top(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                    const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                    uint32_t top, double min_score, alz_node_corr* out, alz_node_out* nodes,
+                                    double* series, uint8_t* present, size_t cap, size_t* n_out, uint32_t* n_points,
+                                    alz_rollup_info* points, alz_corr_info* info);
+int alz_group_node_correlations_top_device(alz_handle* h, uint32_t source, uint32_t side, uint32_t tier, uint32_t k,
+                                           const alz_metric* m, const alz_corr* corr, const alz_corr_target* target,
+                                           uint32_t top, double min_score, const alz_node_corr** dev_out,
+                                           const alz_node_out** dev_nodes, const double** dev_series,
+                                           const uint8_t** dev_present, size_t* n_out, uint32_t* n_points,
+                                           alz_rollup_info* points, alz_corr_info* info);
+
 /* ---- tcp_state sink + temporal socket join (SURVEY §8f.2) -------------------
  * alz_submit_tcp replaces processTcpConnect (aggregator/data.go:404-506) +
  * SocketLine.AddValue (sock_num_line.go:62-80); alz_sock_lookup replaces

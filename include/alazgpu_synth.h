@@ -96,6 +96,17 @@ int alz_debug_cycles_rows(alz_handle* h, const alz_edge_out* dev_rows, size_t n,
                           uint32_t min_size, alz_cycle_node* nodes, size_t node_cap, size_t* n_nodes,
                           uint32_t* row_index, alz_edge_out* rows, size_t row_cap, size_t* n_rows,
                           alz_cycle_info* info);
+/* test/debug: the §29 statistic and selection over n caller series of P points in device memory (values[i * P + j],
+ * present[i * P + j], which may hold layouts no series call makes: any P, rows past 2^20, values at absent points). The
+ * values must be finite with |v| <= 2^64, as every §17 metric is. target->n must be P; its window_last is not read.
+ * Records carry a zero head (`valid` and `lag` set). top = 0: every row's record in row order into out[n]; top > 0:
+ * the first min(top, above) in rank order into out, their rows into top_index. More than 2^30 - 1 rows or slots:
+ * ALZ_E_CAPACITY. *n_out, *valid and *above (each may be NULL but n_out) as alz_corr_info gives them. Uses the edge
+ * correlation calls' buffers. */
+int alz_debug_corr_series(alz_handle* h, const double* dev_values, const uint8_t* dev_present, size_t n, uint32_t P,
+                          const alz_corr_target* target, const alz_corr* corr, uint32_t top, double min_score,
+                          alz_edge_corr* out, uint32_t* top_index, size_t cap, size_t* n_out, uint64_t* valid,
+                          uint64_t* above);
 
 typedef struct alz_synth_dev alz_synth_dev;
 int alz_synth_dev_create(alz_handle* h, const alz_synth_topo* topo, alz_synth_dev** out);
